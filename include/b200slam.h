@@ -351,6 +351,56 @@ int b2s_bow_transform(b2s_vocabulary* v, const uint8_t* features, int n, int lev
 int b2s_bow_transform_device(b2s_vocabulary* v, const uint8_t* d_features, int n, int levelsup, int32_t* d_word_id,
                              double* d_weight, int32_t* d_node_id, void* stream);
 
+/* ------------------------------------------------------------------ keyframe database */
+/* KeyFrameDatabase (src/KeyFrameDatabase.cc): place recognition over the BowVectors of the map's keyframes, with the
+ * reference's candidate semantics (DetectLoopCandidates :104-239 for LoopClosing::DetectLoop, DetectRelocalizationCandidates
+ * :252-374 for Tracking::Relocalization) and DBoW2's L1 score (Thirdparty/DBoW2/DBoW2/ScoringObject.cpp:23-68).
+ * The BowVectors live in a device pool indexed by keyframe id; the per-keyframe query state of include/KeyFrame.h:328-338
+ * (mnLoopQuery, mnLoopWords, mLoopScore, mnRelocQuery, mnRelocWords, mRelocScore) is owned by the database, starts at
+ * 0 / 0 / 0.0f and persists across queries exactly as the reference's KeyFrame fields do (the results depend on it).
+ * A BowVector is passed as `n` (word id, value) pairs in ascending word order (std::map order), n <= B2S_KFDB_MAX_WORDS
+ * (longer: B2S_ERR_CAPACITY).  Keyframe ids are < 2^31.  Queries are serialised on the handle's stream; each does one
+ * upload and one download.
+ * covis: GetBestCovisibilityKeyFrames(10) of every keyframe at query time, by keyframe id: covis_ids[id*10 + k] for
+ * k < covis_n[id], id < n_rows (rows at or beyond n_rows are empty).  Neighbours that are not in the database are allowed.
+ * out_ids receives the candidates in the reference's order; *n_out = their number (B2S_ERR_CAPACITY if > cap). */
+#define B2S_KFDB_MAX_WORDS 8192
+typedef struct b2s_kfdb b2s_kfdb;
+typedef struct {
+  uint64_t loop_query;  /* mnLoopQuery */
+  int32_t loop_words;   /* mnLoopWords */
+  float loop_score;     /* mLoopScore */
+  uint64_t reloc_query; /* mnRelocQuery */
+  int32_t reloc_words;  /* mnRelocWords */
+  float reloc_score;    /* mRelocScore */
+} b2s_kfdb_state;
+typedef struct {
+  const uint64_t* ids;  /* [n_rows][10] */
+  const int32_t* n;     /* [n_rows], each <= 10 */
+  int32_t n_rows;
+} b2s_kfdb_covis;
+/* n_words = ORBVocabulary::size() (word ids must be below it) */
+int b2s_kfdb_create(int n_words, int device, b2s_kfdb** out);
+void b2s_kfdb_destroy(b2s_kfdb* db);
+/* add(pKF) (:53-60).  A keyframe id that is already in the database: B2S_ERR_BAD_ARG (the system adds each keyframe once). */
+int b2s_kfdb_add(b2s_kfdb* db, uint64_t kf_id, const uint32_t* words, const double* values, int n);
+/* erase(pKF) (:63-84): no effect for an id that is not in the database; the keyframe's query state is kept. */
+int b2s_kfdb_erase(b2s_kfdb* db, uint64_t kf_id);
+/* clear() (:87-91); also resets every keyframe's query state (the system then reuses ids for new keyframes). */
+int b2s_kfdb_clear(b2s_kfdb* db);
+int b2s_kfdb_size(const b2s_kfdb* db, int* n);
+/* DetectLoopCandidates(pKF, minScore): connected_ids = pKF->GetConnectedKeyFrames() (any order). */
+int b2s_kfdb_detect_loop_candidates(b2s_kfdb* db, uint64_t query_kf_id, const uint32_t* words, const double* values, int n,
+                                    const uint64_t* connected_ids, int n_connected, float min_score,
+                                    const b2s_kfdb_covis* covis, uint64_t* out_ids, int cap, int* n_out);
+/* DetectRelocalizationCandidates(F): frame_id = F->mnId. */
+int b2s_kfdb_detect_relocalization_candidates(b2s_kfdb* db, uint64_t frame_id, const uint32_t* words, const double* values,
+                                              int n, const b2s_kfdb_covis* covis, uint64_t* out_ids, int cap, int* n_out);
+/* The query state of keyframe kf_id (the initial state for an id the database never saw). */
+int b2s_kfdb_keyframe_state(b2s_kfdb* db, uint64_t kf_id, b2s_kfdb_state* state);
+/* Device time (CUDA events on the handle's stream) of the kernels of the last query, in ms. */
+float b2s_kfdb_last_query_ms(const b2s_kfdb* db);
+
 /* ------------------------------------------------------------------ LocalBA */
 typedef struct {
   int32_t kf;       /* index into Tcw[] */

@@ -644,6 +644,110 @@ class ORBVocabulary:
         return bow, feat
 
 
+class _KfdbState(ctypes.Structure):
+    _fields_ = [("loop_query", ctypes.c_uint64), ("loop_words", ctypes.c_int32), ("loop_score", ctypes.c_float),
+                ("reloc_query", ctypes.c_uint64), ("reloc_words", ctypes.c_int32), ("reloc_score", ctypes.c_float)]
+
+
+class _KfdbCovis(ctypes.Structure):
+    _fields_ = [("ids", _vp), ("n", _vp), ("n_rows", ctypes.c_int32)]
+
+
+class KeyFrameDatabase:
+    """Mirror of ORB_SLAM2::KeyFrameDatabase (include/KeyFrameDatabase.h) on the device (b2s_kfdb_*).
+
+    A BowVector is (words, values): ascending uint32 word ids and their float64 values.  `covis` is the
+    GetBestCovisibilityKeyFrames(10) table at query time, (ids [n_rows, 10] uint64, n [n_rows] int32) indexed by keyframe
+    id, or None.  The Detect* methods return the candidate keyframe ids in the reference's order."""
+
+    def __init__(self, n_words, device=0):
+        self._h = _vp()
+        L = lib()
+        L.b2s_kfdb_create.argtypes = [ctypes.c_int, ctypes.c_int, _vp]
+        L.b2s_kfdb_destroy.argtypes = [_vp]
+        L.b2s_kfdb_destroy.restype = None
+        L.b2s_kfdb_add.argtypes = [_vp, ctypes.c_uint64, _vp, _vp, ctypes.c_int]
+        L.b2s_kfdb_erase.argtypes = [_vp, ctypes.c_uint64]
+        L.b2s_kfdb_clear.argtypes = [_vp]
+        L.b2s_kfdb_size.argtypes = [_vp, _vp]
+        L.b2s_kfdb_detect_loop_candidates.argtypes = [_vp, ctypes.c_uint64, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int,
+                                                      ctypes.c_float, _vp, _vp, ctypes.c_int, _vp]
+        L.b2s_kfdb_detect_relocalization_candidates.argtypes = [_vp, ctypes.c_uint64, _vp, _vp, ctypes.c_int, _vp, _vp,
+                                                                ctypes.c_int, _vp]
+        L.b2s_kfdb_keyframe_state.argtypes = [_vp, ctypes.c_uint64, _vp]
+        L.b2s_kfdb_last_query_ms.argtypes = [_vp]
+        L.b2s_kfdb_last_query_ms.restype = ctypes.c_float
+        _check(L.b2s_kfdb_create(int(n_words), device, ctypes.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().b2s_kfdb_destroy(self._h)
+            self._h = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @staticmethod
+    def _bow(words, values):
+        return np.ascontiguousarray(words, np.uint32), np.ascontiguousarray(values, np.float64)
+
+    def add(self, kf_id, words, values):
+        w, v = self._bow(words, values)
+        _check(lib().b2s_kfdb_add(self._h, int(kf_id), _p(w), _p(v), len(w)))
+
+    def erase(self, kf_id):
+        _check(lib().b2s_kfdb_erase(self._h, int(kf_id)))
+
+    def clear(self):
+        _check(lib().b2s_kfdb_clear(self._h))
+
+    def size(self):
+        n = ctypes.c_int(0)
+        _check(lib().b2s_kfdb_size(self._h, ctypes.byref(n)))
+        return n.value
+
+    @staticmethod
+    def _covis(covis):
+        if covis is None:
+            return _KfdbCovis(None, None, 0), None
+        ids = np.ascontiguousarray(covis[0], np.uint64).reshape(-1, 10)
+        n = np.ascontiguousarray(covis[1], np.int32)
+        assert len(n) == len(ids)
+        return _KfdbCovis(ids.ctypes.data, n.ctypes.data, len(n)), (ids, n)
+
+    def _detect(self, fn, *args, covis):
+        c, keep = self._covis(covis)
+        cap = self.size() + 1
+        out = np.zeros(cap, np.uint64)
+        n = ctypes.c_int(0)
+        _check(fn(self._h, *args, ctypes.byref(c), _p(out), cap, ctypes.byref(n)))
+        return out[:n.value].tolist()
+
+    def DetectLoopCandidates(self, kf_id, words, values, connected, min_score, covis=None):
+        w, v = self._bow(words, values)
+        conn = np.ascontiguousarray(list(connected), np.uint64)
+        return self._detect(lib().b2s_kfdb_detect_loop_candidates, int(kf_id), _p(w), _p(v), len(w), _p(conn), len(conn),
+                            float(min_score), covis=covis)
+
+    def DetectRelocalizationCandidates(self, frame_id, words, values, covis=None):
+        w, v = self._bow(words, values)
+        return self._detect(lib().b2s_kfdb_detect_relocalization_candidates, int(frame_id), _p(w), _p(v), len(w),
+                            covis=covis)
+
+    def keyframe_state(self, kf_id):
+        """(mnLoopQuery, mnLoopWords, mLoopScore, mnRelocQuery, mnRelocWords, mRelocScore) of keyframe kf_id."""
+        s = _KfdbState()
+        _check(lib().b2s_kfdb_keyframe_state(self._h, int(kf_id), ctypes.byref(s)))
+        return (s.loop_query, s.loop_words, s.loop_score, s.reloc_query, s.reloc_words, s.reloc_score)
+
+    def last_query_ms(self):
+        """Device time of the last query's kernels (CUDA events on the database's stream)."""
+        return float(lib().b2s_kfdb_last_query_ms(self._h))
+
+
 class Optimizer:
     """Mirror of ORB_SLAM2::Optimizer::LocalBundleAdjustment (include/Optimizer.h:112) on a flattened window."""
 

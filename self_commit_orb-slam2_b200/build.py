@@ -15,8 +15,9 @@ ORACLE_LIB = os.path.join(ORACLE_DIR, "liborb_oracle.so")
 
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_FLAGS = GENCODE + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-O3"]
-# extractor/matcher: bit-exact float arithmetic, never contract a*b+c; LocalBA is FP64 with a 1e-5 bar -> FMA allowed
-NO_FMAD = {"extractor.cu", "extractor_tile.cu", "matcher.cu", "common.cu"}
+# extractor/matcher/keyframe database: bit-exact float arithmetic, never contract a*b+c; LocalBA is FP64 with a 1e-5 bar
+# -> FMA allowed
+NO_FMAD = {"extractor.cu", "extractor_tile.cu", "matcher.cu", "common.cu", "kfdb.cu"}
 
 
 def _newer(target, sources):
@@ -71,9 +72,10 @@ def build_cuda(force=False, verbose=False):
 def build_oracle(force=False):
     srcs = [os.path.join(ORACLE_DIR, f) for f in os.listdir(ORACLE_DIR) if f.endswith((".cpp", ".h"))]
     srcs.append(os.path.join(ROOT, "data", "orb_pattern_31.inc"))
-    if not force and _newer(ORACLE_LIB, srcs):
-        return ORACLE_LIB
-    subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-B", "liborb_oracle.so"])
+    if force or not _newer(ORACLE_LIB, srcs):
+        subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-B", "liborb_oracle.so"])
+    # the keyframe database's CPU restatement (oracle/kfdb.mk)
+    subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "kfdb.mk"] + (["-B"] if force else []) + ["liborb_kfdb.so"])
     return ORACLE_LIB
 
 
@@ -85,6 +87,7 @@ def build_oracle_ref():
     if not os.path.isdir(os.path.join(ref, "src")):
         return None
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "ref", "REF=" + ref])
+    subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "kfdb.mk", "ref", "REF=" + ref])
     return os.path.join(ORACLE_DIR, "_ref")
 
 

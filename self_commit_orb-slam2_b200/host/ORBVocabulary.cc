@@ -86,4 +86,24 @@ void ORBVocabulary::transform(const uint8_t* descriptors, int n, BowVector& v, F
     for (BowVector::iterator it = v.begin(); it != v.end(); ++it) it->second /= norm;
 }
 
+double ORBVocabulary::score(const BowVector& a, const BowVector& b) const {
+  // L1Scoring::score: over the common words in ascending order, one sequential sum (the lower_bound jumps of the
+  // reference only skip words that are not common)
+  double s = 0.0;
+  BowVector::const_iterator i = a.begin(), j = b.begin();
+  while (i != a.end() && j != b.end()) {
+    if (i->first == j->first) {
+      const double v = i->second, w = j->second;
+      s += std::fabs(v - w) - std::fabs(v) - std::fabs(w);
+      ++i;
+      ++j;
+    } else if (i->first < j->first) {
+      i = a.lower_bound(j->first);
+    } else {
+      j = b.lower_bound(i->first);
+    }
+  }
+  return -s / 2.0;  // ||v - w||_1 scaled to [0, 1] (Nister, 2006)
+}
+
 }  // namespace ORB_SLAM2

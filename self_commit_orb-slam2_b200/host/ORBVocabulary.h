@@ -34,6 +34,11 @@ class ORBVocabulary {
   // for the ORB vocabulary's TF_IDF weighting and L1 scoring; descriptors: n x 32 bytes (cv::Mat rows)
   void transform(const uint8_t* descriptors, int n, BowVector& v, FeatureVector& fv, int levelsup) const;
 
+  // double score(const BowVector& a, const BowVector& b) const (TemplatedVocabulary.h:1199-1203) for the ORB
+  // vocabulary's L1 scoring (ScoringObject.cpp:23-68), on the host: LoopClosing::DetectLoop calls it per covisible
+  // keyframe; the keyframe database scores on the device (b2s_kfdb_*).
+  double score(const BowVector& a, const BowVector& b) const;
+
  protected:
   b2s_vocabulary* mpHandle = nullptr;
   int mScoring = 0, mWeighting = 0;
