@@ -473,6 +473,48 @@ typedef struct {
 int b2s_pose_optimization(b2s_ba_solver* h, const b2s_pose_problem* p, b2s_pose_result* r);
 int b2s_pose_optimization_batch(b2s_ba_solver* h, int batch, const b2s_pose_problem* p, b2s_pose_result* r);
 
+/* ------------------------------------------------------------------ global bundle adjustment */
+/* Optimizer::BundleAdjustment (src/Optimizer.cc:86-341), the body of GlobalBundleAdjustemnt: one Levenberg run of
+ * `iterations` over every keyframe, map point and observation of the map (LoopClosing::RunGlobalBundleAdjustment, monocular
+ * initialisation), from graph construction to the values handed to SetPose / SetWorldPos (or mTcwGBA / mPosGBA).
+ * Keyframes without an edge and the fixed keyframes keep their estimate but are still written back through the Converter
+ * quaternion round trip; points without an edge are excluded (vbNotIncludedMP) and their rows are not written.
+ * With an empty graph, or the stop flag set before the first iteration, nothing is optimised and the write-back still
+ * happens.  The LM loop runs on the host; every stage of a trial (linearisation, Schur complement, the tiled Cholesky of
+ * the reduced camera system over its block envelope, the substitutions, the update) is FP64 kernels without
+ * floating-point atomics, so two calls on the same input give bit-identical outputs. */
+typedef struct {
+  int n_kf;                 /* the non-bad keyframes, ascending mnId */
+  const float* Tcw;         /* n_kf x 16, GetPose() */
+  const uint8_t* fixed;     /* n_kf; the reference fixes exactly mnId == 0 (src/Optimizer.cc:132) */
+  int n_mp;                 /* the non-bad map points, ascending mnId */
+  const float* points;      /* n_mp x 3 */
+  int n_edges;
+  const b2s_ba_edge* edges; /* grouped by point (ascending), one per (keyframe, point) */
+  float fx, fy, cx, cy, bf;
+  int iterations;           /* nIterations */
+  int robust;               /* bRobust: Huber sqrt(5.99) mono / sqrt(7.815) stereo, deltas passed as float (:141-142) */
+} b2s_gba_problem;
+typedef struct {
+  float* Tcw_out;           /* n_kf x 16: every keyframe, via the Converter quaternion round trip (:294-308) */
+  float* points_out;        /* n_mp x 3; rows of excluded points are not written */
+  uint8_t* point_included;  /* n_mp: 0 = the point has no edge (vbNotIncludedMP, :266-274) */
+  int32_t* trace;           /* optional (>= 256): accept(1)/reject(0) per LM trial, -1 terminated */
+  double chi2_final;        /* robustified chi2 of the returned estimate */
+  int n_trials;
+} b2s_gba_result;
+typedef struct b2s_gba_solver b2s_gba_solver;
+/* Capacities of the problem arrays; the reduced-system storage is sized from each call's free keyframes and grows on
+ * demand.  Supports at least max_kf = 2048, max_mp = 262144, max_edges = 2^21. */
+int b2s_gba_create(int max_kf, int max_mp, int max_edges, int device, b2s_gba_solver** out);
+void b2s_gba_destroy(b2s_gba_solver* h);
+/* stop: pbStopFlag (may be NULL), polled before each iteration and in the trial loop.  Sizes above the handle's
+ * capacities: B2S_ERR_CAPACITY; an index out of range, a duplicate (keyframe, point) pair or points not ascending:
+ * B2S_ERR_BAD_ARG. */
+int b2s_global_ba(b2s_gba_solver* h, const b2s_gba_problem* p, const volatile uint8_t* stop, b2s_gba_result* r);
+/* Device time (CUDA events on the solver's stream) of the last b2s_global_ba call and the LM trials it ran. */
+float b2s_gba_last_ms(const b2s_gba_solver* h, long long* lm_trials);
+
 #ifdef __cplusplus
 }
 #endif

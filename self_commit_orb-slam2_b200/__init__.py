@@ -65,6 +65,18 @@ class _BaResult(ctypes.Structure):
                 ("chi2_final", ctypes.c_double), ("n_trials", ctypes.c_int)]
 
 
+class _GbaProblem(ctypes.Structure):
+    _fields_ = [("n_kf", ctypes.c_int), ("Tcw", _vp), ("fixed", _vp), ("n_mp", ctypes.c_int), ("points", _vp),
+                ("n_edges", ctypes.c_int), ("edges", _vp), ("fx", ctypes.c_float), ("fy", ctypes.c_float),
+                ("cx", ctypes.c_float), ("cy", ctypes.c_float), ("bf", ctypes.c_float), ("iterations", ctypes.c_int),
+                ("robust", ctypes.c_int)]
+
+
+class _GbaResult(ctypes.Structure):
+    _fields_ = [("Tcw_out", _vp), ("points_out", _vp), ("point_included", _vp), ("trace", _vp),
+                ("chi2_final", ctypes.c_double), ("n_trials", ctypes.c_int)]
+
+
 def lib():
     """Loads libb200slam.so (built in-tree by build.py). Fails loudly if it is missing."""
     global _lib
@@ -136,6 +148,13 @@ def lib():
             L.b2s_local_ba.argtypes = [_vp, _vp, _vp, _vp]
             L.b2s_ba_set_sm_budget.argtypes = [_vp, ctypes.c_int]
             L.b2s_local_ba_batch.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+        if hasattr(L, "b2s_gba_create"):
+            L.b2s_gba_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+            L.b2s_gba_destroy.argtypes = [_vp]
+            L.b2s_gba_destroy.restype = None
+            L.b2s_global_ba.argtypes = [_vp, _vp, _vp, _vp]
+            L.b2s_gba_last_ms.restype = ctypes.c_float
+            L.b2s_gba_last_ms.argtypes = [_vp, _vp]
         _lib = L
     return _lib
 
@@ -912,3 +931,54 @@ class Optimizer:
             outs[i]["chi2"] = ress[i].chi2_final
             outs[i]["n_trials"] = ress[i].n_trials
         return outs
+
+
+class GlobalOptimizer:
+    """Mirror of ORB_SLAM2::Optimizer::BundleAdjustment (include/Optimizer.h, src/Optimizer.cc:86-341), the body of
+    GlobalBundleAdjustemnt, on a flattened map (b2s_global_ba).  The handle's capacities bound the problem sizes; the
+    reduced-system storage grows with the maps it is given."""
+
+    def __init__(self, max_kf=2048, max_mp=262144, max_edges=1 << 21, device=0):
+        self._h = _vp()
+        _check(lib().b2s_gba_create(max_kf, max_mp, max_edges, device, ctypes.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().b2s_gba_destroy(self._h)
+            self._h = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def last_ms(self):
+        """(ms, trials): device time of the last call (its stream segments between the host's LM decisions, CUDA
+        events) and the LM trials it ran."""
+        n = ctypes.c_longlong(0)
+        ms = lib().b2s_gba_last_ms(self._h, ctypes.byref(n))
+        return float(ms), int(n.value)
+
+    def BundleAdjustment(self, d, iterations=10, robust=True, stop=None):
+        """d: Tcw (n_kf x 16, the non-bad keyframes by ascending mnId), fixed (n_kf), points (n_mp x 3, the non-bad map
+        points by ascending mnId), edges (ba_edge_dtype, grouped by point, one per (keyframe, point)), fx, fy, cx, cy, bf.
+        Returns Tcw (every keyframe), points (rows of excluded points keep their input), point_included, trace, n_trials,
+        chi2 (robustified chi2 of the returned estimate)."""
+        keep = dict(Tcw=np.ascontiguousarray(d["Tcw"], np.float32).reshape(-1, 16),
+                    fixed=np.ascontiguousarray(d["fixed"], np.uint8),
+                    points=np.ascontiguousarray(d["points"], np.float32).reshape(-1, 3),
+                    edges=np.ascontiguousarray(d["edges"]))
+        assert keep["edges"].dtype == ba_edge_dtype
+        nkf, nmp = len(keep["Tcw"]), len(keep["points"])
+        p = _GbaProblem(nkf, keep["Tcw"].ctypes.data, keep["fixed"].ctypes.data, nmp, keep["points"].ctypes.data,
+                        len(keep["edges"]), keep["edges"].ctypes.data, float(d["fx"]), float(d["fy"]), float(d["cx"]),
+                        float(d["cy"]), float(d["bf"]), int(iterations), int(bool(robust)))
+        out = dict(Tcw=np.zeros((nkf, 16), np.float32), points=keep["points"].copy(),
+                   point_included=np.zeros(nmp, np.uint8), trace=np.full(256, -1, np.int32))
+        r = _GbaResult(out["Tcw"].ctypes.data, out["points"].ctypes.data, out["point_included"].ctypes.data,
+                       out["trace"].ctypes.data, 0.0, 0)
+        _check(lib().b2s_global_ba(self._h, ctypes.byref(p), _p(stop), ctypes.byref(r)))
+        out["chi2"] = r.chi2_final
+        out["n_trials"] = r.n_trials
+        return out

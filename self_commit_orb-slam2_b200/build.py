@@ -38,6 +38,8 @@ def _deps_of(src):
     deps = [src, os.path.join(CSRC, "common.cuh"), os.path.join(ROOT, "include", "b200slam.h"), os.path.abspath(__file__)]
     if base.startswith("extractor"):
         deps.append(os.path.join(CSRC, "extractor.cuh"))
+    if base in ("localba.cu", "gba.cu"):
+        deps.append(os.path.join(CSRC, "ba_math.cuh"))
     if base == "extractor.cu":
         deps.append(os.path.join(ROOT, "data", "orb_pattern_31.inc"))
     return deps
@@ -76,6 +78,8 @@ def build_oracle(force=False):
         subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-B", "liborb_oracle.so"])
     # the keyframe database's CPU restatement (oracle/kfdb.mk)
     subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "kfdb.mk"] + (["-B"] if force else []) + ["liborb_kfdb.so"])
+    # the global bundle adjustment's CPU restatement (oracle/gba.mk)
+    subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "gba.mk"] + (["-B"] if force else []) + ["liborb_gba.so"])
     return ORACLE_LIB
 
 
@@ -88,6 +92,7 @@ def build_oracle_ref():
         return None
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "kfdb.mk", "ref", "REF=" + ref])
+    subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "gba.mk", "gba-ref", "REF=" + ref])
     return os.path.join(ORACLE_DIR, "_ref")
 
 

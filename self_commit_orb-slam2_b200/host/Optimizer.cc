@@ -94,4 +94,48 @@ int Optimizer::PoseOptimization(const PoseProblem& f, float TcwOut[16], std::vec
   return r.n_inliers;
 }
 
+// Global BA runs on LoopClosing's GBA thread (and once for the monocular initial map): its own handle, grown on demand
+static b2s_gba_solver* g_gbaSolver = nullptr;
+static int g_gkf = 0, g_gmp = 0, g_ge = 0;
+static std::mutex g_gbaMutex;
+
+void Optimizer::BundleAdjustment(const GlobalBAMap& m, int nIterations, bool* pbStopFlag, bool bRobust,
+                                 GlobalBAResult& out) {
+  std::lock_guard<std::mutex> lock(g_gbaMutex);
+  const int nKF = (int)m.fixed.size(), nMP = (int)m.points.size() / 3, nE = (int)m.edges.size();
+  if (!g_gbaSolver || nKF > g_gkf || nMP > g_gmp || nE > g_ge) {
+    b2s_gba_destroy(g_gbaSolver);
+    g_gbaSolver = nullptr;
+    g_gkf = nKF > 256 ? nKF : 256;
+    g_gmp = nMP > 32768 ? nMP : 32768;
+    g_ge = nE > 262144 ? nE : 262144;
+    const char* e = getenv("B2S_DEVICE");
+    int rc = b2s_gba_create(g_gkf, g_gmp, g_ge, e ? atoi(e) : 0, &g_gbaSolver);
+    if (rc != B2S_OK) {
+      fprintf(stderr, "Optimizer::BundleAdjustment: libb200slam error %d: %s\n", rc, b2s_last_error());
+      throw std::runtime_error(b2s_last_error());
+    }
+  }
+  b2s_gba_problem p;
+  p.n_kf = nKF; p.Tcw = m.Tcw.data(); p.fixed = m.fixed.data();
+  p.n_mp = nMP; p.points = m.points.data();
+  p.n_edges = nE; p.edges = m.edges.data();
+  p.fx = m.fx; p.fy = m.fy; p.cx = m.cx; p.cy = m.cy; p.bf = m.bf;
+  p.iterations = nIterations;
+  p.robust = bRobust ? 1 : 0;
+  out.Tcw.assign((size_t)nKF * 16, 0.f);
+  out.points = m.points;
+  out.included.assign((size_t)(nMP > 0 ? nMP : 1), 0);
+  b2s_gba_result r;
+  r.Tcw_out = out.Tcw.data(); r.points_out = out.points.data(); r.point_included = out.included.data();
+  r.trace = nullptr; r.chi2_final = 0; r.n_trials = 0;
+  static_assert(sizeof(bool) == 1, "bool stop flag is read as a byte");
+  int rc = b2s_global_ba(g_gbaSolver, &p, (const volatile uint8_t*)pbStopFlag, &r);
+  if (rc != B2S_OK) {
+    fprintf(stderr, "Optimizer::BundleAdjustment: libb200slam error %d: %s\n", rc, b2s_last_error());
+    throw std::runtime_error(b2s_last_error());
+  }
+  out.included.resize(nMP);
+}
+
 }  // namespace ORB_SLAM2

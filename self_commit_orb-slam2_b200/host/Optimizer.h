@@ -35,6 +35,20 @@ struct PoseProblem {                 // Optimizer::PoseOptimization(Frame*) on t
   float fx = 0, fy = 0, cx = 0, cy = 0, bf = 0;
 };
 
+struct GlobalBAMap {                 // Optimizer::BundleAdjustment on the flattened map (src/Optimizer.cc:86-275)
+  std::vector<float> Tcw;            // nKF x 16: the non-bad keyframes by ascending mnId (KeyFrame::GetPose())
+  std::vector<uint8_t> fixed;        // nKF: mnId == 0
+  std::vector<float> points;         // nMP x 3: the non-bad map points by ascending mnId
+  std::vector<b2s_ba_edge> edges;    // grouped by point, observations of non-bad keyframes with mnId <= maxKFid
+  float fx = 0, fy = 0, cx = 0, cy = 0, bf = 0;
+};
+
+struct GlobalBAResult {
+  std::vector<float> Tcw;            // nKF x 16 -> SetPose (nLoopKF == 0) or mTcwGBA
+  std::vector<float> points;         // nMP x 3  -> SetWorldPos + UpdateNormalAndDepth, or mPosGBA (included points only)
+  std::vector<uint8_t> included;     // nMP: 0 = no edge (vbNotIncludedMP): not written back
+};
+
 class Optimizer {
  public:
   // int static PoseOptimization(Frame* pFrame) (include/Optimizer.h:100, src/Optimizer.cc:363-605): fills TcwOut (the
@@ -42,6 +56,8 @@ class Optimizer {
   static int PoseOptimization(const PoseProblem& f, float TcwOut[16], std::vector<uint8_t>& outlier);
   // void static LocalBundleAdjustment(KeyFrame* pKF, bool* pbStopFlag, Map* pMap) on the flattened window
   static void LocalBundleAdjustment(const LocalBAWindow& w, bool* pbStopFlag, LocalBAResult& out);
+  // void static BundleAdjustment(vpKF, vpMP, nIterations, pbStopFlag, nLoopKF, bRobust) on the flattened map
+  static void BundleAdjustment(const GlobalBAMap& m, int nIterations, bool* pbStopFlag, bool bRobust, GlobalBAResult& out);
 };
 
 }  // namespace ORB_SLAM2

@@ -1,11 +1,14 @@
 // Optimizer_b200.cc — drop-in bodies of
 //     void Optimizer::LocalBundleAdjustment(KeyFrame* pKF, bool* pbStopFlag, Map* pMap)   include/Optimizer.h:112
 //     int  Optimizer::PoseOptimization(Frame* pFrame)                                      include/Optimizer.h:100
-// with the reference's exact signatures, for the LocalMapping / Tracking threads to call unchanged
-// (src/LocalMapping.cc:123, src/Tracking.cc:1219, 1398, 1834, 2078, 2152 ...).  Compile this file INSIDE the reference
-// tree (it includes the reference's own include/Optimizer.h) in place of those two function bodies of src/Optimizer.cc
-// (:363-605, :629-997) and link libb200slam.so; the other Optimizer functions (global BA, essential graph, Sim3) are
-// outside the hot path (SURVEY.md §8) and stay as they are.
+//     void Optimizer::GlobalBundleAdjustemnt(Map*, int, bool*, unsigned long, bool)       src/Optimizer.cc:55
+//     void Optimizer::BundleAdjustment(const vector<KeyFrame*>&, const vector<MapPoint*>&, int, bool*, unsigned long,
+//                                      bool)                                              src/Optimizer.cc:86
+// with the reference's exact signatures, for the LocalMapping / Tracking / LoopClosing threads to call unchanged
+// (src/LocalMapping.cc:123, src/Tracking.cc:1081, 1219, 1398, 1834, 2078, 2152, src/LoopClosing.cc:880-895 ...).  Compile
+// this file INSIDE the reference tree (it includes the reference's own include/Optimizer.h) in place of those function
+// bodies of src/Optimizer.cc (:55-341, :363-605, :629-997) and link libb200slam.so; the other Optimizer functions
+// (essential graph, Sim3) stay as they are.
 //
 // What stays on the host is what touches the object graph: the window selection (local keyframes = pKF + covisibles,
 // local map points = their matches, fixed cameras = other observers; the mnBALocalForKF / mnBAFixedForKF marks other
@@ -17,6 +20,7 @@
 // tests: oracle/ref_optimizer_glue.cpp builds the same stub object graph for this file (oracle/_ref/libadapter_optimizer.so)
 // and for the reference's own Optimizer.cc (libref_optimizer.so); tests/test_adapters_gpu.py requires identical erase
 // lists and poses / landmarks within the parity bar.
+#include <algorithm>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -59,6 +63,28 @@ struct SolverSlot {
   }
 };
 SolverSlot g_localBA, g_pose;
+
+// The global bundle adjustment's handle (LoopClosing's GBA thread, or Tracking's monocular initialisation), grown on demand.
+struct GbaSlot {
+  b2s_gba_solver* h = nullptr;
+  int kf = 0, mp = 0, edges = 0;
+  std::mutex m;
+  b2s_gba_solver* get(int nKF, int nMP, int nE) {
+    if (h && nKF <= kf && nMP <= mp && nE <= edges) return h;
+    b2s_gba_destroy(h);
+    h = nullptr;
+    kf = nKF > 256 ? nKF : 256;
+    mp = nMP > 32768 ? nMP : 32768;
+    edges = nE > 262144 ? nE : 262144;
+    if (b2s_gba_create(kf, mp, edges, device_index(), &h) != B2S_OK) {
+      fprintf(stderr, "Optimizer (b200): %s\n", b2s_last_error());
+      h = nullptr;
+      kf = mp = edges = 0;
+    }
+    return h;
+  }
+};
+GbaSlot g_gba;
 
 void pose_to_floats(const cv::Mat& T, float* out) {
   for (int i = 0; i < 4; i++)
@@ -259,6 +285,126 @@ int Optimizer::PoseOptimization(Frame* pFrame) {
     for (int j = 0; j < 4; j++) T.at<float>(i, j) = TcwOut[4 * i + j];
   pFrame->SetPose(T);
   return res.n_inliers;
+}
+
+void Optimizer::GlobalBundleAdjustemnt(Map* pMap, int nIterations, bool* pbStopFlag, const unsigned long nLoopKF,
+                                       const bool bRobust) {
+  std::vector<KeyFrame*> vpKFs = pMap->GetAllKeyFrames();
+  std::vector<MapPoint*> vpMP = pMap->GetAllMapPoints();
+  BundleAdjustment(vpKFs, vpMP, nIterations, pbStopFlag, nLoopKF, bRobust);
+}
+
+void Optimizer::BundleAdjustment(const std::vector<KeyFrame*>& vpKFs, const std::vector<MapPoint*>& vpMP, int nIterations,
+                                 bool* pbStopFlag, const unsigned long nLoopKF, const bool bRobust) {
+  // ---- gather (src/Optimizer.cc:117-275): non-bad keyframes by ascending mnId (g2o orders vertices by id), mnId == 0
+  // fixed; non-bad points by ascending mnId, one edge per observation of a non-bad keyframe with mnId <= maxKFid
+  std::vector<KeyFrame*> kfs;
+  unsigned long maxKFid = 0;
+  for (size_t i = 0; i < vpKFs.size(); i++) {
+    if (vpKFs[i]->isBad()) continue;
+    kfs.push_back(vpKFs[i]);
+    if (vpKFs[i]->mnId > maxKFid) maxKFid = vpKFs[i]->mnId;
+  }
+  std::sort(kfs.begin(), kfs.end(), [](KeyFrame* a, KeyFrame* b) { return a->mnId < b->mnId; });
+  std::vector<MapPoint*> mps;
+  for (size_t i = 0; i < vpMP.size(); i++)
+    if (!vpMP[i]->isBad()) mps.push_back(vpMP[i]);
+  std::sort(mps.begin(), mps.end(), [](MapPoint* a, MapPoint* b) { return a->mnId < b->mnId; });
+  const int nKF = (int)kfs.size(), nMP = (int)mps.size();
+  std::map<KeyFrame*, int> kfIndex;
+  std::vector<float> Tcw((size_t)nKF * 16), pts((size_t)nMP * 3);
+  std::vector<uint8_t> fixed((size_t)nKF, 0);
+  float fx = 0, fy = 0, cx = 0, cy = 0, bf = 0;
+  for (int k = 0; k < nKF; k++) {
+    kfIndex[kfs[k]] = k;
+    pose_to_floats(kfs[k]->GetPose(), &Tcw[(size_t)16 * k]);
+    fixed[k] = kfs[k]->mnId == 0;  // :132
+  }
+  std::vector<b2s_ba_edge> edges;
+  for (int m = 0; m < nMP; m++) {
+    const cv::Mat X = mps[m]->GetWorldPos();
+    for (int c = 0; c < 3; c++) pts[(size_t)3 * m + c] = X.at<float>(c);
+    const std::map<KeyFrame*, size_t> observations = mps[m]->GetObservations();
+    for (std::map<KeyFrame*, size_t>::const_iterator it = observations.begin(); it != observations.end(); ++it) {
+      KeyFrame* k = it->first;
+      if (k->isBad() || k->mnId > maxKFid) continue;  // :178-179
+      std::map<KeyFrame*, int>::const_iterator ki = kfIndex.find(k);
+      if (ki == kfIndex.end()) continue;  // (an observer outside the keyframe list: not a vertex of the graph)
+      const cv::KeyPoint& kp = k->mvKeysUn[it->second];
+      b2s_ba_edge e;
+      e.kf = ki->second;
+      e.mp = m;
+      e.obs[0] = kp.pt.x;
+      e.obs[1] = kp.pt.y;
+      e.obs[2] = k->mvuRight[it->second];  // < 0: monocular observation (:186)
+      e.inv_sigma2 = k->mvInvLevelSigma2[kp.octave];
+      edges.push_back(e);
+      if (edges.size() == 1) {
+        fx = k->fx; fy = k->fy; cx = k->cx; cy = k->cy; bf = k->mbf;
+      } else if (k->fx != fx || k->fy != fy || k->cx != cx || k->cy != cy || k->mbf != bf) {
+        fprintf(stderr, "Optimizer::BundleAdjustment (b200): keyframes with different intrinsics are not supported\n");
+        return;
+      }
+    }
+  }
+  const int nE = (int)edges.size();
+  std::vector<float> TcwOut((size_t)(nKF > 0 ? nKF : 1) * 16), ptsOut((size_t)(nMP > 0 ? nMP : 1) * 3);
+  std::vector<uint8_t> included((size_t)(nMP > 0 ? nMP : 1), 0);
+  b2s_gba_problem prob;
+  prob.n_kf = nKF;
+  prob.Tcw = Tcw.data();
+  prob.fixed = fixed.data();
+  prob.n_mp = nMP;
+  prob.points = pts.data();
+  prob.n_edges = nE;
+  prob.edges = edges.data();
+  prob.fx = fx; prob.fy = fy; prob.cx = cx; prob.cy = cy; prob.bf = bf;
+  prob.iterations = nIterations;
+  prob.robust = bRobust ? 1 : 0;
+  b2s_gba_result res;
+  res.Tcw_out = TcwOut.data();
+  res.points_out = ptsOut.data();
+  res.point_included = included.data();
+  res.trace = nullptr;
+  res.chi2_final = 0;
+  res.n_trials = 0;
+  {
+    std::lock_guard<std::mutex> lock(g_gba.m);
+    b2s_gba_solver* solver = g_gba.get(nKF, nMP, nE);
+    if (!solver) return;
+    static_assert(sizeof(bool) == 1, "the stop flag is polled as one byte");
+    if (b2s_global_ba(solver, &prob, reinterpret_cast<const volatile uint8_t*>(pbStopFlag), &res) != B2S_OK) {
+      fprintf(stderr, "Optimizer::BundleAdjustment (b200): %s\n", b2s_last_error());
+      return;
+    }
+  }
+
+  // ---- scatter (:287-340): direct writes for the initial map (nLoopKF == 0), else the GBA copies for LoopClosing
+  for (int k = 0; k < nKF; k++) {
+    cv::Mat T(4, 4, CV_32F);
+    for (int i = 0; i < 4; i++)
+      for (int j = 0; j < 4; j++) T.at<float>(i, j) = TcwOut[(size_t)16 * k + 4 * i + j];
+    if (nLoopKF == 0) {
+      kfs[k]->SetPose(T);
+    } else {
+      kfs[k]->mTcwGBA.create(4, 4, CV_32F);
+      T.copyTo(kfs[k]->mTcwGBA);
+      kfs[k]->mnBAGlobalForKF = nLoopKF;
+    }
+  }
+  for (int m = 0; m < nMP; m++) {
+    if (!included[m]) continue;  // vbNotIncludedMP
+    cv::Mat X(3, 1, CV_32F);
+    for (int c = 0; c < 3; c++) X.at<float>(c) = ptsOut[(size_t)3 * m + c];
+    if (nLoopKF == 0) {
+      mps[m]->SetWorldPos(X);
+      mps[m]->UpdateNormalAndDepth();
+    } else {
+      mps[m]->mPosGBA.create(3, 1, CV_32F);
+      X.copyTo(mps[m]->mPosGBA);
+      mps[m]->mnBAGlobalForKF = nLoopKF;
+    }
+  }
 }
 
 }  // namespace ORB_SLAM2
