@@ -344,8 +344,7 @@ class ORBmatcher:
     def SearchByProjection(self, queries, kpx, kpy, octave, angle, uright, occupied, desc, geom, th, mode=0,
                            th_high=TH_HIGH):
         nf = len(kpx)
-        sf = np.ascontiguousarray(geom["scale_factors"], np.float32)
-        g = _FrameGeom(geom["mnMinX"], geom["mnMinY"], geom["mnMaxX"], geom["mnMaxY"], geom["bf"], sf.ctypes.data, len(sf))
+        g, sf = self.frame_geom(geom)
         match = np.full(nf, -1, np.int32)
         nm = ctypes.c_int(0)
         _check(lib().b2s_search_by_projection_last(self._h, _p(queries), len(queries), _p(kpx), _p(kpy), _p(octave),
@@ -417,8 +416,7 @@ class ORBmatcher:
         n1, n2 = len(octave1), len(kpx2)
         prev_in = np.ascontiguousarray(prev, np.float32)
         px, py = np.ascontiguousarray(prev_in[:, 0]), np.ascontiguousarray(prev_in[:, 1])
-        sf = np.ascontiguousarray(geom["scale_factors"], np.float32)
-        g = _FrameGeom(geom["mnMinX"], geom["mnMinY"], geom["mnMaxX"], geom["mnMaxY"], geom["bf"], sf.ctypes.data, len(sf))
+        g, sf = self.frame_geom(geom)
         keep = [np.ascontiguousarray(octave1, np.int32), np.ascontiguousarray(angle1, np.float32),
                 np.ascontiguousarray(desc1, np.uint8), np.ascontiguousarray(kpx2, np.float32),
                 np.ascontiguousarray(kpy2, np.float32), np.ascontiguousarray(octave2, np.int32),
@@ -451,8 +449,7 @@ class ORBmatcher:
     def SearchByProjectionMap(self, queries, kpx, kpy, octave, uright, occupied, desc, geom, th=1.0, th_high=TH_HIGH):
         """SearchByProjection(Frame&, const vector<MapPoint*>&, th) (src/ORBmatcher.cc:70-175); queries: map_query_dtype."""
         nf = len(kpx)
-        sf = np.ascontiguousarray(geom["scale_factors"], np.float32)
-        g = _FrameGeom(geom["mnMinX"], geom["mnMinY"], geom["mnMaxX"], geom["mnMaxY"], geom["bf"], sf.ctypes.data, len(sf))
+        g, sf = self.frame_geom(geom)
         match = np.full(nf, -1, np.int32)
         nm = ctypes.c_int(0)
         _check(lib().b2s_search_by_projection_map(self._h, _p(queries), len(queries), _p(kpx), _p(kpy), _p(octave),
@@ -466,8 +463,7 @@ class ORBmatcher:
         """Search core of Fuse (src/ORBmatcher.cc:1020-1174, :1179-1310) and SearchByProjection(KeyFrame*, Scw, ...)
         (:388-512); queries: win_query_dtype.  Returns (n_accepted, best_idx, best_dist)."""
         nq, nf = len(queries), len(kpx)
-        sf = np.ascontiguousarray(geom["scale_factors"], np.float32)
-        g = _FrameGeom(geom["mnMinX"], geom["mnMinY"], geom["mnMaxX"], geom["mnMaxY"], geom["bf"], sf.ctypes.data, len(sf))
+        g, sf = self.frame_geom(geom)
         best = np.full(nq, -1, np.int32)
         bdist = np.full(nq, 256, np.int32)
         nacc = ctypes.c_int(0)
@@ -545,8 +541,7 @@ class FrameGrid:
         L.b2s_search_by_projection_map_grid.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_float, ctypes.c_int,
                                                         ctypes.c_float, _vp, _vp]
         L.b2s_search_windows_grid.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]
-        sf = np.ascontiguousarray(geom["scale_factors"], np.float32)
-        g = _FrameGeom(geom["mnMinX"], geom["mnMinY"], geom["mnMaxX"], geom["mnMaxY"], geom["bf"], sf.ctypes.data, len(sf))
+        g, sf = ORBmatcher.frame_geom(geom)
         is2 = None if inv_level_sigma2 is None else np.ascontiguousarray(inv_level_sigma2, np.float32)
         if d_kps_ptr is not None:
             _check(L.b2s_frame_grid_create_device(matcher._h, _vp(d_kps_ptr), _vp(d_desc_ptr), int(nf),

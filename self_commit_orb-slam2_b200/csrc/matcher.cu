@@ -1686,26 +1686,8 @@ extern "C" int b2s_search_by_bow(b2s_matcher* h, const uint8_t* descA, const int
   for (int j = 0; j < nB; j++) matchB[j] = -1;
   if (nA == 0 || nB == 0) return B2S_OK;
   if (!descA || !nodeA || !angA || !descB || !nodeB || !angB) return B2S_ERR_BAD_ARG;
-  B2S_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = h->stream;
-  B2S_CUDA(cudaMemcpyAsync(h->dDescA, descA, (size_t)nA * 32, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dNodeA, nodeA, (size_t)nA * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dAngA, angA, (size_t)nA * 4, cudaMemcpyHostToDevice, st));
-  if (validA) B2S_CUDA(cudaMemcpyAsync(h->dValidA, validA, (size_t)nA, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dDescB, descB, (size_t)nB * 32, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dNodeB, nodeB, (size_t)nB * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dAngB, angB, (size_t)nB * 4, cudaMemcpyHostToDevice, st));
-  if (validB) B2S_CUDA(cudaMemcpyAsync(h->dValidB, validB, (size_t)nB, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dNA, &nA, 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dNB, &nB, 4, cudaMemcpyHostToDevice, st));
-  int rc = b2s_search_by_bow_device(h, 1, h->dDescA, h->dNodeA, validA ? h->dValidA : nullptr, h->dAngA, h->dNA, nA,
-                                    h->dDescB, h->dNodeB, validB ? h->dValidB : nullptr, h->dAngB, h->dNB, nB, th_low,
-                                    nnratio, strict_lt, check_ori, h->dMatch, h->dNMatches, st);
-  if (rc != B2S_OK) return rc;
-  B2S_CUDA(cudaMemcpyAsync(matchB, h->dMatch, (size_t)nB * 4, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaMemcpyAsync(nmatches, h->dNMatches, 4, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaStreamSynchronize(st));
-  return B2S_OK;
+  return b2s_search_by_bow_batch(h, 1, descA, nodeA, validA, angA, &nA, nA, descB, nodeB, validB, angB, &nB, nB, th_low,
+                                 nnratio, strict_lt, check_ori, matchB, nmatches);
 }
 
 extern "C" int b2s_search_by_bow_batch(b2s_matcher* h, int batch, const uint8_t* descA, const int32_t* nodeA,
@@ -1743,6 +1725,162 @@ extern "C" int b2s_search_by_bow_batch(b2s_matcher* h, int batch, const uint8_t*
   return B2S_OK;
 }
 
+// ================================================================================================ projection searches
+// Every projection search runs on a frame grid: a resident b2s_frame_grid, or the matcher's own work buffers seen as one
+// (scratch_grid) for the host-buffer calls, which upload the frame's features and build the grid on every call.
+
+// Grid bounds, cell scales (src/Frame.cc:213-214), bf and the level tables of one frame; a null table reads as zeros.
+// th / mode / thHigh / checkOri / winFlags are left to each search.
+static ProjGeom proj_geom(const b2s_frame_geom* g, const float* inv_level_sigma2) {
+  ProjGeom pg;
+  memset(&pg, 0, sizeof(pg));
+  pg.minX = g->mnMinX; pg.minY = g->mnMinY; pg.maxX = g->mnMaxX; pg.maxY = g->mnMaxY;
+  pg.invW = (float)GRID_COLS / (g->mnMaxX - g->mnMinX);
+  pg.invH = (float)GRID_ROWS / (g->mnMaxY - g->mnMinY);
+  pg.bf = g->bf; pg.nlevels = g->nlevels;
+  for (int i = 0; i < 16 && i < g->nlevels; i++) {
+    pg.scale[i] = g->scale_factors ? g->scale_factors[i] : 0.f;
+    pg.invSigma2[i] = inv_level_sigma2 ? inv_level_sigma2[i] : 0.f;
+  }
+  return pg;
+}
+
+struct b2s_frame_grid {
+  b2s_matcher* owner = nullptr;  // identity check only: never dereferenced after creation-time use by destroy
+  int device = 0;
+  int nf = 0;
+  ProjGeom pg;  // geometry + scale tables (th / mode / thresholds are filled per search)
+  float *kpx = nullptr, *kpy = nullptr, *ang = nullptr, *uright = nullptr;
+  int32_t *oct = nullptr, *order = nullptr, *cellStart = nullptr, *cellKey = nullptr, *nB = nullptr, *qOut = nullptr;
+  uint8_t* desc = nullptr;
+};
+
+// The grid of a host-buffer search: it aliases the matcher's work buffers, owns nothing and is never passed to
+// b2s_frame_grid_destroy.
+static b2s_frame_grid scratch_grid(b2s_matcher* h, int nf, const ProjGeom& pg) {
+  b2s_frame_grid gr;
+  gr.owner = h; gr.device = h->device; gr.nf = nf; gr.pg = pg;
+  gr.kpx = h->dKpx; gr.kpy = h->dKpy; gr.ang = h->dAngB; gr.uright = h->dURight; gr.oct = h->dOct; gr.desc = h->dDescB;
+  gr.order = h->dOrder; gr.cellStart = h->dCellStart; gr.cellKey = h->dCellKey; gr.nB = h->dNB;
+  return gr;
+}
+
+// Frame::AssignFeaturesToGrid (src/Frame.cc:461-491) on the arrays already in gr: cell key, stable rank, cell starts
+static int grid_build(b2s_frame_grid& gr, cudaStream_t st) {
+  const int nf = gr.nf;
+  B2S_CUDA(cudaMemcpyAsync(gr.nB, &gr.nf, 4, cudaMemcpyHostToDevice, st));
+  if (nf > 0) {
+    k_proj_cell_key<<<div_up(nf, 256), 256, 0, st>>>(gr.kpx, gr.kpy, nf, gr.pg, gr.cellKey);
+    k_rank_by_key<<<dim3(div_up(nf, 128), 1), 128, 0, st>>>(gr.cellKey, gr.nB, nf, gr.order);
+  }
+  k_proj_cell_start<<<div_up(nf + 1, 256), 256, 0, st>>>(gr.cellKey, gr.order, nf, gr.cellStart);
+  gr.owner->launches += 3;
+  B2S_CUDA(cudaGetLastError());
+  return B2S_OK;
+}
+
+// host feature arrays into gr, then grid_build.  A null angle or uright array is not uploaded: the searches that do not
+// read it pass none.
+static int grid_upload(b2s_frame_grid& gr, const float* kpx, const float* kpy, const int32_t* octave, const float* angle,
+                       const float* uright, const uint8_t* desc, cudaStream_t st) {
+  const size_t n = (size_t)gr.nf;
+  if (n > 0) {
+    B2S_CUDA(cudaMemcpyAsync(gr.kpx, kpx, n * 4, cudaMemcpyHostToDevice, st));
+    B2S_CUDA(cudaMemcpyAsync(gr.kpy, kpy, n * 4, cudaMemcpyHostToDevice, st));
+    B2S_CUDA(cudaMemcpyAsync(gr.oct, octave, n * 4, cudaMemcpyHostToDevice, st));
+    if (angle) B2S_CUDA(cudaMemcpyAsync(gr.ang, angle, n * 4, cudaMemcpyHostToDevice, st));
+    if (uright) B2S_CUDA(cudaMemcpyAsync(gr.uright, uright, n * 4, cudaMemcpyHostToDevice, st));
+    B2S_CUDA(cudaMemcpyAsync(gr.desc, desc, n * 32, cudaMemcpyHostToDevice, st));
+  }
+  return grid_build(gr, st);
+}
+
+// The three searches on a built grid (nq > 0, gr.nf > 0): upload the queries and the occupancy flags, run, download.
+// SearchByProjection(CurrentFrame, LastFrame) and relocalisation: 4 launches
+static int proj_search_last(b2s_matcher* h, const b2s_frame_grid& gr, const b2s_proj_query* q, int nq, const uint8_t* occupied,
+                            float th, int mode, int th_high, int check_ori, int32_t* match_cur, int* nmatches) {
+  const int nf = gr.nf;
+  cudaStream_t st = h->stream;
+  ProjGeom pg = gr.pg;
+  pg.th = th; pg.mode = mode; pg.thHigh = th_high; pg.checkOri = check_ori;
+  const uint8_t* occ = occupied ? h->dOcc : nullptr;
+  B2S_CUDA(cudaMemcpyAsync(h->dQueries, q, (size_t)nq * sizeof(ProjQuery), cudaMemcpyHostToDevice, st));
+  if (occ) B2S_CUDA(cudaMemcpyAsync(h->dOcc, occupied, (size_t)nf, cudaMemcpyHostToDevice, st));
+  B2S_CUDA(cudaMemsetAsync(h->dTaken, 0, (size_t)nf, st));
+  k_fill_i32<<<div_up(nf, 256), 256, 0, st>>>(h->dMatch, -1, (size_t)nf);
+  k_proj_topk<ProjQuery><<<div_up(nq, 8), 256, 0, st>>>(h->dQueries, nq, gr.kpx, gr.kpy, gr.oct, gr.uright, occ, gr.desc,
+                                                        gr.order, gr.cellStart, pg, h->dTopk, h->dTopkIdx, h->dCandCnt);
+  k_proj_resolve<<<1, 32, 0, st>>>(h->dQueries, nq, gr.kpx, gr.kpy, gr.oct, gr.ang, gr.uright, occ, gr.desc, gr.order,
+                                   gr.cellStart, pg, h->dTopk, h->dTopkIdx, h->dCandCnt, h->dTaken, h->dMatch, h->dPush,
+                                   h->dExtra, h->dHist);
+  k_proj_cull<<<1, 256, 0, st>>>(check_ori, h->dHist, h->dExtra, h->dMatch, h->dPush, h->dNMatches);
+  h->launches += 4;
+  B2S_CUDA(cudaGetLastError());
+  B2S_CUDA(cudaMemcpyAsync(match_cur, h->dMatch, (size_t)nf * 4, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA(cudaMemcpyAsync(nmatches, h->dNMatches, 4, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA(cudaStreamSynchronize(st));
+  return B2S_OK;
+}
+
+// SearchByProjection(Frame&, vector<MapPoint*>&, th): 3 launches
+static int proj_search_map(b2s_matcher* h, const b2s_frame_grid& gr, const b2s_map_query* q, int nq, const uint8_t* occupied,
+                           float th, int th_high, float nnratio, int32_t* match_cur, int* nmatches) {
+  const int nf = gr.nf;
+  cudaStream_t st = h->stream;
+  ProjGeom pg = gr.pg;
+  pg.th = th; pg.mode = 0; pg.thHigh = th_high; pg.checkOri = 0;
+  const uint8_t* occ = occupied ? h->dOcc : nullptr;
+  MapQuery* dQ = reinterpret_cast<MapQuery*>(h->dQueries);
+  B2S_CUDA(cudaMemcpyAsync(dQ, q, (size_t)nq * sizeof(MapQuery), cudaMemcpyHostToDevice, st));
+  if (occ) B2S_CUDA(cudaMemcpyAsync(h->dOcc, occupied, (size_t)nf, cudaMemcpyHostToDevice, st));
+  B2S_CUDA(cudaMemsetAsync(h->dTaken, 0, (size_t)nf, st));
+  k_fill_i32<<<div_up(nf, 256), 256, 0, st>>>(h->dMatch, -1, (size_t)nf);
+  k_proj_topk<MapQuery><<<div_up(nq, 8), 256, 0, st>>>(dQ, nq, gr.kpx, gr.kpy, gr.oct, gr.uright, occ, gr.desc, gr.order,
+                                                       gr.cellStart, pg, h->dTopk, h->dTopkIdx, h->dCandCnt);
+  k_map_resolve<<<1, 32, 0, st>>>(dQ, nq, gr.kpx, gr.kpy, gr.oct, gr.uright, occ, gr.desc, gr.order, gr.cellStart, pg, nnratio,
+                                  h->dTopk, h->dTopkIdx, h->dCandCnt, h->dTaken, h->dMatch, h->dNMatches);
+  h->launches += 3;
+  B2S_CUDA(cudaGetLastError());
+  B2S_CUDA(cudaMemcpyAsync(match_cur, h->dMatch, (size_t)nf * 4, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA(cudaMemcpyAsync(nmatches, h->dNMatches, 4, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA(cudaStreamSynchronize(st));
+  return B2S_OK;
+}
+
+// window search core of Fuse / SearchByProjection(KeyFrame*, Scw, ...): 2 launches; only the greedy form reads occupancy
+static int proj_search_windows(b2s_matcher* h, const b2s_frame_grid& gr, const b2s_win_query* q, int nq,
+                               const uint8_t* occupied, int flags, int th_dist, int32_t* best_idx, int32_t* best_dist,
+                               int* n_accepted) {
+  const int nf = gr.nf;
+  cudaStream_t st = h->stream;
+  ProjGeom pg = gr.pg;
+  pg.th = 1.f; pg.mode = 0; pg.thHigh = th_dist; pg.checkOri = 0; pg.winFlags = flags;
+  const bool greedy = (flags & B2S_WIN_GREEDY) != 0;
+  const uint8_t* occ = (greedy && occupied) ? h->dOcc : nullptr;
+  WinQuery* dQ = reinterpret_cast<WinQuery*>(h->dQueries);
+  B2S_CUDA(cudaMemcpyAsync(dQ, q, (size_t)nq * sizeof(WinQuery), cudaMemcpyHostToDevice, st));
+  if (occ) B2S_CUDA(cudaMemcpyAsync(h->dOcc, occupied, (size_t)nf, cudaMemcpyHostToDevice, st));
+  B2S_CUDA(cudaMemsetAsync(h->dTaken, 0, (size_t)nf, st));
+  B2S_CUDA(cudaMemsetAsync(h->dNMatches, 0, 4, st));
+  k_proj_topk<WinQuery><<<div_up(nq, 8), 256, 0, st>>>(dQ, nq, gr.kpx, gr.kpy, gr.oct, gr.uright, occ, gr.desc, gr.order,
+                                                       gr.cellStart, pg, h->dTopk, h->dTopkIdx, h->dCandCnt);
+  // results: dMatch holds best_idx (nq <= maxF entries), dPush holds best_dist
+  if (greedy)
+    k_win_resolve<<<1, 32, 0, st>>>(dQ, nq, th_dist, gr.kpx, gr.kpy, gr.oct, gr.uright, occ, gr.desc, gr.order, gr.cellStart,
+                                    pg, h->dTopk, h->dTopkIdx, h->dCandCnt, h->dTaken, h->dMatch, h->dPush, h->dNMatches);
+  else
+    k_win_pick<<<div_up(nq, 256), 256, 0, st>>>(nq, th_dist, h->dTopk, h->dTopkIdx, h->dMatch, h->dPush, h->dNMatches);
+  h->launches += 2;
+  B2S_CUDA(cudaGetLastError());
+  B2S_CUDA(cudaMemcpyAsync(best_idx, h->dMatch, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
+  if (best_dist) B2S_CUDA(cudaMemcpyAsync(best_dist, h->dPush, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
+  int acc = 0;
+  B2S_CUDA(cudaMemcpyAsync(&acc, h->dNMatches, 4, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA(cudaStreamSynchronize(st));
+  if (n_accepted) *n_accepted = acc;
+  return B2S_OK;
+}
+
 extern "C" int b2s_search_by_projection_last(b2s_matcher* h, const b2s_proj_query* q, int nq, const float* kpx,
                                              const float* kpy, const int32_t* octave, const float* angle,
                                              const float* uright, const uint8_t* occupied, const uint8_t* desc, int nf,
@@ -1759,41 +1897,10 @@ extern "C" int b2s_search_by_projection_last(b2s_matcher* h, const b2s_proj_quer
   if (nq == 0 || nf == 0) return B2S_OK;
   if (!q || !kpx || !kpy || !octave || !angle || !uright || !desc) return B2S_ERR_BAD_ARG;
   B2S_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = h->stream;
-  ProjGeom pg;
-  memset(&pg, 0, sizeof(pg));
-  pg.minX = g->mnMinX; pg.minY = g->mnMinY; pg.maxX = g->mnMaxX; pg.maxY = g->mnMaxY;
-  pg.invW = (float)GRID_COLS / (g->mnMaxX - g->mnMinX);  // src/Frame.cc:213-214
-  pg.invH = (float)GRID_ROWS / (g->mnMaxY - g->mnMinY);
-  pg.bf = g->bf; pg.th = th; pg.mode = mode; pg.thHigh = th_high; pg.checkOri = check_ori; pg.nlevels = g->nlevels;
-  for (int i = 0; i < 16; i++) pg.scale[i] = i < g->nlevels ? g->scale_factors[i] : 0.f;
-  B2S_CUDA(cudaMemcpyAsync(h->dQueries, q, (size_t)nq * sizeof(ProjQuery), cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dKpx, kpx, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dKpy, kpy, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dOct, octave, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dAngB, angle, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dURight, uright, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-  if (occupied) B2S_CUDA(cudaMemcpyAsync(h->dOcc, occupied, (size_t)nf, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dDescB, desc, (size_t)nf * 32, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dNB, &nf, 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemsetAsync(h->dTaken, 0, (size_t)nf, st));
-  k_fill_i32<<<div_up(nf, 256), 256, 0, st>>>(h->dMatch, -1, (size_t)nf);
-  k_proj_cell_key<<<div_up(nf, 256), 256, 0, st>>>(h->dKpx, h->dKpy, nf, pg, h->dCellKey);
-  k_rank_by_key<<<dim3(div_up(nf, 128), 1), 128, 0, st>>>(h->dCellKey, h->dNB, nf, h->dOrder);
-  k_proj_cell_start<<<div_up(nf + 1, 256), 256, 0, st>>>(h->dCellKey, h->dOrder, nf, h->dCellStart);
-  k_proj_topk<ProjQuery><<<div_up(nq, 8), 256, 0, st>>>(h->dQueries, nq, h->dKpx, h->dKpy, h->dOct, h->dURight,
-                                             occupied ? h->dOcc : nullptr, h->dDescB, h->dOrder, h->dCellStart, pg,
-                                             h->dTopk, h->dTopkIdx, h->dCandCnt);
-  k_proj_resolve<<<1, 32, 0, st>>>(h->dQueries, nq, h->dKpx, h->dKpy, h->dOct, h->dAngB, h->dURight,
-                                   occupied ? h->dOcc : nullptr, h->dDescB, h->dOrder, h->dCellStart, pg, h->dTopk,
-                                   h->dTopkIdx, h->dCandCnt, h->dTaken, h->dMatch, h->dPush, h->dExtra, h->dHist);
-  k_proj_cull<<<1, 256, 0, st>>>(check_ori, h->dHist, h->dExtra, h->dMatch, h->dPush, h->dNMatches);
-  h->launches += 7;
-  B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaMemcpyAsync(match_cur, h->dMatch, (size_t)nf * 4, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaMemcpyAsync(nmatches, h->dNMatches, 4, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaStreamSynchronize(st));
-  return B2S_OK;
+  b2s_frame_grid gr = scratch_grid(h, nf, proj_geom(g, nullptr));
+  const int rc = grid_upload(gr, kpx, kpy, octave, angle, uright, desc, h->stream);
+  if (rc != B2S_OK) return rc;
+  return proj_search_last(h, gr, q, nq, occupied, th, mode, th_high, check_ori, match_cur, nmatches);
 }
 
 // ---------------------------------------------------------------- batched, device-resident SearchByProjection(Cur, Last)
@@ -1880,16 +1987,8 @@ extern "C" int b2s_search_by_projection_last_device(b2s_matcher* h, int batch, c
   }
   B2S_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
-  ProjGeom pg;
-  pg.minX = g->mnMinX; pg.minY = g->mnMinY; pg.maxX = g->mnMaxX; pg.maxY = g->mnMaxY;
-  pg.invW = (float)GRID_COLS / (g->mnMaxX - g->mnMinX);  // src/Frame.cc:213-214
-  pg.invH = (float)GRID_ROWS / (g->mnMaxY - g->mnMinY);
-  pg.bf = g->bf; pg.th = th; pg.mode = mode; pg.thHigh = th_high; pg.checkOri = check_ori; pg.nlevels = g->nlevels;
-  pg.winFlags = 0;
-  for (int i = 0; i < 16; i++) {
-    pg.scale[i] = i < g->nlevels ? g->scale_factors[i] : 0.f;
-    pg.invSigma2[i] = 0.f;
-  }
+  ProjGeom pg = proj_geom(g, nullptr);
+  pg.th = th; pg.mode = mode; pg.thHigh = th_high; pg.checkOri = check_ori;
   pg.strideF = capF; pg.strideQ = capQ; pg.nfArr = d_nf; pg.nqArr = d_nq;
   const size_t FF = (size_t)batch * capF;
   const ProjQuery* dq = reinterpret_cast<const ProjQuery*>(d_q);
@@ -2029,38 +2128,28 @@ extern "C" int b2s_search_for_initialization(b2s_matcher* h, const float* prevx,
     Q.valid = octave1[i] > 0 ? 0 : 1;
     memcpy(Q.desc, desc1 + (size_t)i * 32, 32);
   }
-  ProjGeom pg;
-  memset(&pg, 0, sizeof(pg));
-  pg.minX = g->mnMinX; pg.minY = g->mnMinY; pg.maxX = g->mnMaxX; pg.maxY = g->mnMaxY;
-  pg.invW = (float)GRID_COLS / (g->mnMaxX - g->mnMinX);
-  pg.invH = (float)GRID_ROWS / (g->mnMaxY - g->mnMinY);
+  ProjGeom pg = proj_geom(g, nullptr);
   pg.checkOri = check_ori;
+  b2s_frame_grid gr = scratch_grid(h, n2, pg);
   WinQuery* dQ = reinterpret_cast<WinQuery*>(h->dQueries);
   int32_t* dMatchedDist = h->dNodeA;  // vMatchedDistance
   int32_t* dMatch21 = h->dBin;        // vnMatches21
   B2S_CUDA(cudaMemcpyAsync(dQ, wq.data(), (size_t)n1 * sizeof(WinQuery), cudaMemcpyHostToDevice, st));
   B2S_CUDA(cudaMemcpyAsync(h->dAngA, angle1, (size_t)n1 * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dKpx, kpx2, (size_t)n2 * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dKpy, kpy2, (size_t)n2 * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dOct, octave2, (size_t)n2 * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dAngB, angle2, (size_t)n2 * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dDescB, desc2, (size_t)n2 * 32, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dNB, &n2, 4, cudaMemcpyHostToDevice, st));
   B2S_CUDA(cudaMemsetAsync(h->dURight, 0, (size_t)n2 * 4, st));
+  const int rc = grid_upload(gr, kpx2, kpy2, octave2, angle2, nullptr, desc2, st);
+  if (rc != B2S_OK) return rc;
   B2S_CUDA(cudaStreamSynchronize(st));  // wq is a stack-owned staging vector
   k_fill_i32<<<div_up(n1, 256), 256, 0, st>>>(h->dMatch, -1, (size_t)n1);
   k_fill_i32<<<div_up(n2, 256), 256, 0, st>>>(dMatch21, -1, (size_t)n2);
   k_fill_i32<<<div_up(n2, 256), 256, 0, st>>>(dMatchedDist, 2147483647, (size_t)n2);
-  k_proj_cell_key<<<div_up(n2, 256), 256, 0, st>>>(h->dKpx, h->dKpy, n2, pg, h->dCellKey);
-  k_rank_by_key<<<dim3(div_up(n2, 128), 1), 128, 0, st>>>(h->dCellKey, h->dNB, n2, h->dOrder);
-  k_proj_cell_start<<<div_up(n2 + 1, 256), 256, 0, st>>>(h->dCellKey, h->dOrder, n2, h->dCellStart);
   k_proj_topk<WinQuery><<<div_up(n1, 8), 256, 0, st>>>(dQ, n1, h->dKpx, h->dKpy, h->dOct, h->dURight, nullptr, h->dDescB,
                                                        h->dOrder, h->dCellStart, pg, h->dTopk, h->dTopkIdx, h->dCandCnt);
   k_init_resolve<<<1, 32, 0, st>>>(dQ, n1, h->dAngA, h->dKpx, h->dKpy, h->dOct, h->dAngB, h->dURight, h->dDescB, h->dOrder,
                                    h->dCellStart, pg, th_low, nnratio, h->dTopk, h->dTopkIdx, h->dCandCnt, dMatchedDist,
                                    dMatch21, h->dMatch, h->dPush, h->dExtra, h->dHist);
   k_init_cull<<<1, 256, 0, st>>>(check_ori, n1, h->dHist, h->dExtra, h->dMatch, h->dPush, h->dNMatches);
-  h->launches += 9;
+  h->launches += 6;
   B2S_CUDA(cudaGetLastError());
   B2S_CUDA(cudaMemcpyAsync(match12, h->dMatch, (size_t)n1 * 4, cudaMemcpyDeviceToHost, st));
   B2S_CUDA(cudaMemcpyAsync(nmatches, h->dNMatches, 4, cudaMemcpyDeviceToHost, st));
@@ -2089,40 +2178,10 @@ extern "C" int b2s_search_by_projection_map(b2s_matcher* h, const b2s_map_query*
       return B2S_ERR_BAD_ARG;
     }
   B2S_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = h->stream;
-  ProjGeom pg;
-  memset(&pg, 0, sizeof(pg));
-  pg.minX = g->mnMinX; pg.minY = g->mnMinY; pg.maxX = g->mnMaxX; pg.maxY = g->mnMaxY;
-  pg.invW = (float)GRID_COLS / (g->mnMaxX - g->mnMinX);  // src/Frame.cc:213-214
-  pg.invH = (float)GRID_ROWS / (g->mnMaxY - g->mnMinY);
-  pg.bf = g->bf; pg.th = th; pg.mode = 0; pg.thHigh = th_high; pg.checkOri = 0; pg.nlevels = g->nlevels;
-  for (int i = 0; i < 16; i++) pg.scale[i] = i < g->nlevels ? g->scale_factors[i] : 0.f;
-  MapQuery* dQ = reinterpret_cast<MapQuery*>(h->dQueries);
-  B2S_CUDA(cudaMemcpyAsync(dQ, q, (size_t)nq * sizeof(MapQuery), cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dKpx, kpx, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dKpy, kpy, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dOct, octave, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dURight, uright, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-  if (occupied) B2S_CUDA(cudaMemcpyAsync(h->dOcc, occupied, (size_t)nf, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dDescB, desc, (size_t)nf * 32, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dNB, &nf, 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemsetAsync(h->dTaken, 0, (size_t)nf, st));
-  k_fill_i32<<<div_up(nf, 256), 256, 0, st>>>(h->dMatch, -1, (size_t)nf);
-  k_proj_cell_key<<<div_up(nf, 256), 256, 0, st>>>(h->dKpx, h->dKpy, nf, pg, h->dCellKey);
-  k_rank_by_key<<<dim3(div_up(nf, 128), 1), 128, 0, st>>>(h->dCellKey, h->dNB, nf, h->dOrder);
-  k_proj_cell_start<<<div_up(nf + 1, 256), 256, 0, st>>>(h->dCellKey, h->dOrder, nf, h->dCellStart);
-  k_proj_topk<MapQuery><<<div_up(nq, 8), 256, 0, st>>>(dQ, nq, h->dKpx, h->dKpy, h->dOct, h->dURight,
-                                                       occupied ? h->dOcc : nullptr, h->dDescB, h->dOrder, h->dCellStart,
-                                                       pg, h->dTopk, h->dTopkIdx, h->dCandCnt);
-  k_map_resolve<<<1, 32, 0, st>>>(dQ, nq, h->dKpx, h->dKpy, h->dOct, h->dURight, occupied ? h->dOcc : nullptr, h->dDescB,
-                                  h->dOrder, h->dCellStart, pg, nnratio, h->dTopk, h->dTopkIdx, h->dCandCnt, h->dTaken,
-                                  h->dMatch, h->dNMatches);
-  h->launches += 6;
-  B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaMemcpyAsync(match_cur, h->dMatch, (size_t)nf * 4, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaMemcpyAsync(nmatches, h->dNMatches, 4, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaStreamSynchronize(st));
-  return B2S_OK;
+  b2s_frame_grid gr = scratch_grid(h, nf, proj_geom(g, nullptr));
+  const int rc = grid_upload(gr, kpx, kpy, octave, nullptr, uright, desc, h->stream);
+  if (rc != B2S_OK) return rc;
+  return proj_search_map(h, gr, q, nq, occupied, th, th_high, nnratio, match_cur, nmatches);
 }
 
 extern "C" int b2s_search_windows(b2s_matcher* h, const b2s_win_query* q, int nq, const float* kpx, const float* kpy,
@@ -2143,66 +2202,13 @@ extern "C" int b2s_search_windows(b2s_matcher* h, const b2s_win_query* q, int nq
   if (nq == 0 || nf == 0) return B2S_OK;
   if (!q || !kpx || !kpy || !octave || !uright || !desc) return B2S_ERR_BAD_ARG;
   B2S_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = h->stream;
-  ProjGeom pg;
-  memset(&pg, 0, sizeof(pg));
-  pg.minX = g->mnMinX; pg.minY = g->mnMinY; pg.maxX = g->mnMaxX; pg.maxY = g->mnMaxY;
-  pg.invW = (float)GRID_COLS / (g->mnMaxX - g->mnMinX);  // KeyFrame::mfGridElementWidthInv (copied from the Frame)
-  pg.invH = (float)GRID_ROWS / (g->mnMaxY - g->mnMinY);
-  pg.bf = g->bf; pg.th = 1.f; pg.mode = 0; pg.thHigh = th_dist; pg.checkOri = 0; pg.nlevels = g->nlevels;
-  pg.winFlags = flags;
-  for (int i = 0; i < 16; i++) {
-    pg.scale[i] = (g->scale_factors && i < g->nlevels) ? g->scale_factors[i] : 0.f;
-    pg.invSigma2[i] = (inv_level_sigma2 && i < g->nlevels) ? inv_level_sigma2[i] : 0.f;
-  }
-  const bool greedy = (flags & B2S_WIN_GREEDY) != 0;
-  const bool useOcc = greedy && occupied;
-  WinQuery* dQ = reinterpret_cast<WinQuery*>(h->dQueries);
-  B2S_CUDA(cudaMemcpyAsync(dQ, q, (size_t)nq * sizeof(WinQuery), cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dKpx, kpx, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dKpy, kpy, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dOct, octave, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dURight, uright, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-  if (useOcc) B2S_CUDA(cudaMemcpyAsync(h->dOcc, occupied, (size_t)nf, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dDescB, desc, (size_t)nf * 32, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dNB, &nf, 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemsetAsync(h->dTaken, 0, (size_t)nf, st));
-  B2S_CUDA(cudaMemsetAsync(h->dNMatches, 0, 4, st));
-  k_proj_cell_key<<<div_up(nf, 256), 256, 0, st>>>(h->dKpx, h->dKpy, nf, pg, h->dCellKey);
-  k_rank_by_key<<<dim3(div_up(nf, 128), 1), 128, 0, st>>>(h->dCellKey, h->dNB, nf, h->dOrder);
-  k_proj_cell_start<<<div_up(nf + 1, 256), 256, 0, st>>>(h->dCellKey, h->dOrder, nf, h->dCellStart);
-  k_proj_topk<WinQuery><<<div_up(nq, 8), 256, 0, st>>>(dQ, nq, h->dKpx, h->dKpy, h->dOct, h->dURight,
-                                                       useOcc ? h->dOcc : nullptr, h->dDescB, h->dOrder, h->dCellStart, pg,
-                                                       h->dTopk, h->dTopkIdx, h->dCandCnt);
-  // results: dMatch holds best_idx (nq <= maxF entries), dPush holds best_dist
-  if (greedy)
-    k_win_resolve<<<1, 32, 0, st>>>(dQ, nq, th_dist, h->dKpx, h->dKpy, h->dOct, h->dURight, useOcc ? h->dOcc : nullptr,
-                                    h->dDescB, h->dOrder, h->dCellStart, pg, h->dTopk, h->dTopkIdx, h->dCandCnt, h->dTaken,
-                                    h->dMatch, h->dPush, h->dNMatches);
-  else
-    k_win_pick<<<div_up(nq, 256), 256, 0, st>>>(nq, th_dist, h->dTopk, h->dTopkIdx, h->dMatch, h->dPush, h->dNMatches);
-  h->launches += 5;
-  B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaMemcpyAsync(best_idx, h->dMatch, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
-  if (best_dist) B2S_CUDA(cudaMemcpyAsync(best_dist, h->dPush, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
-  int acc = 0;
-  B2S_CUDA(cudaMemcpyAsync(&acc, h->dNMatches, 4, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaStreamSynchronize(st));
-  if (n_accepted) *n_accepted = acc;
-  return B2S_OK;
+  b2s_frame_grid gr = scratch_grid(h, nf, proj_geom(g, inv_level_sigma2));
+  const int rc = grid_upload(gr, kpx, kpy, octave, nullptr, uright, desc, h->stream);
+  if (rc != B2S_OK) return rc;
+  return proj_search_windows(h, gr, q, nq, occupied, flags, th_dist, best_idx, best_dist, n_accepted);
 }
 
 // ================================================================================================ persistent feature grid
-struct b2s_frame_grid {
-  b2s_matcher* owner = nullptr;  // identity check only: never dereferenced after creation-time use by destroy
-  int device = 0;
-  int nf = 0;
-  ProjGeom pg;  // geometry + scale tables (th / mode / thresholds are filled per search)
-  float *kpx = nullptr, *kpy = nullptr, *ang = nullptr, *uright = nullptr;
-  int32_t *oct = nullptr, *order = nullptr, *cellStart = nullptr, *cellKey = nullptr, *nB = nullptr, *qOut = nullptr;
-  uint8_t* desc = nullptr;
-};
-
 extern "C" void b2s_frame_grid_destroy(b2s_frame_grid* gr) {
   if (!gr) return;
   cudaSetDevice(gr->device);
@@ -2223,16 +2229,7 @@ static int grid_alloc(b2s_matcher* h, int nf, const b2s_frame_geom* g, const flo
   gr->owner = h;
   gr->device = h->device;
   gr->nf = nf;
-  ProjGeom& pg = gr->pg;
-  memset(&pg, 0, sizeof(pg));
-  pg.minX = g->mnMinX; pg.minY = g->mnMinY; pg.maxX = g->mnMaxX; pg.maxY = g->mnMaxY;
-  pg.invW = (float)GRID_COLS / (g->mnMaxX - g->mnMinX);  // src/Frame.cc:213-214
-  pg.invH = (float)GRID_ROWS / (g->mnMaxY - g->mnMinY);
-  pg.bf = g->bf; pg.nlevels = g->nlevels;
-  for (int i = 0; i < 16; i++) {
-    pg.scale[i] = i < g->nlevels ? g->scale_factors[i] : 0.f;
-    pg.invSigma2[i] = (inv_level_sigma2 && i < g->nlevels) ? inv_level_sigma2[i] : 0.f;
-  }
+  gr->pg = proj_geom(g, inv_level_sigma2);
   const size_t n = (size_t)std::max(nf, 1);
   cudaError_t e = cudaSuccess;
   auto A = [&](void** p, size_t bytes) {
@@ -2251,18 +2248,7 @@ static int grid_alloc(b2s_matcher* h, int nf, const b2s_frame_geom* g, const flo
   return B2S_OK;
 }
 
-// Frame::AssignFeaturesToGrid (src/Frame.cc:461-491) on the arrays already in gr: cell key, stable rank, cell starts
-static int grid_build(b2s_frame_grid* gr, cudaStream_t st) {
-  b2s_matcher* h = gr->owner;
-  const int nf = gr->nf;
-  B2S_CUDA(cudaMemcpyAsync(gr->nB, &gr->nf, 4, cudaMemcpyHostToDevice, st));
-  if (nf > 0) {
-    k_proj_cell_key<<<div_up(nf, 256), 256, 0, st>>>(gr->kpx, gr->kpy, nf, gr->pg, gr->cellKey);
-    k_rank_by_key<<<dim3(div_up(nf, 128), 1), 128, 0, st>>>(gr->cellKey, gr->nB, nf, gr->order);
-  }
-  k_proj_cell_start<<<div_up(nf + 1, 256), 256, 0, st>>>(gr->cellKey, gr->order, nf, gr->cellStart);
-  h->launches += 3;
-  B2S_CUDA(cudaGetLastError());
+static int stream_sync(cudaStream_t st) {
   B2S_CUDA(cudaStreamSynchronize(st));
   return B2S_OK;
 }
@@ -2274,16 +2260,8 @@ extern "C" int b2s_frame_grid_create(b2s_matcher* h, const float* kpx, const flo
   int rc = grid_alloc(h, nf, g, inv_level_sigma2, out);
   if (rc != B2S_OK) return rc;
   b2s_frame_grid* gr = *out;
-  cudaStream_t st = h->stream;
-  if (nf > 0) {
-    B2S_CUDA(cudaMemcpyAsync(gr->kpx, kpx, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-    B2S_CUDA(cudaMemcpyAsync(gr->kpy, kpy, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-    B2S_CUDA(cudaMemcpyAsync(gr->oct, octave, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-    B2S_CUDA(cudaMemcpyAsync(gr->ang, angle, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-    B2S_CUDA(cudaMemcpyAsync(gr->uright, uright, (size_t)nf * 4, cudaMemcpyHostToDevice, st));
-    B2S_CUDA(cudaMemcpyAsync(gr->desc, desc, (size_t)nf * 32, cudaMemcpyHostToDevice, st));
-  }
-  rc = grid_build(gr, st);
+  rc = grid_upload(*gr, kpx, kpy, octave, angle, uright, desc, h->stream);
+  if (rc == B2S_OK) rc = stream_sync(h->stream);
   if (rc != B2S_OK) {
     b2s_frame_grid_destroy(gr);
     *out = nullptr;
@@ -2306,7 +2284,8 @@ extern "C" int b2s_frame_grid_create_device(b2s_matcher* h, const b2s_keypoint* 
     else k_fill_i32<<<div_up(nf, 256), 256, 0, st>>>(reinterpret_cast<int32_t*>(gr->uright), (int)0xBF800000, (size_t)nf);  // -1.0f
     B2S_CUDA(cudaMemcpyAsync(gr->desc, d_desc, (size_t)nf * 32, cudaMemcpyDeviceToDevice, st));
   }
-  rc = grid_build(gr, st);
+  rc = grid_build(*gr, st);
+  if (rc == B2S_OK) rc = stream_sync(st);
   if (rc != B2S_OK) {
     b2s_frame_grid_destroy(gr);
     *out = nullptr;
@@ -2355,26 +2334,7 @@ extern "C" int b2s_search_by_projection_last_grid(b2s_matcher* h, b2s_frame_grid
   if (nq == 0 || nf == 0) return B2S_OK;
   if (!q) return B2S_ERR_BAD_ARG;
   B2S_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = h->stream;
-  ProjGeom pg = gr->pg;
-  pg.th = th; pg.mode = mode; pg.thHigh = th_high; pg.checkOri = check_ori;
-  B2S_CUDA(cudaMemcpyAsync(h->dQueries, q, (size_t)nq * sizeof(ProjQuery), cudaMemcpyHostToDevice, st));
-  if (occupied) B2S_CUDA(cudaMemcpyAsync(h->dOcc, occupied, (size_t)nf, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemsetAsync(h->dTaken, 0, (size_t)nf, st));
-  k_fill_i32<<<div_up(nf, 256), 256, 0, st>>>(h->dMatch, -1, (size_t)nf);
-  k_proj_topk<ProjQuery><<<div_up(nq, 8), 256, 0, st>>>(h->dQueries, nq, gr->kpx, gr->kpy, gr->oct, gr->uright,
-                                                        occupied ? h->dOcc : nullptr, gr->desc, gr->order, gr->cellStart, pg,
-                                                        h->dTopk, h->dTopkIdx, h->dCandCnt);
-  k_proj_resolve<<<1, 32, 0, st>>>(h->dQueries, nq, gr->kpx, gr->kpy, gr->oct, gr->ang, gr->uright,
-                                   occupied ? h->dOcc : nullptr, gr->desc, gr->order, gr->cellStart, pg, h->dTopk, h->dTopkIdx,
-                                   h->dCandCnt, h->dTaken, h->dMatch, h->dPush, h->dExtra, h->dHist);
-  k_proj_cull<<<1, 256, 0, st>>>(check_ori, h->dHist, h->dExtra, h->dMatch, h->dPush, h->dNMatches);
-  h->launches += 4;
-  B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaMemcpyAsync(match_cur, h->dMatch, (size_t)nf * 4, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaMemcpyAsync(nmatches, h->dNMatches, 4, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaStreamSynchronize(st));
-  return B2S_OK;
+  return proj_search_last(h, *gr, q, nq, occupied, th, mode, th_high, check_ori, match_cur, nmatches);
 }
 
 extern "C" int b2s_search_by_projection_map_grid(b2s_matcher* h, b2s_frame_grid* gr, const b2s_map_query* q, int nq,
@@ -2395,26 +2355,7 @@ extern "C" int b2s_search_by_projection_map_grid(b2s_matcher* h, b2s_frame_grid*
       return B2S_ERR_BAD_ARG;
     }
   B2S_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = h->stream;
-  ProjGeom pg = gr->pg;
-  pg.th = th; pg.mode = 0; pg.thHigh = th_high; pg.checkOri = 0;
-  MapQuery* dQ = reinterpret_cast<MapQuery*>(h->dQueries);
-  B2S_CUDA(cudaMemcpyAsync(dQ, q, (size_t)nq * sizeof(MapQuery), cudaMemcpyHostToDevice, st));
-  if (occupied) B2S_CUDA(cudaMemcpyAsync(h->dOcc, occupied, (size_t)nf, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemsetAsync(h->dTaken, 0, (size_t)nf, st));
-  k_fill_i32<<<div_up(nf, 256), 256, 0, st>>>(h->dMatch, -1, (size_t)nf);
-  k_proj_topk<MapQuery><<<div_up(nq, 8), 256, 0, st>>>(dQ, nq, gr->kpx, gr->kpy, gr->oct, gr->uright,
-                                                       occupied ? h->dOcc : nullptr, gr->desc, gr->order, gr->cellStart, pg,
-                                                       h->dTopk, h->dTopkIdx, h->dCandCnt);
-  k_map_resolve<<<1, 32, 0, st>>>(dQ, nq, gr->kpx, gr->kpy, gr->oct, gr->uright, occupied ? h->dOcc : nullptr, gr->desc,
-                                  gr->order, gr->cellStart, pg, nnratio, h->dTopk, h->dTopkIdx, h->dCandCnt, h->dTaken,
-                                  h->dMatch, h->dNMatches);
-  h->launches += 3;
-  B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaMemcpyAsync(match_cur, h->dMatch, (size_t)nf * 4, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaMemcpyAsync(nmatches, h->dNMatches, 4, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaStreamSynchronize(st));
-  return B2S_OK;
+  return proj_search_map(h, *gr, q, nq, occupied, th, th_high, nnratio, match_cur, nmatches);
 }
 
 extern "C" int b2s_search_windows_grid(b2s_matcher* h, b2s_frame_grid* gr, const b2s_win_query* q, int nq,
@@ -2433,34 +2374,7 @@ extern "C" int b2s_search_windows_grid(b2s_matcher* h, b2s_frame_grid* gr, const
   if (nq == 0 || nf == 0) return B2S_OK;
   if (!q) return B2S_ERR_BAD_ARG;
   B2S_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = h->stream;
-  ProjGeom pg = gr->pg;
-  pg.th = 1.f; pg.mode = 0; pg.thHigh = th_dist; pg.checkOri = 0; pg.winFlags = flags;
-  const bool greedy = (flags & B2S_WIN_GREEDY) != 0;
-  const bool useOcc = greedy && occupied;
-  WinQuery* dQ = reinterpret_cast<WinQuery*>(h->dQueries);
-  B2S_CUDA(cudaMemcpyAsync(dQ, q, (size_t)nq * sizeof(WinQuery), cudaMemcpyHostToDevice, st));
-  if (useOcc) B2S_CUDA(cudaMemcpyAsync(h->dOcc, occupied, (size_t)nf, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemsetAsync(h->dTaken, 0, (size_t)nf, st));
-  B2S_CUDA(cudaMemsetAsync(h->dNMatches, 0, 4, st));
-  k_proj_topk<WinQuery><<<div_up(nq, 8), 256, 0, st>>>(dQ, nq, gr->kpx, gr->kpy, gr->oct, gr->uright,
-                                                       useOcc ? h->dOcc : nullptr, gr->desc, gr->order, gr->cellStart, pg,
-                                                       h->dTopk, h->dTopkIdx, h->dCandCnt);
-  if (greedy)
-    k_win_resolve<<<1, 32, 0, st>>>(dQ, nq, th_dist, gr->kpx, gr->kpy, gr->oct, gr->uright, useOcc ? h->dOcc : nullptr,
-                                    gr->desc, gr->order, gr->cellStart, pg, h->dTopk, h->dTopkIdx, h->dCandCnt, h->dTaken,
-                                    h->dMatch, h->dPush, h->dNMatches);
-  else
-    k_win_pick<<<div_up(nq, 256), 256, 0, st>>>(nq, th_dist, h->dTopk, h->dTopkIdx, h->dMatch, h->dPush, h->dNMatches);
-  h->launches += 2;
-  B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaMemcpyAsync(best_idx, h->dMatch, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
-  if (best_dist) B2S_CUDA(cudaMemcpyAsync(best_dist, h->dPush, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
-  int acc = 0;
-  B2S_CUDA(cudaMemcpyAsync(&acc, h->dNMatches, 4, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaStreamSynchronize(st));
-  if (n_accepted) *n_accepted = acc;
-  return B2S_OK;
+  return proj_search_windows(h, *gr, q, nq, occupied, flags, th_dist, best_idx, best_dist, n_accepted);
 }
 
 extern "C" int b2s_search_for_triangulation(b2s_matcher* h, const b2s_kf_features* kf1, const b2s_kf_features* kf2,

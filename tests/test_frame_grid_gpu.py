@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 from oracle_binding import FrameGeom
-from synth import synth_projection, synth_projection_map, synth_windows
+from synth import synth_descriptors, synth_projection, synth_projection_map, synth_windows
 
 pytestmark = pytest.mark.gpu
 vp, c_i, c_f = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
@@ -104,6 +104,60 @@ def test_searches_on_resident_grid_equal_host_buffer_calls(pkg, oracle):
         on, ob, obd = oracle.search_windows(d["q"], d["kpx"], d["kpy"], d["octave"], d["uright"], d["inv_sigma2"], occ, d["desc"],
                                             d["geom"], chi2=chi2, greedy=greedy)
         assert n == on and np.array_equal(best, ob) and np.array_equal(bd, obd)
+
+
+def _launches(m, call):
+    before = m.launch_count()
+    out = call()
+    return out, m.launch_count() - before
+
+
+def test_host_buffer_searches_equal_their_grid_twins(pkg, oracle):
+    """A host-buffer projection search is its resident-grid twin plus a grid build (3 launches) on the same inputs:
+    array-for-array identical outputs, and the launch count of every host-buffer matcher call is pinned."""
+    d = synth_projection(seed=21, cluster=True, th=7.0)
+    m = pkg.ORBmatcher(0.9, True)
+    gr = _grid(pkg, m, d)
+    for mode in (0, 1, 2):
+        (nh, mh), lh = _launches(m, lambda: m.SearchByProjection(d["q"], d["kpx"], d["kpy"], d["octave"], d["angle"], d["uright"],
+                                                                 d["occupied"], d["desc"], d["geom"], d["th"], mode=mode))
+        (ng, mg), lg = _launches(m, lambda: gr.SearchByProjection(d["q"], d["occupied"], d["th"], mode=mode))
+        assert (lh, lg) == (7, 4)
+        assert nh == ng > 100 and np.array_equal(mh, mg)
+    d = synth_projection_map(seed=33, cluster=True)
+    m8 = pkg.ORBmatcher(0.8, True)
+    gr = _grid(pkg, m8, d)
+    for th in (1.0, 3.0):
+        (nh, mh), lh = _launches(m8, lambda: m8.SearchByProjectionMap(d["q"], d["kpx"], d["kpy"], d["octave"], d["uright"],
+                                                                      d["occupied"], d["desc"], d["geom"], th=th))
+        (ng, mg), lg = _launches(m8, lambda: gr.SearchByProjectionMap(d["q"], d["occupied"], th=th))
+        assert (lh, lg) == (6, 3)
+        assert nh == ng > 100 and np.array_equal(mh, mg)
+    d = synth_windows(seed=13)
+    gr = _grid(pkg, m8, d, is2=d["inv_sigma2"])
+    for chi2, greedy in ((True, False), (False, False), (False, True)):
+        occ = d["occupied"] if greedy else None
+        (nh, bh, dh), lh = _launches(m8, lambda: m8.SearchWindows(d["q"], d["kpx"], d["kpy"], d["octave"], d["uright"],
+                                                                  d["inv_sigma2"], occ, d["desc"], d["geom"], chi2=chi2,
+                                                                  greedy=greedy))
+        (ng, bg, dg), lg = _launches(m8, lambda: gr.SearchWindows(d["q"], occ, chi2=chi2, greedy=greedy))
+        assert (lh, lg) == (5, 2)
+        assert nh == ng > 100 and np.array_equal(bh, bg) and np.array_equal(dh, dg)
+    # the two host-buffer matchers without a grid twin: launch counts, and the oracle's answer
+    d = synth_projection(nf=1500, nq=1500, seed=41)
+    rng = np.random.RandomState(42)
+    q = d["q"]
+    prev = np.ascontiguousarray(np.stack([q["u"], q["v"]], 1), np.float32)
+    oct1 = np.where(rng.randint(0, 100, size=len(q)) < 50, 0, q["octave"]).astype(np.int32)
+    oct2 = np.where(rng.randint(0, 100, size=len(d["kpx"])) < 60, 0, d["octave"]).astype(np.int32)
+    args = (oct1, q["angle"], q["desc"], d["kpx"], d["kpy"], oct2, d["angle"], d["desc"], d["geom"])
+    (n, m12), l = _launches(m, lambda: m.SearchForInitialization(prev.copy(), *args))
+    on, om = oracle.search_for_initialization(prev.copy(), *args, nnratio=0.9)
+    assert l == 9 and n == on > 100 and np.array_equal(m12, om)
+    A, nA, vA, aA, B, nB, aB = synth_descriptors(1000, seed=5)
+    (n, mb), l = _launches(m, lambda: m.SearchByBoW(A, nA, vA, aA, B, nB, aB))
+    on, om = oracle.search_by_bow(A, nA, vA, aA, B, nB, aB, nnratio=0.9)
+    assert l == 5 and n == on > 100 and np.array_equal(mb, om)
 
 
 def test_grid_from_device_resident_extractor_records(pkg, oracle):
