@@ -515,6 +515,54 @@ int b2s_global_ba(b2s_gba_solver* h, const b2s_gba_problem* p, const volatile ui
 /* Device time (CUDA events on the solver's stream) of the last b2s_global_ba call and the LM trials it ran. */
 float b2s_gba_last_ms(const b2s_gba_solver* h, long long* lm_trials);
 
+/* ------------------------------------------------------------------ essential graph */
+/* Optimizer::OptimizeEssentialGraph (src/Optimizer.cc:1017-1339), the pose-graph step of LoopClosing::CorrectLoop: a Sim3
+ * pose graph over every keyframe of the map, one fixed vertex (the loop keyframe), EdgeSim3 edges with identity
+ * information, 20 Levenberg iterations from lambda 1e-16, g2o's numeric Jacobians (central differences, delta = 1e-9);
+ * then every keyframe gets [R t/s; 0 1] of its optimised Sim3 and every point moves with its reference keyframe.
+ * The caller builds the edge list and its measurements (the reference's loops :1108-1262, in their order); the device
+ * never needs to know which pose an edge's measurement came from.  The LM loop runs on the host; every stage of a trial
+ * is FP64 kernels without floating-point atomics, so two calls on the same input give bit-identical outputs.  With no
+ * edge, nothing is optimised and everything is still written back. */
+typedef struct {
+  double q[4];  /* g2o::Sim3 operator[] order: qx qy qz qw, then t, then s */
+  double t[3];
+  double s;
+} b2s_sim3;
+typedef struct {
+  int32_t i, j;   /* EdgeSim3: vertex 0 = keyframe i, vertex 1 = keyframe j */
+  b2s_sim3 meas;  /* S_ji */
+} b2s_sim3_edge;
+typedef struct {
+  int n_kf;                    /* the map's keyframes, ascending mnId */
+  const b2s_sim3* Siw;         /* n_kf: initial estimates (vScw: CorrectedSim3 if present, else Sim3(Rcw, tcw, 1)) */
+  int fixed_kf;                /* index of the loop keyframe, the only fixed vertex (:1086) */
+  int fix_scale;               /* bFixScale: the scale component of every update is zeroed */
+  int n_edges;
+  const b2s_sim3_edge* edges;  /* in the reference's insertion order */
+  int n_mp;                    /* the non-bad map points */
+  const float* points;         /* n_mp x 3 */
+  const int32_t* ref_kf;       /* n_mp: keyframe index of the point's nIDr (:1311-1322); -1: no such vertex, the point
+                                  is written back unchanged */
+} b2s_eg_problem;
+typedef struct {
+  float* Tcw_out;              /* n_kf x 16: SetPose([R t/s; 0 1]) of every keyframe (:1279-1299) */
+  float* points_out;           /* n_mp x 3: correctedSwr.map(Srw.map(P)) (:1304-1338) */
+  int32_t* trace;              /* optional (>= 256): accept(1)/reject(0) per LM trial, -1 terminated */
+  double chi2_initial, chi2_final;
+  int n_trials;
+} b2s_eg_result;
+typedef struct b2s_eg_solver b2s_eg_solver;
+/* Capacities of the problem arrays; the tile storage of the factorisation is sized from each call's graph and grows on
+ * demand.  Supports at least max_kf = 4096, max_edges = 2^17, max_mp = 2^22. */
+int b2s_eg_create(int max_kf, int max_edges, int max_mp, int device, b2s_eg_solver** out);
+void b2s_eg_destroy(b2s_eg_solver* h);
+/* Sizes above the handle's capacities: B2S_ERR_CAPACITY.  An edge index out of range or i == j, fixed_kf out of range or a
+ * ref_kf outside [-1, n_kf): B2S_ERR_BAD_ARG (the reference would dereference a missing vertex). */
+int b2s_optimize_essential_graph(b2s_eg_solver* h, const b2s_eg_problem* p, b2s_eg_result* r);
+/* Device time (CUDA events on the solver's stream) of the last call and the LM trials it ran. */
+float b2s_eg_last_ms(const b2s_eg_solver* h, long long* lm_trials);
+
 #ifdef __cplusplus
 }
 #endif

@@ -72,6 +72,20 @@ class _GbaProblem(ctypes.Structure):
                 ("robust", ctypes.c_int)]
 
 
+class _EgProblem(ctypes.Structure):
+    _fields_ = [("n_kf", ctypes.c_int), ("Siw", _vp), ("fixed_kf", ctypes.c_int), ("fix_scale", ctypes.c_int),
+                ("n_edges", ctypes.c_int), ("edges", _vp), ("n_mp", ctypes.c_int), ("points", _vp), ("ref_kf", _vp)]
+
+
+class _EgResult(ctypes.Structure):
+    _fields_ = [("Tcw_out", _vp), ("points_out", _vp), ("trace", _vp), ("chi2_initial", ctypes.c_double),
+                ("chi2_final", ctypes.c_double), ("n_trials", ctypes.c_int)]
+
+
+# b2s_sim3_edge: EdgeSim3 between keyframes i (vertex 0) and j (vertex 1), measurement S_ji as qx qy qz qw tx ty tz s
+sim3_edge_dtype = np.dtype([("i", np.int32), ("j", np.int32), ("meas", np.float64, 8)])
+
+
 class _GbaResult(ctypes.Structure):
     _fields_ = [("Tcw_out", _vp), ("points_out", _vp), ("point_included", _vp), ("trace", _vp),
                 ("chi2_final", ctypes.c_double), ("n_trials", ctypes.c_int)]
@@ -155,6 +169,13 @@ def lib():
             L.b2s_global_ba.argtypes = [_vp, _vp, _vp, _vp]
             L.b2s_gba_last_ms.restype = ctypes.c_float
             L.b2s_gba_last_ms.argtypes = [_vp, _vp]
+        if hasattr(L, "b2s_eg_create"):
+            L.b2s_eg_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+            L.b2s_eg_destroy.argtypes = [_vp]
+            L.b2s_eg_destroy.restype = None
+            L.b2s_optimize_essential_graph.argtypes = [_vp, _vp, _vp]
+            L.b2s_eg_last_ms.restype = ctypes.c_float
+            L.b2s_eg_last_ms.argtypes = [_vp, _vp]
         _lib = L
     return _lib
 
@@ -974,6 +995,54 @@ class GlobalOptimizer:
         r = _GbaResult(out["Tcw"].ctypes.data, out["points"].ctypes.data, out["point_included"].ctypes.data,
                        out["trace"].ctypes.data, 0.0, 0)
         _check(lib().b2s_global_ba(self._h, ctypes.byref(p), _p(stop), ctypes.byref(r)))
+        out["chi2"] = r.chi2_final
+        out["n_trials"] = r.n_trials
+        return out
+
+
+class EssentialGraphOptimizer:
+    """Mirror of ORB_SLAM2::Optimizer::OptimizeEssentialGraph (src/Optimizer.cc:1017-1339) on a flattened pose graph
+    (b2s_optimize_essential_graph).  The handle's capacities bound the problem sizes; the factorisation's tile storage
+    grows with the graphs it is given."""
+
+    def __init__(self, max_kf=4096, max_edges=1 << 17, max_mp=1 << 22, device=0):
+        self._h = _vp()
+        _check(lib().b2s_eg_create(max_kf, max_edges, max_mp, device, ctypes.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().b2s_eg_destroy(self._h)
+            self._h = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def last_ms(self):
+        """(ms, trials): device time of the last call (CUDA events) and the LM trials it ran."""
+        n = ctypes.c_longlong(0)
+        ms = lib().b2s_eg_last_ms(self._h, ctypes.byref(n))
+        return float(ms), int(n.value)
+
+    def OptimizeEssentialGraph(self, d):
+        """d: Siw (n_kf x 8: qx qy qz qw tx ty tz s, the keyframes by ascending mnId), fixed_kf, fix_scale, edges
+        (sim3_edge_dtype, in the reference's insertion order), points (n_mp x 3), ref_kf (n_mp, -1: unchanged).
+        Returns Tcw (every keyframe), points, trace, n_trials, chi2_initial, chi2_final."""
+        keep = dict(Siw=np.ascontiguousarray(d["Siw"], np.float64).reshape(-1, 8),
+                    edges=np.ascontiguousarray(d["edges"]),
+                    points=np.ascontiguousarray(d["points"], np.float32).reshape(-1, 3),
+                    ref_kf=np.ascontiguousarray(d["ref_kf"], np.int32))
+        assert keep["edges"].dtype == sim3_edge_dtype
+        nkf, nmp = len(keep["Siw"]), len(keep["points"])
+        p = _EgProblem(nkf, keep["Siw"].ctypes.data, int(d["fixed_kf"]), int(bool(d["fix_scale"])), len(keep["edges"]),
+                       keep["edges"].ctypes.data, nmp, keep["points"].ctypes.data, keep["ref_kf"].ctypes.data)
+        out = dict(Tcw=np.zeros((nkf, 16), np.float32), points=np.zeros((nmp, 3), np.float32),
+                   trace=np.full(256, -1, np.int32))
+        r = _EgResult(out["Tcw"].ctypes.data, out["points"].ctypes.data, out["trace"].ctypes.data, 0.0, 0.0, 0)
+        _check(lib().b2s_optimize_essential_graph(self._h, ctypes.byref(p), ctypes.byref(r)))
+        out["chi2_initial"] = r.chi2_initial
         out["chi2"] = r.chi2_final
         out["n_trials"] = r.n_trials
         return out

@@ -16,8 +16,8 @@ ORACLE_LIB = os.path.join(ORACLE_DIR, "liborb_oracle.so")
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_FLAGS = GENCODE + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-O3"]
 # extractor/matcher/keyframe database: bit-exact float arithmetic, never contract a*b+c; LocalBA is FP64 with a 1e-5 bar
-# -> FMA allowed
-NO_FMAD = {"extractor.cu", "extractor_tile.cu", "matcher.cu", "common.cu", "kfdb.cu"}
+# -> FMA allowed; the essential graph differentiates numerically (delta = 1e-9 amplifies last-bit differences ~5e8 times)
+NO_FMAD = {"extractor.cu", "extractor_tile.cu", "matcher.cu", "common.cu", "kfdb.cu", "essential.cu"}
 
 
 def _newer(target, sources):
@@ -38,8 +38,10 @@ def _deps_of(src):
     deps = [src, os.path.join(CSRC, "common.cuh"), os.path.join(ROOT, "include", "b200slam.h"), os.path.abspath(__file__)]
     if base.startswith("extractor"):
         deps.append(os.path.join(CSRC, "extractor.cuh"))
-    if base in ("localba.cu", "gba.cu"):
+    if base in ("localba.cu", "gba.cu", "essential.cu"):
         deps.append(os.path.join(CSRC, "ba_math.cuh"))
+    if base in ("gba.cu", "essential.cu"):
+        deps.append(os.path.join(CSRC, "chol.cuh"))
     if base == "extractor.cu":
         deps.append(os.path.join(ROOT, "data", "orb_pattern_31.inc"))
     return deps
@@ -80,6 +82,9 @@ def build_oracle(force=False):
     subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "kfdb.mk"] + (["-B"] if force else []) + ["liborb_kfdb.so"])
     # the global bundle adjustment's CPU restatement (oracle/gba.mk)
     subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "gba.mk"] + (["-B"] if force else []) + ["liborb_gba.so"])
+    # the essential graph's CPU restatement (oracle/essential.mk)
+    subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "essential.mk"] + (["-B"] if force else []) +
+                          ["liborb_essential.so"])
     return ORACLE_LIB
 
 
@@ -93,6 +98,7 @@ def build_oracle_ref():
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "kfdb.mk", "ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "gba.mk", "gba-ref", "REF=" + ref])
+    subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "essential.mk", "essential-ref", "REF=" + ref])
     return os.path.join(ORACLE_DIR, "_ref")
 
 

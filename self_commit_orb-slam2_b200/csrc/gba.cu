@@ -35,16 +35,13 @@
 #include <cub/cub.cuh>
 
 #include "ba_math.cuh"
+#include "chol.cuh"
 #include "common.cuh"
 
 namespace b2s {
 namespace gba {
 
-constexpr int TS = 64;           // Cholesky tile (scalar rows / columns)
-constexpr int TT = TS * TS;      // doubles per stored tile (row-major, stride TS)
-constexpr int LDT = 68;          // shared-memory row stride of a tile: the 8 rows of a DMMA fragment spread over the banks
-constexpr int TILE_SMEM = TS * LDT * 8;
-constexpr int RED_BLOCKS = 256;  // fixed grid of the deterministic sums
+using namespace chol;  // tiles, deterministic sums, the tiled Cholesky (chol.cuh)
 constexpr int PSD = 8;           // doubles per pose: q(x,y,z,w), t(x,y,z), pad
 
 struct Cam {
@@ -83,51 +80,6 @@ struct Edges {
   const float* obs;  // 3 per edge
   const float* w;    // inv_sigma2
 };
-
-// ================================================================================================ deterministic sums
-__device__ __forceinline__ double warp_sum(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-// part[blockIdx.x] = sum of v[chunk of this block] (fixed chunking, fixed tree); op 0 = sum, 1 = max |v|
-template <int OP>
-__global__ void __launch_bounds__(256) k_reduce_part(const double* __restrict__ v, long long n, double* part) {
-  __shared__ double sm[8];
-  const long long chunk = (n + gridDim.x - 1) / gridDim.x;
-  const long long beg = chunk * blockIdx.x, end = min(n, beg + chunk);
-  double s = 0;
-  for (long long i = beg + threadIdx.x; i < end; i += 256) s = OP == 0 ? s + v[i] : fmax(s, fabs(v[i]));
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const double t = __shfl_xor_sync(0xffffffffu, s, o);
-    s = OP == 0 ? s + t : fmax(s, t);
-  }
-  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double r = sm[0];
-    for (int i = 1; i < 8; i++) r = OP == 0 ? r + sm[i] : fmax(r, sm[i]);
-    part[blockIdx.x] = r;
-  }
-}
-template <int OP>
-__global__ void __launch_bounds__(256) k_reduce_final(const double* __restrict__ part, int n, double* out) {
-  __shared__ double sm[8];
-  double s = threadIdx.x < n ? part[threadIdx.x] : 0.0;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const double t = __shfl_xor_sync(0xffffffffu, s, o);
-    s = OP == 0 ? s + t : fmax(s, t);
-  }
-  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double r = sm[0];
-    for (int i = 1; i < 8; i++) r = OP == 0 ? r + sm[i] : fmax(r, sm[i]);
-    *out = r;
-  }
-}
 
 // ================================================================================================ set-up and structure
 // Converter::toSE3Quat (src/Converter.cc:57-66) / toVector3d
@@ -417,10 +369,6 @@ __global__ void __launch_bounds__(256) k_rhs(LmArgs a) {
   }
 }
 
-__device__ __forceinline__ double* tile_ptr(const LmArgs& a, int I, int K) {
-  return a.tiles + (size_t)(a.tileOff[I] + (K - a.envT[I])) * TT;
-}
-
 // one warp per lower 6x6 block (i, j) of S, summed over its pair records in order, written into the envelope tiles
 __global__ void __launch_bounds__(256) k_schur(LmArgs a, const unsigned* __restrict__ ukey, const int* __restrict__ blkBeg,
                                                int nBlk, const int4* __restrict__ rec, double lambda) {
@@ -447,173 +395,6 @@ __global__ void __launch_bounds__(256) k_schur(LmArgs a, const unsigned* __restr
     const int R = i * 6 + r, Cc = j * 6 + c;
     tile_ptr(a, R / TS, Cc / TS)[(R % TS) * TS + (Cc % TS)] = v;
   }
-}
-
-// ---------------------------------------------------------------- tiled Cholesky
-__device__ __forceinline__ void load_tile(double* s, const double* g) {
-  for (int k = threadIdx.x; k < TT; k += blockDim.x) s[(k / TS) * LDT + (k % TS)] = g[k];
-}
-// acc = X Y^T for the 8 output rows of this warp (rows 8 w + g, columns 8 n + 2 t + {0, 1}) on the DMMA pipe
-__device__ __forceinline__ void gemm_nt(const double* __restrict__ X, const double* __restrict__ Y, double (&acc)[8][2]) {
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
-#pragma unroll
-  for (int n = 0; n < 8; n++) acc[n][0] = acc[n][1] = 0.0;
-#pragma unroll 4
-  for (int s = 0; s < TS / 4; s++) {
-    const double av = X[(8 * w + g) * LDT + 4 * s + t];
-#pragma unroll
-    for (int n = 0; n < 8; n++) {
-      const double bv = Y[(8 * n + g) * LDT + 4 * s + t];
-      asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                   : "+d"(acc[n][0]), "+d"(acc[n][1])
-                   : "d"(av), "d"(bv));
-    }
-  }
-}
-
-// diagonal tile K: Cholesky in shared memory (right-looking), then Linv = L^-1 (lower) to linv[K]
-__global__ void __launch_bounds__(256) k_potrf(LmArgs a, int K) {
-  extern __shared__ double sm[];
-  double* sA = sm;
-  double* sX = sm + TS * LDT;
-  if (*(volatile int*)a.fail) return;
-  const int tid = threadIdx.x;
-  const double* g = tile_ptr(a, K, K);
-  for (int k = tid; k < TT; k += 256) {
-    const int r = k / TS, c = k % TS;
-    const bool pad = K * TS + r >= a.np || K * TS + c >= a.np;  // padding rows / columns: identity
-    sA[r * LDT + c] = pad ? (r == c ? 1.0 : 0.0) : g[k];
-    sX[r * LDT + c] = 0.0;
-  }
-  for (int j = 0; j < TS; j++) {
-    __syncthreads();
-    const double d = sA[j * LDT + j];
-    if (!(d > 0.0) || !isfinite(d)) {
-      if (tid == 0) *a.fail = 1;
-      return;
-    }
-    const double piv = sqrt(d);
-    __syncthreads();
-    if (tid == 0) sA[j * LDT + j] = piv;
-    for (int i = j + 1 + tid; i < TS; i += 256) sA[i * LDT + j] /= piv;
-    __syncthreads();
-    for (int i = j + 1 + (tid >> 4); i < TS; i += 16) {
-      const double lij = sA[i * LDT + j];
-      for (int c = j + 1 + (tid & 15); c <= i; c += 16) sA[i * LDT + c] -= lij * sA[c * LDT + j];
-    }
-  }
-  __syncthreads();
-  // Linv column c by a group of 4 lanes: X[r][c] = (delta_rc - sum_{k=c}^{r-1} L[r][k] X[k][c]) / L[r][r]
-  {
-    const int c = tid >> 2, q = tid & 3;
-    const unsigned mask = 0xFu << (threadIdx.x & 28);
-    for (int r = c; r < TS; r++) {
-      double s = 0;
-      for (int k = c + q; k < r; k += 4) s += sA[r * LDT + k] * sX[k * LDT + c];
-      s += __shfl_xor_sync(mask, s, 1);
-      s += __shfl_xor_sync(mask, s, 2);
-      if (q == 0) sX[r * LDT + c] = ((r == c ? 1.0 : 0.0) - s) / sA[r * LDT + r];
-      __syncwarp(mask);
-    }
-  }
-  __syncthreads();
-  double* out = a.linv + (size_t)K * TT;
-  for (int k = tid; k < TT; k += 256) out[k] = sX[(k / TS) * LDT + (k % TS)];
-}
-
-// panel: L_IK = A_IK Linv_KK^T for every tile row I > K whose envelope reaches column K
-__global__ void __launch_bounds__(256) k_trsm(LmArgs a, int K) {
-  extern __shared__ double sm[];
-  if (*(volatile int*)a.fail) return;
-  const int I = K + 1 + blockIdx.x;
-  if (a.envT[I] > K) return;
-  double* sA = sm;
-  double* sL = sm + TS * LDT;
-  double* g = tile_ptr(a, I, K);
-  load_tile(sA, g);
-  load_tile(sL, a.linv + (size_t)K * TT);
-  __syncthreads();
-  double acc[8][2];
-  gemm_nt(sA, sL, acc);
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, gi = lane >> 2, t = lane & 3;
-#pragma unroll
-  for (int n = 0; n < 8; n++) {
-    const int r = 8 * w + gi, c = 8 * n + 2 * t;
-    g[r * TS + c] = acc[n][0];
-    g[r * TS + c + 1] = acc[n][1];
-  }
-}
-
-// trailing update: A_IJ -= L_IK L_JK^T for K < J <= I inside both envelopes
-__global__ void __launch_bounds__(256) k_syrk(LmArgs a, int K, int nT) {
-  extern __shared__ double sm[];
-  if (*(volatile int*)a.fail) return;
-  const long long idx = blockIdx.x;
-  long long ii = (long long)((sqrt(8.0 * (double)idx + 1.0) - 1.0) * 0.5);
-  while (ii * (ii + 1) / 2 > idx) ii--;
-  while ((ii + 1) * (ii + 2) / 2 <= idx) ii++;
-  const int I = K + 1 + (int)ii, J = K + 1 + (int)(idx - ii * (ii + 1) / 2);
-  if (I >= nT || a.envT[I] > K || a.envT[J] > K) return;
-  double* sI = sm;
-  double* sJ = sm + TS * LDT;
-  load_tile(sI, tile_ptr(a, I, K));
-  load_tile(sJ, tile_ptr(a, J, K));
-  __syncthreads();
-  double acc[8][2];
-  gemm_nt(sI, sJ, acc);
-  double* g = tile_ptr(a, I, J);
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, gi = lane >> 2, t = lane & 3;
-#pragma unroll
-  for (int n = 0; n < 8; n++) {
-    const int r = 8 * w + gi, c = 8 * n + 2 * t;
-    g[r * TS + c] -= acc[n][0];
-    g[r * TS + c + 1] -= acc[n][1];
-  }
-}
-
-// forward substitution step K: y_K = Linv_KK r_K (block 0 stores it), r_I -= L_IK y_K (block I - K)
-__global__ void __launch_bounds__(TS) k_fwd(LmArgs a, int K) {
-  __shared__ double y[TS];
-  if (*(volatile int*)a.fail) return;
-  const int t = threadIdx.x;
-  const double* Li = a.linv + (size_t)K * TT + (size_t)t * TS;
-  const double* r = a.rhs + (size_t)K * TS;
-  double s = 0;
-  for (int k = 0; k <= t; k++) s += Li[k] * r[k];
-  y[t] = s;
-  __syncthreads();
-  if (blockIdx.x == 0) {
-    a.ybuf[(size_t)K * TS + t] = s;
-    return;
-  }
-  const int I = K + blockIdx.x;
-  if (a.envT[I] > K) return;
-  const double* L = tile_ptr(a, I, K) + (size_t)t * TS;
-  double u = 0;
-  for (int k = 0; k < TS; k++) u += L[k] * y[k];
-  a.rhs[(size_t)I * TS + t] -= u;
-}
-
-// backward substitution step I: x_I = Linv_II^T z_I (block 0 stores it), z_K -= L_IK^T x_I for K in [envT[I], I)
-__global__ void __launch_bounds__(TS) k_bwd(LmArgs a, int I) {
-  __shared__ double x[TS];
-  if (*(volatile int*)a.fail) return;
-  const int t = threadIdx.x;
-  const double* Li = a.linv + (size_t)I * TT;
-  const double* z = a.ybuf + (size_t)I * TS;
-  double s = 0;
-  for (int k = t; k < TS; k++) s += Li[(size_t)k * TS + t] * z[k];
-  x[t] = s;
-  __syncthreads();
-  if (blockIdx.x == 0) {
-    a.x[(size_t)I * TS + t] = s;
-    return;
-  }
-  const int K = a.envT[I] + blockIdx.x - 1;
-  const double* L = tile_ptr(a, I, K);
-  double u = 0;
-  for (int r = 0; r < TS; r++) u += L[(size_t)r * TS + t] * x[r];
-  a.ybuf[(size_t)K * TS + t] -= u;
 }
 
 // x_l = Dinv (b_l - sum_e W_e^T x_p)
@@ -702,7 +483,7 @@ struct b2s_gba_solver {
     size_t bytes = 0;
   };
   Buf pairKey, pairKeyS, pairVal, pairValS, pairRec, pairRecS, uKey, runLen, blkBeg, nRuns, cubTmp, tiles, linv, bvec, xvec,
-      rhs, ybuf, tmp;
+      rhs, ybuf, tmp, rows;
 };
 
 namespace {
@@ -723,8 +504,7 @@ inline int blocks(long long n, int t) { return (int)((n + t - 1) / t); }
 // deterministic sum (OP 0) or max |.| (OP 1) of v[0, n) into *out (device)
 template <int OP>
 void reduce(b2s_gba_solver* h, const double* v, long long n, double* out) {
-  k_reduce_part<OP><<<RED_BLOCKS, 256, 0, h->stream>>>(v, n, h->part);
-  k_reduce_final<OP><<<1, 256, 0, h->stream>>>(h->part, RED_BLOCKS, out);
+  chol::reduce<OP>(v, n, h->part, out, h->stream);
 }
 
 int validate(const b2s_gba_solver* h, const b2s_gba_problem* p) {
@@ -792,9 +572,7 @@ extern "C" int b2s_gba_create(int max_kf, int max_mp, int max_edges, int device,
   A(&h->part, RED_BLOCKS * 8); A(&h->scal, 4 * 8); A(&h->fail, 4);
   if (e == cudaSuccess) e = cudaMallocHost(&h->hScal, 4 * 8);
   if (e == cudaSuccess) e = cudaMallocHost(&h->hFail, 4);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_potrf, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * TILE_SMEM);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_trsm, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * TILE_SMEM);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_syrk, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * TILE_SMEM);
+  if (e == cudaSuccess) e = set_smem_limits();
   if (e != cudaSuccess) {
     set_error("b2s_gba_create: %s", cudaGetErrorString(e));
     b2s_gba_destroy(h);
@@ -810,7 +588,7 @@ extern "C" void b2s_gba_destroy(b2s_gba_solver* h) {
   for (void* p : h->allocs) cudaFree(p);
   b2s_gba_solver::Buf* bufs[] = {&h->pairKey, &h->pairKeyS, &h->pairVal, &h->pairValS, &h->pairRec, &h->pairRecS,
                                  &h->uKey, &h->runLen, &h->blkBeg, &h->nRuns, &h->cubTmp, &h->tiles, &h->linv,
-                                 &h->bvec, &h->xvec, &h->rhs, &h->ybuf, &h->tmp};
+                                 &h->bvec, &h->xvec, &h->rhs, &h->ybuf, &h->tmp, &h->rows};
   for (auto* b : bufs)
     if (b->p) cudaFree(b->p);
   if (h->hScal) cudaFreeHost(h->hScal);
@@ -912,7 +690,7 @@ extern "C" int b2s_global_ba(b2s_gba_solver* h, const b2s_gba_problem* p, const 
 
   int nBlk = 0;
   long long nPairs = 0, nTiles = 0;
-  std::vector<int> envT((size_t)nT);
+  std::vector<int> envT((size_t)nT), rowOff;
   if (nE > 0) {
     // ---- structure: CSR by point and by free keyframe, pair records by lower block, block envelope
     B2S_CUDA(cudaMemsetAsync(h->ptBeg, 0, (size_t)nMp * 4, s));
@@ -987,22 +765,21 @@ extern "C" int b2s_global_ba(b2s_gba_solver* h, const b2s_gba_problem* p, const 
       B2S_CUDA(cudaMemcpyAsync(envBlk.data(), h->envBlk, (size_t)nFree * 4, cudaMemcpyDeviceToHost, s));
       rc = sync_stream();
       if (rc != B2S_OK) return rc;
-      std::vector<long long> off((size_t)nT + 1, 0);
-      for (int T = 0; T < nT; T++) {
-        int e0 = T;
-        for (int i = T * TS / 6; i < nFree && i * 6 < (T + 1) * TS; i++) e0 = std::min(e0, envBlk[(size_t)i] * 6 / TS);
-        envT[(size_t)T] = e0;
-        off[(size_t)T + 1] = off[(size_t)T] + (T - e0 + 1);
-      }
-      nTiles = off[(size_t)nT];
+      std::vector<long long> off;
+      std::vector<int> rows;
+      nTiles = tile_envelope(envBlk, nFree, 6, envT, off, rowOff, rows);
       rc = grow(h->tiles, (size_t)nTiles * TT * 8);
+      if (rc == B2S_OK) rc = grow(h->rows, rows.size() * 4);
       if (rc != B2S_OK) return rc;
       a.tiles = (double*)h->tiles.p;
+      if (!rows.empty())
+        B2S_CUDA(cudaMemcpyAsync(h->rows.p, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, s));
       B2S_CUDA(cudaMemcpyAsync(h->envT, envT.data(), (size_t)nT * 4, cudaMemcpyHostToDevice, s));
       B2S_CUDA(cudaMemcpyAsync(h->tileOff, off.data(), (size_t)(nT + 1) * 8, cudaMemcpyHostToDevice, s));
     }
   }
   const size_t tileBytes = (size_t)nTiles * TT * 8;
+  const TileSys ts = {np, h->envT, h->tileOff, a.tiles, a.linv, a.rhs, a.ybuf, a.x, h->fail};
   B2S_CUDA(cudaMemsetAsync(a.b, 0, (size_t)nx * 8, s));
   B2S_CUDA(cudaMemsetAsync(a.x, 0, (size_t)nx * 8, s));
 
@@ -1055,16 +832,7 @@ extern "C" int b2s_global_ba(b2s_gba_solver* h, const b2s_gba_problem* p, const 
         B2S_CUDA(cudaMemsetAsync(a.tiles, 0, tileBytes, s));
         k_schur<<<blocks((long long)nBlk * 32, 256), 256, 0, s>>>(a, (const unsigned*)h->uKey.p, (const int*)h->blkBeg.p,
                                                                    nBlk, (const int4*)h->pairRecS.p, lambda);
-        for (int K = 0; K < nT; K++) {
-          k_potrf<<<1, 256, 2 * TILE_SMEM, s>>>(a, K);
-          const int m = nT - K - 1;
-          if (m > 0) {
-            k_trsm<<<m, 256, 2 * TILE_SMEM, s>>>(a, K);
-            k_syrk<<<(unsigned)((long long)m * (m + 1) / 2), 256, 2 * TILE_SMEM, s>>>(a, K, nT);
-          }
-        }
-        for (int K = 0; K < nT; K++) k_fwd<<<nT - K, TS, 0, s>>>(a, K);
-        for (int I = nT - 1; I >= 0; I--) k_bwd<<<1 + I - envT[(size_t)I], TS, 0, s>>>(a, I);
+        factor_solve(ts, nT, envT, rowOff, (const int*)h->rows.p, s);
       }
       if (nMp) k_backsub_points<<<blocks(nMp, 128), 128, 0, s>>>(a);
       // ---- SparseOptimizer::update into the trial copy, trial chi2, computeScale

@@ -138,4 +138,43 @@ void Optimizer::BundleAdjustment(const GlobalBAMap& m, int nIterations, bool* pb
   out.included.resize(nMP);
 }
 
+// The essential graph runs on LoopClosing's thread: its own handle, grown on demand
+static b2s_eg_solver* g_egSolver = nullptr;
+static int g_ekf = 0, g_ee = 0, g_emp = 0;
+static std::mutex g_egMutex;
+
+void Optimizer::OptimizeEssentialGraph(const EssentialGraph& g, EssentialGraphResult& out) {
+  std::lock_guard<std::mutex> lock(g_egMutex);
+  const int nKF = (int)g.Siw.size(), nE = (int)g.edges.size(), nMP = (int)g.refKF.size();
+  if (!g_egSolver || nKF > g_ekf || nE > g_ee || nMP > g_emp) {
+    b2s_eg_destroy(g_egSolver);
+    g_egSolver = nullptr;
+    g_ekf = nKF > 1024 ? nKF : 1024;
+    g_ee = nE > 16384 ? nE : 16384;
+    g_emp = nMP > 65536 ? nMP : 65536;
+    const char* e = getenv("B2S_DEVICE");
+    int rc = b2s_eg_create(g_ekf, g_ee, g_emp, e ? atoi(e) : 0, &g_egSolver);
+    if (rc != B2S_OK) {
+      fprintf(stderr, "Optimizer::OptimizeEssentialGraph: libb200slam error %d: %s\n", rc, b2s_last_error());
+      throw std::runtime_error(b2s_last_error());
+    }
+  }
+  b2s_eg_problem p;
+  p.n_kf = nKF; p.Siw = g.Siw.data(); p.fixed_kf = g.fixedKF; p.fix_scale = g.fixScale ? 1 : 0;
+  p.n_edges = nE; p.edges = g.edges.data();
+  p.n_mp = nMP; p.points = g.points.data(); p.ref_kf = g.refKF.data();
+  out.Tcw.assign((size_t)(nKF > 0 ? nKF : 1) * 16, 0.f);
+  out.points.assign((size_t)(nMP > 0 ? nMP : 1) * 3, 0.f);
+  b2s_eg_result r;
+  r.Tcw_out = out.Tcw.data(); r.points_out = out.points.data(); r.trace = nullptr;
+  r.chi2_initial = r.chi2_final = 0; r.n_trials = 0;
+  int rc = b2s_optimize_essential_graph(g_egSolver, &p, &r);
+  if (rc != B2S_OK) {
+    fprintf(stderr, "Optimizer::OptimizeEssentialGraph: libb200slam error %d: %s\n", rc, b2s_last_error());
+    throw std::runtime_error(b2s_last_error());
+  }
+  out.Tcw.resize((size_t)nKF * 16);
+  out.points.resize((size_t)nMP * 3);
+}
+
 }  // namespace ORB_SLAM2

@@ -49,6 +49,20 @@ struct GlobalBAResult {
   std::vector<uint8_t> included;     // nMP: 0 = no edge (vbNotIncludedMP): not written back
 };
 
+struct EssentialGraph {              // Optimizer::OptimizeEssentialGraph on the gathered graph (src/Optimizer.cc:1059-1322)
+  std::vector<b2s_sim3> Siw;         // nKF: vScw of the non-bad keyframes by ascending mnId
+  int fixedKF = 0;                   // vertex of pLoopKF
+  bool fixScale = false;             // bFixScale
+  std::vector<b2s_sim3_edge> edges;  // insertion order of :1108-1262, measurements computed as the reference does
+  std::vector<float> points;         // nMP x 3: the non-bad map points
+  std::vector<int32_t> refKF;        // nMP: vertex of the point's nIDr, -1 for none
+};
+
+struct EssentialGraphResult {
+  std::vector<float> Tcw;            // nKF x 16 -> SetPose
+  std::vector<float> points;         // nMP x 3  -> SetWorldPos + UpdateNormalAndDepth
+};
+
 class Optimizer {
  public:
   // int static PoseOptimization(Frame* pFrame) (include/Optimizer.h:100, src/Optimizer.cc:363-605): fills TcwOut (the
@@ -58,6 +72,9 @@ class Optimizer {
   static void LocalBundleAdjustment(const LocalBAWindow& w, bool* pbStopFlag, LocalBAResult& out);
   // void static BundleAdjustment(vpKF, vpMP, nIterations, pbStopFlag, nLoopKF, bRobust) on the flattened map
   static void BundleAdjustment(const GlobalBAMap& m, int nIterations, bool* pbStopFlag, bool bRobust, GlobalBAResult& out);
+  // void static OptimizeEssentialGraph(pMap, pLoopKF, pCurKF, NonCorrectedSim3, CorrectedSim3, LoopConnections,
+  // bFixScale) on the gathered graph
+  static void OptimizeEssentialGraph(const EssentialGraph& g, EssentialGraphResult& out);
 };
 
 }  // namespace ORB_SLAM2

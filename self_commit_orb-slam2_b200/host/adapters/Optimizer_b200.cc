@@ -4,11 +4,14 @@
 //     void Optimizer::GlobalBundleAdjustemnt(Map*, int, bool*, unsigned long, bool)       src/Optimizer.cc:55
 //     void Optimizer::BundleAdjustment(const vector<KeyFrame*>&, const vector<MapPoint*>&, int, bool*, unsigned long,
 //                                      bool)                                              src/Optimizer.cc:86
+//     void Optimizer::OptimizeEssentialGraph(Map*, KeyFrame*, KeyFrame*, const KeyFrameAndPose&,
+//                                            const KeyFrameAndPose&, const map<KeyFrame*, set<KeyFrame*>>&,
+//                                            const bool&)                                src/Optimizer.cc:1017
 // with the reference's exact signatures, for the LocalMapping / Tracking / LoopClosing threads to call unchanged
-// (src/LocalMapping.cc:123, src/Tracking.cc:1081, 1219, 1398, 1834, 2078, 2152, src/LoopClosing.cc:880-895 ...).  Compile
-// this file INSIDE the reference tree (it includes the reference's own include/Optimizer.h) in place of those function
-// bodies of src/Optimizer.cc (:55-341, :363-605, :629-997) and link libb200slam.so; the other Optimizer functions
-// (essential graph, Sim3) stay as they are.
+// (src/LocalMapping.cc:123, src/Tracking.cc:1081, 1219, 1398, 1834, 2078, 2152, src/LoopClosing.cc:782, 880-895 ...).
+// Compile this file INSIDE the reference tree (it includes the reference's own include/Optimizer.h) in place of those
+// function bodies of src/Optimizer.cc (:55-341, :363-605, :629-997, :1017-1339) and link libb200slam.so; OptimizeSim3
+// stays as it is.
 //
 // What stays on the host is what touches the object graph: the window selection (local keyframes = pKF + covisibles,
 // local map points = their matches, fixed cameras = other observers; the mnBALocalForKF / mnBAFixedForKF marks other
@@ -27,6 +30,8 @@
 #include <list>
 #include <map>
 #include <mutex>
+#include <set>
+#include <utility>
 #include <vector>
 
 #include "Optimizer.h"
@@ -85,6 +90,36 @@ struct GbaSlot {
   }
 };
 GbaSlot g_gba;
+
+// The essential graph's handle (LoopClosing::CorrectLoop), grown on demand.
+struct EgSlot {
+  b2s_eg_solver* h = nullptr;
+  int kf = 0, edges = 0, mp = 0;
+  std::mutex m;
+  b2s_eg_solver* get(int nKF, int nE, int nMP) {
+    if (h && nKF <= kf && nE <= edges && nMP <= mp) return h;
+    b2s_eg_destroy(h);
+    h = nullptr;
+    kf = nKF > 1024 ? nKF : 1024;
+    edges = nE > 16384 ? nE : 16384;
+    mp = nMP > 65536 ? nMP : 65536;
+    if (b2s_eg_create(kf, edges, mp, device_index(), &h) != B2S_OK) {
+      fprintf(stderr, "Optimizer (b200): %s\n", b2s_last_error());
+      h = nullptr;
+      kf = edges = mp = 0;
+    }
+    return h;
+  }
+};
+EgSlot g_eg;
+
+b2s_sim3 to_b2s(const g2o::Sim3& S) {
+  b2s_sim3 o;
+  for (int i = 0; i < 4; i++) o.q[i] = S[i];
+  for (int i = 0; i < 3; i++) o.t[i] = S[4 + i];
+  o.s = S[7];
+  return o;
+}
 
 void pose_to_floats(const cv::Mat& T, float* out) {
   for (int i = 0; i < 4; i++)
@@ -404,6 +439,176 @@ void Optimizer::BundleAdjustment(const std::vector<KeyFrame*>& vpKFs, const std:
       X.copyTo(mps[m]->mPosGBA);
       mps[m]->mnBAGlobalForKF = nLoopKF;
     }
+  }
+}
+
+void Optimizer::OptimizeEssentialGraph(Map* pMap, KeyFrame* pLoopKF, KeyFrame* pCurKF,
+                                       const LoopClosing::KeyFrameAndPose& NonCorrectedSim3,
+                                       const LoopClosing::KeyFrameAndPose& CorrectedSim3,
+                                       const map<KeyFrame*, set<KeyFrame*> >& LoopConnections, const bool& bFixScale) {
+  const std::vector<KeyFrame*> vpKFs = pMap->GetAllKeyFrames();
+  const std::vector<MapPoint*> vpMPs = pMap->GetAllMapPoints();
+  const int minFeat = 100;
+
+  // ---- gather, step 2 (:1059-1098): one vertex per non-bad keyframe, ascending mnId; vScw = CorrectedSim3 if present,
+  // else Sim3(Rcw, tcw, 1)
+  std::vector<KeyFrame*> kfs;
+  for (size_t i = 0; i < vpKFs.size(); i++)
+    if (!vpKFs[i]->isBad()) kfs.push_back(vpKFs[i]);
+  std::sort(kfs.begin(), kfs.end(), [](KeyFrame* a, KeyFrame* b) { return a->mnId < b->mnId; });
+  const int nKF = (int)kfs.size();
+  std::map<unsigned long, int> index;  // mnId -> vertex
+  std::vector<g2o::Sim3, Eigen::aligned_allocator<g2o::Sim3> > vScw((size_t)nKF);
+  std::vector<b2s_sim3> Siw((size_t)nKF);
+  for (int k = 0; k < nKF; k++) {
+    KeyFrame* pKF = kfs[(size_t)k];
+    index[pKF->mnId] = k;
+    LoopClosing::KeyFrameAndPose::const_iterator it = CorrectedSim3.find(pKF);
+    if (it != CorrectedSim3.end()) {
+      vScw[(size_t)k] = it->second;
+    } else {
+      const cv::Mat R = pKF->GetRotation(), t = pKF->GetTranslation();
+      Eigen::Matrix<double, 3, 3> Rcw;
+      Eigen::Matrix<double, 3, 1> tcw;
+      for (int i = 0; i < 3; i++) {
+        for (int j = 0; j < 3; j++) Rcw(i, j) = R.at<float>(i, j);
+        tcw(i) = t.at<float>(i);
+      }
+      vScw[(size_t)k] = g2o::Sim3(Rcw, tcw, 1.0);
+    }
+    Siw[(size_t)k] = to_b2s(vScw[(size_t)k]);
+  }
+  std::map<unsigned long, int>::const_iterator li = index.find(pLoopKF->mnId);
+  if (li == index.end()) {
+    fprintf(stderr, "Optimizer::OptimizeEssentialGraph (b200): the loop keyframe is not in the map\n");
+    return;
+  }
+  auto vertex = [&](KeyFrame* pKF) {
+    std::map<unsigned long, int>::const_iterator it = index.find(pKF->mnId);
+    return it == index.end() ? -1 : it->second;
+  };
+  // the pose an edge's measurement starts from: NonCorrectedSim3 if present, else vScw
+  auto nonCorrected = [&](KeyFrame* pKF, int v) -> g2o::Sim3 {
+    LoopClosing::KeyFrameAndPose::const_iterator it = NonCorrectedSim3.find(pKF);
+    return it != NonCorrectedSim3.end() ? it->second : vScw[(size_t)v];
+  };
+  // an edge whose endpoint has no vertex would dereference a null vertex in the reference; it is left out here
+  std::vector<b2s_sim3_edge> edges;
+  auto add = [&](int i, int j, const g2o::Sim3& Sji) {
+    if (i < 0 || j < 0) return;
+    b2s_sim3_edge e;
+    e.i = i;
+    e.j = j;
+    e.meas = to_b2s(Sji);
+    edges.push_back(e);
+  };
+  std::set<std::pair<unsigned long, unsigned long> > sInsertedEdges;
+
+  // ---- step 3 (:1108-1143): loop connections, measured from vScw
+  for (map<KeyFrame*, set<KeyFrame*> >::const_iterator mit = LoopConnections.begin(); mit != LoopConnections.end(); mit++) {
+    KeyFrame* pKF = mit->first;
+    const unsigned long nIDi = pKF->mnId;
+    const int vi = vertex(pKF);
+    if (vi < 0) continue;
+    const g2o::Sim3 Swi = vScw[(size_t)vi].inverse();
+    for (set<KeyFrame*>::const_iterator sit = mit->second.begin(); sit != mit->second.end(); sit++) {
+      const unsigned long nIDj = (*sit)->mnId;
+      if ((nIDi != pCurKF->mnId || nIDj != pLoopKF->mnId) && pKF->GetWeight(*sit) < minFeat) continue;
+      const int vj = vertex(*sit);
+      if (vj < 0) continue;
+      add(vi, vj, vScw[(size_t)vj] * Swi);
+      sInsertedEdges.insert(std::make_pair(std::min(nIDi, nIDj), std::max(nIDi, nIDj)));
+    }
+  }
+  // ---- step 4 (:1147-1262): spanning tree, loop edges and strong covisibility, measured from NonCorrectedSim3
+  for (size_t i = 0; i < vpKFs.size(); i++) {
+    KeyFrame* pKF = vpKFs[i];
+    const int vi = vertex(pKF);
+    if (vi < 0) continue;
+    const g2o::Sim3 Swi = nonCorrected(pKF, vi).inverse();
+    KeyFrame* pParentKF = pKF->GetParent();
+    if (pParentKF) {
+      const int vj = vertex(pParentKF);
+      if (vj >= 0) add(vi, vj, nonCorrected(pParentKF, vj) * Swi);
+    }
+    const set<KeyFrame*> sLoopEdges = pKF->GetLoopEdges();
+    for (set<KeyFrame*>::const_iterator sit = sLoopEdges.begin(); sit != sLoopEdges.end(); sit++) {
+      KeyFrame* pLKF = *sit;
+      if (pLKF->mnId < pKF->mnId) {
+        const int vl = vertex(pLKF);
+        if (vl >= 0) add(vi, vl, nonCorrected(pLKF, vl) * Swi);
+      }
+    }
+    const std::vector<KeyFrame*> vpConnectedKFs = pKF->GetCovisiblesByWeight(minFeat);
+    for (std::vector<KeyFrame*>::const_iterator vit = vpConnectedKFs.begin(); vit != vpConnectedKFs.end(); vit++) {
+      KeyFrame* pKFn = *vit;
+      if (pKFn && pKFn != pParentKF && !pKF->hasChild(pKFn) && !sLoopEdges.count(pKFn)) {
+        if (!pKFn->isBad() && pKFn->mnId < pKF->mnId) {
+          if (sInsertedEdges.count(std::make_pair(std::min(pKF->mnId, pKFn->mnId), std::max(pKF->mnId, pKFn->mnId))))
+            continue;
+          const int vn = vertex(pKFn);
+          if (vn >= 0) add(vi, vn, nonCorrected(pKFn, vn) * Swi);
+        }
+      }
+    }
+  }
+  // ---- points (:1304-1322): the non-bad ones, each with the vertex of its nIDr (-1: none, the point stays)
+  std::vector<MapPoint*> mps;
+  for (size_t i = 0; i < vpMPs.size(); i++)
+    if (!vpMPs[i]->isBad()) mps.push_back(vpMPs[i]);
+  const int nMP = (int)mps.size(), nE = (int)edges.size();
+  std::vector<float> pts((size_t)(nMP > 0 ? nMP : 1) * 3), ptsOut((size_t)(nMP > 0 ? nMP : 1) * 3),
+      TcwOut((size_t)(nKF > 0 ? nKF : 1) * 16);
+  std::vector<int32_t> refKF((size_t)(nMP > 0 ? nMP : 1));
+  for (int m = 0; m < nMP; m++) {
+    MapPoint* pMP = mps[(size_t)m];
+    const unsigned long nIDr =
+        pMP->mnCorrectedByKF == pCurKF->mnId ? pMP->mnCorrectedReference : pMP->GetReferenceKeyFrame()->mnId;
+    std::map<unsigned long, int>::const_iterator it = index.find(nIDr);
+    refKF[(size_t)m] = it == index.end() ? -1 : it->second;
+    const cv::Mat X = pMP->GetWorldPos();
+    for (int c = 0; c < 3; c++) pts[(size_t)3 * m + c] = X.at<float>(c);
+  }
+  b2s_eg_problem prob;
+  prob.n_kf = nKF;
+  prob.Siw = Siw.data();
+  prob.fixed_kf = li->second;
+  prob.fix_scale = bFixScale ? 1 : 0;
+  prob.n_edges = nE;
+  prob.edges = edges.data();
+  prob.n_mp = nMP;
+  prob.points = pts.data();
+  prob.ref_kf = refKF.data();
+  b2s_eg_result res;
+  res.Tcw_out = TcwOut.data();
+  res.points_out = ptsOut.data();
+  res.trace = nullptr;
+  res.chi2_initial = res.chi2_final = 0;
+  res.n_trials = 0;
+  {
+    std::lock_guard<std::mutex> lock(g_eg.m);
+    b2s_eg_solver* solver = g_eg.get(nKF, nE, nMP);
+    if (!solver) return;
+    if (b2s_optimize_essential_graph(solver, &prob, &res) != B2S_OK) {
+      fprintf(stderr, "Optimizer::OptimizeEssentialGraph (b200): %s\n", b2s_last_error());
+      return;
+    }
+  }
+
+  // ---- scatter (:1274-1338) under the map-update lock: SetPose of every keyframe, SetWorldPos and
+  // UpdateNormalAndDepth of every non-bad point
+  std::unique_lock<std::mutex> lock(pMap->mMutexMapUpdate);
+  for (int k = 0; k < nKF; k++) {
+    cv::Mat T(4, 4, CV_32F);
+    for (int i = 0; i < 4; i++)
+      for (int j = 0; j < 4; j++) T.at<float>(i, j) = TcwOut[(size_t)16 * k + 4 * i + j];
+    kfs[(size_t)k]->SetPose(T);
+  }
+  for (int m = 0; m < nMP; m++) {
+    cv::Mat X(3, 1, CV_32F);
+    for (int c = 0; c < 3; c++) X.at<float>(c) = ptsOut[(size_t)3 * m + c];
+    mps[(size_t)m]->SetWorldPos(X);
+    mps[(size_t)m]->UpdateNormalAndDepth();
   }
 }
 
