@@ -35,6 +35,17 @@ int select_device(int device) {
   }
   return B2S_OK;
 }
+
+int grow(DevBuf& b, size_t bytes) {
+  if (bytes == 0) bytes = 16;
+  if (b.bytes >= bytes) return B2S_OK;
+  if (b.p) cudaFree(b.p);
+  b.p = nullptr;
+  b.bytes = 0;
+  B2S_CUDA(cudaMalloc(&b.p, bytes));
+  b.bytes = bytes;
+  return B2S_OK;
+}
 }  // namespace b2s
 
 extern "C" const char* b2s_last_error(void) { return b2s::g_last_error.c_str(); }

@@ -26,6 +26,14 @@ void set_error(const char* fmt, ...);
 
 int select_device(int device);  // returns B2S_OK / B2S_ERR_NO_DEVICE
 
+// Device buffer grown on demand.  grow() reallocates when `bytes` exceeds the capacity, without keeping the contents
+// (cudaFree synchronises the device); returns B2S_OK or a B2S_CUDA error.
+struct DevBuf {
+  void* p = nullptr;
+  size_t bytes = 0;
+};
+int grow(DevBuf& b, size_t bytes);
+
 static inline int div_up(int a, int b) { return (a + b - 1) / b; }
 static inline size_t align_up(size_t a, size_t b) { return (a + b - 1) / b * b; }
 

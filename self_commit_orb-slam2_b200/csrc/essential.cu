@@ -425,27 +425,12 @@ struct b2s_eg_solver {
          *scal = nullptr;
   double* hScal = nullptr;  // pinned
   int* hFail = nullptr;
-  // grown on demand
-  void* tiles = nullptr;
-  size_t tileBytes = 0;
-  void* rows = nullptr;
-  size_t rowBytes = 0;
+  DevBuf tiles, rows;  // grown on demand
 };
 
 namespace {
 
 inline int blocks(long long n, int t) { return (int)((n + t - 1) / t); }
-
-int grow(void*& p, size_t& have, size_t bytes) {
-  if (bytes == 0) bytes = 16;
-  if (have >= bytes) return B2S_OK;
-  if (p) cudaFree(p);
-  p = nullptr;
-  have = 0;
-  B2S_CUDA(cudaMalloc(&p, bytes));
-  have = bytes;
-  return B2S_OK;
-}
 
 int validate(const b2s_eg_solver* h, const b2s_eg_problem* p) {
   if (!p || p->n_kf < 1 || p->n_edges < 0 || p->n_mp < 0 || !p->Siw || (p->n_edges && !p->edges) ||
@@ -525,8 +510,8 @@ extern "C" void b2s_eg_destroy(b2s_eg_solver* h) {
   if (!h) return;
   if (h->stream) cudaStreamSynchronize(h->stream);
   for (void* p : h->allocs) cudaFree(p);
-  if (h->tiles) cudaFree(h->tiles);
-  if (h->rows) cudaFree(h->rows);
+  if (h->tiles.p) cudaFree(h->tiles.p);
+  if (h->rows.p) cudaFree(h->rows.p);
   if (h->hScal) cudaFreeHost(h->hScal);
   if (h->hFail) cudaFreeHost(h->hFail);
   for (cudaEvent_t ev : h->ev)
@@ -602,8 +587,8 @@ extern "C" int b2s_optimize_essential_graph(b2s_eg_solver* h, const b2s_eg_probl
   std::vector<long long> off;
   const long long nTiles = tile_envelope(envBlk, nFree, 7, envT, off, rowOff, rows);
   const int np = nFree * 7, nT = (int)envT.size(), npPad = nT * TS;
-  rc = grow(h->tiles, h->tileBytes, (size_t)nTiles * TT * 8);
-  if (rc == B2S_OK) rc = grow(h->rows, h->rowBytes, rows.size() * 4);
+  rc = grow(h->tiles, (size_t)nTiles * TT * 8);
+  if (rc == B2S_OK) rc = grow(h->rows, rows.size() * 4);
   if (rc != B2S_OK) return rc;
 
   // device time: the stream segments between the host's synchronisations (the host's LM decisions excluded)
@@ -640,7 +625,7 @@ extern "C" int b2s_optimize_essential_graph(b2s_eg_solver* h, const b2s_eg_probl
     B2S_CUDA(cudaMemsetAsync(h->b, 0, (size_t)npPad * 8, s));
     B2S_CUDA(cudaMemsetAsync(h->x, 0, (size_t)npPad * 8, s));
   }
-  if (!rows.empty()) B2S_CUDA(cudaMemcpyAsync(h->rows, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, s));
+  if (!rows.empty()) B2S_CUDA(cudaMemcpyAsync(h->rows.p, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, s));
   if (nMp) {
     B2S_CUDA(cudaMemcpyAsync(h->P, p->points, (size_t)nMp * 12, cudaMemcpyHostToDevice, s));
     B2S_CUDA(cudaMemcpyAsync(h->ref, p->ref_kf, (size_t)nMp * 4, cudaMemcpyHostToDevice, s));
@@ -651,8 +636,8 @@ extern "C" int b2s_optimize_essential_graph(b2s_eg_solver* h, const b2s_eg_probl
   a.nKf = nKf; a.nE = nE; a.nFree = nFree; a.np = np; a.fixScale = p->fix_scale != 0;
   a.ei = h->ei; a.ej = h->ej; a.meas = h->meas; a.pidx = h->pidx; a.vOff = h->vOff; a.vList = h->vList; a.blk = h->blk;
   a.bOff = h->bOff; a.bList = h->bList; a.err = h->err; a.chi2 = h->chi2; a.J = h->J; a.b = h->b;
-  a.x = h->x; a.tmp = h->tmp; a.envT = h->envT; a.tileOff = h->tileOff; a.tiles = (double*)h->tiles;
-  const TileSys ts = {np, h->envT, h->tileOff, (double*)h->tiles, h->linv, h->rhs, h->ybuf, h->x, h->fail};
+  a.x = h->x; a.tmp = h->tmp; a.envT = h->envT; a.tileOff = h->tileOff; a.tiles = (double*)h->tiles.p;
+  const TileSys ts = {np, h->envT, h->tileOff, (double*)h->tiles.p, h->linv, h->rhs, h->ybuf, h->x, h->fail};
   const size_t tileBytes = (size_t)nTiles * TT * 8;
 
   double* est = h->est;
@@ -687,11 +672,11 @@ extern "C" int b2s_optimize_essential_graph(b2s_eg_solver* h, const b2s_eg_probl
     int qmax = 0;
     do {
       B2S_CUDA(cudaMemsetAsync(h->fail, 0, 4, s));
-      B2S_CUDA(cudaMemsetAsync(h->tiles, 0, tileBytes, s));
+      B2S_CUDA(cudaMemsetAsync(h->tiles.p, 0, tileBytes, s));
       B2S_CUDA(cudaMemcpyAsync(h->rhs, h->b, (size_t)npPad * 8, cudaMemcpyDeviceToDevice, s));
       k_assemble_diag<false><<<blocks((long long)nFree * 32, 256), 256, 0, s>>>(a, lambda);
       if (nBlk) k_assemble_off<<<blocks((long long)nBlk * 32, 256), 256, 0, s>>>(a, nBlk);
-      factor_solve(ts, nT, envT, rowOff, (const int*)h->rows, s);
+      factor_solve(ts, nT, envT, rowOff, (const int*)h->rows.p, s);
       k_update<<<blocks(nKf, 128), 128, 0, s>>>(a, est, estT, lambda);
       chi2_of(estT, h->scal);
       chol::reduce<0>(h->tmp, np, h->part, h->scal + 1, s);

@@ -478,26 +478,11 @@ struct b2s_gba_solver {
   double* hScal = nullptr;  // pinned: [0] sum, [1] second sum; fail read separately
   int* hFail = nullptr;
   // grown on demand
-  struct Buf {
-    void* p = nullptr;
-    size_t bytes = 0;
-  };
-  Buf pairKey, pairKeyS, pairVal, pairValS, pairRec, pairRecS, uKey, runLen, blkBeg, nRuns, cubTmp, tiles, linv, bvec, xvec,
+  DevBuf pairKey, pairKeyS, pairVal, pairValS, pairRec, pairRecS, uKey, runLen, blkBeg, nRuns, cubTmp, tiles, linv, bvec, xvec,
       rhs, ybuf, tmp, rows;
 };
 
 namespace {
-
-int grow(b2s_gba_solver::Buf& b, size_t bytes) {
-  if (bytes == 0) bytes = 16;
-  if (b.bytes >= bytes) return B2S_OK;
-  if (b.p) cudaFree(b.p);
-  b.p = nullptr;
-  b.bytes = 0;
-  B2S_CUDA(cudaMalloc(&b.p, bytes));
-  b.bytes = bytes;
-  return B2S_OK;
-}
 
 inline int blocks(long long n, int t) { return (int)((n + t - 1) / t); }
 
@@ -586,7 +571,7 @@ extern "C" void b2s_gba_destroy(b2s_gba_solver* h) {
   if (!h) return;
   if (h->stream) cudaStreamSynchronize(h->stream);
   for (void* p : h->allocs) cudaFree(p);
-  b2s_gba_solver::Buf* bufs[] = {&h->pairKey, &h->pairKeyS, &h->pairVal, &h->pairValS, &h->pairRec, &h->pairRecS,
+  DevBuf* bufs[] = {&h->pairKey, &h->pairKeyS, &h->pairVal, &h->pairValS, &h->pairRec, &h->pairRecS,
                                  &h->uKey, &h->runLen, &h->blkBeg, &h->nRuns, &h->cubTmp, &h->tiles, &h->linv,
                                  &h->bvec, &h->xvec, &h->rhs, &h->ybuf, &h->tmp, &h->rows};
   for (auto* b : bufs)

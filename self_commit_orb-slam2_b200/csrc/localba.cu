@@ -12,6 +12,7 @@
 // by a per-window barrier in global memory; the LM state machine is a device record per window, so a batch of windows
 // needs a single launch and no host round trips.  All reductions have a fixed order (no floating-point atomics).
 #include <float.h>
+#include <limits.h>
 #include <stddef.h>
 #include <stdlib.h>
 #include <math.h>
@@ -31,8 +32,9 @@ constexpr int CHOL_BS = 32;
 
 struct BaState {
   int active, round, it, qmax, needBuild, restore, doOutlier, solveOk, stop, nTrials, nBad, robust, finishedRound0;
-  int errBuf, errCurrent;  // recompute mode: which err / eWq buffer describes the linearisation state; it is up to date
+  int errBuf, errCurrent;  // which err / eWq buffer describes the linearisation state; it is up to date
   int nLive;               // edges left at level 0 by the outlier pass between the rounds (0: round 2 has nothing to optimise)
+  int pairsOverflow;       // the covisibility pair list did not fit capPairs: the window was not run
   int its[2];
   double lambda, ni, currentChi, iniChi, tempChi, rho, chi2Final;
   unsigned long long maxDiagBits;
@@ -53,23 +55,21 @@ struct BaPtrs {  // strided per-window arrays
   int *eKf, *eMp;
   float *eObs, *eW;
   uint8_t *eStereo, *eLevel, *eOutlier;
-  double *err, *chi2, *W;  // err = errB[0]
-  double *errB[2], *eWqB[2];  // recompute mode: double-buffered (phase_errors fills the other one, an accepted step swaps)
+  double* chi2;
+  // per edge: error vector and rho' * invSigma2 of the linearisation state (0: edge excluded), from which the Schur and
+  // back-substitution phases recompute W_e; double-buffered (phase_errors fills the other one, an accepted step swaps)
+  double *errB[2], *eWqB[2];
   int *mpStart, *mpEdges, *kfStart, *kfEdges;
   double *Hpp, *Hll, *b, *x, *Dinv, *S;
-  double *db, *Y;      // Dinv*b_l per landmark, (Y unused)
+  double* db;          // Dinv*b_l per landmark
   double* DinvP;       // per landmark, 16-byte items: {d00,d01,d02,d11,d12,d22, db0,db1,db2, pad} (Schur gather record)
-  double* hl;          // landmark-side contributions {H00,H01,H02,H11,H12,H22, b0,b1,b2}, layout [window][term][edge]
   int *lmEdge, *freeKf;  // [landmark][free pose] -> edge id or -1 ; free pose index -> keyframe index
-  int *blkOff, *usePairs;  // covisibility pair lists per lower block (built once per window): offsets, fits-flag
-  int4* pairRec;           // pair record {edge of pose i1, edge of pose i2, landmark, 0}
+  int* blkOff;             // covisibility pair lists per lower block (built once per window): offsets
+  int4* pairRec;           // pair record {edge of pose i1, edge of pose i2, landmark, stereo flags}, capPairs per window
   int2* lmRec;             // landmark-CSR order: {edge, free pose index of its keyframe or -1}
   int* blkFirst;           // per block row: first non-empty block column (envelope of the reduced system)
   int *blkOrder, *blkNZ;   // lower blocks sorted by descending pair count; number of non-empty blocks
   int capPairs, capBlk;
-  double* eWq;             // per edge: rho' * invSigma2 of the last build (0: edge excluded), for the W_e recomputation
-  int schurRecompute;      // Schur phase recomputes W_e from (pose, landmark, eWq) instead of gathering the stored blocks
-  int schurDmma;           // ... and forms the 6 x 6 block products on the FP64 tensor pipe (DMMA.8x8x4)
   double *partChi, *partScale;   // per-CTA partial sums [window][nCta]
   unsigned int* bar;             // per-window barrier counters
   long long* prof;               // per-window phase cycle counters (debug): 16 slots
@@ -200,153 +200,9 @@ __device__ __forceinline__ void load_edge_ops(const BaPtrs& p, int w, const Edge
 }
 
 // ---------------------------------------------------------------- phases (device functions, strided over the window's threads)
-// computeActiveErrors + buildSystem, edge side (block_solver.hpp:502-560): one thread per edge in edge order — error,
-// chi2, Huber weight, the landmark-side products {A^T W A, A^T W e} and the pose-landmark block W_e = B^T W A.  The
-// per-edge records are written through a per-warp shared-memory transpose so that 32 consecutive edges leave the SM as
-// contiguous 4.6 KB / 2.3 KB / 0.8 KB bursts instead of 30 scattered 8-byte stores per lane.
-__device__ void phase_build_edges(const BaPtrs& p, const WinCtx& c, const BaWin& W, int robust, double* stage, double* sm) {
-  const int w = c.w;
-  const int lane = threadIdx.x & 31;
-  double* tile = stage + (size_t)(threadIdx.x >> 5) * (30 * 33);
-  const int nE = W.nEdges;
-  const bool skipW = p.schurRecompute && p.usePairs[w];  // W_e is recomputed by its two consumers: neither formed nor stored
-  double chi = 0;
-  for (int base0 = c.gtid - lane; base0 < nE; base0 += 2 * c.gthreads) {
-    EdgeIdx ix[2];
-    EdgeOps op[2];
-#pragma unroll
-    for (int h = 0; h < 2; h++) load_edge_idx(p, w, base0 + h * c.gthreads + lane, nE, ix[h]);
-#pragma unroll
-    for (int h = 0; h < 2; h++) load_edge_ops(p, w, ix[h], op[h]);
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-      const int base = base0 + h * c.gthreads;
-      if (base >= nE) break;  // (warp-uniform)
-      const int e = base + lane;
-      const size_t eo = (size_t)w * p.capE + e;
-      double rec[30];
-#pragma unroll
-      for (int k = 0; k < 30; k++) rec[k] = 0;
-      if (!ix[h].live && e < nE) p.eWqB[0][eo] = 0.0;
-      if (ix[h].live) {
-        const bool stereo = ix[h].stereo;
-        EdgeJac J;
-        edge_jacobians(op[h].P, op[h].X, stereo, W.fx, W.fy, W.bf, J);
-        const double w0 = (double)ix[h].wgt;
-        double er[3];
-        const double c2 = edge_error(J.Xc, stereo, ix[h].ob, w0, W, er);
-        p.chi2[eo] = c2;
-        double rho0 = c2, rho1 = 1.0;
-        if (robust) huber(c2, delta_of(stereo), rho0, rho1);
-        chi += rho0;
-        double omr[3];
-#pragma unroll
-        for (int r = 0; r < 3; r++) {
-          omr[r] = -(w0 * er[r]) * rho1;
-          rec[27 + r] = er[r];
-        }
-        const double wq = rho1 * w0;
-        p.eWqB[0][eo] = wq;
-        // W_e (6x3)
-        if (!skipW) {
-#pragma unroll
-          for (int i = 0; i < 6; i++)
-#pragma unroll
-            for (int j = 0; j < 3; j++) {
-              double hh = 0;
-#pragma unroll
-              for (int r = 0; r < 3; r++) hh += J.B[r][i] * wq * J.A[r][j];
-              rec[i * 3 + j] = hh;
-            }
-        }
-        // A^T (wq) A upper triangle, A^T omega_r
-        int t = 18;
-#pragma unroll
-        for (int i = 0; i < 3; i++)
-#pragma unroll
-          for (int j = i; j < 3; j++) {
-            double hh = 0;
-#pragma unroll
-            for (int r = 0; r < 3; r++) hh += J.A[r][i] * wq * J.A[r][j];
-            rec[t++] = hh;
-          }
-#pragma unroll
-        for (int i = 0; i < 3; i++) {
-          double s2 = 0;
-#pragma unroll
-          for (int r = 0; r < 3; r++) s2 += J.A[r][i] * omr[r];
-          rec[24 + i] = s2;
-        }
-      }
-#pragma unroll
-      for (int k = 0; k < 30; k++)
-        if ((k < 18 && !skipW) || k >= 27) tile[k * 33 + lane] = rec[k];
-      __syncwarp();
-      const int nv = min(32, nE - base);
-      if (!skipW) {
-        double* Wout = p.W + ((size_t)w * p.capE + base) * 18;
-        for (int idx = lane; idx < nv * 18; idx += 32) {
-          const int ed = idx / 18, k = idx - ed * 18;
-          Wout[idx] = tile[k * 33 + ed];
-        }
-      }
-      if (e < nE) {  // landmark-side terms: structure-of-arrays [term][edge], written straight from registers
-#pragma unroll
-        for (int k = 0; k < 9; k++) p.hl[((size_t)w * 9 + k) * p.capE + e] = rec[18 + k];
-      }
-      double* Eout = p.err + ((size_t)w * p.capE + base) * 3;
-      for (int idx = lane; idx < nv * 3; idx += 32) {
-        const int ed = idx / 3, k = idx - ed * 3;
-        Eout[idx] = tile[(27 + k) * 33 + ed];
-      }
-      __syncwarp();
-    }
-  }
-  const double s = block_sum(chi, sm);
-  if (threadIdx.x == 0) p.partChi[(size_t)w * p.nPartE + c.cta] = s;
-}
-
-// landmark side of buildSystem: one thread per landmark sums its edges' contributions in insertion order
-__device__ void phase_reduce_landmarks(const BaPtrs& p, const WinCtx& c, const BaWin& W) {
-  const int w = c.w;
-  const int* ms = p.mpStart + (size_t)w * (p.capMp + 1);
-  const int* me = p.mpEdges + (size_t)w * p.capE;
-  double md = 0;
-  for (int l = c.gtid; l < W.nMp; l += c.gthreads) {
-    const size_t mo = (size_t)w * p.capMp + l;
-    double h[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-    // level-1 edges carry zero terms (phase_build_edges); four edges' loads are issued together, summed in list order
-    const int kBeg = ms[l], kEnd = ms[l + 1];
-    for (int k0 = kBeg; k0 < kEnd; k0 += 4) {
-      int ee[4];
-      double v[4][9];
-#pragma unroll
-      for (int j = 0; j < 4; j++) ee[j] = me[min(k0 + j, kEnd - 1)];
-#pragma unroll
-      for (int j = 0; j < 4; j++)
-#pragma unroll
-        for (int q = 0; q < 9; q++) v[j][q] = p.hl[((size_t)w * 9 + q) * p.capE + ee[j]];
-#pragma unroll
-      for (int j = 0; j < 4; j++)
-        if (k0 + j < kEnd) {
-#pragma unroll
-          for (int q = 0; q < 9; q++) h[q] += v[j][q];
-        }
-    }
-    double* H = p.Hll + mo * 9;
-    H[0] = h[0]; H[1] = h[1]; H[2] = h[2];
-    H[3] = h[1]; H[4] = h[3]; H[5] = h[4];
-    H[6] = h[2]; H[7] = h[4]; H[8] = h[5];
-    double* bb = p.b + (size_t)w * (p.capKf * 6 + p.capMp * 3) + (size_t)W.nFree * 6 + (size_t)l * 3;
-    bb[0] = h[6]; bb[1] = h[7]; bb[2] = h[8];
-    md = fmax(md, fmax(fabs(h[0]), fmax(fabs(h[3]), fabs(h[5]))));
-  }
-  atomic_max_pos_double(&p.st[w].maxDiagBits, md);
-}
-
-// Recompute mode: the landmark side of buildSystem straight from the stored errors and weights — per edge
+// The landmark side of buildSystem straight from the stored errors and weights — per edge
 // A = d e / d X (from R|t of its keyframe and the landmark), H_ll += A^T (rho' Omega) A, b_l -= A^T (rho' Omega) e, in list order.
-__device__ void phase_reduce_landmarks_rc(const BaPtrs& p, const WinCtx& c, const BaWin& W, int cur, double* RtTab) {
+__device__ void phase_reduce_landmarks(const BaPtrs& p, const WinCtx& c, const BaWin& W, int cur, double* RtTab) {
   const int w = c.w;
   for (int k = threadIdx.x; k < W.nKf; k += blockDim.x) {
     const double* P = p.pose + ((size_t)w * p.capKf + k) * PSTRIDE;
@@ -473,7 +329,7 @@ __device__ void phase_build_poses(const BaPtrs& p, const WinCtx& c, const BaWin&
         wgt[h] = p.eW[eo];
         c2v[h] = p.chi2[eo];
 #pragma unroll
-        for (int r = 0; r < 3; r++) er[h][r] = p.errB[cur][eo * 3 + r];  // phase_build_edges / phase_errors
+        for (int r = 0; r < 3; r++) er[h][r] = p.errB[cur][eo * 3 + r];  // phase_errors
       }
 #pragma unroll
       for (int h = 0; h < 2; h++) {
@@ -639,31 +495,18 @@ __device__ __forceinline__ double warp_reduce_scatter32(double (&v)[32], int lan
 }
 
 
-// Warp-cooperative gather of one record per lane (REC16 16-byte items each, record index `rec` held by the lane) into a
-// shared-memory tile laid out [lane][N16]: consecutive lanes fetch consecutive 16-byte items, so one load instruction
-// touches ~32*16/128 lines per record run instead of 32 lines (a lane reading its own record costs one LSU wavefront
-// per lane per instruction; that wavefront rate, not HBM, is what bounded the Schur and back-substitution phases).
-// Only the first N16 items of each record are fetched.  Tile reads by the owning lane (stride N16*16 B, N16 odd) are
-// bank-conflict free for 128-bit accesses.
-template <int N16, int REC16>
-__device__ __forceinline__ void warp_gather16(double2* tile, const double2* base, int rec, int lane) {
-#pragma unroll
-  for (int r = 0; r < N16; r++) {
-    const int idx = lane + 32 * r;
-    const int pr = idx / N16, el = idx - pr * N16;
-    const int src = __shfl_sync(0xffffffffu, rec, pr);
-    tile[idx] = base[(size_t)src * REC16 + el];
-  }
-}
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
   const unsigned sa = (unsigned)__cvta_generic_to_shared(smem);
   asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(sa), "l"(gmem) : "memory");
 }
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-// the same gather as an asynchronous global->shared copy (no registers held across the memory latency)
+// Warp-cooperative asynchronous gather of one record per lane (REC16 16-byte items each, record index `rec` held by the
+// lane) into a shared-memory tile laid out [lane][N16]: consecutive lanes fetch consecutive 16-byte items, so one copy
+// instruction touches ~32*16/128 lines per record run instead of 32 lines, and no registers are held across the memory
+// latency.  Only the first N16 items of each record are fetched.  Tile reads by the owning lane (stride N16*16 B, N16
+// odd) are bank-conflict free for 128-bit accesses.
 template <int N16, int REC16>
 __device__ __forceinline__ void warp_gather16_async(double2* tile, const double2* base, int rec, int lane) {
 #pragma unroll
@@ -674,7 +517,6 @@ __device__ __forceinline__ void warp_gather16_async(double2* tile, const double2
     cp_async16(tile + idx, base + (size_t)src * REC16 + el);
   }
 }
-constexpr int GATHER_TILE16 = 32 * 9 * 2 + 32 * 5;  // per-warp staging: two W records + one packed Dinv record per lane
 
 // One covisibility pair per lane out of the staged records: acc += (W_a Dinv_l) W_c^T (36 entries: 32 in acc, 4 in
 // tail[0..3]); diagonal blocks also accumulate W_a (Dinv_l b_l) into tail[4..9].
@@ -719,66 +561,6 @@ __device__ __forceinline__ void schur_accumulate(const double2* tA, const double
       if (DIAG) tail[4 + r] += w0 * b0 + w1 * b1 + w2 * b2;
     }
   }
-}
-
-// Pair-list Schur accumulation of one block, software pipelined: while the lanes multiply the records of iteration i,
-// the cp.async gathers of iteration i+1 are in flight and the pair records of iteration i+2 are being loaded.  (At
-// 8 warps per SM the phase is bound by the index -> record -> arithmetic dependency chain, not by bandwidth.)
-// Edges excluded from the optimisation (level 1) carry W_e = 0 (phase_build_edges), so they need no test here.
-template <bool DIAG>
-__device__ __forceinline__ void schur_block_pairs(const int4* prs, int qBeg, int qEnd, const double2* Wb, const double2* Db,
-                                                  double2* buf, int lane, double (&acc)[32], double (&tail)[10]) {
-  const int nIt = (qEnd - qBeg + 31) >> 5;
-  auto issue = [&](double2* t, const int4& r) {
-    warp_gather16_async<9, 9>(t, Wb, r.x, lane);
-    if (!DIAG) {
-      warp_gather16_async<9, 9>(t + 32 * 9, Wb, r.y, lane);
-      warp_gather16_async<3, 5>(t + 32 * 18, Db, r.z, lane);
-    } else {
-      warp_gather16_async<5, 5>(t + 32 * 18, Db, r.z, lane);
-    }
-  };
-  auto loadRec = [&](int it, int4& r, bool& v) {
-    const int q = qBeg + it * 32 + lane;
-    v = q < qEnd;
-    r = v ? prs[q] : make_int4(0, 0, 0, 0);
-  };
-  int4 r0, r1 = make_int4(0, 0, 0, 0);
-  bool v0, v1 = false;
-  loadRec(0, r0, v0);
-  issue(buf, r0);
-  cp_async_commit();
-  if (nIt > 1) loadRec(1, r1, v1);
-  for (int it = 0; it < nIt; it++) {
-    double2* cur = buf + (size_t)(it & 1) * GATHER_TILE16;
-    double2* nxt = buf + (size_t)((it & 1) ^ 1) * GATHER_TILE16;
-    if (it + 1 < nIt) issue(nxt, r1);
-    cp_async_commit();
-    int4 r2 = make_int4(0, 0, 0, 0);
-    bool v2 = false;
-    if (it + 2 < nIt) {
-      loadRec(it + 2, r2, v2);
-      // 32 windows' records (~10 MB each) do not stay in L2: pull the lines of step it+2 into L2 now so that its
-      // cp.async gathers (issued one step later) see L2 latency instead of DRAM latency
-      if (v2) {
-        prefetch_l2(Wb + (size_t)r2.x * 9);
-        prefetch_l2(Wb + (size_t)r2.x * 9 + 8);
-        if (!DIAG) {
-          prefetch_l2(Wb + (size_t)r2.y * 9);
-          prefetch_l2(Wb + (size_t)r2.y * 9 + 8);
-        }
-        prefetch_l2(Db + (size_t)r2.z * 5);
-      }
-    }
-    cp_async_wait<1>();
-    __syncwarp();
-    if (v0) schur_accumulate<DIAG>(cur, cur + 32 * 9, cur + 32 * 18, lane, acc, tail);
-    __syncwarp();
-    v0 = v1;
-    r1 = r2;
-    v1 = v2;
-  }
-  cp_async_wait<0>();
 }
 
 // W_e = B^T (rho' Omega) A of one edge from the camera's rotation / translation (Rt: R row-major, then t), the landmark and
@@ -839,17 +621,17 @@ __device__ __forceinline__ void cp_async8(void* smem, const void* gmem) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(sa), "l"(gmem) : "memory");
 }
 
-// per-warp staging of the recomputing Schur loop (double2 units): W_a | W_c tiles (one 9-double2 record per lane each),
-// two Dinv tiles (5 per lane) and two operand tiles (3 per lane: X0 X1 | X2 wq_a | wq_c -), then R|t of the block's two poses
-constexpr int RC_W = 0, RC_D = 32 * 18, RC_OP = RC_D + 2 * 32 * 5, RC_RT = RC_OP + 2 * 32 * 3, RC_DB = RC_RT + 12,
-              RC_TOTAL = RC_DB + 48;  // RC_DB: Dinv b_l of the 32 pairs of an iteration (DMMA variant, diagonal blocks)
-static_assert(RC_TOTAL <= 2 * GATHER_TILE16, "the recomputing loop reuses the gather staging area");
+// per-warp staging of the Schur loop (double2 units): W_a | W_c tiles (one 9-double2 record per lane each), two Dinv
+// tiles (5 per lane) and two operand tiles (3 per lane: X0 X1 | X2 wq_a | wq_c -), then R|t of the block's two poses
+constexpr int RC_W = 0, RC_D = 32 * 18, RC_OP = RC_D + 2 * 32 * 5, RC_RT = RC_OP + 2 * 32 * 3, RC_TOTAL = RC_RT + 12;
 
-// Same accumulation as schur_block_pairs, but W_a / W_c are recomputed per pair from 40 bytes of operands that stay
-// resident in L2 (landmark position, two edge weights) instead of gathering two 144-byte blocks from a 4.3 MB array that
-// 32 concurrent windows push out of L2 (the gathers are ~all of the stored form's DRAM reads).
+// Pair-list Schur accumulation of one block, software pipelined: while the lanes multiply the pairs of iteration i, the
+// cp.async copies of iteration i+1 are in flight and the pair records of iteration i+2 are being loaded.  W_a / W_c are
+// recomputed per pair from 40 bytes of operands that stay resident in L2 (landmark position, two edge weights) instead
+// of being stored per edge and gathered (144 bytes each from an array that 32 concurrent windows push out of L2).
+// Edges excluded from the optimisation (level 1) have weight 0 and so an exact zero W_e: they need no test here.
 template <bool DIAG>
-__device__ __forceinline__ void schur_block_pairs_rc(const int4* prs, int qBeg, int qEnd, const double* __restrict__ pts,
+__device__ __forceinline__ void schur_block_pairs(const int4* prs, int qBeg, int qEnd, const double* __restrict__ pts,
                                                      const double* __restrict__ eWq, const double2* Db, double2* buf, int lane,
                                                      double fx, double fy, double bf, double (&acc)[32], double (&tail)[10]) {
   const int nIt = (qEnd - qBeg + 31) >> 5;
@@ -902,127 +684,6 @@ __device__ __forceinline__ void schur_block_pairs_rc(const int4* prs, int qBeg, 
   cp_async_wait<0>();
 }
 
-// The same block sum on the FP64 tensor pipe.  With the pairs p of the block stacked along k = 3 p + j,
-//   S(i1,i2) -= A B,   A[r][k] = W_a,p[r][j]  (6 x 3P),   B[k][c] = (W_c,p Dinv_p)[c][j]  (3P x 6),
-// and for a diagonal block one more column B[k][6] = (Dinv_p b_p)[j], which makes column 6 of the product the block's
-// right-hand-side sum W_a (Dinv b).  An iteration handles 32 pairs: every lane recomputes its pair's W_a (and W_c), forms
-// Z = W_c Dinv in registers and leaves W_a | Z | Dinv b in the warp's staging tile; 24 mma.sync.m8n8k4.f64 (SASS DMMA.8x8x4)
-// then consume the 96 k-positions, each lane feeding A[g][k0+t] and B[k0+t][g] (g = lane / 4, t = lane % 4; rows / columns
-// 6, 7 of the 8 x 8 tile are zero padding).  The warp's whole block lives in two accumulator registers per lane
-// (C[g][2t], C[g][2t+1]): no per-lane 6 x 6 partial sums and no 36-value warp reduction at the end of the block.
-template <bool DIAG>
-__device__ __forceinline__ void schur_block_pairs_dmma(const int4* prs, int qBeg, int qEnd, const double* __restrict__ pts,
-                                                       const double* __restrict__ eWq, const double2* Db, double2* buf, int lane,
-                                                       double fx, double fy, double bf, double& c0, double& c1) {
-  const int nIt = (qEnd - qBeg + 31) >> 5;
-  double* sA = reinterpret_cast<double*>(buf + RC_W);            // [pair][r * 3 + j]
-  double* sZ = reinterpret_cast<double*>(buf + RC_W + 32 * 9);   // [pair][c * 3 + j]
-  double* sDb = reinterpret_cast<double*>(buf + RC_DB);          // [pair][j]
-  const double* Rt = reinterpret_cast<const double*>(buf + RC_RT);
-  const int g = lane >> 2, t = lane & 3;
-  auto issue = [&](int slot, const int4& r, bool v) {
-    double2* op = buf + RC_OP + slot * (32 * 3) + lane * 3;
-    if (v) {
-      const double* X = pts + (size_t)r.z * 3;
-      double* o = reinterpret_cast<double*>(op);
-      cp_async8(o, X);
-      cp_async8(o + 1, X + 1);
-      cp_async8(o + 2, X + 2);
-      cp_async8(o + 3, eWq + r.x);
-      if (!DIAG) cp_async8(o + 4, eWq + r.y);
-    }
-    warp_gather16_async<DIAG ? 5 : 3, 5>(buf + RC_D + slot * (32 * 5), Db, r.z, lane);
-  };
-  auto loadRec = [&](int it, int4& r, bool& v) {
-    const int q = qBeg + it * 32 + lane;
-    v = q < qEnd;
-    r = v ? prs[q] : make_int4(0, 0, 0, 0);
-  };
-  int4 r0, r1 = make_int4(0, 0, 0, 0);
-  bool v0, v1 = false;
-  loadRec(0, r0, v0);
-  issue(0, r0, v0);
-  cp_async_commit();
-  if (nIt > 1) loadRec(1, r1, v1);
-  for (int it = 0; it < nIt; it++) {
-    const int slot = it & 1;
-    if (it + 1 < nIt) issue(slot ^ 1, r1, v1);
-    cp_async_commit();
-    int4 r2 = make_int4(0, 0, 0, 0);
-    bool v2 = false;
-    if (it + 2 < nIt) loadRec(it + 2, r2, v2);
-    cp_async_wait<1>();
-    __syncwarp();
-    {
-      double wa[18], z[18];
-      double db0 = 0.0, db1 = 0.0, db2 = 0.0;
-      if (v0) {
-        const double* o = reinterpret_cast<const double*>(buf + RC_OP + slot * (32 * 3) + lane * 3);
-        const double X0 = o[0], X1 = o[1], X2 = o[2];
-        edge_W_regs(Rt, X0, X1, X2, (r0.w & 1) != 0, o[3], fx, fy, bf, wa);
-        double wc[18];
-        if (!DIAG) edge_W_regs(Rt + 12, X0, X1, X2, (r0.w & 2) != 0, o[4], fx, fy, bf, wc);
-        const double2* rd = buf + RC_D + slot * (32 * 5) + lane * (DIAG ? 5 : 3);
-        const double2 dA = rd[0], dB = rd[1], dC = rd[2];
-        const double d00 = dA.x, d01 = dA.y, d02 = dB.x, d11 = dB.y, d12 = dC.x, d22 = dC.y;
-        if (DIAG) {
-          const double2 e0 = rd[3], e1 = rd[4];
-          db0 = e0.x; db1 = e0.y; db2 = e1.x;
-        }
-#pragma unroll
-        for (int cc = 0; cc < 6; cc++) {
-          const double w0 = DIAG ? wa[cc * 3] : wc[cc * 3], w1 = DIAG ? wa[cc * 3 + 1] : wc[cc * 3 + 1],
-                       w2 = DIAG ? wa[cc * 3 + 2] : wc[cc * 3 + 2];
-          z[cc * 3] = w0 * d00 + w1 * d01 + w2 * d02;
-          z[cc * 3 + 1] = w0 * d01 + w1 * d11 + w2 * d12;
-          z[cc * 3 + 2] = w0 * d02 + w1 * d12 + w2 * d22;
-        }
-      } else {
-#pragma unroll
-        for (int k = 0; k < 18; k++) {
-          wa[k] = 0.0;
-          z[k] = 0.0;
-        }
-      }
-      double2* oa = reinterpret_cast<double2*>(sA + lane * 18);
-      double2* oz = reinterpret_cast<double2*>(sZ + lane * 18);
-#pragma unroll
-      for (int k = 0; k < 9; k++) {
-        oa[k] = make_double2(wa[2 * k], wa[2 * k + 1]);
-        oz[k] = make_double2(z[2 * k], z[2 * k + 1]);
-      }
-      if (DIAG) {
-        sDb[lane * 3] = db0;
-        sDb[lane * 3 + 1] = db1;
-        sDb[lane * 3 + 2] = db2;
-      }
-    }
-    __syncwarp();
-    const int kEnd = min(32, qEnd - qBeg - it * 32) * 3;  // k-positions that carry a pair (the rest of the tile is zero)
-#pragma unroll 4
-    for (int k0 = 0; k0 < 96; k0 += 4) {
-      if (k0 >= kEnd) break;  // (warp-uniform)
-      const int k = k0 + t;
-      const int pr = (k * 0xAAABu) >> 17;  // k / 3 for k < 98304
-      const int j = k - 3 * pr;
-      double av = 0.0, bv = 0.0;
-      if (g < 6) {
-        av = sA[pr * 18 + g * 3 + j];
-        bv = sZ[pr * 18 + g * 3 + j];
-      } else if (DIAG && g == 6) {
-        bv = sDb[pr * 3 + j];
-      }
-      asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-                   : "+d"(c0), "+d"(c1)
-                   : "d"(av), "d"(bv));
-    }
-    __syncwarp();
-    r0 = r1; v0 = v1;
-    r1 = r2; v1 = v2;
-  }
-  cp_async_wait<0>();
-}
-
 // Schur complement (block_solver.hpp:381-439): one warp per lower block (i1 >= i2); lanes stride over the block's
 // covisibility pairs (edge a of pose i1, edge c of pose i2, same landmark l) and accumulate (W_a Dinv_l) W_c^T; the
 // diagonal blocks also accumulate W_a (Dinv_l b_l) for the right-hand side.  S(i1,i2) = [Hpp + lambda I] - sum.
@@ -1033,21 +694,17 @@ __device__ void phase_schur_blocks(const BaPtrs& p, const WinCtx& c, const BaWin
   const int nWarps = c.gthreads >> 5, gw = c.gtid >> 5;
   const int nb = W.nFree * (W.nFree + 1) / 2;
   const int n = W.nFree * 6;
-  const int usePairs = p.usePairs[w];
   const int* off = p.blkOff + (size_t)w * (p.capBlk + 1);
   const int* order = p.blkOrder + (size_t)w * p.capBlk;
   const int4* prs = p.pairRec + (size_t)w * p.capPairs;
-  const int* ks = p.kfStart + (size_t)w * (p.capKf + 1);
-  const int* ke = p.kfEdges + (size_t)w * p.capE;
-  const int* lm = p.lmEdge + (size_t)w * p.capMp * p.capKf;
-  const int* eMp = p.eMp + (size_t)w * p.capE;
-  const double2* Wb = reinterpret_cast<const double2*>(p.W + (size_t)w * p.capE * 18);
   const double2* Db = reinterpret_cast<const double2*>(p.DinvP + (size_t)w * p.capMp * 10);
-  double2* buf = reinterpret_cast<double2*>(stage) + (size_t)(threadIdx.x >> 5) * (2 * GATHER_TILE16);
+  const double* ptsW = p.pts + (size_t)w * p.capMp * 3;
+  const double* wqW = p.eWqB[cur] + (size_t)w * p.capE;
+  double2* buf = reinterpret_cast<double2*>(stage) + (size_t)(threadIdx.x >> 5) * RC_TOTAL;
   for (int k0 = 0; k0 < nb; k0 += nWarps) {
     const int k = k0 + (((k0 / nWarps) & 1) ? nWarps - 1 - gw : gw);
     if (k >= nb) continue;
-    const int t = usePairs ? order[k] : k;
+    const int t = order[k];
     int i1, i2;
     decode_block(t, i1, i2);
     const bool diag = (i1 == i2);
@@ -1056,108 +713,26 @@ __device__ void phase_schur_blocks(const BaPtrs& p, const WinCtx& c, const BaWin
     for (int z = 0; z < 32; z++) acc[z] = 0;
 #pragma unroll
     for (int z = 0; z < 10; z++) tail[z] = 0;
-    bool any = true;
-    const bool dmma = usePairs && p.schurRecompute && p.schurDmma;
-    double c0 = 0.0, c1 = 0.0;  // DMMA variant: C[g][2t], C[g][2t+1] of the block's 8 x 8 product tile
-    if (usePairs) {
-      const int qBeg = off[t], qEnd = off[t + 1];
-      any = qEnd > qBeg;
-      if (any && dmma) {
-        __syncwarp();
-        if (lane < 2) {
-          const int kf = p.freeKf[(size_t)w * p.capKf + (lane ? i2 : i1)];
-          const double* P = p.pose + ((size_t)w * p.capKf + kf) * PSTRIDE;
-          double R[3][3];
-          quat_to_R(P, R);
-          double* o = reinterpret_cast<double*>(buf + RC_RT) + lane * 12;
+    const int qBeg = off[t], qEnd = off[t + 1];
+    const bool any = qEnd > qBeg;
+    if (any) {
+      // rotation / translation of the block's two cameras, staged once per block for the whole warp
+      __syncwarp();
+      if (lane < 2) {
+        const int kf = p.freeKf[(size_t)w * p.capKf + (lane ? i2 : i1)];
+        const double* P = p.pose + ((size_t)w * p.capKf + kf) * PSTRIDE;
+        double R[3][3];
+        quat_to_R(P, R);
+        double* o = reinterpret_cast<double*>(buf + RC_RT) + lane * 12;
 #pragma unroll
-          for (int a = 0; a < 3; a++)
+        for (int a = 0; a < 3; a++)
 #pragma unroll
-            for (int b2 = 0; b2 < 3; b2++) o[a * 3 + b2] = R[a][b2];
-          o[9] = P[4]; o[10] = P[5]; o[11] = P[6];
-        }
-        __syncwarp();
-        const double* ptsW = p.pts + (size_t)w * p.capMp * 3;
-        const double* wqW = p.eWqB[cur] + (size_t)w * p.capE;
-        if (diag) schur_block_pairs_dmma<true>(prs, qBeg, qEnd, ptsW, wqW, Db, buf, lane, W.fx, W.fy, W.bf, c0, c1);
-        else schur_block_pairs_dmma<false>(prs, qBeg, qEnd, ptsW, wqW, Db, buf, lane, W.fx, W.fy, W.bf, c0, c1);
-      } else if (any && p.schurRecompute) {
-        // rotation / translation of the block's two cameras, staged once per block for the whole warp
-        __syncwarp();
-        if (lane < 2) {
-          const int kf = p.freeKf[(size_t)w * p.capKf + (lane ? i2 : i1)];
-          const double* P = p.pose + ((size_t)w * p.capKf + kf) * PSTRIDE;
-          double R[3][3];
-          quat_to_R(P, R);
-          double* o = reinterpret_cast<double*>(buf + RC_RT) + lane * 12;
-#pragma unroll
-          for (int a = 0; a < 3; a++)
-#pragma unroll
-            for (int b2 = 0; b2 < 3; b2++) o[a * 3 + b2] = R[a][b2];
-          o[9] = P[4]; o[10] = P[5]; o[11] = P[6];
-        }
-        __syncwarp();
-        const double* ptsW = p.pts + (size_t)w * p.capMp * 3;
-        const double* wqW = p.eWqB[cur] + (size_t)w * p.capE;
-        if (diag) schur_block_pairs_rc<true>(prs, qBeg, qEnd, ptsW, wqW, Db, buf, lane, W.fx, W.fy, W.bf, acc, tail);
-        else schur_block_pairs_rc<false>(prs, qBeg, qEnd, ptsW, wqW, Db, buf, lane, W.fx, W.fy, W.bf, acc, tail);
-      } else if (any) {
-        if (diag) schur_block_pairs<true>(prs, qBeg, qEnd, Wb, Db, buf, lane, acc, tail);
-        else schur_block_pairs<false>(prs, qBeg, qEnd, Wb, Db, buf, lane, acc, tail);
+          for (int b2 = 0; b2 < 3; b2++) o[a * 3 + b2] = R[a][b2];
+        o[9] = P[4]; o[10] = P[5]; o[11] = P[6];
       }
-    } else {  // pair list did not fit: walk pose i1's edges and probe the landmark->edge table (same order)
-      const int kf1 = p.freeKf[(size_t)w * p.capKf + i1];
-      const int qBeg = ks[kf1], qEnd = ks[kf1 + 1];
-      for (int q0 = qBeg; q0 < qEnd; q0 += 32) {
-        const int q = q0 + lane;
-        bool valid = q < qEnd;
-        int ea = 0, ec = 0, mp = 0;
-        if (valid) {
-          ea = ke[q];
-          mp = eMp[ea];
-          ec = lm[(size_t)mp * p.capKf + i2];
-          if (ec < 0) {
-            valid = false;
-            ec = 0;
-          }
-        }
-        if (!__any_sync(0xffffffffu, valid)) continue;
-        warp_gather16<9, 9>(buf, Wb, ea, lane);
-        if (!diag) {
-          warp_gather16<9, 9>(buf + 32 * 9, Wb, ec, lane);
-          warp_gather16<3, 5>(buf + 32 * 18, Db, mp, lane);
-        } else {
-          warp_gather16<5, 5>(buf + 32 * 18, Db, mp, lane);
-        }
-        __syncwarp();
-        if (valid) {
-          if (diag) schur_accumulate<true>(buf, buf + 32 * 9, buf + 32 * 18, lane, acc, tail);
-          else schur_accumulate<false>(buf, buf + 32 * 9, buf + 32 * 18, lane, acc, tail);
-        }
-        __syncwarp();
-      }
-    }
-    if (dmma) {  // lane (g, t) holds columns 2t, 2t+1 of row g; column 6 of a diagonal block is its right-hand-side sum
-      double* Sb = p.S + (size_t)w * p.ldS * p.ldS + (size_t)(i1 * 6) * p.ldS + i2 * 6;
-      const double* Hp = p.Hpp + ((size_t)w * p.capKf + i1) * 36;
-      const int g = lane >> 2, t4 = lane & 3;
-      if (g < 6 && t4 < 3) {
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-          const int cc = 2 * t4 + h;
-          double base = 0;
-          if (diag) {
-            base = Hp[g * 6 + cc];
-            if (g == cc) base += lambda;
-          }
-          Sb[(size_t)g * p.ldS + cc] = base - (h ? c1 : c0);
-        }
-      }
-      if (diag && g < 6 && t4 == 3) {
-        const double* bp = p.b + (size_t)w * (p.capKf * 6 + p.capMp * 3) + (size_t)i1 * 6;
-        p.S[(size_t)w * p.ldS * p.ldS + (size_t)n * p.ldS + i1 * 6 + g] = bp[g] - c0;
-      }
-      continue;
+      __syncwarp();
+      if (diag) schur_block_pairs<true>(prs, qBeg, qEnd, ptsW, wqW, Db, buf, lane, W.fx, W.fy, W.bf, acc, tail);
+      else schur_block_pairs<false>(prs, qBeg, qEnd, ptsW, wqW, Db, buf, lane, W.fx, W.fy, W.bf, acc, tail);
     }
     double mine = 0;
     if (any) {  // (warp-uniform) a block without pairs is just its Hpp part
@@ -1404,11 +979,8 @@ __device__ void phase_backsub_update(const BaPtrs& p, const WinCtx& c, const BaW
   double sc = 0;
   const int lane = threadIdx.x & 31;
   const int2* lrec = p.lmRec + (size_t)w * p.capE;
-  const double2* Wb2 = reinterpret_cast<const double2*>(p.W + (size_t)w * p.capE * 18);
-  double2* tA = reinterpret_cast<double2*>(stage) + (size_t)(threadIdx.x >> 5) * (2 * GATHER_TILE16);
-  const bool recompute = p.schurRecompute && p.usePairs[w];
-  double* RtTab = stage + (size_t)(blockDim.x >> 5) * (2 * GATHER_TILE16) * 2;  // R | t of every free pose (behind the gather tiles)
-  if (recompute && solveOk) {
+  double* RtTab = stage + (size_t)(blockDim.x >> 5) * RC_TOTAL * 2;  // R | t of every free pose (behind the Schur staging)
+  if (solveOk) {
     for (int i = threadIdx.x; i < W.nFree; i += blockDim.x) {
       const double* P = p.pose + ((size_t)w * p.capKf + p.freeKf[(size_t)w * p.capKf + i]) * PSTRIDE;
       double R[3][3];
@@ -1438,81 +1010,37 @@ __device__ void phase_backsub_update(const BaPtrs& p, const WinCtx& c, const BaW
     const double* bl = p.b + xo + (size_t)W.nFree * 6 + (size_t)(live ? l : 0) * 3;
     double cl[3] = {bl[0], bl[1], bl[2]};
     const int kBeg = live ? ms[l] : 0, deg = live ? ms[l + 1] - kBeg : 0;
-    int maxDeg = deg;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) maxDeg = max(maxDeg, __shfl_xor_sync(0xffffffffu, maxDeg, o));
-    // Edges k .. k+4 of every landmark of the group at once: their {edge, pose} records, then their W records (gathered
-    // cooperatively with cp.async into five tiles) are all in flight together, so a group costs two memory latencies
-    // instead of three per edge.  Level-1 edges carry W_e = 0 and subtract exact zeros.
-    constexpr int NBUF = 5, TILE = 32 * 9;
-    if (recompute) {
-      // W_e^T x_p with W_e recomputed from (R|t of the pose, this landmark, edge weight): five edges' records, then their
-      // weights and flags, are loaded together; no W block is read
-      const double X0 = live ? X[0] : 0.0, X1 = live ? X[1] : 0.0, X2 = live ? X[2] : 1.0;
-      for (int kb0 = 0; kb0 < deg; kb0 += NBUF) {
-        int ee[NBUF], pp[NBUF];
-        double wq[NBUF];
-        bool st[NBUF];
-#pragma unroll
-        for (int j = 0; j < NBUF; j++) {
-          const int2 r = (kb0 + j < deg) ? lrec[kBeg + kb0 + j] : make_int2(0, -1);
-          ee[j] = r.x;
-          pp[j] = r.y;
-        }
-#pragma unroll
-        for (int j = 0; j < NBUF; j++) {
-          wq[j] = wqW[ee[j]];
-          st[j] = stW[ee[j]] != 0;
-        }
-#pragma unroll
-        for (int j = 0; j < NBUF; j++) {
-          if (pp[j] < 0) continue;
-          double wb[18];
-          edge_W_regs(RtTab + (size_t)pp[j] * 12, X0, X1, X2, st[j], wq[j], W.fx, W.fy, W.bf, wb);
-          const double* xp = p.x + xo + (size_t)pp[j] * 6;
-#pragma unroll
-          for (int cc = 0; cc < 3; cc++)
-#pragma unroll
-            for (int r = 0; r < 6; r++) cl[cc] -= wb[r * 3 + cc] * xp[r];
-        }
-      }
-    } else
-    for (int kb0 = 0; kb0 < maxDeg; kb0 += NBUF) {
+    // W_e^T x_p with W_e recomputed from (R|t of the pose, this landmark, edge weight): five edges' {edge, pose} records,
+    // then their weights and flags, are loaded together, so the five edges share two memory latencies.  Level-1 edges
+    // have weight 0 and subtract exact zeros.
+    constexpr int NBUF = 5;
+    const double X0 = live ? X[0] : 0.0, X1 = live ? X[1] : 0.0, X2 = live ? X[2] : 1.0;
+    for (int kb0 = 0; kb0 < deg; kb0 += NBUF) {
       int ee[NBUF], pp[NBUF];
+      double wq[NBUF];
+      bool st[NBUF];
 #pragma unroll
       for (int j = 0; j < NBUF; j++) {
-        const int k = kb0 + j;
-        const int2 r = (k < deg) ? lrec[kBeg + k] : make_int2(0, -1);
+        const int2 r = (kb0 + j < deg) ? lrec[kBeg + kb0 + j] : make_int2(0, -1);
         ee[j] = r.x;
         pp[j] = r.y;
       }
 #pragma unroll
-      for (int j = 0; j < NBUF; j++)
-        if (kb0 + j < maxDeg) warp_gather16_async<9, 9>(tA + j * TILE, Wb2, ee[j], lane);
-      cp_async_commit();
-      cp_async_wait<0>();
-      __syncwarp();
+      for (int j = 0; j < NBUF; j++) {
+        wq[j] = wqW[ee[j]];
+        st[j] = stW[ee[j]] != 0;
+      }
 #pragma unroll
       for (int j = 0; j < NBUF; j++) {
         if (pp[j] < 0) continue;
-        const double2* ra = tA + j * TILE + lane * 9;
         double wb[18];
-#pragma unroll
-        for (int z = 0; z < 9; z++) {
-          const double2 t2 = ra[z];
-          wb[2 * z] = t2.x;
-          wb[2 * z + 1] = t2.y;
-        }
+        edge_W_regs(RtTab + (size_t)pp[j] * 12, X0, X1, X2, st[j], wq[j], W.fx, W.fy, W.bf, wb);
         const double* xp = p.x + xo + (size_t)pp[j] * 6;
-        double xv[6];
-#pragma unroll
-        for (int r = 0; r < 6; r++) xv[r] = xp[r];
 #pragma unroll
         for (int cc = 0; cc < 3; cc++)
 #pragma unroll
-          for (int r = 0; r < 6; r++) cl[cc] -= wb[r * 3 + cc] * xv[r];
+          for (int r = 0; r < 6; r++) cl[cc] -= wb[r * 3 + cc] * xp[r];
       }
-      __syncwarp();
     }
     if (!live) continue;
     const double* Di = p.Dinv + mo * 9;
@@ -1544,11 +1072,11 @@ __device__ void phase_backsub_update(const BaPtrs& p, const WinCtx& c, const BaW
   if (threadIdx.x == 0) p.partScale[(size_t)w * p.nPartM + c.cta] = s;
 }
 
-// computeActiveErrors + activeRobustChi2 after the update (sparse_optimizer.cpp:61-113), one thread per edge
-// storeBuf >= 0 (recompute mode): also keep the error vectors and the edge weights rho' * invSigma2 in buffer storeBuf, so
-// that an accepted step needs no separate error pass before the next buildSystem (the values are the same);
+// computeActiveErrors + activeRobustChi2 after the update (sparse_optimizer.cpp:61-113), one thread per edge; also keeps
+// the error vectors and the edge weights rho' * invSigma2 in buffer storeBuf, so that an accepted step needs no separate
+// error pass before the next buildSystem (the values are the same);
 // zeroDead: excluded edges get weight 0 (first pass of a round).
-__device__ void phase_errors(const BaPtrs& p, const WinCtx& c, const BaWin& W, int robust, double* sm, int storeBuf = -1,
+__device__ void phase_errors(const BaPtrs& p, const WinCtx& c, const BaWin& W, int robust, double* sm, int storeBuf,
                              bool zeroDead = false) {
   const int w = c.w;
   double chi = 0;
@@ -1577,11 +1105,9 @@ __device__ void phase_errors(const BaPtrs& p, const WinCtx& c, const BaWin& W, i
       double rho0 = c2, rho1 = 1.0;
       if (robust) huber(c2, delta_of(ix[h].stereo), rho0, rho1);
       chi += rho0;
-      if (storeBuf >= 0) {
-        double* eb = p.errB[storeBuf] + eo * 3;
-        eb[0] = er[0]; eb[1] = er[1]; eb[2] = er[2];
-        p.eWqB[storeBuf][eo] = rho1 * (double)ix[h].wgt;
-      }
+      double* eb = p.errB[storeBuf] + eo * 3;
+      eb[0] = er[0]; eb[1] = er[1]; eb[2] = er[2];
+      p.eWqB[storeBuf][eo] = rho1 * (double)ix[h].wgt;
     }
   }
   const double s = block_sum(chi, sm);
@@ -1614,10 +1140,8 @@ __device__ void control_end(const BaPtrs& p, int w, int nCta) {
     st.lambda *= fmax(1. / 3., alpha);
     st.ni = 2;
     st.currentChi = tempChi;
-    if (p.schurRecompute && p.usePairs[w]) {  // phase_errors just stored this state's errors / weights in the other buffer
-      st.errBuf ^= 1;
-      st.errCurrent = 1;
-    }
+    st.errBuf ^= 1;  // phase_errors just stored this state's errors / weights in the other buffer
+    st.errCurrent = 1;
   } else {
     st.lambda *= st.ni;
     st.ni *= 2;
@@ -1723,24 +1247,16 @@ __global__ void __launch_bounds__(BA_T) k_local_ba(BaPtrs p, int nCtaUniform, in
   for (int guard = 0; guard < 4096; guard++) {
     if (!vst->active || *hung) break;
     const int needBuild = vst->needBuild, robust = vst->robust;
-    const bool rcMode = p.schurRecompute && p.usePairs[w];
-    const int cur = rcMode ? vst->errBuf : 0;
+    const int cur = vst->errBuf;
     if (needBuild) {
       for (int rr = ((dbgRepeat >> 8) == 2 ? (dbgRepeat & 255) : 1); rr > 0; rr--) {
-        if (rcMode) {
-          // errors + weights: after an accepted step they were stored by that step's phase_errors (same state, same values)
-          if (!vst->errCurrent) {
-            phase_errors(p, c, W, robust, red, cur, true);
-            win_barrier(bar, epoch, nCta, hung);
-          }
-          BA_PROF(0)
-          phase_reduce_landmarks_rc(p, c, W, cur, dsm);
-        } else {
-          phase_build_edges(p, c, W, robust, dsm, red);
+        // errors + weights: after an accepted step they were stored by that step's phase_errors (same state, same values)
+        if (!vst->errCurrent) {
+          phase_errors(p, c, W, robust, red, cur, true);
           win_barrier(bar, epoch, nCta, hung);
-          BA_PROF(0)
-          phase_reduce_landmarks(p, c, W);
         }
+        BA_PROF(0)
+        phase_reduce_landmarks(p, c, W, cur, dsm);
         phase_build_poses(p, c, W, robust, cur);
         win_barrier(bar, epoch, nCta, hung);
         BA_PROF(1)
@@ -1767,7 +1283,7 @@ __global__ void __launch_bounds__(BA_T) k_local_ba(BaPtrs p, int nCtaUniform, in
     win_barrier(bar, epoch, nCta, hung);
     BA_PROF(7)
     for (int rr = ((dbgRepeat >> 8) == 3 ? (dbgRepeat & 255) : 1); rr > 0; rr--) {
-      phase_errors(p, c, W, robust, red, rcMode ? (cur ^ 1) : -1);
+      phase_errors(p, c, W, robust, red, cur ^ 1);
       win_barrier(bar, epoch, nCta, hung);
     }
     BA_PROF(8)
@@ -1815,7 +1331,7 @@ __global__ void __launch_bounds__(64) k_pair_build(BaPtrs p, int fill) {
   __shared__ int wsum[2];
   __shared__ int running;
   const int w = blockIdx.y;
-  if (!p.usePairs[w]) return;
+  if (fill && p.st[w].pairsOverflow) return;
   const BaWin W = p.win[w];
   int i1, i2;
   decode_block(blockIdx.x, i1, i2);
@@ -1856,7 +1372,7 @@ __global__ void __launch_bounds__(64) k_pair_build(BaPtrs p, int fill) {
 
 __global__ void k_pair_scan(BaPtrs p, int batch) {
   const int w = blockIdx.x * blockDim.x + threadIdx.x;
-  if (w >= batch || !p.usePairs[w]) return;
+  if (w >= batch) return;
   const BaWin W = p.win[w];
   int* off = p.blkOff + (size_t)w * (p.capBlk + 1);
   const int nb = W.nFree * (W.nFree + 1) / 2;
@@ -1866,7 +1382,10 @@ __global__ void k_pair_scan(BaPtrs p, int batch) {
     run += off[t + 1];
     off[t + 1] = run;
   }
-  if (run > p.capPairs) p.usePairs[w] = 0;  // does not fit: fall back to probing every trial
+  if (run > p.capPairs) {  // cannot happen with capPairs >= the host's bound (ba_run); guards the fill pass
+    p.st[w].pairsOverflow = 1;
+    p.st[w].active = 0;
+  }
 }
 
 // lower blocks sorted by descending pair count (ties by block id): the Schur phase deals them to its warps in this order
@@ -1877,12 +1396,6 @@ __global__ void __launch_bounds__(256) k_block_order(BaPtrs p) {
   const int* off = p.blkOff + (size_t)w * (p.capBlk + 1);
   int* order = p.blkOrder + (size_t)w * p.capBlk;
   int* first = p.blkFirst + (size_t)w * p.capKf;
-  if (!p.usePairs[w]) {
-    for (int t = threadIdx.x; t < nb; t += blockDim.x) order[t] = t;
-    for (int i = threadIdx.x; i < W.nFree; i += blockDim.x) first[i] = 0;  // structure unknown: dense
-    if (threadIdx.x == 0) p.blkNZ[w] = nb;
-    return;
-  }
   for (int i1 = threadIdx.x; i1 < W.nFree; i1 += blockDim.x) {
     int f = i1;
     const int t0 = i1 * (i1 + 1) / 2;
@@ -2257,7 +1770,7 @@ using namespace b2s;
 struct BaHostStage {  // pinned mirror of the uploaded per-window arrays (same strides as the device arrays)
   double *pose = nullptr, *pts = nullptr;
   int *pidx = nullptr, *freeKf = nullptr, *eKf = nullptr, *eMp = nullptr, *mpStart = nullptr, *kfStart = nullptr,
-      *mpEdges = nullptr, *kfEdges = nullptr, *usePairs = nullptr;
+      *mpEdges = nullptr, *kfEdges = nullptr;
   float *eObs = nullptr, *eW = nullptr;
   uint8_t *eSt = nullptr, *eOutlier = nullptr;
   BaWin* win = nullptr;
@@ -2281,6 +1794,7 @@ struct b2s_ba_solver {
   long long lastTrials = 0;
   int *dCtaMap = nullptr, *dWinCtas = nullptr;  // balanced launch tables (see ba_run)
   int smBudget = 0;  // CTAs (= SMs) one LocalBA batch may occupy; 0 = all (b2s_ba_set_sm_budget)
+  DevBuf pairRec;    // d.pairRec: batch x d.capPairs records, grown by ba_run when a window needs more
 };
 
 static void quat_from_R_host(const double m[3][3], double* q) {
@@ -2359,30 +1873,18 @@ extern "C" int b2s_ba_create(int max_kf, int max_mp, int max_edges, int max_batc
   A(&d.eKf, B * max_edges * 4); A(&d.eMp, B * max_edges * 4);
   A(&d.eObs, B * max_edges * 12); A(&d.eW, B * max_edges * 4);
   A(&d.eStereo, B * max_edges); A(&d.eLevel, B * max_edges); A(&d.eOutlier, B * max_edges);
-  A(&d.err, B * max_edges * 24); A(&d.chi2, B * max_edges * 8); A(&d.W, B * max_edges * 18 * 8);
-  A(&d.eWq, B * max_edges * 8);
-  d.eWqB[0] = d.eWq;
-  A(&d.eWqB[1], B * max_edges * 8);
-  d.errB[0] = d.err;
-  A(&d.errB[1], B * max_edges * 24);
-  d.schurRecompute = 1;
-  if (const char* ev = getenv("B2S_BA_SCHUR_RC")) d.schurRecompute = atoi(ev) != 0;  // 0: gather the stored W blocks
-  // The DMMA form of the Schur products is off by default: measured on H100 (bench.py, 32 windows on 64 SMs) the LM kernel
-  // takes 19.9 ms with it against 15.0-15.2 ms with the per-lane FMA form.  A 6 x 3 . 3 x 6 product fills 42 % of an
-  // 8 x 8 x 4 tile and the 24 DMMAs of an iteration form one dependent chain, so the tensor pipe's higher FP64 rate does
-  // not pay.  Kept as a tested option (results identical within the LM tolerances, same traces).
-  d.schurDmma = 0;
-  if (const char* ev = getenv("B2S_BA_SCHUR_DMMA")) d.schurDmma = atoi(ev) != 0;     // 1: block products on DMMA.8x8x4
+  A(&d.chi2, B * max_edges * 8);
+  A(&d.errB[0], B * max_edges * 24); A(&d.errB[1], B * max_edges * 24);
+  A(&d.eWqB[0], B * max_edges * 8); A(&d.eWqB[1], B * max_edges * 8);
   A(&d.mpStart, B * (max_mp + 1) * 4); A(&d.mpEdges, B * max_edges * 4);
   A(&d.kfStart, B * (max_kf + 1) * 4); A(&d.kfEdges, B * max_edges * 4);
   A(&d.Hpp, B * max_kf * 36 * 8); A(&d.Hll, B * max_mp * 9 * 8);
   A(&d.b, B * ((size_t)max_kf * 6 + (size_t)max_mp * 3) * 8); A(&d.x, B * ((size_t)max_kf * 6 + (size_t)max_mp * 3) * 8);
   A(&d.Dinv, B * max_mp * 9 * 8); A(&d.S, B * (size_t)d.ldS * d.ldS * 8);
-  A(&d.db, B * max_mp * 3 * 8); A(&d.DinvP, B * max_mp * 10 * 8); A(&d.hl, B * (size_t)max_edges * 9 * 8);
+  A(&d.db, B * max_mp * 3 * 8); A(&d.DinvP, B * max_mp * 10 * 8);
   A(&d.lmEdge, B * (size_t)max_mp * max_kf * 4); A(&d.freeKf, B * max_kf * 4);
-  A(&d.blkOff, B * (size_t)(d.capBlk + 1) * 4); A(&d.pairRec, B * (size_t)d.capPairs * 16);
+  A(&d.blkOff, B * (size_t)(d.capBlk + 1) * 4);
   A(&d.lmRec, B * (size_t)max_edges * 8); A(&d.blkFirst, B * (size_t)max_kf * 4); A(&d.blkOrder, B * (size_t)d.capBlk * 4); A(&d.blkNZ, B * 4);
-  A(&d.usePairs, B * 4);
   A(&d.partChi, B * d.nPartE * 8); A(&d.partScale, B * d.nPartM * 8);
   A(&d.bar, B * 4);
   A(&d.prof, B * 16 * 8);
@@ -2395,13 +1897,13 @@ extern "C" int b2s_ba_create(int max_kf, int max_mp, int max_edges, int max_batc
   HA(&s.eKf, B * max_edges * 4); HA(&s.eMp, B * max_edges * 4);
   HA(&s.mpStart, B * (max_mp + 1) * 4); HA(&s.kfStart, B * (max_kf + 1) * 4);
   HA(&s.mpEdges, B * max_edges * 4); HA(&s.kfEdges, B * max_edges * 4);
-  HA(&s.usePairs, B * 4);
   HA(&s.eObs, B * max_edges * 12); HA(&s.eW, B * max_edges * 4);
   HA(&s.eSt, B * max_edges); HA(&s.eOutlier, B * max_edges);
   HA(&s.win, B * sizeof(BaWin)); HA(&s.st, B * sizeof(BaState));
+  if (e == cudaSuccess && grow(h->pairRec, B * (size_t)d.capPairs * 16) != B2S_OK) e = cudaErrorMemoryAllocation;
+  d.pairRec = (int4*)h->pairRec.p;
   h->smemBytes = (size_t)((CHOL_BS + 1) * CHOL_PP + (size_t)(d.ldS + 8) * CHOL_PP + 2 * d.ldS) * 8 + (size_t)(d.ldS + 8 + max_kf) * 4;
-  h->smemBytes = std::max(h->smemBytes, (size_t)(BA_T / 32) * 30 * 33 * 8);  // per-warp staging tiles of phase_build_edges
-  h->smemBytes = std::max(h->smemBytes, (size_t)(BA_T / 32) * 2 * GATHER_TILE16 * 16  // double-buffered gather tiles (Schur)
+  h->smemBytes = std::max(h->smemBytes, (size_t)(BA_T / 32) * RC_TOTAL * 16  // per-warp staging of the Schur loop
                                             + (size_t)max_kf * 12 * 8);                  // + R|t table (back-substitution)
   if (e == cudaSuccess && h->smemBytes > 48 * 1024)
     e = cudaFuncSetAttribute(k_local_ba, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smemBytes);
@@ -2419,6 +1921,7 @@ extern "C" void b2s_ba_destroy(b2s_ba_solver* h) {
   cudaSetDevice(h->device);
   pose_scratch_free(h->pose);
   for (void* p : h->allocs) cudaFree(p);
+  cudaFree(h->pairRec.p);
   for (void* p : h->hostAllocs) cudaFreeHost(p);
   for (auto& e : h->evLm)
     if (e) cudaEventDestroy(e);
@@ -2442,7 +1945,7 @@ static int ba_host_threads(int batch) {
   return std::max(1, std::min(batch, std::min(cap, (int)std::thread::hardware_concurrency())));
 }
 
-static int ba_prepare_window(b2s_ba_solver* h, int w, const b2s_ba_problem& P, int* nFreeOut) {
+static int ba_prepare_window(b2s_ba_solver* h, int w, const b2s_ba_problem& P, int* nFreeOut, long long* pairBoundOut) {
   const BaPtrs& d = h->d;
   BaHostStage& s = h->hs;
   double* pose = s.pose + (size_t)w * d.capKf * PSTRIDE;
@@ -2498,7 +2001,17 @@ static int ba_prepare_window(b2s_ba_solver* h, int w, const b2s_ba_problem& P, i
       kfEdges[ck[eKf[e]]++] = e;
     }
   }
+  // Upper bound on the window's covisibility pair records (k_pair_build): a landmark with f edges on free keyframes has
+  // at most f (f + 1) / 2, because once its free edges are sorted by pose, the k-th of them pairs with at most k distinct
+  // poses at or below its own (also when one keyframe observes the landmark twice).
+  long long pairs = 0;
+  for (int l = 0; l < P.n_mp; l++) {
+    long long f = 0;
+    for (int k = mpStart[l]; k < mpStart[l + 1]; k++) f += pidx[eKf[mpEdges[k]]] >= 0;
+    pairs += f * (f + 1) / 2;
+  }
   *nFreeOut = nFree;
+  *pairBoundOut = pairs;
   return 0;
 }
 
@@ -2529,16 +2042,18 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
   }
   // ---- host preparation of all windows in parallel (pinned staging), then one H2D per array
   std::vector<int> nFree(batch, 0), prc(batch, 0);
+  std::vector<long long> pairBound(batch, 0);
   {
     const int nth = ba_host_threads(batch);
     std::vector<std::thread> th;
     for (int t = 0; t < nth; t++)
       th.emplace_back([&, t]() {
-        for (int w = t; w < batch; w += nth) prc[w] = ba_prepare_window(h, w, probs[w], &nFree[w]);
+        for (int w = t; w < batch; w += nth) prc[w] = ba_prepare_window(h, w, probs[w], &nFree[w], &pairBound[w]);
       });
     for (auto& t : th) t.join();
   }
   int maxE = 0, maxMp = 0, maxFree = 0;
+  long long maxPairs = 8LL * h->maxE;  // the stride b2s_ba_create allocated for: windows bounded by it never grow the list
   for (int w = 0; w < batch; w++) {
     if (prc[w]) {
       set_error("b2s_local_ba: window %d: an edge references a vertex out of range", w);
@@ -2555,8 +2070,19 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
     S0.robust = 1;
     S0.its[0] = P.its1; S0.its[1] = P.its2;
     S0.ni = 2;
-    s.usePairs[w] = 1;
     maxE = std::max(maxE, P.n_edges); maxMp = std::max(maxMp, P.n_mp); maxFree = std::max(maxFree, nFree[w]);
+    maxPairs = std::max(maxPairs, pairBound[w]);
+  }
+  // the pair list of every window fits: grow it before anything is enqueued (cudaFree synchronises the device)
+  if (maxPairs > INT_MAX) {
+    set_error("b2s_local_ba: a window may have %lld covisibility pairs (at most %d)", maxPairs, INT_MAX);
+    return B2S_ERR_CAPACITY;
+  }
+  d.capPairs = (int)maxPairs;
+  {
+    const int rc = grow(h->pairRec, (size_t)batch * d.capPairs * 16);
+    if (rc != B2S_OK) return rc;
+    d.pairRec = (int4*)h->pairRec.p;
   }
   const size_t nb = (size_t)batch;
 #define UPALL(dst, src, stride, type) \
@@ -2574,7 +2100,6 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
   UPALL(d.mpEdges, s.mpEdges, d.capE, int);
   UPALL(d.kfStart, s.kfStart, d.capKf + 1, int);
   UPALL(d.kfEdges, s.kfEdges, d.capE, int);
-  UPALL(d.usePairs, s.usePairs, 1, int);
   UPALL(d.win, s.win, 1, BaWin);
   UPALL(d.st, s.st, 1, BaState);
 #undef UPALL
@@ -2707,6 +2232,11 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
     if (s.st[w].finishedRound0) {
       set_error("b2s_local_ba: window %d: LM kernel barrier timed out (CTAs not co-resident?)", w);
       return B2S_ERR_CUDA;
+    }
+  for (int w = 0; w < batch; w++)
+    if (s.st[w].pairsOverflow) {
+      set_error("b2s_local_ba: window %d: covisibility pair list exceeds its capacity of %d", w, d.capPairs);
+      return B2S_ERR_CAPACITY;
     }
   const auto tLoop = std::chrono::steady_clock::now();
   {

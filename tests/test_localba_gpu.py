@@ -125,11 +125,31 @@ def test_local_ba_shuffled_keyframes(pkg, oracle):
     _check(opt.LocalBundleAdjustment(d), oracle.local_ba(d), d)
 
 
-def test_local_ba_pair_list_overflow(pkg, oracle):
-    """High-degree landmarks with a tight edge capacity: the covisibility pair list does not fit (8 x max_edges) and the
-    Schur phase falls back to probing the landmark -> edge table."""
+def _high_degree_window():
+    """High-degree landmarks: the window's covisibility pair list is larger than the initial capacity (8 x max_edges) of
+    a handle sized to its edge count."""
     d = synth_local_ba(n_kf=24, n_fixed=2, n_mp=150, obs_per_mp=20, seed=31)
     deg = np.bincount(d["edges"]["mp"][d["fixed"][d["edges"]["kf"]] == 0])
     assert (deg * (deg + 1) // 2).sum() > 8 * len(d["edges"])
+    return d
+
+
+def test_local_ba_pair_list_grows(pkg, oracle):
+    """A pair list larger than the initial capacity: the handle grows it on demand."""
+    d = _high_degree_window()
     opt = pkg.Optimizer(max_kf=24, max_mp=150, max_edges=len(d["edges"]))
     _check(opt.LocalBundleAdjustment(d), oracle.local_ba(d), d)
+
+
+def test_local_ba_pair_list_grows_in_reused_handle(pkg, oracle):
+    """One handle: the high-degree window alone, then in a batch with two ordinary windows (the per-window stride of the
+    grown pair list applies to every window of the batch), then an ordinary window again."""
+    hd = _high_degree_window()
+    ds = [synth_local_ba(n_kf=10, n_fixed=2, n_mp=150, obs_per_mp=5, seed=11),
+          synth_local_ba(n_kf=14, n_fixed=4, n_mp=120, obs_per_mp=6, seed=12, mono_frac=0.2)]
+    opt = pkg.Optimizer(max_kf=24, max_mp=150, max_edges=len(hd["edges"]), max_batch=3)
+    _check(opt.LocalBundleAdjustment(hd), oracle.local_ba(hd), hd)
+    batch = [ds[0], hd, ds[1]]
+    for d, out in zip(batch, opt.LocalBundleAdjustmentBatch(batch)):
+        _check(out, oracle.local_ba(d), d)
+    _check(opt.LocalBundleAdjustment(ds[1]), oracle.local_ba(ds[1]), ds[1])
