@@ -65,6 +65,17 @@ class _BaResult(ctypes.Structure):
                 ("chi2_final", ctypes.c_double), ("n_trials", ctypes.c_int)]
 
 
+class _PoseProblem(ctypes.Structure):
+    _fields_ = [("Tcw", _vp), ("n", ctypes.c_int32), ("has_mp", _vp), ("Xw", _vp), ("kpx", _vp), ("kpy", _vp),
+                ("uright", _vp), ("inv_sigma2", _vp), ("fx", ctypes.c_float), ("fy", ctypes.c_float),
+                ("cx", ctypes.c_float), ("cy", ctypes.c_float), ("bf", ctypes.c_float)]
+
+
+class _PoseResult(ctypes.Structure):
+    _fields_ = [("Tcw_out", _vp), ("outlier", _vp), ("trace", _vp), ("n_inliers", ctypes.c_int32),
+                ("n_trials", ctypes.c_int32)]
+
+
 class _GbaProblem(ctypes.Structure):
     _fields_ = [("n_kf", ctypes.c_int), ("Tcw", _vp), ("fixed", _vp), ("n_mp", ctypes.c_int), ("points", _vp),
                 ("n_edges", ctypes.c_int), ("edges", _vp), ("fx", ctypes.c_float), ("fy", ctypes.c_float),
@@ -162,6 +173,7 @@ def lib():
             L.b2s_local_ba.argtypes = [_vp, _vp, _vp, _vp]
             L.b2s_ba_set_sm_budget.argtypes = [_vp, ctypes.c_int]
             L.b2s_local_ba_batch.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+            L.b2s_pose_optimization_batch.argtypes = [_vp, ctypes.c_int, _vp, _vp]
         if hasattr(L, "b2s_gba_create"):
             L.b2s_gba_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
             L.b2s_gba_destroy.argtypes = [_vp]
@@ -847,16 +859,8 @@ class Optimizer:
     def PoseOptimizationBatch(self, ds):
         """Optimizer::PoseOptimization (src/Optimizer.cc:363-605) for a batch of independent frames; ds: dicts with Tcw,
         has_mp, Xw, kpx, kpy, uright, inv_sigma2, fx, fy, cx, cy, bf.  Returns a list of result dicts."""
-        class PP(ctypes.Structure):
-            _fields_ = [("Tcw", _vp), ("n", ctypes.c_int32), ("has_mp", _vp), ("Xw", _vp), ("kpx", _vp), ("kpy", _vp),
-                        ("uright", _vp), ("inv_sigma2", _vp), ("fx", ctypes.c_float), ("fy", ctypes.c_float),
-                        ("cx", ctypes.c_float), ("cy", ctypes.c_float), ("bf", ctypes.c_float)]
-
-        class PR(ctypes.Structure):
-            _fields_ = [("Tcw_out", _vp), ("outlier", _vp), ("trace", _vp), ("n_inliers", ctypes.c_int32),
-                        ("n_trials", ctypes.c_int32)]
         B = len(ds)
-        probs, ress, keep, outs = (PP * B)(), (PR * B)(), [], []
+        probs, ress, keep, outs = (_PoseProblem * B)(), (_PoseResult * B)(), [], []
         for i, d in enumerate(ds):
             a = dict(Tcw=np.ascontiguousarray(d["Tcw"], np.float32).reshape(16),
                      has_mp=np.ascontiguousarray(d["has_mp"], np.uint8), Xw=np.ascontiguousarray(d["Xw"], np.float32),
@@ -866,14 +870,13 @@ class Optimizer:
             n = len(a["has_mp"])
             o = dict(Tcw=np.zeros(16, np.float32), outlier=np.zeros(max(n, 1), np.uint8), trace=np.full(256, -1, np.int32))
             keep.append((a, o))
-            probs[i] = PP(a["Tcw"].ctypes.data, n, a["has_mp"].ctypes.data, a["Xw"].ctypes.data, a["kpx"].ctypes.data,
-                          a["kpy"].ctypes.data, a["uright"].ctypes.data, a["inv_sigma2"].ctypes.data, float(d["fx"]),
-                          float(d["fy"]), float(d["cx"]), float(d["cy"]), float(d["bf"]))
-            ress[i] = PR(o["Tcw"].ctypes.data, o["outlier"].ctypes.data, o["trace"].ctypes.data, 0, 0)
+            probs[i] = _PoseProblem(a["Tcw"].ctypes.data, n, a["has_mp"].ctypes.data, a["Xw"].ctypes.data,
+                                    a["kpx"].ctypes.data, a["kpy"].ctypes.data, a["uright"].ctypes.data,
+                                    a["inv_sigma2"].ctypes.data, float(d["fx"]), float(d["fy"]), float(d["cx"]),
+                                    float(d["cy"]), float(d["bf"]))
+            ress[i] = _PoseResult(o["Tcw"].ctypes.data, o["outlier"].ctypes.data, o["trace"].ctypes.data, 0, 0)
             outs.append((o, n))
-        L = lib()
-        L.b2s_pose_optimization_batch.argtypes = [_vp, ctypes.c_int, _vp, _vp]
-        _check(L.b2s_pose_optimization_batch(self._h, B, ctypes.cast(probs, _vp), ctypes.cast(ress, _vp)))
+        _check(lib().b2s_pose_optimization_batch(self._h, B, ctypes.cast(probs, _vp), ctypes.cast(ress, _vp)))
         return [dict(n_inliers=ress[i].n_inliers, n_trials=ress[i].n_trials, Tcw=o["Tcw"], outlier=o["outlier"][:n],
                      trace=o["trace"]) for i, (o, n) in enumerate(outs)]
 
@@ -882,16 +885,8 @@ class Optimizer:
 
     # ---- prepared batches: the ctypes problem / result arrays are built once, a step is then one C call (stream.py)
     def prepare_pose_batch(self, ds):
-        class PP(ctypes.Structure):
-            _fields_ = [("Tcw", _vp), ("n", ctypes.c_int32), ("has_mp", _vp), ("Xw", _vp), ("kpx", _vp), ("kpy", _vp),
-                        ("uright", _vp), ("inv_sigma2", _vp), ("fx", ctypes.c_float), ("fy", ctypes.c_float),
-                        ("cx", ctypes.c_float), ("cy", ctypes.c_float), ("bf", ctypes.c_float)]
-
-        class PR(ctypes.Structure):
-            _fields_ = [("Tcw_out", _vp), ("outlier", _vp), ("trace", _vp), ("n_inliers", ctypes.c_int32),
-                        ("n_trials", ctypes.c_int32)]
         B = len(ds)
-        probs, ress, keep = (PP * B)(), (PR * B)(), []
+        probs, ress, keep = (_PoseProblem * B)(), (_PoseResult * B)(), []
         for i, d in enumerate(ds):
             a = [np.ascontiguousarray(d["Tcw"], np.float32).reshape(16), np.ascontiguousarray(d["has_mp"], np.uint8),
                  np.ascontiguousarray(d["Xw"], np.float32), np.ascontiguousarray(d["kpx"], np.float32),
@@ -900,12 +895,10 @@ class Optimizer:
             n = len(a[1])
             o = [np.zeros(16, np.float32), np.zeros(max(n, 1), np.uint8)]
             keep.append((a, o))
-            probs[i] = PP(a[0].ctypes.data, n, a[1].ctypes.data, a[2].ctypes.data, a[3].ctypes.data, a[4].ctypes.data,
-                          a[5].ctypes.data, a[6].ctypes.data, float(d["fx"]), float(d["fy"]), float(d["cx"]), float(d["cy"]),
-                          float(d["bf"]))
-            ress[i] = PR(o[0].ctypes.data, o[1].ctypes.data, None, 0, 0)
-        L = lib()
-        L.b2s_pose_optimization_batch.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+            probs[i] = _PoseProblem(a[0].ctypes.data, n, a[1].ctypes.data, a[2].ctypes.data, a[3].ctypes.data,
+                                    a[4].ctypes.data, a[5].ctypes.data, a[6].ctypes.data, float(d["fx"]), float(d["fy"]),
+                                    float(d["cx"]), float(d["cy"]), float(d["bf"]))
+            ress[i] = _PoseResult(o[0].ctypes.data, o[1].ctypes.data, None, 0, 0)
         return dict(B=B, probs=probs, ress=ress, keep=keep)
 
     def run_prepared_pose(self, prep):
@@ -932,21 +925,7 @@ class Optimizer:
         return prep["outs"]
 
     def LocalBundleAdjustmentBatch(self, ds, its1=5, its2=10):
-        B = len(ds)
-        probs = (_BaProblem * B)()
-        ress = (_BaResult * B)()
-        keeps, outs = [], []
-        for i, d in enumerate(ds):
-            p, keep = self._problem(d, its1, its2)
-            r, out = self._result(d)
-            probs[i], ress[i] = p, r
-            keeps.append(keep)
-            outs.append(out)
-        _check(lib().b2s_local_ba_batch(self._h, B, ctypes.cast(probs, _vp), ctypes.cast(ress, _vp)))
-        for i in range(B):
-            outs[i]["chi2"] = ress[i].chi2_final
-            outs[i]["n_trials"] = ress[i].n_trials
-        return outs
+        return self.run_prepared_ba(self.prepare_ba_batch(ds, its1, its2))
 
 
 class GlobalOptimizer:

@@ -40,6 +40,7 @@ def _deps_of(src):
         deps.append(os.path.join(CSRC, "extractor.cuh"))
     if base in ("localba.cu", "gba.cu", "essential.cu"):
         deps.append(os.path.join(CSRC, "ba_math.cuh"))
+        deps.append(os.path.join(CSRC, "levenberg.cuh"))
     if base in ("gba.cu", "essential.cu"):
         deps.append(os.path.join(CSRC, "chol.cuh"))
     if base == "extractor.cu":

@@ -2,8 +2,11 @@
 // PoseOptimization; gba.cu: global bundle adjustment).
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
 
 namespace b2s {
+
+constexpr int POSE_STRIDE = 8;  // doubles per SE3Quat pose: q(x,y,z,w), t(x,y,z), pad
 
 // ---------------------------------------------------------------- small FP64 helpers
 __device__ __forceinline__ void quat_rotate(const double* q, const double* v, double* o) {
@@ -17,7 +20,7 @@ __device__ __forceinline__ void pose_map(const double* P, const double* X, doubl
   quat_rotate(P, X, o);
   o[0] += P[4]; o[1] += P[5]; o[2] += P[6];
 }
-__device__ __forceinline__ void quat_to_R(const double* q, double R[3][3]) {
+__host__ __device__ __forceinline__ void quat_to_R(const double* q, double R[3][3]) {
   const double tx = 2 * q[0], ty = 2 * q[1], tz = 2 * q[2];
   const double twx = tx * q[3], twy = ty * q[3], twz = tz * q[3];
   const double txx = tx * q[0], txy = ty * q[0], txz = tz * q[0];
@@ -26,7 +29,7 @@ __device__ __forceinline__ void quat_to_R(const double* q, double R[3][3]) {
   R[1][0] = txy + twz; R[1][1] = 1 - (txx + tzz); R[1][2] = tyz - twx;
   R[2][0] = txz - twy; R[2][1] = tyz + twx; R[2][2] = 1 - (txx + tyy);
 }
-__device__ __forceinline__ void quat_from_R(const double m[3][3], double* q) {  // Eigen::Quaterniond(Matrix3d)
+__host__ __device__ __forceinline__ void quat_from_R(const double m[3][3], double* q) {  // Eigen::Quaterniond(Matrix3d)
   double t = m[0][0] + m[1][1] + m[2][2];
   if (t > 0.0) {
     t = sqrt(t + 1.0);
@@ -50,12 +53,32 @@ __device__ __forceinline__ void quat_from_R(const double m[3][3], double* q) {  
     q[0] = v[0]; q[1] = v[1]; q[2] = v[2];
   }
 }
-__device__ __forceinline__ void normalize_rot(double* q) {  // SE3Quat::normalizeRotation
+__host__ __device__ __forceinline__ void normalize_rot(double* q) {  // SE3Quat::normalizeRotation
   if (q[3] < 0) {
     q[0] = -q[0]; q[1] = -q[1]; q[2] = -q[2]; q[3] = -q[3];
   }
   const double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
   q[0] /= n; q[1] /= n; q[2] /= n; q[3] /= n;
+}
+
+// Converter::toSE3Quat (src/Converter.cc:57-66): row-major float 4x4 Tcw -> pose P (POSE_STRIDE doubles)
+__host__ __device__ __forceinline__ void se3quat_from_Tcw(const float* T, double* P) {
+  double R[3][3];
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++) R[i][j] = T[i * 4 + j];
+  quat_from_R(R, P);
+  normalize_rot(P);
+  P[4] = T[3]; P[5] = T[7]; P[6] = T[11]; P[7] = 0;
+}
+// Converter::toCvMat(SE3Quat) (src/Converter.cc:96-107): pose P -> row-major float 4x4 Tcw
+__host__ __device__ __forceinline__ void se3quat_to_Tcw(const double* P, float* T) {
+  double R[3][3];
+  quat_to_R(P, R);
+  for (int r = 0; r < 3; r++) {
+    for (int c = 0; c < 3; c++) T[r * 4 + c] = (float)R[r][c];
+    T[r * 4 + 3] = (float)P[4 + r];
+  }
+  T[12] = 0.f; T[13] = 0.f; T[14] = 0.f; T[15] = 1.f;
 }
 
 // SE3Quat::exp(update) * estimate  (se3quat.h:223-257, :103-109)

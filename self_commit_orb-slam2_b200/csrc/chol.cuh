@@ -259,6 +259,39 @@ static __global__ void __launch_bounds__(TS) k_bwd(TileSys a, int I) {
 }
 
 // ================================================================================================ host side
+// The host-driven LM loop's synchronisations.  busyMs adds up the stream segments between them (CUDA events): the device
+// time of a solve, without the host's decisions in between.  start() opens the first segment.
+struct HostSync {
+  cudaStream_t s;
+  cudaEvent_t* ev;        // ev[0]: start of the open segment, ev[1]: its end
+  double* hScal;          // pinned host copy of the solver's scalars
+  const double* scal;     // device scalars (chi2, scale / max |diag|)
+  int* hFail;             // pinned host copy of the factorisation's fail flag
+  const int* fail;
+  float busyMs;
+
+  int start() {
+    B2S_CUDA(cudaEventRecord(ev[0], s));
+    return B2S_OK;
+  }
+  // wait for the stream and close the segment
+  int stream() {
+    B2S_CUDA(cudaEventRecord(ev[1], s));
+    B2S_CUDA(cudaStreamSynchronize(s));
+    float ms = 0.f;
+    B2S_CUDA(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+    busyMs += ms;
+    B2S_CUDA(cudaEventRecord(ev[0], s));
+    return B2S_OK;
+  }
+  // the first n scalars and the fail flag to the host, then stream()
+  int scalars(int n) {
+    B2S_CUDA(cudaMemcpyAsync(hScal, scal, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
+    B2S_CUDA(cudaMemcpyAsync(hFail, fail, 4, cudaMemcpyDeviceToHost, s));
+    return stream();
+  }
+};
+
 // the kernels above need 2 tiles of dynamic shared memory
 static cudaError_t set_smem_limits() {
   cudaError_t e = cudaFuncSetAttribute(k_potrf, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * TILE_SMEM);

@@ -31,6 +31,7 @@
 #include "ba_math.cuh"
 #include "chol.cuh"
 #include "common.cuh"
+#include "levenberg.cuh"
 
 namespace b2s {
 namespace eg {
@@ -591,18 +592,9 @@ extern "C" int b2s_optimize_essential_graph(b2s_eg_solver* h, const b2s_eg_probl
   if (rc == B2S_OK) rc = grow(h->rows, rows.size() * 4);
   if (rc != B2S_OK) return rc;
 
-  // device time: the stream segments between the host's synchronisations (the host's LM decisions excluded)
-  float busyMs = 0.f;
-  B2S_CUDA(cudaEventRecord(h->ev[0], s));
-  auto sync_stream = [&]() -> int {
-    B2S_CUDA(cudaEventRecord(h->ev[1], s));
-    B2S_CUDA(cudaStreamSynchronize(s));
-    float ms = 0.f;
-    B2S_CUDA(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
-    busyMs += ms;
-    B2S_CUDA(cudaEventRecord(h->ev[0], s));
-    return B2S_OK;
-  };
+  HostSync sync = {s, h->ev, h->hScal, h->scal, h->hFail, h->fail, 0.f};
+  rc = sync.start();
+  if (rc != B2S_OK) return rc;
   // ---- upload
   B2S_CUDA(cudaMemcpyAsync(h->est0, p->Siw, (size_t)nKf * SD * 8, cudaMemcpyHostToDevice, s));
   B2S_CUDA(cudaMemcpyAsync(h->est, p->Siw, (size_t)nKf * SD * 8, cudaMemcpyHostToDevice, s));
@@ -646,69 +638,36 @@ extern "C" int b2s_optimize_essential_graph(b2s_eg_solver* h, const b2s_eg_probl
     k_errors<<<blocks(nE, 128), 128, 0, s>>>(a, S);
     chol::reduce<0>(h->chi2, nE, h->part, out, s);
   };
-  auto sync_scalars = [&](int nScal) -> int {
-    B2S_CUDA(cudaMemcpyAsync(h->hScal, h->scal, (size_t)nScal * 8, cudaMemcpyDeviceToHost, s));
-    B2S_CUDA(cudaMemcpyAsync(h->hFail, h->fail, 4, cudaMemcpyDeviceToHost, s));
-    return sync_stream();
-  };
 
   // ---- SparseOptimizer::optimize(20) + OptimizationAlgorithmLevenberg::solve (an empty graph optimises nothing)
-  std::vector<int32_t> trace;
-  int nTrials = 0;
+  Levenberg lm = {};
+  int32_t trace[256];
   double chi2Initial = 0;
-  double lambda = 1e-16, ni = 2;  // computeLambdaInit returns the user lambda (setUserLambdaInit(1e-16), :1035)
-  int nBad = 0;
+  lm.init_lambda(1e-16);  // computeLambdaInit returns the user lambda (setUserLambdaInit(1e-16), :1035)
   bool ok = nE > 0;
   for (int it = 0; it < 20 && ok; it++) {
     chi2_of(est, h->scal);
     k_linearize<<<blocks((long long)nE * 14, 128), 128, 0, s>>>(a, est);
     k_assemble_diag<true><<<blocks((long long)nFree * 32, 256), 256, 0, s>>>(a, 0.0);
-    rc = sync_scalars(1);
+    rc = sync.scalars(1);
     if (rc != B2S_OK) return rc;
-    double currentChi = h->hScal[0];
-    const double iniChi = currentChi;
-    if (it == 0) chi2Initial = currentChi;
-    double rho = 0;
-    int qmax = 0;
+    lm.begin(h->hScal[0]);
+    if (it == 0) chi2Initial = lm.currentChi;
     do {
       B2S_CUDA(cudaMemsetAsync(h->fail, 0, 4, s));
       B2S_CUDA(cudaMemsetAsync(h->tiles.p, 0, tileBytes, s));
       B2S_CUDA(cudaMemcpyAsync(h->rhs, h->b, (size_t)npPad * 8, cudaMemcpyDeviceToDevice, s));
-      k_assemble_diag<false><<<blocks((long long)nFree * 32, 256), 256, 0, s>>>(a, lambda);
+      k_assemble_diag<false><<<blocks((long long)nFree * 32, 256), 256, 0, s>>>(a, lm.lambda);
       if (nBlk) k_assemble_off<<<blocks((long long)nBlk * 32, 256), 256, 0, s>>>(a, nBlk);
       factor_solve(ts, nT, envT, rowOff, (const int*)h->rows.p, s);
-      k_update<<<blocks(nKf, 128), 128, 0, s>>>(a, est, estT, lambda);
+      k_update<<<blocks(nKf, 128), 128, 0, s>>>(a, est, estT, lm.lambda);
       chi2_of(estT, h->scal);
       chol::reduce<0>(h->tmp, np, h->part, h->scal + 1, s);
-      rc = sync_scalars(2);
+      rc = sync.scalars(2);
       if (rc != B2S_OK) return rc;
-      const bool solved = *h->hFail == 0;
-      const double tempChi = solved ? h->hScal[0] : DBL_MAX;
-      rho = currentChi - tempChi;
-      double scale = solved ? h->hScal[1] : 0.0;
-      scale += 1e-3;
-      rho /= scale;
-      if (!solved) rho = -1;
-      const bool good = rho > 0 && std::isfinite(tempChi);
-      if (trace.size() < 255) trace.push_back(good ? 1 : 0);
-      nTrials++;
-      if (good) {
-        double alpha = 1. - pow((2 * rho - 1), 3);
-        alpha = std::min(alpha, 2. / 3.);
-        lambda *= std::max(1. / 3., alpha);
-        ni = 2;
-        currentChi = tempChi;
-        std::swap(est, estT);
-      } else {
-        lambda *= ni;
-        ni *= 2;
-      }
-      qmax++;
-    } while (rho < 0 && qmax < 10);
-    if (qmax == 10 || rho == 0) break;
-    if ((iniChi - currentChi) * 1e3 < iniChi) nBad++;
-    else nBad = 0;
-    if (nBad >= 3) break;
+      if (lm.trial(*h->hFail == 0, h->hScal[0], h->hScal[1], trace)) std::swap(est, estT);
+    } while (lm.retry(false));
+    if (lm.end_iteration()) break;
   }
 
   // ---- write-back and the chi2 of the returned estimate
@@ -718,17 +677,18 @@ extern "C" int b2s_optimize_essential_graph(b2s_eg_solver* h, const b2s_eg_probl
   B2S_CUDA(cudaMemcpyAsync(r->Tcw_out, h->Tcw, (size_t)nKf * 64, cudaMemcpyDeviceToHost, s));
   if (nMp) B2S_CUDA(cudaMemcpyAsync(r->points_out, h->Pout, (size_t)nMp * 12, cudaMemcpyDeviceToHost, s));
   B2S_CUDA(cudaMemcpyAsync(h->hScal, h->scal, 8, cudaMemcpyDeviceToHost, s));
-  rc = sync_stream();
+  rc = sync.stream();
   if (rc != B2S_OK) return rc;
   B2S_CUDA(cudaGetLastError());
   r->chi2_initial = nE ? chi2Initial : 0.0;
   r->chi2_final = h->hScal[0];
-  r->n_trials = nTrials;
+  r->n_trials = lm.nTrials;
   if (r->trace) {
-    for (size_t i = 0; i < trace.size(); i++) r->trace[i] = trace[i];
-    r->trace[trace.size()] = -1;
+    const int n = std::min(lm.nTrials, 255);
+    for (int i = 0; i < n; i++) r->trace[i] = trace[i];
+    r->trace[n] = -1;
   }
-  h->lastMs = busyMs;
-  h->lastTrials = nTrials;
+  h->lastMs = sync.busyMs;
+  h->lastTrials = lm.nTrials;
   return B2S_OK;
 }

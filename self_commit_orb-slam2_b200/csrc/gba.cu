@@ -37,12 +37,12 @@
 #include "ba_math.cuh"
 #include "chol.cuh"
 #include "common.cuh"
+#include "levenberg.cuh"
 
 namespace b2s {
 namespace gba {
 
 using namespace chol;  // tiles, deterministic sums, the tiled Cholesky (chol.cuh)
-constexpr int PSD = 8;           // doubles per pose: q(x,y,z,w), t(x,y,z), pad
 
 struct Cam {
   float fx, fy, cx, cy, bf;
@@ -69,7 +69,8 @@ __device__ __forceinline__ double edge_error(const double* Xc, bool stereo, cons
   return e[0] * (wgt * e[0]) + e[1] * (wgt * e[1]);
 }
 
-// const float thHuber2D = sqrt(5.99), thHuber3D = sqrt(7.815)  (src/Optimizer.cc:141-142)
+// const float thHuber2D = sqrt(5.99), thHuber3D = sqrt(7.815)  (src/Optimizer.cc:141-142).  BundleAdjustment's own
+// constants: its monocular threshold is sqrt(5.99), not LocalBA / PoseOptimization's sqrt(5.991) (delta_of, localba.cu).
 __device__ __forceinline__ double gba_delta(bool stereo) {
   return stereo ? (double)(float)2.795532150593156 : (double)(float)2.4474476501040834;
 }
@@ -86,14 +87,7 @@ struct Edges {
 __global__ void k_pose_init(const float* __restrict__ Tcw, int nKf, double* pose) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= nKf) return;
-  const float* T = Tcw + (size_t)k * 16;
-  double R[3][3];
-  for (int i = 0; i < 3; i++)
-    for (int j = 0; j < 3; j++) R[i][j] = T[i * 4 + j];
-  double* P = pose + (size_t)k * PSD;
-  quat_from_R(R, P);
-  normalize_rot(P);
-  P[4] = T[3]; P[5] = T[7]; P[6] = T[11]; P[7] = 0;
+  se3quat_from_Tcw(Tcw + (size_t)k * 16, pose + (size_t)k * POSE_STRIDE);
 }
 __global__ void k_point_init(const float* __restrict__ X, int n, double* pts) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -203,7 +197,7 @@ __global__ void k_errors(LmArgs a, const double* __restrict__ pose, const double
   if (e >= a.nE) return;
   const double* X = pts + (size_t)a.E.mp[e] * 3;
   double Xc[3];
-  pose_map(pose + (size_t)a.E.kf[e] * PSD, X, Xc);
+  pose_map(pose + (size_t)a.E.kf[e] * POSE_STRIDE, X, Xc);
   const float* ob = a.E.obs + (size_t)e * 3;
   const bool st = !(ob[2] < 0);
   double er[3];
@@ -226,7 +220,7 @@ struct EdgeLin {
 __device__ __forceinline__ void edge_lin(const LmArgs& a, const double* pose, const double* pts, int e, EdgeLin& L) {
   const float* ob = a.E.obs + (size_t)e * 3;
   const bool st = !(ob[2] < 0);
-  edge_jacobians(pose + (size_t)a.E.kf[e] * PSD, pts + (size_t)a.E.mp[e] * 3, st, (double)a.C.fx, (double)a.C.fy,
+  edge_jacobians(pose + (size_t)a.E.kf[e] * POSE_STRIDE, pts + (size_t)a.E.mp[e] * 3, st, (double)a.C.fx, (double)a.C.fy,
                  (double)a.C.bf, L.J);
   const double w0 = (double)a.E.w[e];
   double rho1 = 1.0;
@@ -422,11 +416,11 @@ __global__ void k_update(LmArgs a, const double* __restrict__ pose, const double
                          double* ptsT, double lambda) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < a.nKf) {
-    double P[PSD];
-    for (int k = 0; k < PSD; k++) P[k] = pose[(size_t)i * PSD + k];
+    double P[POSE_STRIDE];
+    for (int k = 0; k < POSE_STRIDE; k++) P[k] = pose[(size_t)i * POSE_STRIDE + k];
     const int p = a.pidx[i];
     if (p >= 0) pose_oplus(P, a.x + (size_t)p * 6);
-    for (int k = 0; k < PSD; k++) poseT[(size_t)i * PSD + k] = P[k];
+    for (int k = 0; k < POSE_STRIDE; k++) poseT[(size_t)i * POSE_STRIDE + k] = P[k];
   }
   if (i < a.nMp * 3) ptsT[i] = pts[i] + a.x[(size_t)a.npPad + i];
   if (i < a.npPad + a.nMp * 3) a.tmp[i] = a.x[i] * (lambda * a.x[i] + a.b[i]);
@@ -436,17 +430,7 @@ __global__ void k_update(LmArgs a, const double* __restrict__ pose, const double
 __global__ void k_writeback(LmArgs a, const double* __restrict__ pose, const double* __restrict__ pts, float* Tcw,
                             float* X) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < a.nKf) {
-    const double* P = pose + (size_t)i * PSD;
-    double R[3][3];
-    quat_to_R(P, R);
-    float* T = Tcw + (size_t)i * 16;
-    for (int r = 0; r < 3; r++) {
-      for (int c = 0; c < 3; c++) T[r * 4 + c] = (float)R[r][c];
-      T[r * 4 + 3] = (float)P[4 + r];
-    }
-    T[12] = 0.f; T[13] = 0.f; T[14] = 0.f; T[15] = 1.f;
-  }
+  if (i < a.nKf) se3quat_to_Tcw(pose + (size_t)i * POSE_STRIDE, Tcw + (size_t)i * 16);
   if (i < a.nMp * 3) X[i] = (float)pts[i];
 }
 
@@ -551,7 +535,7 @@ extern "C" int b2s_gba_create(int max_kf, int max_mp, int max_edges, int device,
   A(&h->err, E * 24); A(&h->chi2, E * 8); A(&h->rho, E * 8); A(&h->W, E * 18 * 8);
   A(&h->pidx, K * 4); A(&h->fixedD, K); A(&h->Tcw, K * 64); A(&h->kfBeg, K * 4); A(&h->kfEnd, K * 4);
   A(&h->envBlk, K * 4); A(&h->envT, K * 4 + 4); A(&h->tileOff, (K + 1) * 8);
-  A(&h->pose, K * PSD * 8); A(&h->poseT, K * PSD * 8); A(&h->Hpp, K * 36 * 8);
+  A(&h->pose, K * POSE_STRIDE * 8); A(&h->poseT, K * POSE_STRIDE * 8); A(&h->Hpp, K * 36 * 8);
   A(&h->X, M * 12); A(&h->pts, M * 24); A(&h->ptsT, M * 24); A(&h->ptBeg, M * 4); A(&h->ptEnd, M * 4);
   A(&h->Hll, M * 72); A(&h->Dinv, M * 72); A(&h->db, M * 24); A(&h->pairCnt, (M + 1) * 8); A(&h->pairOff, (M + 1) * 8);
   A(&h->part, RED_BLOCKS * 8); A(&h->scal, 4 * 8); A(&h->fail, 4);
@@ -615,18 +599,9 @@ extern "C" int b2s_global_ba(b2s_gba_solver* h, const b2s_gba_problem* p, const 
     if (active[(size_t)k] && !p->fixed[k]) pidx[(size_t)k] = nFree++;
   const int np = nFree * 6, nT = (np + TS - 1) / TS, npPad = nT * TS;
 
-  // device time: the stream segments between the host's synchronisations (the host's LM decisions excluded)
-  float busyMs = 0.f;
-  B2S_CUDA(cudaEventRecord(h->ev[0], s));
-  auto sync_stream = [&]() -> int {
-    B2S_CUDA(cudaEventRecord(h->ev[1], s));
-    B2S_CUDA(cudaStreamSynchronize(s));
-    float ms = 0.f;
-    B2S_CUDA(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
-    busyMs += ms;
-    B2S_CUDA(cudaEventRecord(h->ev[0], s));
-    return B2S_OK;
-  };
+  HostSync sync = {s, h->ev, h->hScal, h->scal, h->hFail, h->fail, 0.f};
+  rc = sync.start();
+  if (rc != B2S_OK) return rc;
   // ---- upload
   std::vector<int> ek((size_t)nE), em((size_t)nE);
   std::vector<float> eo((size_t)nE * 3), ew((size_t)nE);
@@ -651,8 +626,6 @@ extern "C" int b2s_global_ba(b2s_gba_solver* h, const b2s_gba_problem* p, const 
     B2S_CUDA(cudaMemcpyAsync(h->X, p->points, (size_t)nMp * 12, cudaMemcpyHostToDevice, s));
     k_point_init<<<blocks((long long)nMp * 3, 256), 256, 0, s>>>(h->X, nMp * 3, h->pts);
   }
-  std::vector<int32_t> trace;
-  int nTrials = 0;
   LmArgs a;
   memset(&a, 0, sizeof(a));
   a.E.kf = h->eKf; a.E.mp = h->eMp; a.E.obs = h->eObs; a.E.w = h->eW;
@@ -701,7 +674,7 @@ extern "C" int b2s_global_ba(b2s_gba_solver* h, const b2s_gba_problem* p, const 
     if (rc != B2S_OK) return rc;
     B2S_CUDA(cub::DeviceScan::ExclusiveSum(h->cubTmp.p, tb, h->pairCnt, h->pairOff, nMp + 1, s));
     B2S_CUDA(cudaMemcpyAsync(h->hScal, h->pairOff + nMp, 8, cudaMemcpyDeviceToHost, s));
-    rc = sync_stream();
+    rc = sync.stream();
     if (rc != B2S_OK) return rc;
     memcpy(&nPairs, h->hScal, 8);
     if (nPairs > 0x7fffffffLL) {
@@ -737,7 +710,7 @@ extern "C" int b2s_global_ba(b2s_gba_solver* h, const b2s_gba_problem* p, const 
       k_pair_gather<<<blocks(nPairs, 256), 256, 0, s>>>(pvS, (const int4*)h->pairRec.p, nPairs, (int4*)h->pairRecS.p);
       B2S_CUDA(cub::DeviceRunLengthEncode::Encode(h->cubTmp.p, t2, pkS, uk, rl, nr, nP, s));
       B2S_CUDA(cudaMemcpyAsync(h->hFail, nr, 4, cudaMemcpyDeviceToHost, s));
-      rc = sync_stream();
+      rc = sync.stream();
       if (rc != B2S_OK) return rc;
       nBlk = *h->hFail;
       B2S_CUDA(cudaMemsetAsync(rl + nBlk, 0, 4, s));
@@ -748,7 +721,7 @@ extern "C" int b2s_global_ba(b2s_gba_solver* h, const b2s_gba_problem* p, const 
       // tile envelope: first tile column any scalar row of the tile row reaches; tile storage sized from it
       std::vector<int> envBlk((size_t)nFree);
       B2S_CUDA(cudaMemcpyAsync(envBlk.data(), h->envBlk, (size_t)nFree * 4, cudaMemcpyDeviceToHost, s));
-      rc = sync_stream();
+      rc = sync.stream();
       if (rc != B2S_OK) return rc;
       std::vector<long long> off;
       std::vector<int> rows;
@@ -777,15 +750,10 @@ extern "C" int b2s_global_ba(b2s_gba_solver* h, const b2s_gba_problem* p, const 
     k_errors<<<blocks(nE, 256), 256, 0, s>>>(a, P, X);
     reduce<0>(h, h->rho, nE, out);
   };
-  auto sync_scalars = [&](int nScal) -> int {
-    B2S_CUDA(cudaMemcpyAsync(h->hScal, h->scal, (size_t)nScal * 8, cudaMemcpyDeviceToHost, s));
-    B2S_CUDA(cudaMemcpyAsync(h->hFail, h->fail, 4, cudaMemcpyDeviceToHost, s));
-    return sync_stream();
-  };
 
   // ---- SparseOptimizer::optimize + OptimizationAlgorithmLevenberg::solve ("empty graph": nothing to optimise)
-  double lambda = -1, ni = 2;
-  int nBad = 0;
+  Levenberg lm = {};
+  int32_t trace[256];
   bool ok = nE > 0;
   for (int it = 0; it < p->iterations && !terminate() && ok; it++) {
     chi2_of(pose, pts, h->scal);
@@ -796,67 +764,35 @@ extern "C" int b2s_global_ba(b2s_gba_solver* h, const b2s_gba_problem* p, const 
       k_diag<<<blocks(nd, 256), 256, 0, s>>>(a);
       reduce<1>(h, a.tmp, nd, h->scal + 1);
     }
-    rc = sync_scalars(2);
+    rc = sync.scalars(2);
     if (rc != B2S_OK) return rc;
-    double currentChi = h->hScal[0];
-    const double iniChi = currentChi;
-    if (it == 0) {
-      lambda = 1e-5 * h->hScal[1];
-      ni = 2;
-      nBad = 0;
-    }
-    double rho = 0;
-    int qmax = 0;
+    lm.begin(h->hScal[0]);
+    if (it == 0) lm.init_lambda(1e-5 * h->hScal[1]);
     do {
       // ---- BlockSolver::solve: Schur complement, tiled Cholesky, substitutions, point back-substitution
       B2S_CUDA(cudaMemsetAsync(h->fail, 0, 4, s));
-      if (nMp) k_dinv<<<blocks(nMp, 128), 128, 0, s>>>(a, lambda);
+      if (nMp) k_dinv<<<blocks(nMp, 128), 128, 0, s>>>(a, lm.lambda);
       if (nFree) {
         B2S_CUDA(cudaMemsetAsync(a.rhs, 0, (size_t)npPad * 8, s));
         k_rhs<<<blocks((long long)nFree * 32, 256), 256, 0, s>>>(a);
         B2S_CUDA(cudaMemsetAsync(a.tiles, 0, tileBytes, s));
         k_schur<<<blocks((long long)nBlk * 32, 256), 256, 0, s>>>(a, (const unsigned*)h->uKey.p, (const int*)h->blkBeg.p,
-                                                                   nBlk, (const int4*)h->pairRecS.p, lambda);
+                                                                   nBlk, (const int4*)h->pairRecS.p, lm.lambda);
         factor_solve(ts, nT, envT, rowOff, (const int*)h->rows.p, s);
       }
       if (nMp) k_backsub_points<<<blocks(nMp, 128), 128, 0, s>>>(a);
       // ---- SparseOptimizer::update into the trial copy, trial chi2, computeScale
-      k_update<<<blocks(nUpd, 256), 256, 0, s>>>(a, pose, pts, poseT, ptsT, lambda);
+      k_update<<<blocks(nUpd, 256), 256, 0, s>>>(a, pose, pts, poseT, ptsT, lm.lambda);
       chi2_of(poseT, ptsT, h->scal);
       reduce<0>(h, a.tmp, nx, h->scal + 1);
-      rc = sync_scalars(2);
+      rc = sync.scalars(2);
       if (rc != B2S_OK) return rc;
-      const bool solved = *h->hFail == 0;
-      double tempChi = solved ? h->hScal[0] : DBL_MAX;
-      rho = currentChi - tempChi;
-      double scale = solved ? h->hScal[1] : 0.0;
-      scale += 1e-3;
-      rho /= scale;
-      if (!solved) rho = -1;
-      const bool good = rho > 0 && std::isfinite(tempChi);
-      if (trace.size() < 255) trace.push_back(good ? 1 : 0);
-      nTrials++;
-      if (good) {
-        double alpha = 1. - pow((2 * rho - 1), 3);
-        alpha = std::min(alpha, 2. / 3.);
-        lambda *= std::max(1. / 3., alpha);
-        ni = 2;
-        currentChi = tempChi;
+      if (lm.trial(*h->hFail == 0, h->hScal[0], h->hScal[1], trace)) {
         std::swap(pose, poseT);
         std::swap(pts, ptsT);
-      } else {
-        lambda *= ni;
-        ni *= 2;
       }
-      qmax++;
-    } while (rho < 0 && qmax < 10 && !terminate());
-    if (qmax == 10 || rho == 0) {
-      ok = false;
-      continue;
-    }
-    if ((iniChi - currentChi) * 1e3 < iniChi) nBad++;
-    else nBad = 0;
-    if (nBad >= 3) ok = false;
+    } while (lm.retry(terminate()));
+    ok = !lm.end_iteration();
   }
 
   // ---- write-back (every keyframe through Converter; points with an edge) and the chi2 of the returned estimate
@@ -867,19 +803,20 @@ extern "C" int b2s_global_ba(b2s_gba_solver* h, const b2s_gba_problem* p, const 
   if (nKf) B2S_CUDA(cudaMemcpyAsync(r->Tcw_out, h->Tcw, (size_t)nKf * 64, cudaMemcpyDeviceToHost, s));
   if (nMp) B2S_CUDA(cudaMemcpyAsync(Xout.data(), h->X, (size_t)nMp * 12, cudaMemcpyDeviceToHost, s));
   B2S_CUDA(cudaMemcpyAsync(h->hScal, h->scal, 8, cudaMemcpyDeviceToHost, s));
-  rc = sync_stream();
+  rc = sync.stream();
   if (rc != B2S_OK) return rc;
   B2S_CUDA(cudaGetLastError());
   for (int m = 0; m < nMp; m++)
     if (r->point_included[m])
       for (int c = 0; c < 3; c++) r->points_out[(size_t)m * 3 + c] = Xout[(size_t)m * 3 + c];
   r->chi2_final = h->hScal[0];
-  r->n_trials = nTrials;
+  r->n_trials = lm.nTrials;
   if (r->trace) {
-    for (size_t i = 0; i < trace.size(); i++) r->trace[i] = trace[i];
-    r->trace[trace.size()] = -1;
+    const int n = std::min(lm.nTrials, 255);
+    for (int i = 0; i < n; i++) r->trace[i] = trace[i];
+    r->trace[n] = -1;
   }
-  h->lastMs = busyMs;
-  h->lastTrials = nTrials;
+  h->lastMs = sync.busyMs;
+  h->lastTrials = lm.nTrials;
   return B2S_OK;
 }

@@ -5,7 +5,8 @@
 //   types/types_six_dof_expmap.{h,cpp}   computeError / linearizeOplus of EdgeSE3ProjectXYZ, EdgeStereoSE3ProjectXYZ
 //   core/base_binary_edge.hpp:55-120     constructQuadraticForm (Huber weighted)      -> k_build_landmarks / k_build_poses
 //   core/block_solver.hpp:354-486        Schur complement + back substitution         -> k_schur / k_chol / k_backsub
-//   core/optimization_algorithm_levenberg.cpp:61-189   LM control                     -> k_control_begin / k_control_end
+//   core/optimization_algorithm_levenberg.cpp:61-189   LM control                     -> control_begin / control_end
+//                                                      (the step policy itself: Levenberg, levenberg.cuh)
 //   types/se3quat.h:223-257, types_sba.h:52-56         oplus updates                  -> k_update_poses / k_backsub
 // The whole Levenberg-Marquardt loop of a window runs inside ONE persistent kernel: a window owns `nCta` thread blocks
 // that move through the phases (linearise -> Schur -> Cholesky -> back-substitute -> evaluate -> accept/reject) separated
@@ -24,19 +25,20 @@
 
 #include "common.cuh"
 #include "ba_math.cuh"  // quat / pose helpers, huber, edge_jacobians
+#include "levenberg.cuh"
 
 namespace b2s {
 
-constexpr int PSTRIDE = 8;  // doubles per pose: q(x,y,z,w), t(x,y,z), pad
 constexpr int CHOL_BS = 32;
 
 struct BaState {
-  int active, round, it, qmax, needBuild, restore, doOutlier, solveOk, stop, nTrials, nBad, robust, finishedRound0;
+  int active, round, it, needBuild, restore, doOutlier, solveOk, stop, robust, finishedRound0;
   int errBuf, errCurrent;  // which err / eWq buffer describes the linearisation state; it is up to date
   int nLive;               // edges left at level 0 by the outlier pass between the rounds (0: round 2 has nothing to optimise)
   int pairsOverflow;       // the covisibility pair list did not fit capPairs: the window was not run
   int its[2];
-  double lambda, ni, currentChi, iniChi, tempChi, rho, chi2Final;
+  Levenberg lm;
+  double chi2Final;
   unsigned long long maxDiagBits;
   int trace[256];
 };
@@ -191,7 +193,7 @@ __device__ __forceinline__ void load_edge_idx(const BaPtrs& p, int w, int e, int
   x.stereo = p.eStereo[eo] != 0;
 }
 __device__ __forceinline__ void load_edge_ops(const BaPtrs& p, int w, const EdgeIdx& x, EdgeOps& o) {
-  const double* P = p.pose + ((size_t)w * p.capKf + x.kf) * PSTRIDE;
+  const double* P = p.pose + ((size_t)w * p.capKf + x.kf) * POSE_STRIDE;
   const double* X = p.pts + ((size_t)w * p.capMp + x.mp) * 3;
 #pragma unroll
   for (int k = 0; k < 7; k++) o.P[k] = P[k];
@@ -205,7 +207,7 @@ __device__ __forceinline__ void load_edge_ops(const BaPtrs& p, int w, const Edge
 __device__ void phase_reduce_landmarks(const BaPtrs& p, const WinCtx& c, const BaWin& W, int cur, double* RtTab) {
   const int w = c.w;
   for (int k = threadIdx.x; k < W.nKf; k += blockDim.x) {
-    const double* P = p.pose + ((size_t)w * p.capKf + k) * PSTRIDE;
+    const double* P = p.pose + ((size_t)w * p.capKf + k) * POSE_STRIDE;
     double R[3][3];
     quat_to_R(P, R);
     double* o = RtTab + (size_t)k * 12;
@@ -304,7 +306,7 @@ __device__ void phase_build_poses(const BaPtrs& p, const WinCtx& c, const BaWin&
     double acc[27];
 #pragma unroll
     for (int k = 0; k < 27; k++) acc[k] = 0;
-    const double* P = p.pose + ((size_t)w * p.capKf + kf) * PSTRIDE;
+    const double* P = p.pose + ((size_t)w * p.capKf + kf) * POSE_STRIDE;
     double Pv[7];
 #pragma unroll
     for (int k = 0; k < 7; k++) Pv[k] = P[k];
@@ -404,16 +406,8 @@ __device__ void control_begin(const BaPtrs& p, int w, int nCta) {
   if (st.needBuild) {
     double chi = 0;
     for (int k = 0; k < nCta; k++) chi += p.partChi[(size_t)w * p.nPartE + k];
-    st.currentChi = chi;
-    st.iniChi = chi;
-    st.tempChi = chi;
-    if (st.it == 0) {  // computeLambdaInit (levenberg.cpp:93-97,166-180)
-      st.lambda = 1e-5 * __longlong_as_double((long long)st.maxDiagBits);
-      st.ni = 2;
-      st.nBad = 0;
-    }
-    st.rho = 0;
-    st.qmax = 0;
+    st.lm.begin(chi);
+    if (st.it == 0) st.lm.init_lambda(1e-5 * __longlong_as_double((long long)st.maxDiagBits));
     st.needBuild = 0;
   }
   st.maxDiagBits = 0ull;
@@ -720,7 +714,7 @@ __device__ void phase_schur_blocks(const BaPtrs& p, const WinCtx& c, const BaWin
       __syncwarp();
       if (lane < 2) {
         const int kf = p.freeKf[(size_t)w * p.capKf + (lane ? i2 : i1)];
-        const double* P = p.pose + ((size_t)w * p.capKf + kf) * PSTRIDE;
+        const double* P = p.pose + ((size_t)w * p.capKf + kf) * POSE_STRIDE;
         double R[3][3];
         quat_to_R(P, R);
         double* o = reinterpret_cast<double*>(buf + RC_RT) + lane * 12;
@@ -982,7 +976,7 @@ __device__ void phase_backsub_update(const BaPtrs& p, const WinCtx& c, const BaW
   double* RtTab = stage + (size_t)(blockDim.x >> 5) * RC_TOTAL * 2;  // R | t of every free pose (behind the Schur staging)
   if (solveOk) {
     for (int i = threadIdx.x; i < W.nFree; i += blockDim.x) {
-      const double* P = p.pose + ((size_t)w * p.capKf + p.freeKf[(size_t)w * p.capKf + i]) * PSTRIDE;
+      const double* P = p.pose + ((size_t)w * p.capKf + p.freeKf[(size_t)w * p.capKf + i]) * POSE_STRIDE;
       double R[3][3];
       quat_to_R(P, R);
       double* o = RtTab + (size_t)i * 12;
@@ -1056,8 +1050,8 @@ __device__ void phase_backsub_update(const BaPtrs& p, const WinCtx& c, const BaW
   // poses: the last CTA of the window also backs up and updates the keyframe poses
   if (c.cta == c.nCta - 1) {
     for (int kf = threadIdx.x; kf < W.nKf; kf += blockDim.x) {
-      double* P = p.pose + ((size_t)w * p.capKf + kf) * PSTRIDE;
-      double* Pb = p.poseBak + ((size_t)w * p.capKf + kf) * PSTRIDE;
+      double* P = p.pose + ((size_t)w * p.capKf + kf) * POSE_STRIDE;
+      double* Pb = p.poseBak + ((size_t)w * p.capKf + kf) * POSE_STRIDE;
       for (int k = 0; k < 7; k++) Pb[k] = P[k];
       const int pi = p.poseIndex[(size_t)w * p.capKf + kf];
       if (pi >= 0 && solveOk) {
@@ -1124,42 +1118,15 @@ __device__ void control_end(const BaPtrs& p, int w, int nCta) {
   for (int k = 0; k < nCta; k++) tempChi += p.partChi[(size_t)w * p.nPartE + k];
   for (int k = 0; k < nCta; k++) scale += p.partScale[(size_t)w * p.nPartM + k];
   st.chi2Final = tempChi;  // activeRobustChi2() of the last evaluated state (diagnostic)
-  if (!st.solveOk) {
-    tempChi = DBL_MAX;
-    scale = 0;
-  }
-  scale += 1e-3;
-  double rho = (st.currentChi - tempChi) / scale;
-  if (!st.solveOk) rho = -1;
-  const bool good = rho > 0 && isfinite(tempChi);
-  if (st.nTrials < 255) st.trace[st.nTrials] = good ? 1 : 0;
-  st.nTrials++;
-  if (good) {
-    double alpha = 1. - pow((2 * rho - 1), 3);
-    alpha = fmin(alpha, 2. / 3.);
-    st.lambda *= fmax(1. / 3., alpha);
-    st.ni = 2;
-    st.currentChi = tempChi;
+  if (st.lm.trial(st.solveOk, tempChi, scale, st.trace)) {
     st.errBuf ^= 1;  // phase_errors just stored this state's errors / weights in the other buffer
     st.errCurrent = 1;
   } else {
-    st.lambda *= st.ni;
-    st.ni *= 2;
     st.restore = 1;
   }
-  st.rho = rho;
-  st.tempChi = tempChi;
-  st.qmax++;
   const int stop = *((volatile int*)&st.stop);
-  if (rho < 0 && st.qmax < 10 && !stop) return;  // another trial with the larger lambda
-  bool roundEnd = false;
-  if (st.qmax == 10 || rho == 0) {
-    roundEnd = true;
-  } else {
-    if ((st.iniChi - st.currentChi) * 1e3 < st.iniChi) st.nBad++;
-    else st.nBad = 0;
-    if (st.nBad >= 3) roundEnd = true;
-  }
+  if (st.lm.retry(stop)) return;  // another trial with the larger lambda
+  bool roundEnd = st.lm.end_iteration();
   st.it++;
   if (st.it >= st.its[st.round] || stop) roundEnd = true;
   if (!roundEnd) {
@@ -1183,8 +1150,8 @@ __device__ void control_end(const BaPtrs& p, int w, int nCta) {
 __device__ void phase_restore(const BaPtrs& p, const WinCtx& c, const BaWin& W) {
   const int w = c.w;
   for (int i = c.gtid; i < W.nMp * 3; i += c.gthreads) p.pts[(size_t)w * p.capMp * 3 + i] = p.ptsBak[(size_t)w * p.capMp * 3 + i];
-  for (int i = c.gtid; i < W.nKf * PSTRIDE; i += c.gthreads)
-    p.pose[(size_t)w * p.capKf * PSTRIDE + i] = p.poseBak[(size_t)w * p.capKf * PSTRIDE + i];
+  for (int i = c.gtid; i < W.nKf * POSE_STRIDE; i += c.gthreads)
+    p.pose[(size_t)w * p.capKf * POSE_STRIDE + i] = p.poseBak[(size_t)w * p.capKf * POSE_STRIDE + i];
 }
 
 // chi2 / depth outlier tests (src/Optimizer.cc:880-958)
@@ -1194,7 +1161,7 @@ __device__ void phase_outliers(const BaPtrs& p, const WinCtx& c, const BaWin& W,
   for (int e = c.gtid; e < W.nEdges; e += c.gthreads) {
     const size_t eo = (size_t)w * p.capE + e;
     double Xc[3];
-    pose_map(p.pose + ((size_t)w * p.capKf + p.eKf[eo]) * PSTRIDE, p.pts + ((size_t)w * p.capMp + p.eMp[eo]) * 3, Xc);
+    pose_map(p.pose + ((size_t)w * p.capKf + p.eKf[eo]) * POSE_STRIDE, p.pts + ((size_t)w * p.capMp + p.eMp[eo]) * 3, Xc);
     const double th = p.eStereo[eo] ? 7.815 : 5.991;
     const bool out = p.chi2[eo] > th || !(Xc[2] > 0.0);
     if (mode == 1) {
@@ -1265,7 +1232,7 @@ __global__ void __launch_bounds__(BA_T) k_local_ba(BaPtrs p, int nCtaUniform, in
     if (c.cta == 0 && threadIdx.x == 0) control_begin(p, w, nCta);
     win_barrier(bar, epoch, nCta, hung);
     BA_PROF(2)
-    const double lambda = vst->lambda;
+    const double lambda = vst->lm.lambda;
     phase_dinv(p, c, W, lambda);
     win_barrier(bar, epoch, nCta, hung);
     BA_PROF(3)
@@ -1503,20 +1470,21 @@ __device__ bool po_solve6(const double* H, double lambda, const double* b, doubl
 
 constexpr int PO_T = 256;
 __global__ void __launch_bounds__(PO_T) k_pose_opt(PoPtrs p) {
-  __shared__ double sPose[8], sInit[8], sBackup[8], sH[27], sX[6], sRed[32];
-  __shared__ double sCur, sTemp, sLambda, sNi, sIni, sRho;
-  __shared__ int sOk, sAgain, sRobust, sNBadLM, sTrials, sQmax, sNActive, sNBad;
+  __shared__ double sPose[POSE_STRIDE], sInit[POSE_STRIDE], sBackup[POSE_STRIDE], sH[27], sX[6], sRed[32];
+  __shared__ double sTemp;
+  __shared__ Levenberg lm;
+  __shared__ int sOk, sAgain, sRobust, sNActive, sNBad;
   const int fr = blockIdx.x;
   const PoFrame F = p.frames[fr];
   const int tid = threadIdx.x;
   const int nE = F.nEdges, e0 = F.edgeOff;
-  if (tid < 8) {
-    sInit[tid] = p.poseInit[(size_t)fr * 8 + tid];
+  if (tid < POSE_STRIDE) {
+    sInit[tid] = p.poseInit[(size_t)fr * POSE_STRIDE + tid];
     sPose[tid] = sInit[tid];
   }
   if (tid == 0) {
     sRobust = 1;
-    sTrials = 0;
+    lm.nTrials = 0;
     sNBad = 0;
   }
   for (int e = tid; e < nE; e += PO_T) {
@@ -1525,14 +1493,13 @@ __global__ void __launch_bounds__(PO_T) k_pose_opt(PoPtrs p) {
   }
   __syncthreads();
   if (nE < 3) {  // :492-493: return 0, pose untouched
-    if (tid < 8) p.poseOut[(size_t)fr * 8 + tid] = sInit[tid];
+    if (tid < POSE_STRIDE) p.poseOut[(size_t)fr * POSE_STRIDE + tid] = sInit[tid];
     if (tid == 0) {
       p.nInliers[fr] = 0;
       p.nTrials[fr] = 0;
     }
     return;
   }
-  const double dMono = (double)(float)2.4476519360399226, dStereo = (double)(float)2.795532150593156;  // (float)sqrt(5.991|7.815)
   auto eval_errors = [&]() -> void {  // computeActiveErrors + activeRobustChi2 -> sTemp
     double chi = 0;
     const int robust = sRobust;
@@ -1546,7 +1513,7 @@ __global__ void __launch_bounds__(PO_T) k_pose_opt(PoPtrs p) {
       p.err[(size_t)ge * 3 + 2] = er[2];
       p.chi2[ge] = c2;
       double r0 = c2, r1;
-      if (robust) huber(c2, (p.obs[(size_t)ge * 3 + 2] < 0) ? dMono : dStereo, r0, r1);
+      if (robust) huber(c2, delta_of(!(p.obs[(size_t)ge * 3 + 2] < 0)), r0, r1);
       chi += r0;
     }
     const double tot = block_sum(chi, sRed);
@@ -1554,7 +1521,7 @@ __global__ void __launch_bounds__(PO_T) k_pose_opt(PoPtrs p) {
     __syncthreads();
   };
   for (int round = 0; round < 4; round++) {
-    if (tid < 8) sPose[tid] = sInit[tid];  // vSE3->setEstimate(Converter::toSE3Quat(pFrame->mTcw)) (:505)
+    if (tid < POSE_STRIDE) sPose[tid] = sInit[tid];  // vSE3->setEstimate(Converter::toSE3Quat(pFrame->mTcw)) (:505)
     int act = 0;
     for (int e = tid; e < nE; e += PO_T) act += p.level[e0 + e] == 0;
     __syncthreads();
@@ -1563,7 +1530,6 @@ __global__ void __launch_bounds__(PO_T) k_pose_opt(PoPtrs p) {
       if (tid == 0) {
         sNActive = (int)a;
         sOk = 1;
-        sNBadLM = 0;
       }
       __syncthreads();
     }
@@ -1571,10 +1537,7 @@ __global__ void __launch_bounds__(PO_T) k_pose_opt(PoPtrs p) {
       for (int it = 0; it < 10; it++) {
         if (!sOk) break;
         eval_errors();
-        if (tid == 0) {
-          sCur = sTemp;
-          sIni = sTemp;
-        }
+        if (tid == 0) lm.begin(sTemp);
         // buildSystem: J^T (rho' Omega) J (upper triangle, 21) and -J^T Omega e rho' (6)
         double acc[27];
 #pragma unroll
@@ -1613,7 +1576,7 @@ __global__ void __launch_bounds__(PO_T) k_pose_opt(PoPtrs p) {
           double rho1 = 1.0;
           if (robust) {
             double r0;
-            huber(p.chi2[ge], st ? dStereo : dMono, r0, rho1);
+            huber(p.chi2[ge], delta_of(st), r0, rho1);
           }
           const double* er = p.err + (size_t)ge * 3;
           double omr[3];
@@ -1653,16 +1616,13 @@ __global__ void __launch_bounds__(PO_T) k_pose_opt(PoPtrs p) {
                 if (i == j) mx = fmax(fabs(sH[t]), mx);
                 t++;
               }
-            sLambda = 1e-5 * mx;
-            sNi = 2;
-            sNBadLM = 0;
+            lm.init_lambda(1e-5 * mx);
           }
-          sQmax = 0;
         }
         __syncthreads();
         do {
           if (tid == 0) {
-            for (int k = 0; k < 8; k++) sBackup[k] = sPose[k];
+            for (int k = 0; k < POSE_STRIDE; k++) sBackup[k] = sPose[k];
             double Hf[36], bb[6];
             int t = 0;
             for (int i = 0; i < 6; i++)
@@ -1673,7 +1633,7 @@ __global__ void __launch_bounds__(PO_T) k_pose_opt(PoPtrs p) {
               }
             for (int i = 0; i < 6; i++) bb[i] = sH[21 + i];
             double xx[6];
-            const bool ok2 = po_solve6(Hf, sLambda, bb, xx);
+            const bool ok2 = po_solve6(Hf, lm.lambda, bb, xx);
             sAgain = ok2 ? 1 : 0;  // (temporarily: solve status)
             if (ok2) {
               for (int i = 0; i < 6; i++) sX[i] = xx[i];
@@ -1684,43 +1644,16 @@ __global__ void __launch_bounds__(PO_T) k_pose_opt(PoPtrs p) {
           const int ok2 = sAgain;
           eval_errors();
           if (tid == 0) {
-            double tempChi = ok2 ? sTemp : DBL_MAX;
-            double rho = sCur - tempChi;
             double scale = 0;
             if (ok2)
-              for (int j = 0; j < 6; j++) scale += sX[j] * (sLambda * sX[j] + sH[21 + j]);
-            scale += 1e-3;
-            rho /= scale;
-            if (!ok2) rho = -1;
-            const bool good = rho > 0 && isfinite(tempChi);
-            if (sTrials < 255) p.trace[(size_t)fr * 256 + sTrials] = good ? 1 : 0;
-            sTrials++;
-            if (good) {
-              double alpha = 1. - pow((2 * rho - 1), 3);
-              alpha = fmin(alpha, 2. / 3.);
-              sLambda *= fmax(1. / 3., alpha);
-              sNi = 2;
-              sCur = tempChi;
-            } else {
-              sLambda *= sNi;
-              sNi *= 2;
-              for (int k = 0; k < 8; k++) sPose[k] = sBackup[k];
-            }
-            sRho = rho;
-            sQmax++;
-            sAgain = (rho < 0 && sQmax < 10) ? 1 : 0;
+              for (int j = 0; j < 6; j++) scale += sX[j] * (lm.lambda * sX[j] + sH[21 + j]);
+            if (!lm.trial(ok2, sTemp, scale, p.trace + (size_t)fr * 256))
+              for (int k = 0; k < POSE_STRIDE; k++) sPose[k] = sBackup[k];
+            sAgain = lm.retry(false) ? 1 : 0;
           }
           __syncthreads();
         } while (sAgain);
-        if (tid == 0) {
-          if (sQmax == 10 || sRho == 0) {
-            sOk = 0;
-          } else {
-            if ((sIni - sCur) * 1e3 < sIni) sNBadLM++;
-            else sNBadLM = 0;
-            if (sNBadLM >= 3) sOk = 0;
-          }
-        }
+        if (tid == 0 && lm.end_iteration()) sOk = 0;
         __syncthreads();
       }
     }
@@ -1754,11 +1687,11 @@ __global__ void __launch_bounds__(PO_T) k_pose_opt(PoPtrs p) {
     }
     if (nE < 10) break;  // optimizer.edges().size() < 10 (:569-570)
   }
-  if (tid < 8) p.poseOut[(size_t)fr * 8 + tid] = sPose[tid];
+  if (tid < POSE_STRIDE) p.poseOut[(size_t)fr * POSE_STRIDE + tid] = sPose[tid];
   if (tid == 0) {
     p.nInliers[fr] = nE - sNBad;
-    p.nTrials[fr] = sTrials;
-    if (sTrials < 256) p.trace[(size_t)fr * 256 + min(sTrials, 255)] = -1;
+    p.nTrials[fr] = lm.nTrials;
+    if (lm.nTrials < 256) p.trace[(size_t)fr * 256 + min(lm.nTrials, 255)] = -1;
   }
 }
 
@@ -1796,36 +1729,6 @@ struct b2s_ba_solver {
   int smBudget = 0;  // CTAs (= SMs) one LocalBA batch may occupy; 0 = all (b2s_ba_set_sm_budget)
   DevBuf pairRec;    // d.pairRec: batch x d.capPairs records, grown by ba_run when a window needs more
 };
-
-static void quat_from_R_host(const double m[3][3], double* q) {
-  double t = m[0][0] + m[1][1] + m[2][2];
-  if (t > 0.0) {
-    t = sqrt(t + 1.0);
-    q[3] = 0.5 * t;
-    t = 0.5 / t;
-    q[0] = (m[2][1] - m[1][2]) * t;
-    q[1] = (m[0][2] - m[2][0]) * t;
-    q[2] = (m[1][0] - m[0][1]) * t;
-  } else {
-    int i = 0;
-    if (m[1][1] > m[0][0]) i = 1;
-    if (m[2][2] > m[i][i]) i = 2;
-    const int j = (i + 1) % 3, k = (j + 1) % 3;
-    t = sqrt(m[i][i] - m[j][j] - m[k][k] + 1.0);
-    double v[3];
-    v[i] = 0.5 * t;
-    t = 0.5 / t;
-    q[3] = (m[k][j] - m[j][k]) * t;
-    v[j] = (m[j][i] + m[i][j]) * t;
-    v[k] = (m[k][i] + m[i][k]) * t;
-    q[0] = v[0]; q[1] = v[1]; q[2] = v[2];
-  }
-  if (q[3] < 0) {
-    q[0] = -q[0]; q[1] = -q[1]; q[2] = -q[2]; q[3] = -q[3];
-  }
-  const double n = sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
-  q[0] /= n; q[1] /= n; q[2] /= n; q[3] /= n;
-}
 
 extern "C" int b2s_ba_create(int max_kf, int max_mp, int max_edges, int max_batch, int device, b2s_ba_solver** out) {
   if (!out || max_kf < 1 || max_kf > 128 || max_mp < 1 || max_edges < 1 || max_batch < 1) {
@@ -1867,7 +1770,7 @@ extern "C" int b2s_ba_create(int max_kf, int max_mp, int max_edges, int max_batc
     }
   };
   A(&d.win, B * sizeof(BaWin)); A(&d.st, B * sizeof(BaState));
-  A(&d.pose, B * max_kf * PSTRIDE * 8); A(&d.poseBak, B * max_kf * PSTRIDE * 8);
+  A(&d.pose, B * max_kf * POSE_STRIDE * 8); A(&d.poseBak, B * max_kf * POSE_STRIDE * 8);
   A(&d.pts, B * max_mp * 3 * 8); A(&d.ptsBak, B * max_mp * 3 * 8);
   A(&d.poseIndex, B * max_kf * 4);
   A(&d.eKf, B * max_edges * 4); A(&d.eMp, B * max_edges * 4);
@@ -1892,7 +1795,7 @@ extern "C" int b2s_ba_create(int max_kf, int max_mp, int max_edges, int max_batc
   d.ctaMap = nullptr;
   d.winCtas = nullptr;
   BaHostStage& s = h->hs;
-  HA(&s.pose, B * max_kf * PSTRIDE * 8); HA(&s.pts, B * max_mp * 3 * 8);
+  HA(&s.pose, B * max_kf * POSE_STRIDE * 8); HA(&s.pts, B * max_mp * 3 * 8);
   HA(&s.pidx, B * max_kf * 4); HA(&s.freeKf, B * max_kf * 4);
   HA(&s.eKf, B * max_edges * 4); HA(&s.eMp, B * max_edges * 4);
   HA(&s.mpStart, B * (max_mp + 1) * 4); HA(&s.kfStart, B * (max_kf + 1) * 4);
@@ -1948,20 +1851,12 @@ static int ba_host_threads(int batch) {
 static int ba_prepare_window(b2s_ba_solver* h, int w, const b2s_ba_problem& P, int* nFreeOut, long long* pairBoundOut) {
   const BaPtrs& d = h->d;
   BaHostStage& s = h->hs;
-  double* pose = s.pose + (size_t)w * d.capKf * PSTRIDE;
+  double* pose = s.pose + (size_t)w * d.capKf * POSE_STRIDE;
   int* pidx = s.pidx + (size_t)w * d.capKf;
   int* freeKf = s.freeKf + (size_t)w * d.capKf;
   int nFree = 0;
   for (int k = 0; k < P.n_kf; k++) {
-    const float* T = P.Tcw + (size_t)k * 16;
-    double R[3][3];
-    for (int i = 0; i < 3; i++)
-      for (int j = 0; j < 3; j++) R[i][j] = T[i * 4 + j];  // Converter::toSE3Quat (src/Converter.cc:57-66)
-    quat_from_R_host(R, pose + (size_t)k * PSTRIDE);
-    pose[(size_t)k * PSTRIDE + 4] = T[3];
-    pose[(size_t)k * PSTRIDE + 5] = T[7];
-    pose[(size_t)k * PSTRIDE + 6] = T[11];
-    pose[(size_t)k * PSTRIDE + 7] = 0;
+    se3quat_from_Tcw(P.Tcw + (size_t)k * 16, pose + (size_t)k * POSE_STRIDE);
     if (!P.fixed[k]) {
       pidx[k] = nFree;
       freeKf[nFree++] = k;
@@ -2069,7 +1964,7 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
     S0.needBuild = 1;
     S0.robust = 1;
     S0.its[0] = P.its1; S0.its[1] = P.its2;
-    S0.ni = 2;
+    S0.lm.ni = 2;
     maxE = std::max(maxE, P.n_edges); maxMp = std::max(maxMp, P.n_mp); maxFree = std::max(maxFree, nFree[w]);
     maxPairs = std::max(maxPairs, pairBound[w]);
   }
@@ -2087,7 +1982,7 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
   const size_t nb = (size_t)batch;
 #define UPALL(dst, src, stride, type) \
   B2S_CUDA(cudaMemcpyAsync((dst), (src), nb * (size_t)(stride) * sizeof(type), cudaMemcpyHostToDevice, st))
-  UPALL(d.pose, s.pose, d.capKf * PSTRIDE, double);
+  UPALL(d.pose, s.pose, d.capKf * POSE_STRIDE, double);
   UPALL(d.pts, s.pts, (size_t)d.capMp * 3, double);
   UPALL(d.poseIndex, s.pidx, d.capKf, int);
   UPALL(d.freeKf, s.freeKf, d.capKf, int);
@@ -2218,7 +2113,7 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
     }
   }
   // write-back values (src/Optimizer.cc:961-996): SetPose(toCvMat(SE3quat)), SetWorldPos(toCvMat(estimate))
-  B2S_CUDA(cudaMemcpyAsync(s.pose, d.pose, nb * d.capKf * PSTRIDE * 8, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA(cudaMemcpyAsync(s.pose, d.pose, nb * d.capKf * POSE_STRIDE * 8, cudaMemcpyDeviceToHost, st));
   B2S_CUDA(cudaMemcpyAsync(s.pts, d.pts, nb * (size_t)d.capMp * 3 * 8, cudaMemcpyDeviceToHost, st));
   B2S_CUDA(cudaMemcpyAsync(s.eOutlier, d.eOutlier, nb * d.capE, cudaMemcpyDeviceToHost, st));
   B2S_CUDA(cudaMemcpyAsync(s.st, d.st, nb * sizeof(BaState), cudaMemcpyDeviceToHost, st));
@@ -2227,7 +2122,7 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
   B2S_CUDA(cudaGetLastError());
   cudaEventElapsedTime(&h->lastLmMs, h->evLm[0], h->evLm[1]);
   h->lastTrials = 0;
-  for (int w = 0; w < batch; w++) h->lastTrials += s.st[w].nTrials;
+  for (int w = 0; w < batch; w++) h->lastTrials += s.st[w].lm.nTrials;
   for (int w = 0; w < batch; w++)
     if (s.st[w].finishedRound0) {
       set_error("b2s_local_ba: window %d: LM kernel barrier timed out (CTAs not co-resident?)", w);
@@ -2247,29 +2142,17 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
         for (int w = t; w < batch; w += nth) {
           const b2s_ba_problem& P = probs[w];
           b2s_ba_result& R = res[w];
-          const double* pose = s.pose + (size_t)w * d.capKf * PSTRIDE;
+          const double* pose = s.pose + (size_t)w * d.capKf * POSE_STRIDE;
           const double* pts = s.pts + (size_t)w * d.capMp * 3;
-          if (R.Tcw_out) {
-            for (int k = 0; k < P.n_local; k++) {
-              const double* q = pose + (size_t)k * PSTRIDE;
-              const double tx = 2 * q[0], ty = 2 * q[1], tz = 2 * q[2];
-              const double twx = tx * q[3], twy = ty * q[3], twz = tz * q[3];
-              const double txx = tx * q[0], txy = ty * q[0], txz = tz * q[0];
-              const double tyy = ty * q[1], tyz = tz * q[1], tzz = tz * q[2];
-              float* T = R.Tcw_out + (size_t)k * 16;
-              T[0] = (float)(1 - (tyy + tzz)); T[1] = (float)(txy - twz); T[2] = (float)(txz + twy); T[3] = (float)q[4];
-              T[4] = (float)(txy + twz); T[5] = (float)(1 - (txx + tzz)); T[6] = (float)(tyz - twx); T[7] = (float)q[5];
-              T[8] = (float)(txz - twy); T[9] = (float)(tyz + twx); T[10] = (float)(1 - (txx + tyy)); T[11] = (float)q[6];
-              T[12] = 0.f; T[13] = 0.f; T[14] = 0.f; T[15] = 1.f;
-            }
-          }
+          if (R.Tcw_out)
+            for (int k = 0; k < P.n_local; k++) se3quat_to_Tcw(pose + (size_t)k * POSE_STRIDE, R.Tcw_out + (size_t)k * 16);
           if (R.points_out)
             for (size_t i = 0; i < (size_t)P.n_mp * 3; i++) R.points_out[i] = (float)pts[i];
           if (R.edge_outlier && P.n_edges) memcpy(R.edge_outlier, s.eOutlier + (size_t)w * d.capE, P.n_edges);
           R.chi2_final = s.st[w].chi2Final;
-          R.n_trials = s.st[w].nTrials;
+          R.n_trials = s.st[w].lm.nTrials;
           if (R.trace) {
-            const int n = std::min(s.st[w].nTrials, 255);
+            const int n = std::min(s.st[w].lm.nTrials, 255);
             for (int i = 0; i < n; i++) R.trace[i] = s.st[w].trace[i];
             R.trace[n] = -1;
           }
@@ -2298,7 +2181,7 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
         long long tot = 0;
         for (int k = 0; k <= 10; k++) tot += q[k];
         fprintf(stderr, "[b2s_local_ba]   w%02d free=%d mp=%d e=%d trials=%d total=%.2f Mcyc: build=%.2f schur=%.2f chol=%.2f(diag %.2f) backsub=%.2f err=%.2f\n",
-                w, nFree[w], probs[w].n_mp, probs[w].n_edges, s.st[w].nTrials, tot / 1e6, (q[0] + q[1]) / 1e6, q[5] / 1e6,
+                w, nFree[w], probs[w].n_mp, probs[w].n_edges, s.st[w].lm.nTrials, tot / 1e6, (q[0] + q[1]) / 1e6, q[5] / 1e6,
                 q[6] / 1e6, q[11] / 1e6, q[7] / 1e6, q[8] / 1e6);
       }
     }
@@ -2357,7 +2240,7 @@ extern "C" int b2s_pose_optimization_batch(b2s_ba_solver* h, int batch, const b2
   cudaStream_t st = h->stream;
   // pack the edges (features with a MapPoint, ascending feature index = g2o insertion order, :411-487)
   std::vector<PoFrame> frames(batch);
-  std::vector<double> poseInit((size_t)batch * 8);
+  std::vector<double> poseInit((size_t)batch * POSE_STRIDE);
   size_t totalE = 0;
   for (int f = 0; f < batch; f++) {
     const b2s_pose_problem& P = probs[f];
@@ -2372,12 +2255,7 @@ extern "C" int b2s_pose_optimization_batch(b2s_ba_solver* h, int batch, const b2
     frames[f].edgeOff = (int)totalE;
     frames[f].fx = P.fx; frames[f].fy = P.fy; frames[f].cx = P.cx; frames[f].cy = P.cy; frames[f].bf = P.bf;
     totalE += ne;
-    double R[3][3];
-    for (int i = 0; i < 3; i++)
-      for (int j = 0; j < 3; j++) R[i][j] = P.Tcw[i * 4 + j];  // Converter::toSE3Quat (src/Converter.cc:57-66)
-    double* q = &poseInit[(size_t)f * 8];
-    quat_from_R_host(R, q);
-    q[4] = P.Tcw[3]; q[5] = P.Tcw[7]; q[6] = P.Tcw[11]; q[7] = 0;
+    se3quat_from_Tcw(P.Tcw, &poseInit[(size_t)f * POSE_STRIDE]);
   }
   std::vector<float> Xw(totalE * 3 + 3), obs(totalE * 3 + 3), invS(totalE + 1);
   std::vector<int> featOf(totalE + 1);
@@ -2406,7 +2284,7 @@ extern "C" int b2s_pose_optimization_batch(b2s_ba_solver* h, int batch, const b2
     auto A = [&](void* pp, size_t bytes) {
       if (e == cudaSuccess) e = cudaMalloc((void**)pp, bytes);
     };
-    A(&s->dFrames, s->capF * sizeof(PoFrame)); A(&s->dPoseInit, (size_t)s->capF * 64); A(&s->dPoseOut, (size_t)s->capF * 64);
+    A(&s->dFrames, s->capF * sizeof(PoFrame)); A(&s->dPoseInit, (size_t)s->capF * POSE_STRIDE * 8); A(&s->dPoseOut, (size_t)s->capF * POSE_STRIDE * 8);
     A(&s->dErr, s->capE * 24); A(&s->dChi2, s->capE * 8); A(&s->dXw, s->capE * 12); A(&s->dObs, s->capE * 12);
     A(&s->dInvS, s->capE * 4); A(&s->dLevel, s->capE); A(&s->dOutlier, s->capE);
     A(&s->dNInl, (size_t)s->capF * 4); A(&s->dNTr, (size_t)s->capF * 4); A(&s->dTrace, (size_t)s->capF * 256 * 4);
@@ -2416,7 +2294,7 @@ extern "C" int b2s_pose_optimization_batch(b2s_ba_solver* h, int batch, const b2
     }
   }
   B2S_CUDA(cudaMemcpyAsync(s->dFrames, frames.data(), batch * sizeof(PoFrame), cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(s->dPoseInit, poseInit.data(), (size_t)batch * 64, cudaMemcpyHostToDevice, st));
+  B2S_CUDA(cudaMemcpyAsync(s->dPoseInit, poseInit.data(), (size_t)batch * POSE_STRIDE * 8, cudaMemcpyHostToDevice, st));
   if (totalE) {
     B2S_CUDA(cudaMemcpyAsync(s->dXw, Xw.data(), totalE * 12, cudaMemcpyHostToDevice, st));
     B2S_CUDA(cudaMemcpyAsync(s->dObs, obs.data(), totalE * 12, cudaMemcpyHostToDevice, st));
@@ -2429,10 +2307,10 @@ extern "C" int b2s_pose_optimization_batch(b2s_ba_solver* h, int batch, const b2
   k_pose_opt<<<batch, PO_T, 0, st>>>(pp);
   h->launches++;
   B2S_CUDA(cudaGetLastError());
-  std::vector<double> poseOut((size_t)batch * 8);
+  std::vector<double> poseOut((size_t)batch * POSE_STRIDE);
   std::vector<uint8_t> outl(totalE + 1);
   std::vector<int> nInl(batch), nTr(batch), trace((size_t)batch * 256);
-  B2S_CUDA(cudaMemcpyAsync(poseOut.data(), s->dPoseOut, (size_t)batch * 64, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA(cudaMemcpyAsync(poseOut.data(), s->dPoseOut, (size_t)batch * POSE_STRIDE * 8, cudaMemcpyDeviceToHost, st));
   if (totalE) B2S_CUDA(cudaMemcpyAsync(outl.data(), s->dOutlier, totalE, cudaMemcpyDeviceToHost, st));
   B2S_CUDA(cudaMemcpyAsync(nInl.data(), s->dNInl, (size_t)batch * 4, cudaMemcpyDeviceToHost, st));
   B2S_CUDA(cudaMemcpyAsync(nTr.data(), s->dNTr, (size_t)batch * 4, cudaMemcpyDeviceToHost, st));
@@ -2448,16 +2326,7 @@ extern "C" int b2s_pose_optimization_batch(b2s_ba_solver* h, int batch, const b2
     if (frames[f].nEdges < 3) {
       for (int k = 0; k < 16; k++) R.Tcw_out[k] = P.Tcw[k];  // untouched (:492-493)
     } else {
-      const double* q = &poseOut[(size_t)f * 8];  // Converter::toCvMat(SE3Quat) (src/Converter.cc:96-107)
-      const double tx = 2 * q[0], ty = 2 * q[1], tz = 2 * q[2];
-      const double twx = tx * q[3], twy = ty * q[3], twz = tz * q[3];
-      const double txx = tx * q[0], txy = ty * q[0], txz = tz * q[0];
-      const double tyy = ty * q[1], tyz = tz * q[1], tzz = tz * q[2];
-      float* T = R.Tcw_out;
-      T[0] = (float)(1 - (tyy + tzz)); T[1] = (float)(txy - twz); T[2] = (float)(txz + twy); T[3] = (float)q[4];
-      T[4] = (float)(txy + twz); T[5] = (float)(1 - (txx + tzz)); T[6] = (float)(tyz - twx); T[7] = (float)q[5];
-      T[8] = (float)(txz - twy); T[9] = (float)(tyz + twx); T[10] = (float)(1 - (txx + tyy)); T[11] = (float)q[6];
-      T[12] = 0.f; T[13] = 0.f; T[14] = 0.f; T[15] = 1.f;
+      se3quat_to_Tcw(&poseOut[(size_t)f * POSE_STRIDE], R.Tcw_out);
     }
     if (R.trace) {
       const int n = std::min(nTr[f], 255);
