@@ -563,6 +563,44 @@ int b2s_optimize_essential_graph(b2s_eg_solver* h, const b2s_eg_problem* p, b2s_
 /* Device time (CUDA events on the solver's stream) of the last call and the LM trials it ran. */
 float b2s_eg_last_ms(const b2s_eg_solver* h, long long* lm_trials);
 
+/* ------------------------------------------------------------------ Sim3 refinement (loop-closure verification) */
+/* Optimizer::OptimizeSim3 (src/Optimizer.cc:1364-1590) after the graph is built: one free Sim3 S12 (fixed scale if
+ * fix_scale), two Huber-robust projection edges per correspondence (S12 X2c into pKF1, S12^-1 X1c into pKF2), g2o's
+ * numeric Jacobians (central differences, delta = 1e-9) and Levenberg steps; optimize(5), drop the pairs with an edge
+ * chi2 above th2, return 0 if fewer than 10 remain, else optimize(10 if any was dropped, else 5) and count the inliers.
+ * The caller applies the reference's skip rules (:1429-1520) and passes the surviving correspondences in its order.
+ * One launch runs a whole batch, one CTA per problem; every sum is serial in edge order, so two calls on the same input
+ * give bit-identical outputs and a batch equals its problems run one by one. */
+typedef struct {
+  int32_t n;                 /* correspondences that entered the graph, in the reference's order (vnIndexEdge) */
+  const float* X1c;          /* n x 3: R1w*P3D1w + t1w as the caller's cv::Mat expression produced it */
+  const float* X2c;          /* n x 3: R2w*P3D2w + t2w */
+  const float* obs1;         /* n x 2: mvKeysUn[i] of pKF1 */
+  const float* obs2;         /* n x 2: mvKeysUn[i2] of pKF2 */
+  const float* inv_sigma2_1; /* n: pKF1->mvInvLevelSigma2[octave] */
+  const float* inv_sigma2_2; /* n */
+  float fx1, fy1, cx1, cy1, fx2, fy2, cx2, cy2;
+  b2s_sim3 S12;              /* g2oS12 on entry */
+  float th2;
+  int32_t fix_scale;
+} b2s_sim3_problem;
+typedef struct {
+  b2s_sim3 S12_out;          /* the optimised g2oS12; equals S12 on the early return */
+  uint8_t* keep;             /* n: 0 -> vpMatches1[vnIndexEdge[k]] = NULL */
+  int32_t* trace;            /* optional (>= 256): accept(1)/reject(0) per trial of both optimize() calls, -1 terminated */
+  int32_t n_inliers;         /* the return value */
+  int32_t n_trials;
+} b2s_sim3_result;
+typedef struct b2s_sim3opt_solver b2s_sim3opt_solver;
+/* max_matches <= 65536 correspondences per problem, max_batch problems per call. */
+int b2s_sim3opt_create(int max_matches, int max_batch, int device, b2s_sim3opt_solver** out);
+void b2s_sim3opt_destroy(b2s_sim3opt_solver* h);
+/* n > max_matches or batch > max_batch: B2S_ERR_CAPACITY.  batch < 1, n < 0, a null array with n > 0 or th2 <= 0:
+ * B2S_ERR_BAD_ARG.  Nothing is written unless every problem is valid. */
+int b2s_optimize_sim3(b2s_sim3opt_solver* h, int batch, const b2s_sim3_problem* p, b2s_sim3_result* r);
+/* Device time (CUDA events on the solver's stream: upload, kernel, download) of the last call and its LM trials. */
+float b2s_sim3opt_last_ms(const b2s_sim3opt_solver* h, long long* lm_trials);
+
 #ifdef __cplusplus
 }
 #endif

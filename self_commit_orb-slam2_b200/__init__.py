@@ -97,6 +97,22 @@ class _EgResult(ctypes.Structure):
 sim3_edge_dtype = np.dtype([("i", np.int32), ("j", np.int32), ("meas", np.float64, 8)])
 
 
+class _Sim3(ctypes.Structure):
+    _fields_ = [("v", ctypes.c_double * 8)]  # b2s_sim3: qx qy qz qw tx ty tz s
+
+
+class _Sim3Problem(ctypes.Structure):
+    _fields_ = [("n", ctypes.c_int32), ("X1c", _vp), ("X2c", _vp), ("obs1", _vp), ("obs2", _vp), ("inv_sigma2_1", _vp),
+                ("inv_sigma2_2", _vp)] + [(k, ctypes.c_float) for k in ("fx1", "fy1", "cx1", "cy1", "fx2", "fy2", "cx2",
+                                                                         "cy2")] + [
+        ("S12", _Sim3), ("th2", ctypes.c_float), ("fix_scale", ctypes.c_int32)]
+
+
+class _Sim3Result(ctypes.Structure):
+    _fields_ = [("S12_out", _Sim3), ("keep", _vp), ("trace", _vp), ("n_inliers", ctypes.c_int32),
+                ("n_trials", ctypes.c_int32)]
+
+
 class _GbaResult(ctypes.Structure):
     _fields_ = [("Tcw_out", _vp), ("points_out", _vp), ("point_included", _vp), ("trace", _vp),
                 ("chi2_final", ctypes.c_double), ("n_trials", ctypes.c_int)]
@@ -188,6 +204,13 @@ def lib():
             L.b2s_optimize_essential_graph.argtypes = [_vp, _vp, _vp]
             L.b2s_eg_last_ms.restype = ctypes.c_float
             L.b2s_eg_last_ms.argtypes = [_vp, _vp]
+        if hasattr(L, "b2s_sim3opt_create"):
+            L.b2s_sim3opt_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+            L.b2s_sim3opt_destroy.argtypes = [_vp]
+            L.b2s_sim3opt_destroy.restype = None
+            L.b2s_optimize_sim3.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+            L.b2s_sim3opt_last_ms.restype = ctypes.c_float
+            L.b2s_sim3opt_last_ms.argtypes = [_vp, _vp]
         _lib = L
     return _lib
 
@@ -1025,3 +1048,68 @@ class EssentialGraphOptimizer:
         out["chi2"] = r.chi2_final
         out["n_trials"] = r.n_trials
         return out
+
+
+class Sim3Optimizer:
+    """Mirror of ORB_SLAM2::Optimizer::OptimizeSim3 (src/Optimizer.cc:1364-1590) on flattened correspondences
+    (b2s_optimize_sim3).  A batch of independent problems runs in one launch."""
+
+    def __init__(self, max_matches=4096, max_batch=64, device=0):
+        self._h = _vp()
+        _check(lib().b2s_sim3opt_create(max_matches, max_batch, device, ctypes.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().b2s_sim3opt_destroy(self._h)
+            self._h = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def last_ms(self):
+        """(ms, trials): device time of the last call (CUDA events) and the LM trials of all its problems."""
+        n = ctypes.c_longlong(0)
+        ms = lib().b2s_sim3opt_last_ms(self._h, ctypes.byref(n))
+        return float(ms), int(n.value)
+
+    def OptimizeSim3(self, d):
+        """d: X1c, X2c (n x 3 float32), obs1, obs2 (n x 2), inv_sigma2_1, inv_sigma2_2 (n), K1, K2 (fx fy cx cy), S12
+        (qx qy qz qw tx ty tz s), th2, fix_scale.  Returns S12, keep (n, uint8), trace, n_inliers, n_trials."""
+        return self.OptimizeSim3Batch([d])[0]
+
+    def OptimizeSim3Batch(self, ds):
+        keep, probs, outs = [], (_Sim3Problem * len(ds))(), []
+        res = (_Sim3Result * len(ds))()
+        for i, d in enumerate(ds):
+            a = dict(X1c=np.ascontiguousarray(d["X1c"], np.float32).reshape(-1, 3),
+                     X2c=np.ascontiguousarray(d["X2c"], np.float32).reshape(-1, 3),
+                     obs1=np.ascontiguousarray(d["obs1"], np.float32).reshape(-1, 2),
+                     obs2=np.ascontiguousarray(d["obs2"], np.float32).reshape(-1, 2),
+                     inv_sigma2_1=np.ascontiguousarray(d["inv_sigma2_1"], np.float32).reshape(-1),
+                     inv_sigma2_2=np.ascontiguousarray(d["inv_sigma2_2"], np.float32).reshape(-1))
+            keep.append(a)
+            n = len(a["X1c"])
+            P = probs[i]
+            P.n = n
+            for k in a:
+                setattr(P, k, a[k].ctypes.data)
+            for k, v in zip(("fx1", "fy1", "cx1", "cy1"), d["K1"]):
+                setattr(P, k, float(v))
+            for k, v in zip(("fx2", "fy2", "cx2", "cy2"), d["K2"]):
+                setattr(P, k, float(v))
+            P.S12.v[:] = [float(v) for v in np.asarray(d["S12"], np.float64).reshape(8)]
+            P.th2 = float(d["th2"])
+            P.fix_scale = int(bool(d["fix_scale"]))
+            out = dict(keep=np.zeros(n, np.uint8), trace=np.full(256, -1, np.int32))
+            outs.append(out)
+            res[i].keep = out["keep"].ctypes.data
+            res[i].trace = out["trace"].ctypes.data
+        _check(lib().b2s_optimize_sim3(self._h, len(ds), probs, res))
+        for i, out in enumerate(outs):
+            out["S12"] = np.array(res[i].S12_out.v[:], np.float64)
+            out["n_inliers"] = res[i].n_inliers
+            out["n_trials"] = res[i].n_trials
+        return outs

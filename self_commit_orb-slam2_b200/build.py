@@ -17,7 +17,7 @@ GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 NVCC_FLAGS = GENCODE + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-O3"]
 # extractor/matcher/keyframe database: bit-exact float arithmetic, never contract a*b+c; LocalBA is FP64 with a 1e-5 bar
 # -> FMA allowed; the essential graph differentiates numerically (delta = 1e-9 amplifies last-bit differences ~5e8 times)
-NO_FMAD = {"extractor.cu", "extractor_tile.cu", "matcher.cu", "common.cu", "kfdb.cu", "essential.cu"}
+NO_FMAD = {"extractor.cu", "extractor_tile.cu", "matcher.cu", "common.cu", "kfdb.cu", "essential.cu", "sim3opt.cu"}
 
 
 def _newer(target, sources):
@@ -38,9 +38,11 @@ def _deps_of(src):
     deps = [src, os.path.join(CSRC, "common.cuh"), os.path.join(ROOT, "include", "b200slam.h"), os.path.abspath(__file__)]
     if base.startswith("extractor"):
         deps.append(os.path.join(CSRC, "extractor.cuh"))
-    if base in ("localba.cu", "gba.cu", "essential.cu"):
+    if base in ("localba.cu", "gba.cu", "essential.cu", "sim3opt.cu"):
         deps.append(os.path.join(CSRC, "ba_math.cuh"))
         deps.append(os.path.join(CSRC, "levenberg.cuh"))
+    if base in ("essential.cu", "sim3opt.cu"):
+        deps.append(os.path.join(CSRC, "sim3.cuh"))
     if base in ("gba.cu", "essential.cu"):
         deps.append(os.path.join(CSRC, "chol.cuh"))
     if base == "extractor.cu":
@@ -86,6 +88,9 @@ def build_oracle(force=False):
     # the essential graph's CPU restatement (oracle/essential.mk)
     subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "essential.mk"] + (["-B"] if force else []) +
                           ["liborb_essential.so"])
+    # OptimizeSim3's CPU restatement (oracle/sim3opt.mk)
+    subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "sim3opt.mk"] + (["-B"] if force else []) +
+                          ["liborb_sim3opt.so"])
     return ORACLE_LIB
 
 
@@ -100,6 +105,7 @@ def build_oracle_ref():
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "kfdb.mk", "ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "gba.mk", "gba-ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "essential.mk", "essential-ref", "REF=" + ref])
+    subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "sim3opt.mk", "sim3opt-ref", "REF=" + ref])
     return os.path.join(ORACLE_DIR, "_ref")
 
 

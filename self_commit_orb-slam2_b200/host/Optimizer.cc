@@ -177,4 +177,44 @@ void Optimizer::OptimizeEssentialGraph(const EssentialGraph& g, EssentialGraphRe
   out.points.resize((size_t)nMP * 3);
 }
 
+// OptimizeSim3 runs on LoopClosing's thread: its own handle, grown on demand
+static b2s_sim3opt_solver* g_s3Solver = nullptr;
+static int g_s3n = 0;
+static std::mutex g_s3Mutex;
+
+int Optimizer::OptimizeSim3(const Sim3Problem& p, Sim3Result& out) {
+  std::lock_guard<std::mutex> lock(g_s3Mutex);
+  const int n = (int)p.invSigma2_1.size();
+  if (!g_s3Solver || n > g_s3n) {
+    b2s_sim3opt_destroy(g_s3Solver);
+    g_s3Solver = nullptr;
+    g_s3n = n > 4096 ? n : 4096;
+    const char* e = getenv("B2S_DEVICE");
+    int rc = b2s_sim3opt_create(g_s3n, 1, e ? atoi(e) : 0, &g_s3Solver);
+    if (rc != B2S_OK) {
+      fprintf(stderr, "Optimizer::OptimizeSim3: libb200slam error %d: %s\n", rc, b2s_last_error());
+      throw std::runtime_error(b2s_last_error());
+    }
+  }
+  b2s_sim3_problem q;
+  q.n = n;
+  q.X1c = p.X1c.data(); q.X2c = p.X2c.data(); q.obs1 = p.obs1.data(); q.obs2 = p.obs2.data();
+  q.inv_sigma2_1 = p.invSigma2_1.data(); q.inv_sigma2_2 = p.invSigma2_2.data();
+  q.fx1 = p.K1[0]; q.fy1 = p.K1[1]; q.cx1 = p.K1[2]; q.cy1 = p.K1[3];
+  q.fx2 = p.K2[0]; q.fy2 = p.K2[1]; q.cx2 = p.K2[2]; q.cy2 = p.K2[3];
+  q.S12 = p.S12; q.th2 = p.th2; q.fix_scale = p.fixScale ? 1 : 0;
+  out.keep.assign((size_t)(n > 0 ? n : 1), 0);
+  b2s_sim3_result r;
+  r.keep = out.keep.data(); r.trace = nullptr; r.n_inliers = r.n_trials = 0;
+  int rc = b2s_optimize_sim3(g_s3Solver, 1, &q, &r);
+  if (rc != B2S_OK) {
+    fprintf(stderr, "Optimizer::OptimizeSim3: libb200slam error %d: %s\n", rc, b2s_last_error());
+    throw std::runtime_error(b2s_last_error());
+  }
+  out.keep.resize((size_t)n);
+  out.S12 = r.S12_out;
+  out.nInliers = r.n_inliers;
+  return r.n_inliers;
+}
+
 }  // namespace ORB_SLAM2

@@ -63,6 +63,22 @@ struct EssentialGraphResult {
   std::vector<float> points;         // nMP x 3  -> SetWorldPos + UpdateNormalAndDepth
 };
 
+struct Sim3Problem {                 // Optimizer::OptimizeSim3 on the gathered correspondences (src/Optimizer.cc:1429-1520)
+  std::vector<float> X1c, X2c;       // n x 3: R1w*P3D1w + t1w, R2w*P3D2w + t2w as the cv::Mat expression gives them
+  std::vector<float> obs1, obs2;     // n x 2: mvKeysUn[i] of pKF1, mvKeysUn[i2] of pKF2
+  std::vector<float> invSigma2_1, invSigma2_2;  // n: mvInvLevelSigma2 at the keypoints' octaves
+  float K1[4], K2[4];                // fx fy cx cy
+  b2s_sim3 S12;                      // g2oS12
+  float th2 = 10.f;
+  bool fixScale = false;
+};
+
+struct Sim3Result {
+  b2s_sim3 S12;                      // -> g2oS12 (the input itself after the early return)
+  std::vector<uint8_t> keep;         // n: 0 -> vpMatches1[vnIndexEdge[k]] = NULL
+  int nInliers = 0;                  // the return value
+};
+
 class Optimizer {
  public:
   // int static PoseOptimization(Frame* pFrame) (include/Optimizer.h:100, src/Optimizer.cc:363-605): fills TcwOut (the
@@ -75,6 +91,8 @@ class Optimizer {
   // void static OptimizeEssentialGraph(pMap, pLoopKF, pCurKF, NonCorrectedSim3, CorrectedSim3, LoopConnections,
   // bFixScale) on the gathered graph
   static void OptimizeEssentialGraph(const EssentialGraph& g, EssentialGraphResult& out);
+  // int static OptimizeSim3(pKF1, pKF2, vpMatches1, g2oS12, th2, bFixScale) on the gathered correspondences
+  static int OptimizeSim3(const Sim3Problem& p, Sim3Result& out);
 };
 
 }  // namespace ORB_SLAM2

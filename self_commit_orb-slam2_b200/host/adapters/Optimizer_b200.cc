@@ -7,11 +7,13 @@
 //     void Optimizer::OptimizeEssentialGraph(Map*, KeyFrame*, KeyFrame*, const KeyFrameAndPose&,
 //                                            const KeyFrameAndPose&, const map<KeyFrame*, set<KeyFrame*>>&,
 //                                            const bool&)                                src/Optimizer.cc:1017
+//     int  Optimizer::OptimizeSim3(KeyFrame*, KeyFrame*, vector<MapPoint*>&, g2o::Sim3&, const float, const bool)
+//                                                                                         src/Optimizer.cc:1364
 // with the reference's exact signatures, for the LocalMapping / Tracking / LoopClosing threads to call unchanged
-// (src/LocalMapping.cc:123, src/Tracking.cc:1081, 1219, 1398, 1834, 2078, 2152, src/LoopClosing.cc:782, 880-895 ...).
+// (src/LocalMapping.cc:123, src/Tracking.cc:1081, 1219, 1398, 1834, 2078, 2152, src/LoopClosing.cc:460, 782, 880-895 ...).
 // Compile this file INSIDE the reference tree (it includes the reference's own include/Optimizer.h) in place of those
-// function bodies of src/Optimizer.cc (:55-341, :363-605, :629-997, :1017-1339) and link libb200slam.so; OptimizeSim3
-// stays as it is.
+// function bodies of src/Optimizer.cc (:55-341, :363-605, :629-997, :1017-1339, :1364-1590), that is every body of that
+// file, and link libb200slam.so.
 //
 // What stays on the host is what touches the object graph: the window selection (local keyframes = pKF + covisibles,
 // local map points = their matches, fixed cameras = other observers; the mnBALocalForKF / mnBAFixedForKF marks other
@@ -112,6 +114,26 @@ struct EgSlot {
   }
 };
 EgSlot g_eg;
+
+// OptimizeSim3's handle (LoopClosing::ComputeSim3), one problem per call, grown on demand.
+struct Sim3Slot {
+  b2s_sim3opt_solver* h = nullptr;
+  int n = 0;
+  std::mutex m;
+  b2s_sim3opt_solver* get(int nMatches) {
+    if (h && nMatches <= n) return h;
+    b2s_sim3opt_destroy(h);
+    h = nullptr;
+    n = nMatches > 4096 ? nMatches : 4096;
+    if (b2s_sim3opt_create(n, 1, device_index(), &h) != B2S_OK) {
+      fprintf(stderr, "Optimizer (b200): %s\n", b2s_last_error());
+      h = nullptr;
+      n = 0;
+    }
+    return h;
+  }
+};
+Sim3Slot g_sim3;
 
 b2s_sim3 to_b2s(const g2o::Sim3& S) {
   b2s_sim3 o;
@@ -610,6 +632,84 @@ void Optimizer::OptimizeEssentialGraph(Map* pMap, KeyFrame* pLoopKF, KeyFrame* p
     mps[(size_t)m]->SetWorldPos(X);
     mps[(size_t)m]->UpdateNormalAndDepth();
   }
+}
+
+int Optimizer::OptimizeSim3(KeyFrame* pKF1, KeyFrame* pKF2, vector<MapPoint*>& vpMatches1, g2o::Sim3& g2oS12,
+                            const float th2, const bool bFixScale) {
+  const cv::Mat& K1 = pKF1->mK;
+  const cv::Mat& K2 = pKF2->mK;
+  const cv::Mat R1w = pKF1->GetRotation();
+  const cv::Mat t1w = pKF1->GetTranslation();
+  const cv::Mat R2w = pKF2->GetRotation();
+  const cv::Mat t2w = pKF2->GetTranslation();
+
+  // ---- gather (:1429-1520): the reference's skip rules in its order; the camera-frame points by its cv::Mat expression
+  const int N = (int)vpMatches1.size();
+  const std::vector<MapPoint*> vpMapPoints1 = pKF1->GetMapPointMatches();
+  std::vector<size_t> vnIndexEdge;
+  std::vector<float> X1c, X2c, obs1, obs2, is1, is2;
+  for (int i = 0; i < N; i++) {
+    if (!vpMatches1[i]) continue;
+    MapPoint* pMP1 = vpMapPoints1[i];
+    MapPoint* pMP2 = vpMatches1[i];
+    const int i2 = pMP2->GetIndexInKeyFrame(pKF2);
+    if (!pMP1 || !pMP2 || pMP1->isBad() || pMP2->isBad() || i2 < 0) continue;
+    const cv::Mat P3D1c = R1w * pMP1->GetWorldPos() + t1w;
+    const cv::Mat P3D2c = R2w * pMP2->GetWorldPos() + t2w;
+    for (int c = 0; c < 3; c++) {
+      X1c.push_back(P3D1c.at<float>(c));
+      X2c.push_back(P3D2c.at<float>(c));
+    }
+    const cv::KeyPoint& kpUn1 = pKF1->mvKeysUn[i];
+    const cv::KeyPoint& kpUn2 = pKF2->mvKeysUn[i2];
+    obs1.push_back(kpUn1.pt.x);
+    obs1.push_back(kpUn1.pt.y);
+    obs2.push_back(kpUn2.pt.x);
+    obs2.push_back(kpUn2.pt.y);
+    is1.push_back(pKF1->mvInvLevelSigma2[kpUn1.octave]);
+    is2.push_back(pKF2->mvInvLevelSigma2[kpUn2.octave]);
+    vnIndexEdge.push_back((size_t)i);
+  }
+  const int n = (int)vnIndexEdge.size();
+  b2s_sim3_problem prob;
+  prob.n = n;
+  prob.X1c = X1c.data();
+  prob.X2c = X2c.data();
+  prob.obs1 = obs1.data();
+  prob.obs2 = obs2.data();
+  prob.inv_sigma2_1 = is1.data();
+  prob.inv_sigma2_2 = is2.data();
+  prob.fx1 = K1.at<float>(0, 0);
+  prob.fy1 = K1.at<float>(1, 1);
+  prob.cx1 = K1.at<float>(0, 2);
+  prob.cy1 = K1.at<float>(1, 2);
+  prob.fx2 = K2.at<float>(0, 0);
+  prob.fy2 = K2.at<float>(1, 1);
+  prob.cx2 = K2.at<float>(0, 2);
+  prob.cy2 = K2.at<float>(1, 2);
+  prob.S12 = to_b2s(g2oS12);
+  prob.th2 = th2;
+  prob.fix_scale = bFixScale ? 1 : 0;
+  std::vector<uint8_t> keep((size_t)(n > 0 ? n : 1));
+  b2s_sim3_result res;
+  res.keep = keep.data();
+  res.trace = nullptr;
+  res.n_inliers = res.n_trials = 0;
+  {
+    std::lock_guard<std::mutex> lock(g_sim3.m);
+    b2s_sim3opt_solver* solver = g_sim3.get(n);
+    if (!solver) return 0;
+    if (b2s_optimize_sim3(solver, 1, &prob, &res) != B2S_OK) {
+      fprintf(stderr, "Optimizer::OptimizeSim3 (b200): %s\n", b2s_last_error());
+      return 0;
+    }
+  }
+
+  // ---- scatter: null the rejected matches; g2oS12 (S12_out is the input itself after the early return, :1549-1551)
+  for (int k = 0; k < n; k++)
+    if (!keep[(size_t)k]) vpMatches1[vnIndexEdge[(size_t)k]] = static_cast<MapPoint*>(NULL);
+  for (int i = 0; i < 8; i++) g2oS12[i] = (&res.S12_out.q[0])[i];
+  return res.n_inliers;
 }
 
 }  // namespace ORB_SLAM2
