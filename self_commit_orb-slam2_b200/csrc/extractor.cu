@@ -1,5 +1,6 @@
-// extractor.cu — H100 (sm_90a) ORB extractor: pyramid, per-cell FAST-9/16 + NMS + dual threshold, parallel
-// order-preserving quadtree, intensity-centroid orientation, Q8 Gaussian blur, steered rBRIEF.
+// extractor.cu — H100 (sm_90a) ORB extractor: per-cell minThFAST fallback, parallel order-preserving quadtree,
+// intensity-centroid orientation, steered rBRIEF and the host side (pyramid, FAST strength and Q8 Gaussian blur are the
+// fused front end of extractor_tile.cu).
 //
 // Replaces the body of ORBextractor::operator() (/root/reference/src/ORBextractor.cc:1544-1668) and the OpenCV
 // primitives it calls.  Every stage is integer- or explicitly-rounded-float arithmetic so results are bit-identical
@@ -21,47 +22,9 @@ __constant__ int8_t c_pattern[1024];
 __constant__ int c_umax[16];
 
 // ------------------------------------------------------------------------------------------------
-// K1: pyramid level l from level l-1 — cv::resize INTER_LINEAR u8 fixed-point recipe (SURVEY §8c),
-//     called at src/ORBextractor.cc:1696.  Tables are built on the host with the same float arithmetic.
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) k_resize(ExtractGeom g, int l, uint8_t* __restrict__ pyr,
-                                                const int16_t* __restrict__ rxOfs, const uint32_t* __restrict__ rxAlpha,
-                                                const int16_t* __restrict__ ryOfs, const uint32_t* __restrict__ ryBeta) {
-  // four destination pixels per thread: one 8-byte + one 16-byte table load, one 32-bit store (the x tables of every
-  // level are padded to a multiple of 4 entries; rows are padded to 16 bytes, padding bytes are written as 0)
-  const LevelGeom& S = g.lv[l - 1];
-  const LevelGeom& D = g.lv[l];
-  const int x0 = (blockIdx.x * 32 + threadIdx.x) * 4;  // block = 32 x 4 threads = 128 pixels x 4 rows
-  const int y = blockIdx.y * 4 + threadIdx.y;
-  if (x0 >= D.w || y >= D.h) return;
-  const uint8_t* src = pyr + (size_t)blockIdx.z * g.pyrBytes + S.off;
-  uint8_t* dst = pyr + (size_t)blockIdx.z * g.pyrBytes + D.off;
-  const int sy = ryOfs[D.ryOff + y];
-  const uint32_t bb = ryBeta[D.ryOff + y];
-  const int b0 = (int16_t)(bb & 0xffffu), b1 = (int16_t)(bb >> 16);
-  const int sy0 = min(max(sy, 0), S.h - 1), sy1 = min(max(sy + 1, 0), S.h - 1);
-  const uint8_t* r0 = src + (size_t)sy0 * S.pitch;
-  const uint8_t* r1 = src + (size_t)sy1 * S.pitch;
-  const short4 sx4 = *reinterpret_cast<const short4*>(rxOfs + D.rxOff + x0);
-  const uint4 aa4 = *reinterpret_cast<const uint4*>(rxAlpha + D.rxOff + x0);
-  const int sxs[4] = {sx4.x, sx4.y, sx4.z, sx4.w};
-  const uint32_t aas[4] = {aa4.x, aa4.y, aa4.z, aa4.w};
-  uint32_t word = 0;
-#pragma unroll
-  for (int i = 0; i < 4; i++) {
-    const int sx = sxs[i], sx1 = min(sx + 1, S.w - 1);
-    const int a0 = (int16_t)(aas[i] & 0xffffu), a1 = (int16_t)(aas[i] >> 16);
-    const int h0 = r0[sx] * a0 + r0[sx1] * a1;
-    const int h1 = r1[sx] * a0 + r1[sx1] * a1;
-    const uint32_t v = (uint32_t)(uint8_t)((((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2);
-    if (x0 + i < D.w) word |= v << (8 * i);
-  }
-  *reinterpret_cast<uint32_t*>(dst + (size_t)y * D.pitch + x0) = word;
-}
-
-// ------------------------------------------------------------------------------------------------
-// K2: per-cell FAST-9/16 score + 3x3 NMS + ini->min threshold fallback.
-//     One CTA per 30-px cell of src/ORBextractor.cc:1089-1157 (cv::FAST on the cell ROI, :1126,1135).
+// K2: the minThFAST pass of the cells that the fused front end (extractor_tile.cu) found without a maximum above
+//     iniThFAST: per listed 30-px cell of src/ORBextractor.cc:1089-1157 (cv::FAST on the cell ROI, :1126,1135) one CTA
+//     computes the FAST-9/16 score, the 3x3 NMS and the ini->min threshold rule.
 //     M = max over the 16 arcs of min|v-p| (same sign); corner at th <=> M > th; response = M-1.
 // ------------------------------------------------------------------------------------------------
 constexpr int FP = 80;   // byte pitch of the raw ROI / score map (ROI width <= 66, + alignment slack)
@@ -337,15 +300,6 @@ __device__ __forceinline__ void fast_cell(const ExtractGeom& g, const uint8_t* _
     candKey[cbase + slot] = ((uint32_t)c << 12) | ((uint32_t)(y - 3) << 6) | (uint32_t)(x - 3);
     candResp[cbase + slot] = (uint8_t)(M - 1);
   }
-}
-
-// every cell of every image (the per-stage path, B2S_EXTRACT_PATH=0)
-__global__ void __launch_bounds__(128) k_fast_cells(ExtractGeom g, const uint8_t* __restrict__ pyr,
-                                                    const uint32_t* __restrict__ cellInfo,
-                                                    uint32_t* __restrict__ candXY, uint32_t* __restrict__ candKey,
-                                                    uint8_t* __restrict__ candResp, int32_t* __restrict__ candCount,
-                                                    int32_t* __restrict__ status) {
-  fast_cell(g, pyr, cellInfo, candXY, candKey, candResp, candCount, status, blockIdx.y, blockIdx.x);
 }
 
 // the fused front end's minThFAST fallback: only the cells listed by k_cells (those without a maximum above iniThFAST,
@@ -727,113 +681,6 @@ __global__ void __launch_bounds__(256) k_quadtree(ExtractGeom g, int capMax, con
 }
 
 // ------------------------------------------------------------------------------------------------
-// K5a: GaussianBlur 7x7 sigma 2, BORDER_REFLECT_101, OpenCV-4 fixed point (Q8 taps, one final rounding).
-//      src/ORBextractor.cc:1626-1634.  Each lane owns 4 consecutive columns and marches down a 32-row strip:
-//      one coalesced 32-bit load per input row (+2 shuffles for the neighbours' words), the horizontal 7 taps are
-//      two DP4A per pixel on byte-aligned windows (PRMT), the vertical 7 taps run on a register window of the last
-//      7 horizontal sums, and every output row is one coalesced 32-bit store per lane.
-// ------------------------------------------------------------------------------------------------
-constexpr int BL_ROWS = 32;        // output rows per warp strip
-constexpr int BL_COLS = 128;       // columns per warp (32 lanes x 4)
-__device__ __forceinline__ int reflect101(int p, int n) {
-  if (n == 1) return 0;
-  while (p < 0 || p >= n) p = (p < 0) ? -p : 2 * (n - 1) - p;
-  return p;
-}
-
-__global__ void __launch_bounds__(128) k_blur(ExtractGeom g, const uint8_t* __restrict__ pyr, uint8_t* __restrict__ blur) {
-  const int b = blockIdx.y;
-  int l = 0;
-  while (l + 1 < g.nlevels && (int)blockIdx.x >= g.lv[l + 1].blurTileStart) l++;
-  const LevelGeom& L = g.lv[l];
-  const int lane = threadIdx.x & 31;
-  const int task = (blockIdx.x - L.blurTileStart) * 4 + (threadIdx.x >> 5);
-  if (task >= L.blurTilesX * L.blurTilesY) return;
-  const int ty = task / L.blurTilesX, tx = task - ty * L.blurTilesX;
-  const int x0 = tx * BL_COLS + lane * 4, oy = ty * BL_ROWS;
-  const uint8_t* src = pyr + (size_t)b * g.pyrBytes + L.off;
-  uint8_t* dst = blur + (size_t)b * g.pyrBytes + L.off;
-  const int Wd = L.w, Hd = L.h;
-  const bool laneIn = x0 < L.pitch;  // this lane's own word exists in the padded row
-  int hw[7][4];
-  // left / right border handling without per-byte loops: reflect101 of the 12-byte window x0-4 .. x0+7
-  const bool leftEdge = (x0 == 0);
-  const int nValid = Wd - x0;                  // pixels of this lane's window that exist, counted from x0
-  const bool rightEdge = laneIn && (nValid < 8) && (x0 < Wd);  // x0+7 >= Wd : some of bytes 4..11 are beyond the image
-  const int pitch = L.pitch;
-  const uint8_t* colBase = src + x0;
-  // lanes 0 and 31 fetch the word left / right of the warp's 128-byte span (one predicated load, no branches)
-  const bool wantExtra = (lane == 0 && x0 >= 4) || (lane == 31 && x0 + 4 < pitch);
-  const int extraOff = (lane == 0) ? -4 : 4;
-#pragma unroll 1
-  for (int i0 = 0; i0 < BL_ROWS + 6; i0 += 7) {
-    // the seven row loads of the body are issued together (one exposed memory latency per seven rows)
-    uint32_t w1v[7], exv[7];
-    int syv[7];
-#pragma unroll
-    for (int u = 0; u < 7; u++) {
-      int sy = oy - 3 + i0 + u;
-      if (Hd >= 8) {  // (uniform) one reflection is enough
-        sy = sy < 0 ? -sy : sy;
-        sy = sy >= Hd ? 2 * (Hd - 1) - sy : sy;
-      } else {
-        sy = reflect101(sy, Hd);
-      }
-      sy = min(max(sy, 0), Hd - 1);  // rows of a partial last tile that are never stored
-      syv[u] = sy;
-      const uint8_t* rp = colBase + (size_t)sy * pitch;
-      w1v[u] = laneIn ? __ldg(reinterpret_cast<const uint32_t*>(rp)) : 0u;
-      exv[u] = wantExtra ? __ldg(reinterpret_cast<const uint32_t*>(rp + extraOff)) : 0u;
-    }
-#pragma unroll
-    for (int u = 0; u < 7; u++) {
-      const int i = i0 + u;
-      if (i < BL_ROWS + 6) {  // warp-uniform
-        uint32_t w1 = w1v[u];
-        uint32_t w0 = __shfl_up_sync(0xffffffffu, w1, 1);
-        uint32_t w2 = __shfl_down_sync(0xffffffffu, w1, 1);
-        if (lane == 0) w0 = exv[u];
-        if (lane == 31) w2 = exv[u];
-        if (leftEdge) w0 = __byte_perm(w1, w2, 0x1234);  // pixels 4,3,2,1 (reflect101 of -4..-1)
-        if (rightEdge) {                                   // few lanes per row: rebuild bytes 4..11 by reflection
-          const uint8_t* row = src + (size_t)syv[u] * pitch;
-          uint32_t ww1 = 0u, ww2 = 0u;
-#pragma unroll
-          for (int k = 0; k < 4; k++) {
-            int px = x0 + k;
-            px = (px >= Wd) ? 2 * (Wd - 1) - px : px;
-            ww1 |= (uint32_t)row[px] << (8 * k);
-            int px2 = x0 + 4 + k;
-            px2 = (px2 >= Wd) ? 2 * (Wd - 1) - px2 : px2;
-            ww2 |= (uint32_t)row[px2] << (8 * k);
-          }
-          w1 = ww1;
-          w2 = ww2;
-        }
-        const uint32_t KA = 0x38302212u, KB = 0x00122230u;  // taps (18,34,48,56) and (48,34,18,0)
-        hw[u][0] = (int)__dp4a(__byte_perm(w1, w2, 0x4321), KB, __dp4a(__byte_perm(w0, w1, 0x4321), KA, 0u));
-        hw[u][1] = (int)__dp4a(__byte_perm(w1, w2, 0x5432), KB, __dp4a(__byte_perm(w0, w1, 0x5432), KA, 0u));
-        hw[u][2] = (int)__dp4a(__byte_perm(w1, w2, 0x6543), KB, __dp4a(__byte_perm(w0, w1, 0x6543), KA, 0u));
-        hw[u][3] = (int)__dp4a(w2, KB, __dp4a(w1, KA, 0u));
-        if (i >= 6) {
-          const int y = oy + i - 6;
-          uint32_t outw = 0;
-#pragma unroll
-          for (int j = 0; j < 4; j++) {
-            // the window holds rows i-6..i at slots (u+1)%7 .. u
-            const int q0 = hw[(u + 1) % 7][j], q1 = hw[(u + 2) % 7][j], q2 = hw[(u + 3) % 7][j], q3 = hw[(u + 4) % 7][j],
-                      q4 = hw[(u + 5) % 7][j], q5 = hw[(u + 6) % 7][j], q6 = hw[u][j];
-            const uint32_t acc = 18u * (uint32_t)(q0 + q6) + 34u * (uint32_t)(q1 + q5) + 48u * (uint32_t)(q2 + q4) + 56u * (uint32_t)q3;
-            outw |= ((acc + 32768u) >> 16) << (8 * j);
-          }
-          if (y < Hd && x0 < Wd) *reinterpret_cast<uint32_t*>(dst + (size_t)y * pitch + x0) = outw;
-        }
-      }
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
 // K4+K5b: IC_Angle (:108-161) + cv::fastAtan2 (:160) + computeOrbDescriptor (:173-227), one warp per keypoint.
 //      cosf/sinf restate glibc 2.39's FMA sincosf kernels operation by operation (DESIGN.md "float trig");
 //      tap coordinates use unfused float mul/add and round-half-even, like the oracle's -ffp-contract=off build.
@@ -1056,7 +903,7 @@ static int build_geometry(b2s_extractor* h, int W, int H) {
   g.iniTh = h->iniTh;
   g.minTh = h->minTh;
   uint32_t off = 0;
-  int cellStart = 0, candOff = 0, selOff = 0, tileStart = 0;
+  int cellStart = 0, candOff = 0, selOff = 0;
   uint32_t rxOff = 0, ryOff = 0;
   std::vector<int16_t> rxOfs, ryOfs;
   std::vector<uint32_t> rxAlpha, ryBeta;
@@ -1100,10 +947,6 @@ static int build_geometry(b2s_extractor* h, int W, int H) {
     selOff += L.nodeCap;
     L.scale = h->scale[l];
     L.kpsize = (float)(int)(kPatch * h->scale[l]);
-    L.blurTileStart = tileStart;
-    L.blurTilesX = div_up(L.w, BL_COLS);  // warp tasks: 128 columns x 32 rows each, 4 per CTA
-    L.blurTilesY = div_up(L.h, BL_ROWS);
-    tileStart += div_up(L.blurTilesX * L.blurTilesY, 4);
     L.rxOff = rxOff;
     L.ryOff = ryOff;
     if (l > 0) {
@@ -1127,11 +970,7 @@ static int build_geometry(b2s_extractor* h, int W, int H) {
         const int16_t b0 = (int16_t)cv_roundf((1.f - fy) * 2048.f), b1 = (int16_t)cv_roundf(fy * 2048.f);
         ryBeta.push_back((uint32_t)(uint16_t)b0 | ((uint32_t)(uint16_t)b1 << 16));
       }
-      for (int dx = L.w; dx & 3; dx++) {  // pad to 4 entries (k_resize loads the x tables four at a time)
-        rxOfs.push_back(rxOfs.back());
-        rxAlpha.push_back(rxAlpha.back());
-      }
-      rxOff += (uint32_t)align_up((size_t)L.w, 4);
+      rxOff += L.w;
       ryOff += L.h;
     }
   }
@@ -1151,7 +990,6 @@ static int build_geometry(b2s_extractor* h, int W, int H) {
   }
   g.totalCandCap = candOff;
   g.totalSelCap = selOff;
-  g.totalBlurTiles = tileStart;
   if (g.pyrBytes > h->pyrBytesAlloc || (size_t)g.totalCandCap > h->candCapAlloc || (size_t)g.totalSelCap > h->selCapAlloc ||
       rxOfs.size() > h->rxAlloc || ryOfs.size() > h->ryAlloc) {
     set_error("image %dx%d exceeds the extractor's max_width/max_height (%dx%d)", W, H, h->maxW, h->maxH);
@@ -1253,44 +1091,24 @@ static int run_pipeline(b2s_extractor* h, const DeviceBuffers& d, int batch, b2s
     if (h->evPending) b2s_extractor_timing_collect(h);
     cudaEventRecord(h->ev[0], st);
   }
-  const int path = h->path;
-  if (path < 3) {
-    for (int l = 1; l < g.nlevels; l++) {
-      dim3 grid(div_up(g.lv[l].w, 128), div_up(g.lv[l].h, 4), batch);
-      k_resize<<<grid, dim3(32, 4), 0, st>>>(g, l, d.pyr, d.rxOfs, d.rxAlpha, d.ryOfs, d.ryBeta);
-      h->launches++;
-    }
-  }
+  // fused front end: per level one tile kernel (TMA-staged tile -> FAST strength map, blur, level l+1), then the per-cell
+  // NMS / threshold rules.  `d` may be a slice of the handle's buffers: pass its image offset.
+  const int bBase = (int)((size_t)(d.pyr - h->d.pyr) / g.pyrBytes);
+  const int rc = tile_run(h, bBase, batch, st);
+  if (rc != B2S_OK) return rc;
   if (tm) cudaEventRecord(h->ev[1], st);
-  if (path == 0) {
-    k_fast_cells<<<dim3(g.totalCells, batch), 128, 0, st>>>(g, d.pyr, d.cellInfo, d.candXY, d.candKey, d.candResp, d.candCount,
-                                                            d.status);
-    h->launches++;
-  } else {
-    // fused front end: per level one tile kernel (TMA-staged tile -> FAST strength map [+ blur] [+ level l+1]), then the
-    // per-cell NMS / threshold rules.  `d` may be a slice of the handle's buffers: pass its image offset.
-    const int bBase = (int)((size_t)(d.pyr - h->d.pyr) / g.pyrBytes);
-    const int rc = tile_run(h, bBase, batch, path, st, nullptr);
-    if (rc != B2S_OK) return rc;
-  }
-  if (tm) cudaEventRecord(h->ev[2], st);
   int capMax = 0;
   for (int l = 0; l < g.nlevels; l++) capMax = std::max(capMax, g.lv[l].nodeCap);
   const size_t qsm = quadtree_smem_bytes(capMax);
   k_quadtree<<<dim3(g.nlevels, batch), 256, qsm, st>>>(g, capMax, d.candXY, d.candKey, d.candResp, d.candNode, d.candQ,
                                                        d.candCount, d.selXYR, d.selCount, d.status);
   h->launches++;
-  if (tm) cudaEventRecord(h->ev[3], st);
-  if (path < 2) {
-    k_blur<<<dim3(g.totalBlurTiles, batch), 128, 0, st>>>(g, d.pyr, d.blur);
-    h->launches++;
-  }
-  if (tm) cudaEventRecord(h->ev[4], st);
+  if (tm) cudaEventRecord(h->ev[2], st);
   k_orient_describe<<<dim3(div_up(g.totalSelCap, 8), batch), 256, 0, st>>>(g, d.pyr, d.blur, d.selXYR, d.selCount, dKps,
                                                                            dDesc, dCounts, cap, d.status);
   h->launches++;
   if (tm) {
-    cudaEventRecord(h->ev[5], st);
+    cudaEventRecord(h->ev[3], st);
     h->evPending = 1;
   }
   B2S_CUDA(cudaGetLastError());
@@ -1299,10 +1117,11 @@ static int run_pipeline(b2s_extractor* h, const DeviceBuffers& d, int batch, b2s
 
 static void b2s_extractor_timing_collect(b2s_extractor* h) {
   if (!h->evPending) return;
-  if (cudaEventSynchronize(h->ev[5]) != cudaSuccess) return;
-  for (int k = 0; k < 5; k++) {
+  static const int kSlot[3] = {1, 2, 4};  // stage slot of the span ev[k] -> ev[k + 1]: tiles + cells, quadtree, describe
+  if (cudaEventSynchronize(h->ev[3]) != cudaSuccess) return;
+  for (int k = 0; k < 3; k++) {
     float ms = 0;
-    if (cudaEventElapsedTime(&ms, h->ev[k], h->ev[k + 1]) == cudaSuccess) h->stageMs[k] += ms;
+    if (cudaEventElapsedTime(&ms, h->ev[k], h->ev[k + 1]) == cudaSuccess) h->stageMs[kSlot[k]] += ms;
   }
   h->timedCalls++;
   h->evPending = 0;
@@ -1539,7 +1358,7 @@ extern "C" int b2s_extractor_set_timing(b2s_extractor* h, int enable) {
   if (!h) return B2S_ERR_BAD_ARG;
   B2S_CUDA(cudaSetDevice(h->device));
   if (enable && !h->ev[0])
-    for (int k = 0; k < 6; k++) B2S_CUDA(cudaEventCreate(&h->ev[k]));
+    for (int k = 0; k < 4; k++) B2S_CUDA(cudaEventCreate(&h->ev[k]));
   b2s_extractor_timing_collect(h);
   h->timing = enable;
   for (int k = 0; k < 5; k++) h->stageMs[k] = 0;
@@ -1547,7 +1366,8 @@ extern "C" int b2s_extractor_set_timing(b2s_extractor* h, int enable) {
   return B2S_OK;
 }
 
-/* accumulated device milliseconds per stage since set_timing(1): resize chain, FAST, quadtree, blur, orient+describe */
+/* accumulated device milliseconds per stage since set_timing(1): resize chain, FAST, quadtree, blur, orient+describe;
+ * the resize chain and the blur run inside the tile kernels, whose time is slot 1, so slots 0 and 3 stay 0 */
 extern "C" int b2s_extractor_get_timing(b2s_extractor* h, double* stage_ms5, long long* calls) {
   if (!h || !stage_ms5) return B2S_ERR_BAD_ARG;
   B2S_CUDA(cudaSetDevice(h->device));
@@ -1587,7 +1407,6 @@ extern "C" int b2s_extractor_create(int nfeatures, float scaleFactor, int nlevel
   h->maxH = max_height;
   h->maxBatch = max_batch;
   h->device = device;
-  if (const char* pe = getenv("B2S_EXTRACT_PATH")) h->path = std::min(3, std::max(0, atoi(pe)));
   // scale tables and per-level quotas — src/ORBextractor.cc:500-554
   h->scale.resize(nlevels);
   h->sigma2.resize(nlevels);

@@ -26,7 +26,6 @@ struct LevelGeom {
   int nodeCap, selOff;    // quadtree node capacity / offset of the level's selected keypoints
   float scale;            // mvScaleFactor[level]
   float kpsize;           // (float)(int)(PATCH_SIZE*scale) (:1175,1189)
-  int blurTileStart, blurTilesX, blurTilesY;
   uint32_t rxOff, ryOff;  // resize tables (entries) for producing this level from level-1
   int tilesX, tilesY;     // 128 x 32 tiles of the fused front end (extractor_tile.cu)
   uint32_t tdxOff, tdyOff;  // per tile column / row: first level l+1 column / row whose source sample starts in it
@@ -36,7 +35,7 @@ struct LevelGeom {
 struct ExtractGeom {
   int nlevels;
   int iniTh, minTh;
-  int totalCells, totalCandCap, totalSelCap, totalBlurTiles;
+  int totalCells, totalCandCap, totalSelCap;
   uint32_t pyrBytes;  // bytes of one image's pyramid
   uint32_t bmWords;   // words of one image's NMS bitmap (fused front end)
   LevelGeom lv[kMaxLevels];
@@ -77,7 +76,7 @@ struct DeviceBuffers {
 struct b2s_extractor;
 namespace b2s {
 int tile_build(b2s_extractor* h);  // tensor maps + resize ownership tables for the current geometry
-int tile_run(b2s_extractor* h, int bBase, int batch, int path, cudaStream_t st, cudaEvent_t evAfterTiles);
+int tile_run(b2s_extractor* h, int bBase, int batch, cudaStream_t st);
 int launch_fast_fallback(const ExtractGeom& g, const DeviceBuffers& d, const uint2* fbList, const int32_t* fbCount, int gridCtas,
                          cudaStream_t st);  // extractor.cu
 }  // namespace b2s
@@ -108,15 +107,15 @@ struct b2s_extractor {
   int32_t* hCounts = nullptr;
   int32_t* hStatus = nullptr;
   long long launches = 0;
-  // fused front end (extractor_tile.cu): 0 = per-stage kernels, 1 = tile FAST, 2 = + blur, 3 = + pyramid (default)
-  int path = 3;
+  // fused front end (extractor_tile.cu)
   size_t tileTabAlloc = 0, bmWordsAlloc = 0;
   alignas(64) unsigned char tmPyr[b2s::kMaxLevels][128];    // CUtensorMap: level images (TMA load, 144 x 38 box)
   alignas(64) unsigned char tmScore[b2s::kMaxLevels][128];  // strength map (TMA store, 128 x 32 box)
   alignas(64) unsigned char tmBlur[b2s::kMaxLevels][128];   // blurred level (TMA store)
-  // optional per-stage CUDA-event timing (bench.py roofline): resize chain, FAST, quadtree, blur, describe
+  // optional per-stage CUDA-event timing (bench.py roofline): resize chain, FAST, quadtree, blur, describe; events
+  // around the tile front end, the quadtree and the description (resize chain and blur are part of the tile front end)
   int timing = 0;
-  cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
   double stageMs[5] = {0, 0, 0, 0, 0};
   long long timedCalls = 0;
   int evPending = 0;

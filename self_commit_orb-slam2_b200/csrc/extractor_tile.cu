@@ -10,8 +10,8 @@
 //
 // Replaces ComputePyramid (/root/reference/src/ORBextractor.cc:1674-1734), the cell loop + cv::FAST of
 // ComputeKeyPointsOctTree (:1060-1157) and the GaussianBlur of operator() (:1626-1634).  Bit-exact: the arithmetic is
-// the same integer recipe as the per-stage kernels in extractor.cu (which remain as the B2S_EXTRACT_PATH=0 fallback and
-// as the parity cross-check).
+// the integer recipe of cv::resize INTER_LINEAR, FAST and the Q8 GaussianBlur (SURVEY.md §8c), checked level by level
+// against the oracle (tests/test_extractor_gpu.py).
 #include <cuda.h>  // CUtensorMap (types only: the encoder is fetched through cudaGetDriverEntryPoint, libcuda is not linked)
 
 #include <algorithm>
@@ -93,7 +93,7 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* tm, uint32_t src
 }
 
 struct TileArgs {
-  int level, bBase, doFast, doBlur, doResize;
+  int level, bBase;
   uint8_t* pyr;  // base of the batch's pyramids (image 0 of the handle), for the level l+1 stores
   const int16_t* rxOfs;
   const uint32_t* rxAlpha;
@@ -204,7 +204,7 @@ __global__ void __launch_bounds__(TILE_THREADS) k_tile(const __grid_constant__ C
   const int Wd = L.w, Hd = L.h;
   const bool edgeX = (X0 + HX - 3 < 0) || (X0 + HX + TW + 3 > Wd);
   const bool edgeY = (Y0 + HY - 3 < 0) || (Y0 + HY + TH + 3 > Hd);
-  if (a.doBlur && (edgeX || edgeY)) {
+  if (edgeX || edgeY) {
     if (edgeX) {
       for (int k = tid; k < BH * 6; k += TILE_THREADS) {
         const int ly = k / 6, c6 = k - ly * 6;
@@ -235,7 +235,7 @@ __global__ void __launch_bounds__(TILE_THREADS) k_tile(const __grid_constant__ C
   }
 
   // ---- FAST: pixel-pair planes, then the dense arc strength of the interior and of a 1-pixel ring around it
-  if (a.doFast) {
+  {
     const uint32_t* rw = reinterpret_cast<const uint32_t*>(S.raw);
     // (only the words the 16-point circles can reach: box columns [HX - 8, HX + TW + 8))
     constexpr int Q0 = HX / 4 - 2, QN = TW / 4 + 4;
@@ -393,7 +393,7 @@ __global__ void __launch_bounds__(TILE_THREADS) k_tile(const __grid_constant__ C
   // ---- Gaussian blur 7x7, sigma 2, Q8 taps [18,34,48,56,48,34,18] (OpenCV >= 4 fixed point; SURVEY.md §8c)
   // (its horizontal sums overwrite the pixel-pair planes: every warp is past the strength passes after the barrier that
   // precedes the NMS loop)
-  if (a.doBlur) {
+  {
     const uint32_t* rw = reinterpret_cast<const uint32_t*>(S.raw);
     const uint32_t KA = 0x38302212u, KB = 0x00122230u;  // taps (18,34,48,56) and (48,34,18,0)
     for (int k = tid; k < (TH + 6) * (TW / 4); k += TILE_THREADS) {
@@ -440,7 +440,7 @@ __global__ void __launch_bounds__(TILE_THREADS) k_tile(const __grid_constant__ C
 
   // ---- level l+1: cv::resize INTER_LINEAR fixed point, every destination pixel whose top-left source sample lies in
   // this tile's interior (the +1 neighbours are inside the halo)
-  if (a.doResize && a.level + 1 < g.nlevels) {
+  if (a.level + 1 < g.nlevels) {
     const LevelGeom& D = g.lv[a.level + 1];
     const int16_t* tdx = a.tileDx + L.tdxOff;
     const int16_t* tdy = a.tileDy + L.tdyOff;
@@ -495,8 +495,8 @@ __global__ void __launch_bounds__(TILE_THREADS) k_tile(const __grid_constant__ C
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   __syncthreads();
   if (tid == 0) {
-    if (a.doFast) tma_store_3d(&tmScore, s32(S.scoreT), tx * TW, ty * TH, a.bBase + b);
-    if (a.doBlur) tma_store_3d(&tmBlur, s32(S.blurT), tx * TW, ty * TH, a.bBase + b);
+    tma_store_3d(&tmScore, s32(S.scoreT), tx * TW, ty * TH, a.bBase + b);
+    tma_store_3d(&tmBlur, s32(S.blurT), tx * TW, ty * TH, a.bBase + b);
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
     asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
   }
@@ -715,17 +715,13 @@ int tile_build(b2s_extractor* h) {
 }
 
 // Enqueue the fused front end for `batch` images starting at image `bBase` of the handle's buffers.
-// path: 1 = strength map only (pyramid and blur by the per-stage kernels), 2 = + blur, 3 = + pyramid (everything fused).
-int tile_run(b2s_extractor* h, int bBase, int batch, int path, cudaStream_t st, cudaEvent_t evAfterTiles) {
+int tile_run(b2s_extractor* h, int bBase, int batch, cudaStream_t st) {
   const ExtractGeom& g = h->geom;
   const DeviceBuffers& d = h->d;
   for (int l = 0; l < g.nlevels; l++) {
     TileArgs a;
     a.level = l;
     a.bBase = bBase;
-    a.doFast = 1;
-    a.doBlur = path >= 2;
-    a.doResize = path >= 3;
     a.pyr = d.pyr;
     a.rxOfs = d.rxOfs;
     a.rxAlpha = d.rxAlpha;
@@ -739,7 +735,6 @@ int tile_run(b2s_extractor* h, int bBase, int batch, int path, cudaStream_t st, 
         *reinterpret_cast<const CUtensorMap*>(h->tmBlur[l]), g, a);
     h->launches++;
   }
-  if (evAfterTiles) cudaEventRecord(evAfterTiles, st);
   // chunks of one batch run concurrently on two streams: each owns a slice of the fallback list and its own counter
   uint2* fbList = d.fbList + (size_t)bBase * g.totalCells;
   int32_t* fbCount = d.fbCount + bBase;

@@ -101,80 +101,9 @@ __global__ void k_rank_by_key(const int32_t* __restrict__ keyBase, const int32_t
 // ------------------------------------------------------------------------------------------------
 // SearchByBoW, stage 1: per keyframe-side row, K best frame-side candidates of the same vocabulary node
 // key = dist<<16 | j   (j ascending == the reference's candidate iteration order inside a node)
-// ------------------------------------------------------------------------------------------------
 // Only candidates closer than `cut` are listed and counted (bow_distance_cut below): no other candidate can change a
 // decision of the resolver.
-// One thread per keyframe-side row (its descriptor and K-list live in registers); the frame-side descriptors of the pair
-// are staged once per CTA in shared memory and read as warp-wide broadcasts, so every distance costs
-// 8 XOR + 8 POPC + 8 IADD per lane and no cross-lane merge is needed.
-constexpr int BOW_TILE = 1024;  // frame-side descriptors per shared-memory stage (32 KB) + node ids (4 KB) + valid (1 KB)
-__global__ void __launch_bounds__(256) k_bow_topk(const uint8_t* __restrict__ descA, const int32_t* __restrict__ nodeA,
-                                                  const uint8_t* __restrict__ validA, const int32_t* __restrict__ nAarr,
-                                                  int capA, const uint8_t* __restrict__ descB,
-                                                  const int32_t* __restrict__ nodeB, const uint8_t* __restrict__ validB,
-                                                  const int32_t* __restrict__ nBarr, int capB, int cut,
-                                                  uint32_t* __restrict__ topk, int32_t* __restrict__ candCnt) {
-  __shared__ __align__(32) uint32_t sB[BOW_TILE * 8];
-  __shared__ __align__(16) int32_t sNode[BOW_TILE];
-  __shared__ __align__(16) uint8_t sValid[BOW_TILE];
-  const int pair = blockIdx.y;
-  const int nA = min(nAarr[pair], capA), nB = min(nBarr[pair], capB);  // (clamped: device-side counts are untrusted)
-  if ((int)(blockIdx.x * blockDim.x) >= nA) return;
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t oa = (size_t)pair * capA, ob = (size_t)pair * capB;
-  const bool rowOk = (i < nA) && (!validA || validA[oa + i]);
-  u256 da;
-  int na = -1;
-  if (rowOk) {
-    da = ld_desc(descA + oa * 32, i);
-    na = nodeA[oa + i];
-  } else {
-#pragma unroll
-    for (int k = 0; k < 8; k++) da.w[k] = 0;
-  }
-  uint32_t t[TOPK];
-#pragma unroll
-  for (int k = 0; k < TOPK; k++) t[k] = EMPTY;
-  int cnt = 0;
-  for (int j0 = 0; j0 < nB; j0 += BOW_TILE) {
-    const int tn = min(BOW_TILE, nB - j0);
-    __syncthreads();
-    const uint32_t* gB = reinterpret_cast<const uint32_t*>(descB + (ob + j0) * 32);
-    for (int q = threadIdx.x; q < tn * 8; q += blockDim.x) sB[q] = gB[q];
-    for (int q = threadIdx.x; q < tn; q += blockDim.x) {
-      sNode[q] = nodeB[ob + j0 + q];
-      sValid[q] = validB ? validB[ob + j0 + q] : 1;
-    }
-    __syncthreads();
-    if (rowOk) {
-      // four frame-side descriptors per iteration, branch-free distance; only the (rare) K-list insertion branches
-      for (int j = 0; j < tn; j += 4) {
-        const int4 nd = *reinterpret_cast<const int4*>(&sNode[j]);
-        const uint32_t vv = *reinterpret_cast<const uint32_t*>(&sValid[j]);
-        const int nds[4] = {nd.x, nd.y, nd.z, nd.w};
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-          const uint4 b0 = *reinterpret_cast<const uint4*>(&sB[(j + q) * 8]);
-          const uint4 b1 = *reinterpret_cast<const uint4*>(&sB[(j + q) * 8 + 4]);
-          const int d = hamming256_words(da.w[0] ^ b0.x, da.w[1] ^ b0.y, da.w[2] ^ b0.z, da.w[3] ^ b0.w, da.w[4] ^ b1.x,
-                                         da.w[5] ^ b1.y, da.w[6] ^ b1.z, da.w[7] ^ b1.w);
-          const bool ok = (nds[q] == na) && ((vv >> (8 * q)) & 0xffu) && (j + q < tn) && (d < cut);
-          cnt += ok ? 1 : 0;
-          const uint32_t key = ok ? (((uint32_t)d << 16) | (uint32_t)(j0 + j + q)) : EMPTY;
-          if (key < t[TOPK - 1]) topk_insert(t, key);
-        }
-      }
-    }
-  }
-  if (i < nA) {
-#pragma unroll
-    for (int k = 0; k < TOPK; k++) topk[(oa + i) * TOPK + k] = t[k];
-    candCnt[oa + i] = cnt;
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// The same stage on the integer tensor pipe.  popc(a ^ b) = popc(a) + popc(b) - 2 popc(a & b), and popc(a & b) of two
+// The distances run on the integer tensor pipe.  popc(a ^ b) = popc(a) + popc(b) - 2 popc(a & b), and popc(a & b) of two
 // 256-bit strings is the dot product of their bits written as 0 / 1 bytes: a 16 x 8 tile of distances is eight
 // mma.sync.m16n8k32.u8 (IMMA.16832; bench.py reports the issue rate measured on the device, b2s_measure_peaks slot 5).
 // A CTA owns 128 keyframe-side rows (4 warps x 32 rows, bit-expanded A fragments live in registers for the whole sweep) and
@@ -183,9 +112,10 @@ __global__ void __launch_bounds__(256) k_bow_topk(const uint8_t* __restrict__ de
 // descriptor byte 4 s + t, on both sides, so a B fragment is one conflict-free LDS.64 (column pitch 288 B).
 // Selection: lane (g, t) sees rows {g, g+8, g+16, g+24} x columns {2t, 2t+1} of every 8-column block and keeps a K-list
 // per row; keys are unique (column index in the low half), so the K smallest of the four lanes' lists are exactly the K
-// smallest of the row — the lists are merged once at the end and written in ascending order like k_bow_topk's.
+// smallest of the row.  The lists are merged once at the end: each row's K-list is written in ascending key order, i.e.
+// by distance and then by frame-side index, with EMPTY filling the slots past the row's candidates.
 // ------------------------------------------------------------------------------------------------
-constexpr int BI_ROWS = 128, BI_PITCH = 288;
+constexpr int BI_ROWS = 128, BI_COLS = 64, BI_PITCH = 288;
 __device__ __forceinline__ void expand_byte(uint32_t x, uint32_t& lo, uint32_t& hi) {  // bit i of x -> byte i (0 / 1)
   lo = ((x & 0xFu) * 0x00204081u) & 0x01010101u;
   hi = (((x >> 4) & 0xFu) * 0x00204081u) & 0x01010101u;
@@ -195,8 +125,7 @@ __device__ __forceinline__ void imma_16832(int (&c)[4], const uint32_t (&a)[4], 
                : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-template <int BI_COLS, int MINB>
-__global__ void __launch_bounds__(128, MINB) k_bow_topk_imma(const uint8_t* __restrict__ descA, const int32_t* __restrict__ nodeA,
+__global__ void __launch_bounds__(128, 3) k_bow_topk_imma(const uint8_t* __restrict__ descA, const int32_t* __restrict__ nodeA,
                                                        const uint8_t* __restrict__ validA, const int32_t* __restrict__ nAarr,
                                                        int capA, const uint8_t* __restrict__ descB,
                                                        const int32_t* __restrict__ nodeB, const uint8_t* __restrict__ validB,
@@ -1649,22 +1578,9 @@ extern "C" int b2s_search_by_bow_device(b2s_matcher* h, int batch, const uint8_t
   MatchParams mp{th_low, nnratio, strict_lt, check_ori};
   k_fill_i32<<<div_up(batch * capB, 256), 256, 0, st>>>(d_matchB, -1, (size_t)batch * capB);
   k_rank_by_key<<<dim3(div_up(capA, 128), batch), 128, 0, st>>>(d_nodeA, d_nA, capA, h->dOrder);
-  static const int scalarTopk = getenv("B2S_BOW_SCALAR") ? atoi(getenv("B2S_BOW_SCALAR")) : 0;  // (A/B switch for profiling)
   const int cut = bow_distance_cut(th_low, nnratio);
-  if (scalarTopk)
-    k_bow_topk<<<dim3(div_up(capA, 256), batch), 256, 0, st>>>(d_descA, d_nodeA, d_validA, d_nA, capA, d_descB, d_nodeB,
-                                                             d_validB, d_nB, capB, cut, h->dTopk, h->dCandCnt);
-  else
-  {
-    static const int variant = getenv("B2S_BOW_VARIANT") ? atoi(getenv("B2S_BOW_VARIANT")) : 0;  // (tuning switch)
-    const dim3 grid(div_up(capA, BI_ROWS), batch);
-#define B2S_BOW_ARGS d_descA, d_nodeA, d_validA, d_nA, capA, d_descB, d_nodeB, d_validB, d_nB, capB, cut, h->dTopk, h->dCandCnt
-    if (variant == 1) k_bow_topk_imma<64, 4><<<grid, 128, 0, st>>>(B2S_BOW_ARGS);
-    else if (variant == 2) k_bow_topk_imma<128, 3><<<grid, 128, 0, st>>>(B2S_BOW_ARGS);
-    else if (variant == 3) k_bow_topk_imma<128, 4><<<grid, 128, 0, st>>>(B2S_BOW_ARGS);
-    else k_bow_topk_imma<64, 3><<<grid, 128, 0, st>>>(B2S_BOW_ARGS);
-#undef B2S_BOW_ARGS
-  }
+  k_bow_topk_imma<<<dim3(div_up(capA, BI_ROWS), batch), 128, 0, st>>>(d_descA, d_nodeA, d_validA, d_nA, capA, d_descB, d_nodeB,
+                                                                     d_validB, d_nB, capB, cut, h->dTopk, h->dCandCnt);
   k_bow_resolve<<<dim3(div_up(capA, 4), batch), 128, 0, st>>>(d_descA, d_nodeA, d_validA, d_angA, d_nA, capA, d_descB,
                                                               d_nodeB, d_validB, d_angB, d_nB, capB, h->dOrder, h->dTopk,
                                                               h->dCandCnt, mp, d_matchB, h->dBin);

@@ -1,5 +1,5 @@
 """CUDA-event time of the batched SearchByBoW (160 pairs, 2000 x 2000, one vocabulary node) — whole call and per kernel under
-ncu:  python tools/bow_time.py            (B2S_BOW_SCALAR=1 for the scalar K-list kernel)"""
+ncu:  python tools/bow_time.py"""
 import ctypes, importlib, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -31,4 +31,4 @@ for _ in range(10):
     run()
 e1.record(st)
 torch.cuda.synchronize()
-print("scalar" if os.environ.get("B2S_BOW_SCALAR") == "1" else "imma", "ms per batched call: %.3f" % (e0.elapsed_time(e1) / 10), "matches", int(nm.sum()))
+print("ms per batched call: %.3f" % (e0.elapsed_time(e1) / 10), "matches", int(nm.sum()))
