@@ -19,7 +19,6 @@
 #include <math.h>
 
 #include <algorithm>
-#include <chrono>
 #include <thread>
 #include <vector>
 
@@ -74,10 +73,8 @@ struct BaPtrs {  // strided per-window arrays
   int capPairs, capBlk;
   double *partChi, *partScale;   // per-CTA partial sums [window][nCta]
   unsigned int* bar;             // per-window barrier counters
-  long long* prof;               // per-window phase cycle counters (debug): 16 slots
-  // balanced launch: CTA -> (window << 8 | index inside the window) and CTAs per window; null = uniform nCta per window
-  const int* ctaMap;
-  const int* winCtas;
+  // launch plan (ba_run): CTA of the launch -> (window << 8 | index inside the window), and CTAs per window
+  int *ctaMap, *winCtas;
 };
 
 __device__ __forceinline__ double delta_of(bool stereo) {
@@ -781,9 +778,6 @@ __device__ void phase_schur_blocks(const BaPtrs& p, const WinCtx& c, const BaWin
 // keeps each row in registers, the trailing update is 4x4 register tiled out of the shared-memory panel.
 constexpr int CHOL_PP = CHOL_BS + 1;
 __device__ void phase_chol(const BaPtrs& p, int w, const BaWin& W, double* dsm) {
-  long long tc = clock64();
-  long long* prof = p.prof + (size_t)w * 16;
-#define CH_PROF(slot) if (threadIdx.x == 0) { const long long tn = clock64(); prof[slot] += tn - tc; tc = tn; }
   BaState& st = p.st[w];
   const int n = W.nFree * 6, ld = p.ldS;
   double* S = p.S + (size_t)w * ld * ld;
@@ -848,7 +842,6 @@ __device__ void phase_chol(const BaPtrs& p, int w, const BaWin& W, double* dsm) 
       mRows = cnt;
     }
     __syncthreads();
-    CH_PROF(11)
     for (int idx = tid; idx < wd * wd; idx += T) {
       const int r = idx / wd, cc = idx - r * wd;
       if (cc <= r) S[(size_t)(kb + r) * ld + kb + cc] = Dblk[r * CHOL_PP + cc];
@@ -877,7 +870,6 @@ __device__ void phase_chol(const BaPtrs& p, int w, const BaWin& W, double* dsm) 
     }
     for (int idx = tid; idx < 8 * CHOL_PP; idx += T) panel[(m + idx / CHOL_PP) * CHOL_PP + idx % CHOL_PP] = 0.0;  // pad to a multiple of 8 rows
     __syncthreads();
-    CH_PROF(12)
     // trailing update S[i][j] -= sum_k panel[i][k] * panel[j][k] on the FP64 tensor pipe: one warp per 8 x 8 tile of the
     // (compacted) row list, eight DMMA.8x8x4 per tile (k = 32), fragments loaded straight from the panel in shared memory.
     // mma.m8n8k4 f64 fragments: A[g][t] and B[t][g] one value per lane (g = lane / 4, t = lane % 4), C[g][2t], C[g][2t+1].
@@ -915,7 +907,6 @@ __device__ void phase_chol(const BaPtrs& p, int w, const BaWin& W, double* dsm) 
       }
     }
     __syncthreads();
-    CH_PROF(13)
   }
   // back substitution L^T x = y
   for (int i = tid; i < n; i += T) xs[i] = S[(size_t)n * ld + i];
@@ -960,8 +951,6 @@ __device__ void phase_chol(const BaPtrs& p, int w, const BaWin& W, double* dsm) 
   for (int i = tid; i < n; i += T) x[i] = xs[i];
   if (tid == 0) st.solveOk = fail ? 0 : 1;
   __syncthreads();
-  CH_PROF(14)
-#undef CH_PROF
 }
 
 // landmark back-substitution (block_solver.hpp:461-481) + updates (types_sba.h:52-56, se3quat oplus) + computeScale
@@ -1177,23 +1166,16 @@ __device__ void phase_outliers(const BaPtrs& p, const WinCtx& c, const BaWin& W,
   }
 }
 
-// ---------------------------------------------------------------- the persistent kernel: grid = batch * nCta CTAs
+// ---------------------------------------------------------------- the persistent kernel: one CTA per entry of p.ctaMap
 constexpr int BA_T = 256;
-__global__ void __launch_bounds__(BA_T) k_local_ba(BaPtrs p, int nCtaUniform, int wBase, int dbgRepeat) {
+__global__ void __launch_bounds__(BA_T) k_local_ba(BaPtrs p) {
   extern __shared__ __align__(16) double dsm[];
   __shared__ double red[32];
   WinCtx c;
-  int nCta = nCtaUniform;
-  if (p.ctaMap) {  // balanced launch: bigger windows own more CTAs
-    const int m = p.ctaMap[blockIdx.x];
-    c.w = m >> 8;
-    c.cta = m & 255;
-    nCta = p.winCtas[c.w];
-  } else {
-    c.w = blockIdx.x / nCta;
-    c.cta = blockIdx.x - c.w * nCta;
-  }
-  c.w += wBase;
+  const int m = p.ctaMap[blockIdx.x];
+  c.w = m >> 8;
+  c.cta = m & 255;
+  const int nCta = p.winCtas[c.w];
   c.nCta = nCta;
   c.gtid = c.cta * blockDim.x + threadIdx.x;
   c.gthreads = nCta * blockDim.x;
@@ -1203,60 +1185,35 @@ __global__ void __launch_bounds__(BA_T) k_local_ba(BaPtrs p, int nCtaUniform, in
   unsigned int epoch = 0;
   volatile BaState* vst = p.st + w;
   volatile int* hung = &(p.st + w)->finishedRound0;  // (field reused as the barrier-timeout flag)
-  const bool profOn = (c.cta == 0 && threadIdx.x == 0);
-  long long tPrev = clock64();
-#define BA_PROF(slot)                                   \
-  if (profOn) {                                         \
-    const long long tn = clock64();                     \
-    p.prof[(size_t)w * 16 + (slot)] += tn - tPrev;      \
-    tPrev = tn;                                         \
-  }
   for (int guard = 0; guard < 4096; guard++) {
     if (!vst->active || *hung) break;
     const int needBuild = vst->needBuild, robust = vst->robust;
     const int cur = vst->errBuf;
     if (needBuild) {
-      for (int rr = ((dbgRepeat >> 8) == 2 ? (dbgRepeat & 255) : 1); rr > 0; rr--) {
-        // errors + weights: after an accepted step they were stored by that step's phase_errors (same state, same values)
-        if (!vst->errCurrent) {
-          phase_errors(p, c, W, robust, red, cur, true);
-          win_barrier(bar, epoch, nCta, hung);
-        }
-        BA_PROF(0)
-        phase_reduce_landmarks(p, c, W, cur, dsm);
-        phase_build_poses(p, c, W, robust, cur);
+      // errors + weights: after an accepted step they were stored by that step's phase_errors (same state, same values)
+      if (!vst->errCurrent) {
+        phase_errors(p, c, W, robust, red, cur, true);
         win_barrier(bar, epoch, nCta, hung);
-        BA_PROF(1)
       }
+      phase_reduce_landmarks(p, c, W, cur, dsm);
+      phase_build_poses(p, c, W, robust, cur);
+      win_barrier(bar, epoch, nCta, hung);
     }
     if (c.cta == 0 && threadIdx.x == 0) control_begin(p, w, nCta);
     win_barrier(bar, epoch, nCta, hung);
-    BA_PROF(2)
     const double lambda = vst->lm.lambda;
     phase_dinv(p, c, W, lambda);
     win_barrier(bar, epoch, nCta, hung);
-    BA_PROF(3)
-    // dbgRepeat (profiling only, B2S_BA_REPEAT=phase*256+count): re-run one idempotent phase so that a whole-kernel
-    // ncu capture is dominated by it; 0 in production
-    for (int rr = ((dbgRepeat >> 8) == 1 ? (dbgRepeat & 255) : 1); rr > 0; rr--) {
-      phase_schur_blocks(p, c, W, lambda, dsm, cur);
-      win_barrier(bar, epoch, nCta, hung);
-    }
-    BA_PROF(5)
+    phase_schur_blocks(p, c, W, lambda, dsm, cur);
+    win_barrier(bar, epoch, nCta, hung);
     if (c.cta == 0) phase_chol(p, w, W, dsm);
     win_barrier(bar, epoch, nCta, hung);
-    BA_PROF(6)
     phase_backsub_update(p, c, W, lambda, vst->solveOk, red, dsm, cur);
     win_barrier(bar, epoch, nCta, hung);
-    BA_PROF(7)
-    for (int rr = ((dbgRepeat >> 8) == 3 ? (dbgRepeat & 255) : 1); rr > 0; rr--) {
-      phase_errors(p, c, W, robust, red, cur ^ 1);
-      win_barrier(bar, epoch, nCta, hung);
-    }
-    BA_PROF(8)
+    phase_errors(p, c, W, robust, red, cur ^ 1);
+    win_barrier(bar, epoch, nCta, hung);
     if (c.cta == 0 && threadIdx.x == 0) control_end(p, w, nCta);
     win_barrier(bar, epoch, nCta, hung);
-    BA_PROF(9)
     if (vst->restore) phase_restore(p, c, W);
     const int doOutlier = vst->doOutlier;
     if (doOutlier) {
@@ -1274,9 +1231,7 @@ __global__ void __launch_bounds__(BA_T) k_local_ba(BaPtrs p, int nCtaUniform, in
       }
       win_barrier(bar, epoch, nCta, hung);
     }
-    BA_PROF(10)
   }
-#undef BA_PROF
 }
 
 // ---------------------------------------------------------------- structure kernels (once per window)
@@ -1703,7 +1658,7 @@ using namespace b2s;
 struct BaHostStage {  // pinned mirror of the uploaded per-window arrays (same strides as the device arrays)
   double *pose = nullptr, *pts = nullptr;
   int *pidx = nullptr, *freeKf = nullptr, *eKf = nullptr, *eMp = nullptr, *mpStart = nullptr, *kfStart = nullptr,
-      *mpEdges = nullptr, *kfEdges = nullptr;
+      *mpEdges = nullptr, *kfEdges = nullptr, *ctaMap = nullptr, *winCtas = nullptr;
   float *eObs = nullptr, *eW = nullptr;
   uint8_t *eSt = nullptr, *eOutlier = nullptr;
   BaWin* win = nullptr;
@@ -1725,7 +1680,6 @@ struct b2s_ba_solver {
   cudaEvent_t evLm[2] = {nullptr, nullptr};  // around the persistent LM kernel of the last batch (b2s_ba_last_kernel_ms)
   float lastLmMs = 0.f;
   long long lastTrials = 0;
-  int *dCtaMap = nullptr, *dWinCtas = nullptr;  // balanced launch tables (see ba_run)
   int smBudget = 0;  // CTAs (= SMs) one LocalBA batch may occupy; 0 = all (b2s_ba_set_sm_budget)
   DevBuf pairRec;    // d.pairRec: batch x d.capPairs records, grown by ba_run when a window needs more
 };
@@ -1790,11 +1744,11 @@ extern "C" int b2s_ba_create(int max_kf, int max_mp, int max_edges, int max_batc
   A(&d.lmRec, B * (size_t)max_edges * 8); A(&d.blkFirst, B * (size_t)max_kf * 4); A(&d.blkOrder, B * (size_t)d.capBlk * 4); A(&d.blkNZ, B * 4);
   A(&d.partChi, B * d.nPartE * 8); A(&d.partScale, B * d.nPartM * 8);
   A(&d.bar, B * 4);
-  A(&d.prof, B * 16 * 8);
-  A(&h->dCtaMap, 1024 * 4); A(&h->dWinCtas, B * 4);
-  d.ctaMap = nullptr;
-  d.winCtas = nullptr;
+  // launch plan (ba_run): a batch of at most numSMs windows has at most numSMs CTAs, a larger one one CTA per window
+  const size_t mapLen = std::max(B, (size_t)h->numSMs);
+  A(&d.ctaMap, mapLen * 4); A(&d.winCtas, B * 4);
   BaHostStage& s = h->hs;
+  HA(&s.ctaMap, mapLen * 4); HA(&s.winCtas, B * 4);
   HA(&s.pose, B * max_kf * POSE_STRIDE * 8); HA(&s.pts, B * max_mp * 3 * 8);
   HA(&s.pidx, B * max_kf * 4); HA(&s.freeKf, B * max_kf * 4);
   HA(&s.eKf, B * max_edges * 4); HA(&s.eMp, B * max_edges * 4);
@@ -1839,7 +1793,6 @@ extern "C" int b2s_ba_set_sm_budget(b2s_ba_solver* h, int sms) {
   return B2S_OK;
 }
 
-// Converter::toSE3Quat / toVector3d + CSR structure of one window, written into the pinned staging area
 // host threads for window preparation / write-back: min(batch, 16, cores), or B2S_BA_HOST_THREADS (several ranks per box
 // share the host cores)
 static int ba_host_threads(int batch) {
@@ -1848,6 +1801,19 @@ static int ba_host_threads(int batch) {
   return std::max(1, std::min(batch, std::min(cap, (int)std::thread::hardware_concurrency())));
 }
 
+template <class F>
+static void ba_for_windows(int batch, const F& fn) {  // fn(w) for every window, on ba_host_threads(batch) threads
+  const int nth = ba_host_threads(batch);
+  auto share = [&](int t) {
+    for (int w = t; w < batch; w += nth) fn(w);
+  };
+  std::vector<std::thread> th;
+  for (int t = 1; t < nth; t++) th.emplace_back(share, t);
+  share(0);  // the calling thread takes the first share instead of waiting idle (one window: no thread is started)
+  for (auto& t : th) t.join();
+}
+
+// Converter::toSE3Quat / toVector3d + CSR structure of one window, written into the pinned staging area
 static int ba_prepare_window(b2s_ba_solver* h, int w, const b2s_ba_problem& P, int* nFreeOut, long long* pairBoundOut) {
   const BaPtrs& d = h->d;
   BaHostStage& s = h->hs;
@@ -1910,6 +1876,47 @@ static int ba_prepare_window(b2s_ba_solver* h, int w, const b2s_ba_problem& P, i
   return 0;
 }
 
+// Launch plan of k_local_ba: n[w] CTAs for window w, and map[] = (w << 8) | CTA index inside the window, windows in
+// order; returns the number of CTAs.  One window takes min(16, numSMs) CTAs (the SM budget does not apply to it).  A batch
+// that fits on the GPU deals its budget by estimated cost, because the launch ends with its slowest window.  Cost model
+// (per-phase cycle counts measured on 32 windows of 23-51 free keyframes / 16-40 k edges): a serial part (single-CTA
+// factorisation, control) that grows with the number of free keyframes, and a part that divides over the window's CTAs
+// (linearisation, Schur pairs ~ edges x observations per point, back-substitution, error pass).  Greedy: every window
+// starts with one CTA, the currently slowest gets the next.  A batch larger than numSMs runs one CTA per window.
+static int ba_launch_plan(const b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, const int* nFree, int* n,
+                          int* map) {
+  const int numSMs = h->numSMs;
+  if (batch == 1) {
+    n[0] = std::min(16, numSMs);
+  } else if (batch > numSMs) {
+    for (int w = 0; w < batch; w++) n[w] = 1;
+  } else {
+    const int budget = h->smBudget > 0 ? std::max(batch, std::min(numSMs, h->smBudget)) : numSMs;
+    std::vector<double> ser(batch), par(batch);
+    for (int w = 0; w < batch; w++) {
+      const double e = probs[w].n_edges * 1e-3, obs = probs[w].n_mp > 0 ? (double)probs[w].n_edges / probs[w].n_mp : 0.0;
+      ser[w] = 0.8 + 0.12 * nFree[w];
+      par[w] = 4.0 * (1.65 + 0.127 * e + 0.024 * e * obs);
+      n[w] = 1;
+    }
+    for (int used = batch; used < budget; used++) {
+      int worst = -1;
+      double tw = -1.0;
+      for (int w = 0; w < batch; w++) {
+        if (n[w] >= 16) continue;
+        const double t = ser[w] + par[w] / n[w];
+        if (t > tw) { tw = t; worst = w; }
+      }
+      if (worst < 0) break;
+      n[worst]++;
+    }
+  }
+  int total = 0;
+  for (int w = 0; w < batch; w++)
+    for (int k = 0; k < n[w]; k++) map[total++] = (w << 8) | k;
+  return total;
+}
+
 static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, const volatile uint8_t* stop,
                   b2s_ba_result* res) {
   if (!h || !probs || !res || batch < 1 || batch > h->maxBatch) {
@@ -1921,8 +1928,6 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
   B2S_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = h->stream;
   if (stop && *stop) return B2S_ERR_ABORTED;  // src/Optimizer.cc:858-860: return without write-back
-  const bool dbg = getenv("B2S_DEBUG_TIMING") != nullptr;
-  const auto tStart = std::chrono::steady_clock::now();
   for (int w = 0; w < batch; w++) {
     const b2s_ba_problem& P = probs[w];
     if (P.its1 < 1 || P.its2 < 0) {
@@ -1938,15 +1943,7 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
   // ---- host preparation of all windows in parallel (pinned staging), then one H2D per array
   std::vector<int> nFree(batch, 0), prc(batch, 0);
   std::vector<long long> pairBound(batch, 0);
-  {
-    const int nth = ba_host_threads(batch);
-    std::vector<std::thread> th;
-    for (int t = 0; t < nth; t++)
-      th.emplace_back([&, t]() {
-        for (int w = t; w < batch; w += nth) prc[w] = ba_prepare_window(h, w, probs[w], &nFree[w], &pairBound[w]);
-      });
-    for (auto& t : th) t.join();
-  }
+  ba_for_windows(batch, [&](int w) { prc[w] = ba_prepare_window(h, w, probs[w], &nFree[w], &pairBound[w]); });
   int maxE = 0, maxMp = 0, maxFree = 0;
   long long maxPairs = 8LL * h->maxE;  // the stride b2s_ba_create allocated for: windows bounded by it never grow the list
   for (int w = 0; w < batch; w++) {
@@ -1979,6 +1976,7 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
     if (rc != B2S_OK) return rc;
     d.pairRec = (int4*)h->pairRec.p;
   }
+  const int nCtas = ba_launch_plan(h, batch, probs, nFree.data(), s.winCtas, s.ctaMap);
   const size_t nb = (size_t)batch;
 #define UPALL(dst, src, stride, type) \
   B2S_CUDA(cudaMemcpyAsync((dst), (src), nb * (size_t)(stride) * sizeof(type), cudaMemcpyHostToDevice, st))
@@ -1997,18 +1995,13 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
   UPALL(d.kfEdges, s.kfEdges, d.capE, int);
   UPALL(d.win, s.win, 1, BaWin);
   UPALL(d.st, s.st, 1, BaState);
+  UPALL(d.winCtas, s.winCtas, 1, int);
 #undef UPALL
+  B2S_CUDA(cudaMemcpyAsync(d.ctaMap, s.ctaMap, (size_t)nCtas * 4, cudaMemcpyHostToDevice, st));
   B2S_CUDA(cudaMemsetAsync(d.eLevel, 0, nb * d.capE, st));
   B2S_CUDA(cudaMemsetAsync(d.chi2, 0, nb * d.capE * 8, st));
   B2S_CUDA(cudaMemsetAsync(d.lmEdge, 0xFF, nb * (size_t)d.capMp * d.capKf * 4, st));
   B2S_CUDA(cudaMemsetAsync(d.bar, 0, nb * 4, st));
-  B2S_CUDA(cudaMemsetAsync(d.prof, 0, nb * 16 * 8, st));
-  const auto tPrep = std::chrono::steady_clock::now();
-  cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  if (dbg) {
-    for (auto& e : ev) cudaEventCreate(&e);
-    cudaEventRecord(ev[0], st);  // uploads + memsets enqueued before this point
-  }
   const int gE = std::max(1, div_up(maxE, 256));
   k_lm_edge<<<dim3(gE, batch), 256, 0, st>>>(d);
   const int nblk = std::max(1, maxFree * (maxFree + 1) / 2);
@@ -2017,87 +2010,29 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
   k_pair_build<<<dim3(nblk, batch), 64, 0, st>>>(d, 1);
   B2S_CUDA(cudaMemsetAsync(d.blkNZ, 0, nb * 4, st));
   k_block_order<<<batch, 256, 0, st>>>(d);
-  // ---- the whole LM loop of every window: one persistent launch, nCta co-resident CTAs per window
-  if (dbg) cudaEventRecord(ev[1], st);
+  // ---- the whole LM loop of every window: persistent cooperative launches, all CTAs of a launch co-resident
   if (!h->evLm[0]) {
     B2S_CUDA(cudaEventCreate(&h->evLm[0]));
     B2S_CUDA(cudaEventCreate(&h->evLm[1]));
   }
   B2S_CUDA(cudaEventRecord(h->evLm[0], st));
-  int chunk = std::min(batch, h->numSMs);  // windows per cooperative launch (all their CTAs must be co-resident)
-  if (const char* ev = getenv("B2S_BA_CHUNK")) chunk = std::max(1, std::min(chunk, atoi(ev)));  // tuning knob
-  int nCta = std::max(1, std::min(16, h->numSMs / chunk));
-  if (const char* ev = getenv("B2S_BA_NCTA")) nCta = std::max(1, std::min(nCta, atoi(ev)));  // tuning knob
-  // Balanced launch (one chunk, more than one window): the kernel ends with its slowest window, so the SMs are dealt by
-  // estimated cost instead of evenly.  Cost model (cycles of the phases measured with B2S_DEBUG_TIMING on 32 windows of
-  // 23-51 free keyframes / 16-40 k edges): a serial part (single-CTA factorisation, control) that grows with the number of
-  // free keyframes, and a part that divides over the window's CTAs (linearisation, Schur pairs ~ edges x observations per
-  // point, back-substitution, error pass).  Greedy: every window starts with one CTA, the currently slowest gets the next.
-  d.ctaMap = nullptr;
-  d.winCtas = nullptr;
-  bool balanced = false;
-  {
-    const char* ev = getenv("B2S_BA_BALANCE");
-    const bool want = !ev || atoi(ev) != 0;
-    int budget = h->smBudget > 0 ? std::max(batch, std::min(h->numSMs, h->smBudget)) : h->numSMs;
-    if (const char* e2 = getenv("B2S_BA_SMS")) budget = std::max(batch, std::min(h->numSMs, atoi(e2)));
-    if (want && batch > 1 && chunk == batch && batch <= budget && !getenv("B2S_BA_NCTA")) {
-      std::vector<double> ser(batch), par(batch);
-      std::vector<int> n(batch, 1);
-      for (int w = 0; w < batch; w++) {
-        const double e = probs[w].n_edges * 1e-3, obs = probs[w].n_mp > 0 ? (double)probs[w].n_edges / probs[w].n_mp : 0.0;
-        ser[w] = 0.8 + 0.12 * nFree[w];
-        par[w] = 4.0 * (1.65 + 0.127 * e + 0.024 * e * obs);
-      }
-      for (int used = batch; used < budget; used++) {
-        int worst = -1;
-        double tw = -1.0;
-        for (int w = 0; w < batch; w++) {
-          if (n[w] >= 16) continue;
-          const double t = ser[w] + par[w] / n[w];
-          if (t > tw) { tw = t; worst = w; }
-        }
-        if (worst < 0) break;
-        n[worst]++;
-      }
-      std::vector<int> map;
-      for (int w = 0; w < batch; w++)
-        for (int k = 0; k < n[w]; k++) map.push_back((w << 8) | k);
-      B2S_CUDA(cudaMemcpyAsync(h->dCtaMap, map.data(), map.size() * 4, cudaMemcpyHostToDevice, st));
-      B2S_CUDA(cudaMemcpyAsync(h->dWinCtas, n.data(), (size_t)batch * 4, cudaMemcpyHostToDevice, st));
-      B2S_CUDA(cudaStreamSynchronize(st));  // (the vectors are pageable host memory)
-      d.ctaMap = h->dCtaMap;
-      d.winCtas = h->dWinCtas;
-      balanced = true;
-      int gridCtas = (int)map.size(), dbgRepeat = 0, wBase = 0, one = 1;
-      if (const char* e3 = getenv("B2S_BA_REPEAT")) dbgRepeat = atoi(e3);
-      void* args[] = {(void*)&d, (void*)&one, (void*)&wBase, (void*)&dbgRepeat};
-      if (h->smemBytes > 48 * 1024)
-        B2S_CUDA(cudaFuncSetAttribute(k_local_ba, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smemBytes));
-      B2S_CUDA(cudaLaunchCooperativeKernel((const void*)k_local_ba, dim3(gridCtas), dim3(BA_T), args, h->smemBytes, st));
-      h->launches++;
-      if (dbg) {
-        fprintf(stderr, "[b2s_local_ba] balanced launch, %d CTAs:", gridCtas);
-        for (int w = 0; w < batch; w++) fprintf(stderr, " %d", n[w]);
-        fprintf(stderr, "\n");
-      }
-    }
-  }
-  for (int wBase = 0; wBase < batch && !balanced; wBase += chunk) {
-    int nw = std::min(chunk, batch - wBase);
-    int dbgRepeat = 0;
-    if (const char* ev = getenv("B2S_BA_REPEAT")) dbgRepeat = atoi(ev);  // profiling aid, see k_local_ba
-    void* args[] = {(void*)&d, (void*)&nCta, (void*)&wBase, (void*)&dbgRepeat};
-    // the attribute is per FUNCTION, not per handle: another solver handle (different capacities) may have set a smaller
-    // limit since this one was created, which makes the cooperative launch fail with "too many blocks"
-    if (h->smemBytes > 48 * 1024)
-      B2S_CUDA(cudaFuncSetAttribute(k_local_ba, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smemBytes));
-    B2S_CUDA(cudaLaunchCooperativeKernel((const void*)k_local_ba, dim3(nw * nCta), dim3(BA_T), args, h->smemBytes, st));
+  // the attribute is per FUNCTION, not per handle: another solver handle (different capacities) may have set a smaller
+  // limit since this one was created, which makes the cooperative launch fail with "too many blocks"
+  if (h->smemBytes > 48 * 1024)
+    B2S_CUDA(cudaFuncSetAttribute(k_local_ba, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smemBytes));
+  // consecutive windows share a launch while their CTAs fit on the SMs (the plan gives no window more than numSMs)
+  for (int w0 = 0, c0 = 0; w0 < batch;) {
+    int grid = 0;
+    for (; w0 < batch && grid + s.winCtas[w0] <= h->numSMs; w0++) grid += s.winCtas[w0];
+    BaPtrs dl = d;
+    dl.ctaMap = d.ctaMap + c0;
+    void* args[] = {(void*)&dl};
+    B2S_CUDA(cudaLaunchCooperativeKernel((const void*)k_local_ba, dim3(grid), dim3(BA_T), args, h->smemBytes, st));
     h->launches++;
+    c0 += grid;
   }
   h->launches += 5;
   B2S_CUDA(cudaEventRecord(h->evLm[1], st));
-  if (dbg) cudaEventRecord(ev[2], st);
   // asynchronous abort (LocalMapping::InsertKeyFrame sets mbAbortBA): forward the flag while the kernel runs
   if (stop) {
     bool sent = false;
@@ -2117,7 +2052,6 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
   B2S_CUDA(cudaMemcpyAsync(s.pts, d.pts, nb * (size_t)d.capMp * 3 * 8, cudaMemcpyDeviceToHost, st));
   B2S_CUDA(cudaMemcpyAsync(s.eOutlier, d.eOutlier, nb * d.capE, cudaMemcpyDeviceToHost, st));
   B2S_CUDA(cudaMemcpyAsync(s.st, d.st, nb * sizeof(BaState), cudaMemcpyDeviceToHost, st));
-  if (dbg) cudaEventRecord(ev[3], st);
   B2S_CUDA(cudaStreamSynchronize(st));
   B2S_CUDA(cudaGetLastError());
   cudaEventElapsedTime(&h->lastLmMs, h->evLm[0], h->evLm[1]);
@@ -2133,67 +2067,24 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
       set_error("b2s_local_ba: window %d: covisibility pair list exceeds its capacity of %d", w, d.capPairs);
       return B2S_ERR_CAPACITY;
     }
-  const auto tLoop = std::chrono::steady_clock::now();
-  {
-    const int nth = ba_host_threads(batch);
-    std::vector<std::thread> th;
-    for (int t = 0; t < nth; t++)
-      th.emplace_back([&, t]() {
-        for (int w = t; w < batch; w += nth) {
-          const b2s_ba_problem& P = probs[w];
-          b2s_ba_result& R = res[w];
-          const double* pose = s.pose + (size_t)w * d.capKf * POSE_STRIDE;
-          const double* pts = s.pts + (size_t)w * d.capMp * 3;
-          if (R.Tcw_out)
-            for (int k = 0; k < P.n_local; k++) se3quat_to_Tcw(pose + (size_t)k * POSE_STRIDE, R.Tcw_out + (size_t)k * 16);
-          if (R.points_out)
-            for (size_t i = 0; i < (size_t)P.n_mp * 3; i++) R.points_out[i] = (float)pts[i];
-          if (R.edge_outlier && P.n_edges) memcpy(R.edge_outlier, s.eOutlier + (size_t)w * d.capE, P.n_edges);
-          R.chi2_final = s.st[w].chi2Final;
-          R.n_trials = s.st[w].lm.nTrials;
-          if (R.trace) {
-            const int n = std::min(s.st[w].lm.nTrials, 255);
-            for (int i = 0; i < n; i++) R.trace[i] = s.st[w].trace[i];
-            R.trace[n] = -1;
-          }
-        }
-      });
-    for (auto& t : th) t.join();
-  }
-  if (dbg) {
-    const auto tEnd = std::chrono::steady_clock::now();
-    auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) {
-      return std::chrono::duration<double, std::milli>(b - a).count();
-    };
-    long long prof[16];
-    cudaMemcpy(prof, d.prof, sizeof(prof), cudaMemcpyDeviceToHost);
-    static const char* names[15] = {"build_lm", "build_pose", "ctl_begin", "dinv", "-", "schur_blk", "chol",
-                                    "backsub", "errors", "ctl_end", "restore/outl", "chol.diag", "chol.panel",
-                                    "chol.trail", "chol.backsub"};
-    fprintf(stderr, "[b2s_local_ba] window 0 phase Mcycles:");
-    for (int k = 0; k < 15; k++) fprintf(stderr, " %s=%.2f", names[k], prof[k] / 1e6);
-    fprintf(stderr, "\n");
-    {  // every window: total of the phase slots (cycles of its CTA 0), size, and the three main phases
-      std::vector<long long> all((size_t)batch * 16);
-      cudaMemcpy(all.data(), d.prof, all.size() * sizeof(long long), cudaMemcpyDeviceToHost);
-      for (int w = 0; w < batch; w++) {
-        const long long* q = all.data() + (size_t)w * 16;
-        long long tot = 0;
-        for (int k = 0; k <= 10; k++) tot += q[k];
-        fprintf(stderr, "[b2s_local_ba]   w%02d free=%d mp=%d e=%d trials=%d total=%.2f Mcyc: build=%.2f schur=%.2f chol=%.2f(diag %.2f) backsub=%.2f err=%.2f\n",
-                w, nFree[w], probs[w].n_mp, probs[w].n_edges, s.st[w].lm.nTrials, tot / 1e6, (q[0] + q[1]) / 1e6, q[5] / 1e6,
-                q[6] / 1e6, q[11] / 1e6, q[7] / 1e6, q[8] / 1e6);
-      }
+  ba_for_windows(batch, [&](int w) {
+    const b2s_ba_problem& P = probs[w];
+    b2s_ba_result& R = res[w];
+    const double* pose = s.pose + (size_t)w * d.capKf * POSE_STRIDE;
+    const double* pts = s.pts + (size_t)w * d.capMp * 3;
+    if (R.Tcw_out)
+      for (int k = 0; k < P.n_local; k++) se3quat_to_Tcw(pose + (size_t)k * POSE_STRIDE, R.Tcw_out + (size_t)k * 16);
+    if (R.points_out)
+      for (size_t i = 0; i < (size_t)P.n_mp * 3; i++) R.points_out[i] = (float)pts[i];
+    if (R.edge_outlier && P.n_edges) memcpy(R.edge_outlier, s.eOutlier + (size_t)w * d.capE, P.n_edges);
+    R.chi2_final = s.st[w].chi2Final;
+    R.n_trials = s.st[w].lm.nTrials;
+    if (R.trace) {
+      const int n = std::min(s.st[w].lm.nTrials, 255);
+      for (int i = 0; i < n; i++) R.trace[i] = s.st[w].trace[i];
+      R.trace[n] = -1;
     }
-    fprintf(stderr, "[b2s_local_ba] batch=%d nCta=%d prep+upload %.2f ms, structure+LM kernel %.2f ms, write-back %.2f ms\n",
-            batch, nCta, ms(tStart, tPrep), ms(tPrep, tLoop), ms(tLoop, tEnd));
-    float e01 = 0, e12 = 0, e23 = 0;
-    cudaEventElapsedTime(&e01, ev[0], ev[1]);
-    cudaEventElapsedTime(&e12, ev[1], ev[2]);
-    cudaEventElapsedTime(&e23, ev[2], ev[3]);
-    fprintf(stderr, "[b2s_local_ba] device: structure kernels %.2f ms, LM kernel %.2f ms, D2H %.2f ms\n", e01, e12, e23);
-    for (auto& e : ev) cudaEventDestroy(e);
-  }
+  });
   return B2S_OK;
 }
 

@@ -153,3 +153,34 @@ def test_local_ba_pair_list_grows_in_reused_handle(pkg, oracle):
     for d, out in zip(batch, opt.LocalBundleAdjustmentBatch(batch)):
         _check(out, oracle.local_ba(d), d)
     _check(opt.LocalBundleAdjustment(ds[1]), oracle.local_ba(ds[1]), ds[1])
+
+
+def _num_sms():
+    import torch
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def _small_windows(n):
+    return [synth_local_ba(n_kf=5, n_fixed=1, n_mp=60, obs_per_mp=4, seed=100 + i) for i in range(n)]
+
+
+def test_local_ba_batch_larger_than_sms(pkg, oracle):
+    """More windows than SMs: one CTA per window, consecutive windows packed into ceil(batch / SMs) cooperative
+    launches; every window must still reproduce the oracle."""
+    ds = _small_windows(_num_sms() + 4)
+    opt = pkg.Optimizer(max_kf=8, max_mp=64, max_edges=512, max_batch=len(ds))
+    for d, out in zip(ds, opt.LocalBundleAdjustmentBatch(ds)):
+        _check(out, oracle.local_ba(d), d)
+
+
+@pytest.mark.parametrize("batch", ["1", "5", "sms+4"])
+def test_local_ba_launch_count(pkg, batch):
+    """Five structure kernels, then one cooperative LM launch per group of consecutive windows whose CTAs fit on the
+    SMs: one for a batch of at most one window per SM, ceil(batch / SMs) beyond that."""
+    sms = _num_sms()
+    nb = sms + 4 if batch == "sms+4" else int(batch)
+    ds = _small_windows(nb)
+    opt = pkg.Optimizer(max_kf=8, max_mp=64, max_edges=512, max_batch=nb)
+    before = opt.launch_count()
+    opt.LocalBundleAdjustmentBatch(ds)
+    assert opt.launch_count() - before == 5 + -(-nb // sms)

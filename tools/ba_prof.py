@@ -1,7 +1,6 @@
-"""One 32-window LocalBA batch (for ncu captures; B2S_BA_REPEAT=phase*256+count repeats one phase)."""
+"""One 32-window LocalBA batch (for ncu captures)."""
 import sys, time, importlib, os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
-os.environ.setdefault('B2S_DEBUG_TIMING', '1')
 from synth import synth_local_ba
 pkg = importlib.import_module('self_commit_orb-slam2_b200')
 d = synth_local_ba()

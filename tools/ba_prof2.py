@@ -1,8 +1,7 @@
-"""One batch of 32 DIFFERENT LocalBA windows (bench.py's set) with the per-phase cycle counters (B2S_DEBUG_TIMING=1)."""
+"""One batch of 32 DIFFERENT LocalBA windows (bench.py's set)."""
 import sys, time, importlib, os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
-os.environ.setdefault('B2S_DEBUG_TIMING', '1')
 import importlib.util
 spec = importlib.util.spec_from_file_location("bench", os.path.join(ROOT, "bench.py")); b = importlib.util.module_from_spec(spec); spec.loader.exec_module(b)
 pkg = importlib.import_module('self_commit_orb-slam2_b200')

@@ -1,6 +1,5 @@
 import sys, time, importlib, os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
-os.environ['B2S_DEBUG_TIMING']='1'
 from synth import synth_local_ba
 pkg=importlib.import_module('self_commit_orb-slam2_b200')
 d=synth_local_ba()

@@ -1,7 +1,6 @@
 #!/bin/bash
 mkdir -p tools/runs
 # ncu --set full capture of one kernel of the bench step (run from the repo root): tools/profile_kernel.sh k_tile
-# LocalBA phases: B2S_BA_REPEAT=$((phase*256+8)) tools/profile_kernel.sh k_local_ba   (phase 1 Schur, 2 build, 3 errors)
 k=${1:-k_tile}
 timeout 900 ncu --set full --import-source on --clock-control none -k regex:$k -s 1 -c 1 -f -o tools/runs/prof_$k \
     python bench.py --steps 1 --warmup 1 --e2e-steps 1 --no-cpu-baseline > tools/runs/ncu_$k.log 2>&1

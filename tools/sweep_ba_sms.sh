@@ -2,7 +2,7 @@
 mkdir -p tools/runs
 # bench.py (GPU arm only) for several SM budgets of the balanced LocalBA launch: tools/sweep_ba_sms.sh "48 64 80" [extra bench args]
 for s in $1; do
-  B2S_BA_SMS=$s timeout 300 python bench.py --no-cpu-baseline ${@:2} > tools/runs/sweep_sms$s.json 2> tools/runs/sweep_err.log
+  timeout 300 python bench.py --no-cpu-baseline --ba-sms $s ${@:2} > tools/runs/sweep_sms$s.json 2> tools/runs/sweep_err.log
   python - "$s" <<'PY'
 import json, sys
 s = sys.argv[1]
