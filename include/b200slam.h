@@ -33,7 +33,7 @@ enum {
   B2S_ERR_NO_DEVICE = 1,    /* no CUDA device / driver: the product does not fall back to the CPU */
   B2S_ERR_BAD_ARG = 2,
   B2S_ERR_CUDA = 3,         /* a CUDA call failed; b2s_last_error() has the text */
-  B2S_ERR_CAPACITY = 4,     /* caller buffer (cap) or an internal candidate buffer too small */
+  B2S_ERR_CAPACITY = 4,     /* caller buffer (cap) too small */
   B2S_ERR_ABORTED = 5       /* LocalBA: stop flag was set before the first round (no write-back) */
 };
 
@@ -55,7 +55,16 @@ typedef struct {
 /* ------------------------------------------------------------------ extractor */
 typedef struct b2s_extractor b2s_extractor;
 
-/* ctor: src/ORBextractor.cc:492-609. max_width/max_height/max_batch size the device buffers. */
+/* ctor: src/ORBextractor.cc:492-609. max_width/max_height/max_batch size the device buffers.
+ * Accepted parameters: nfeatures >= 1 (up to the quadtree's shared-memory limit, about 12,000 at 1.2 / 8 levels: above
+ * it B2S_ERR_BAD_ARG), scaleFactor > 1, nlevels 1..12, 1 <= minThFAST <= iniThFAST <= 254, max_width / max_height
+ * 64..8192, max_batch >= 1.
+ * Accepted images: width <= max_width, height <= max_height, and every pyramid level w_l x h_l
+ * (w_l = cvRound(width / scaleFactor^l)) at least 62 x 62 (one 30-px FAST cell inside the 16-px border; 221 x 221 for
+ * 8 levels at 1.2) with width >= about half the height.  Other images fail with B2S_ERR_BAD_ARG ("pyramid level l
+ * (w x h) is too small for the 30-px FAST cell grid"); the reference would still return the keypoints of the larger
+ * levels there.  Within that domain extraction succeeds for any image content: the internal candidate buffers are sized
+ * for the worst case; B2S_ERR_CAPACITY reports a record cap (`cap`) that is too small. */
 int b2s_extractor_create(int nfeatures, float scaleFactor, int nlevels, int iniThFAST, int minThFAST, int max_width,
                          int max_height, int max_batch, int device, b2s_extractor** out);
 void b2s_extractor_destroy(b2s_extractor* h);
@@ -98,6 +107,11 @@ int b2s_extractor_get_timing(b2s_extractor* h, double* stage_ms5, long long* cal
 int b2s_extractor_debug_level(b2s_extractor* h, int b, int level, int blurred, uint8_t* out, int* w, int* hgt);
 int b2s_extractor_debug_candidates(b2s_extractor* h, int b, int level, int32_t* xy /*2*cap*/, int32_t* resp, int cap,
                                    int* n);
+/* test hook, host only (needs no device): the per-image buffer sizes of a handle created for max_width x max_height and
+ * the pyramid / cell geometry of a width x height image in it.  out: 8 + 8 * nlevels entries (layout in extractor.cu);
+ * returns the status extraction of such an image would get from its geometry (B2S_OK or B2S_ERR_BAD_ARG). */
+int b2s_debug_extractor_plan(int nfeatures, float scaleFactor, int nlevels, int max_width, int max_height, int width,
+                             int height, int64_t* out);
 
 /* ------------------------------------------------------------------ stereo matching (SURVEY.md §8f rank 1) */
 /* Frame::ComputeStereoMatches (src/Frame.cc:1026-1421) for the stereo pairs of the batch this handle extracted last; the

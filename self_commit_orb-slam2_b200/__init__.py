@@ -349,10 +349,11 @@ class ORBextractor:
         return out
 
     def debug_candidates(self, b, level):
-        cap = 70000
+        n = ctypes.c_int(0)
+        _check(lib().b2s_extractor_debug_candidates(self._h, b, level, None, None, 0, ctypes.byref(n)))
+        cap = max(n.value, 1)
         xy = np.zeros((cap, 2), np.int32)
         resp = np.zeros(cap, np.int32)
-        n = ctypes.c_int(0)
         _check(lib().b2s_extractor_debug_candidates(self._h, b, level, _p(xy), _p(resp), cap, ctypes.byref(n)))
         return xy[:n.value].copy(), resp[:n.value].copy()
 

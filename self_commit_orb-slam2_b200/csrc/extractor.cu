@@ -30,6 +30,9 @@ __constant__ int c_umax[16];
 constexpr int FP = 80;   // byte pitch of the raw ROI / score map (ROI width <= 66, + alignment slack)
 constexpr int FR = 68;   // max ROI rows
 constexpr int PW = 40;   // word pitch of the packed pixel-pair planes (<= 38 pair words per row, even => 8-byte stores)
+// a cell's detectable area is at most 60 x 62 (plan_geometry) and its strict 3x3 maxima take one pixel of each 2x2
+// block at most, so the survivor list of fast_cell never overflows
+static_assert(((60 + 1) / 2) * ((FR - 6 + 1) / 2) <= kFastCellCap, "fast_cell survivor list");
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void sts_v2(uint32_t a, uint32_t x, uint32_t y) {
@@ -895,8 +898,43 @@ static size_t quadtree_smem_bytes(int cap) {
   return (size_t)cap * (8 + 16 + 16 + 4 * 5 + 2 * 4 + 2 * 8 + 2) + 64;
 }
 
-// Builds per-level geometry for a WxH image and (re)uploads the resize tables.
-static int build_geometry(b2s_extractor* h, int W, int H) {
+// Level size (:1680-1682) and 30-px FAST cell grid (:1064-1086) of a WxH image at inverse scale s.  A level too small
+// for the grid gets nCols or nRows <= 0.
+static void level_grid(int W, int H, float s, LevelGeom& L) {
+  L.w = cv_roundf((float)W * s);
+  L.h = cv_roundf((float)H * s);
+  L.maxBX = L.w - kEdge + 3;
+  L.maxBY = L.h - kEdge + 3;
+  const float width = (float)(L.maxBX - kMinBorder), height = (float)(L.maxBY - kMinBorder);
+  L.nCols = (int)(width / 30.f);
+  L.nRows = (int)(height / 30.f);
+  L.wCell = L.nCols > 0 ? (int)ceilf(width / L.nCols) : 0;
+  L.hCell = L.nRows > 0 ? (int)ceilf(height / L.nRows) : 0;
+}
+
+// Sum over the n cells of one grid row (or column) of ceil(d / 2), d = the extent of the cell's detectable area; cells
+// the reference skips (:1099 with margin 3, :1116 with margin 6) count 0.  A strict 3x3 maximum of the cell NMS takes at
+// most one pixel of each 2x2 block inside a cell, and the NMS never looks across a seam, so (column sum) x (row sum)
+// bounds a level's candidates whatever the texture.  (ceil(band / 2) over the whole band is NOT a bound: two cells can
+// both keep a maximum on their common seam.)
+static int half_span_sum(int n, int cell, int maxB, int skipMargin) {
+  int s = 0;
+  for (int j = 0; j < n; j++) {
+    const int ini = kMinBorder + j * cell;
+    if (ini >= maxB - skipMargin) break;
+    const int mx = std::min(ini + cell + 6, maxB);
+    if (mx - ini >= 7) s += (mx - ini - 6 + 1) / 2;
+  }
+  return s;
+}
+static int cand_bound(const LevelGeom& L) {
+  return half_span_sum(L.nCols, L.wCell, L.maxBX, 6) * half_span_sum(L.nRows, L.hCell, L.maxBY, 3);
+}
+
+// Builds per-level geometry for a WxH image (host arithmetic only) and checks it against the handle's allocations; the
+// resize tables and the cell list go to the vectors for build_geometry to upload.
+static int plan_geometry(b2s_extractor* h, int W, int H, std::vector<int16_t>& rxOfs, std::vector<uint32_t>& rxAlpha,
+                         std::vector<int16_t>& ryOfs, std::vector<uint32_t>& ryBeta, std::vector<uint32_t>& info) {
   ExtractGeom& g = h->geom;
   memset(&g, 0, sizeof(g));
   g.nlevels = h->nlevels;
@@ -905,27 +943,18 @@ static int build_geometry(b2s_extractor* h, int W, int H) {
   uint32_t off = 0;
   int cellStart = 0, candOff = 0, selOff = 0;
   uint32_t rxOff = 0, ryOff = 0;
-  std::vector<int16_t> rxOfs, ryOfs;
-  std::vector<uint32_t> rxAlpha, ryBeta;
   for (int l = 0; l < g.nlevels; l++) {
     LevelGeom& L = g.lv[l];
-    const float s = h->invScale[l];
-    L.w = cv_roundf((float)W * s);  // :1680-1682
-    L.h = cv_roundf((float)H * s);
+    level_grid(W, H, h->invScale[l], L);
     L.pitch = (int)align_up((size_t)L.w, 16);
     L.off = off;
     off += (uint32_t)align_up((size_t)L.pitch * L.h, 256);
-    L.maxBX = L.w - kEdge + 3;
-    L.maxBY = L.h - kEdge + 3;
-    const float width = (float)(L.maxBX - kMinBorder), height = (float)(L.maxBY - kMinBorder);
-    L.nCols = (int)(width / 30.f);
-    L.nRows = (int)(height / 30.f);
     if (L.nCols <= 0 || L.nRows <= 0) {
       set_error("pyramid level %d (%dx%d) is too small for the 30-px FAST cell grid", l, L.w, L.h);
       return B2S_ERR_BAD_ARG;
     }
-    L.wCell = (int)ceilf(width / L.nCols);
-    L.hCell = (int)ceilf(height / L.nRows);
+    const float width = (float)(L.maxBX - kMinBorder), height = (float)(L.maxBY - kMinBorder);
+    // (nCols = floor(width / 30) gives wCell <= 60; hCell <= 60 likewise: never refused, kept as the kernels' limits)
     if (L.wCell + 6 > 66 || L.hCell + 6 > FR || L.wCell > 63 || L.hCell > 63) {
       set_error("cell %dx%d at level %d exceeds the kernel tile", L.wCell, L.hCell, l);
       return B2S_ERR_BAD_ARG;
@@ -939,9 +968,14 @@ static int build_geometry(b2s_extractor* h, int W, int H) {
       return B2S_ERR_BAD_ARG;
     }
     L.hX = width / L.nIni;
-    L.candCap = std::min(65535, std::max(1024, (L.w * L.h) / 10));
+    L.candCap = cand_bound(L);
     L.candOff = candOff;
     candOff += (int)align_up((size_t)L.candCap, 64);
+    // k_cells: whole cells per CTA such that their maxima fit its shared list (>= 8: a cell is at most 60 x 60), the
+    // row split into equal column ranges
+    const int maxPerCta = std::min(kCellsMaxCols, kCellsListCap / (((L.wCell + 1) / 2) * ((L.hCell + 1) / 2)));
+    L.nChunks = div_up(L.nCols, maxPerCta);
+    L.cellsPerCta = div_up(L.nCols, L.nChunks);
     L.nodeCap = (int)align_up((size_t)std::max(L.N + 4, 4 * L.nIni), 8);
     L.selOff = selOff;
     selOff += L.nodeCap;
@@ -976,17 +1010,14 @@ static int build_geometry(b2s_extractor* h, int W, int H) {
   }
   g.pyrBytes = off;
   g.totalCells = cellStart;
-  {
-    std::vector<uint32_t> info(cellStart);
-    for (int l = 0; l < g.nlevels; l++)
-      for (int ci = 0; ci < g.lv[l].nRows; ci++)
-        for (int cj = 0; cj < g.lv[l].nCols; cj++)
-          info[g.lv[l].cellStart + ci * g.lv[l].nCols + cj] = ((uint32_t)l << 28) | ((uint32_t)ci << 14) | (uint32_t)cj;
-    if ((size_t)cellStart > h->cellAlloc) {
-      set_error("image %dx%d needs %d FAST cells, more than allocated", W, H, cellStart);
-      return B2S_ERR_BAD_ARG;
-    }
-    B2S_CUDA(cudaMemcpy(h->d.cellInfo, info.data(), info.size() * 4, cudaMemcpyHostToDevice));
+  info.assign(cellStart, 0u);
+  for (int l = 0; l < g.nlevels; l++)
+    for (int ci = 0; ci < g.lv[l].nRows; ci++)
+      for (int cj = 0; cj < g.lv[l].nCols; cj++)
+        info[g.lv[l].cellStart + ci * g.lv[l].nCols + cj] = ((uint32_t)l << 28) | ((uint32_t)ci << 14) | (uint32_t)cj;
+  if ((size_t)cellStart > h->cellAlloc) {
+    set_error("image %dx%d needs %d FAST cells, more than allocated", W, H, cellStart);
+    return B2S_ERR_BAD_ARG;
   }
   g.totalCandCap = candOff;
   g.totalSelCap = selOff;
@@ -995,6 +1026,25 @@ static int build_geometry(b2s_extractor* h, int W, int H) {
     set_error("image %dx%d exceeds the extractor's max_width/max_height (%dx%d)", W, H, h->maxW, h->maxH);
     return B2S_ERR_BAD_ARG;
   }
+  int capMax = 0;
+  for (int l = 0; l < g.nlevels; l++) capMax = std::max(capMax, g.lv[l].nodeCap);
+  if (quadtree_smem_bytes(capMax) > 220 * 1024) {
+    set_error("quadtree node capacity %d needs %zu B of shared memory", capMax, quadtree_smem_bytes(capMax));
+    return B2S_ERR_BAD_ARG;
+  }
+  return B2S_OK;
+}
+
+// Builds the geometry of a WxH image and uploads its tables.  Until it succeeds the handle has no current size, so a
+// refused image never leaves a half-built geometry behind for the next call.
+static int build_geometry(b2s_extractor* h, int W, int H) {
+  h->curW = h->curH = 0;
+  std::vector<int16_t> rxOfs, ryOfs;
+  std::vector<uint32_t> rxAlpha, ryBeta, info;
+  const int rc0 = plan_geometry(h, W, H, rxOfs, rxAlpha, ryOfs, ryBeta, info);
+  if (rc0 != B2S_OK) return rc0;
+  const ExtractGeom& g = h->geom;
+  B2S_CUDA(cudaMemcpy(h->d.cellInfo, info.data(), info.size() * 4, cudaMemcpyHostToDevice));
   if (!rxOfs.empty()) {
     B2S_CUDA(cudaMemcpyAsync(h->d.rxOfs, rxOfs.data(), rxOfs.size() * 2, cudaMemcpyHostToDevice, h->stream));
     B2S_CUDA(cudaMemcpyAsync(h->d.rxAlpha, rxAlpha.data(), rxAlpha.size() * 4, cudaMemcpyHostToDevice, h->stream));
@@ -1006,10 +1056,6 @@ static int build_geometry(b2s_extractor* h, int W, int H) {
     int capMax = 0;
     for (int l = 0; l < g.nlevels; l++) capMax = std::max(capMax, g.lv[l].nodeCap);
     const size_t qsm = quadtree_smem_bytes(capMax);
-    if (qsm > 220 * 1024) {
-      set_error("quadtree node capacity %d needs %zu B of shared memory", capMax, qsm);
-      return B2S_ERR_BAD_ARG;
-    }
     B2S_CUDA(cudaFuncSetAttribute(k_quadtree, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(qsm, (size_t)49152)));
   }
   {
@@ -1377,6 +1423,107 @@ extern "C" int b2s_extractor_get_timing(b2s_extractor* h, double* stage_ms5, lon
   return B2S_OK;
 }
 
+// scale tables and per-level quotas — src/ORBextractor.cc:500-554 (from h->nfeatures, nlevels, scaleFactor)
+static void init_tables(b2s_extractor* h) {
+  const int nlevels = h->nlevels;
+  h->scale.resize(nlevels);
+  h->sigma2.resize(nlevels);
+  h->scale[0] = 1.0f;
+  h->sigma2[0] = 1.0f;
+  for (int i = 1; i < nlevels; i++) {
+    h->scale[i] = (float)(h->scale[i - 1] * h->scaleFactor);
+    h->sigma2[i] = h->scale[i] * h->scale[i];
+  }
+  h->invScale.resize(nlevels);
+  h->invSigma2.resize(nlevels);
+  for (int i = 0; i < nlevels; i++) {
+    h->invScale[i] = 1.0f / h->scale[i];
+    h->invSigma2[i] = 1.0f / h->sigma2[i];
+  }
+  h->nFeat.resize(nlevels);
+  float factor = (float)(1.0f / h->scaleFactor);
+  float nDesired = h->nfeatures * (1 - factor) / (1 - (float)pow((double)factor, (double)nlevels));
+  int sum = 0;
+  for (int l = 0; l < nlevels - 1; l++) {
+    h->nFeat[l] = cv_roundf(nDesired);
+    sum += h->nFeat[l];
+    nDesired *= factor;
+  }
+  h->nFeat[nlevels - 1] = std::max(h->nfeatures - sum, 0);
+}
+
+// Per-image buffer sizes for images up to maxW x maxH, from the geometry arithmetic itself (no device access).  Level
+// sizes grow monotonically with the image size, and so do the cell grid (nCols = floor((w - 32) / 30)) and the tile
+// grid, so the largest image bounds every smaller one.  Candidates: plan_geometry gives each level its exact bound
+// cand_bound, which is not monotonic in the size; the allocation uses a monotonic bound of it.
+static void size_buffers(b2s_extractor* h) {
+  size_t pyrBytes = 0, candCap = 0, selCap = 0, rx = 0, ry = 0, cells = 0, bmWords = 0, tiles = 0;
+  for (int l = 0; l < h->nlevels; l++) {
+    LevelGeom L;
+    level_grid(h->maxW, h->maxH, h->invScale[l], L);
+    pyrBytes += align_up(align_up((size_t)L.w, 16) * L.h, 256);
+    // cand_bound's column sum adds ceil(d / 2) over at most nCols cells whose extents d sum to at most w - 38, so it is
+    // <= (w - 38 + nCols) / 2, which grows with w (rows alike)
+    const size_t colHalf = (size_t)std::max(L.w - 2 * kEdge + std::max(L.nCols, 0), 0) / 2;
+    const size_t rowHalf = (size_t)std::max(L.h - 2 * kEdge + std::max(L.nRows, 0), 0) / 2;
+    candCap += align_up(colHalf * rowHalf, 64);
+    // quadtree nodes: plan_geometry's nodeCap = max(N + 4, 4 * nIni), nIni = round(width / height) with height >= 30
+    const int nIniMax = std::max(1, (int)roundf((float)std::max(L.w - 2 * kMinBorder, 0) / 30.f));
+    selCap += align_up((size_t)std::max({h->nFeat[l] + 4, 4 * nIniMax, 64}), 8);
+    if (l > 0) {
+      rx += L.w;
+      ry += L.h;
+    }
+    cells += (size_t)std::max(L.nCols, 0) * (size_t)std::max(L.nRows, 0);
+    bmWords += (size_t)(div_up(L.w, 128) * 4) * (size_t)(div_up(L.h, 32) * 32);  // tile_build: per 128 x 32 tile 4 x 32 words
+    tiles = std::max(tiles, (size_t)(div_up(L.w, 128) + div_up(L.h, 32) + 2));
+  }
+  h->pyrBytesAlloc = pyrBytes + 4096;  // (slack for the 256-byte level alignment of smaller images)
+  h->candCapAlloc = candCap;
+  h->selCapAlloc = selCap + 64 * h->nlevels;
+  h->rxAlloc = rx + 16;
+  h->ryAlloc = ry + 16;
+  h->cellAlloc = cells;
+  h->bmWordsAlloc = bmWords;
+  h->tileTabAlloc = tiles * h->nlevels;
+  h->outCap = h->nfeatures + 4 * h->nlevels + 16;
+}
+
+/* test hook, host only (no device): the buffer sizes b2s_extractor_create gives a handle for max_width x max_height and
+ * the geometry of a width x height image in it.  out[0..7]: candidate entries allocated / needed per image, FAST cells
+ * allocated / needed, NMS bitmap words allocated, k_cells list capacity, k_cells cell columns per CTA at most,
+ * k_fast_cells_list maxima per cell; then per level 8 entries: w, h, nCols, nRows, wCell, hCell, candCap, cellsPerCta.
+ * Returns plan_geometry's status (B2S_ERR_BAD_ARG with b2s_last_error() for a refused image). */
+extern "C" int b2s_debug_extractor_plan(int nfeatures, float scaleFactor, int nlevels, int max_width, int max_height, int width,
+                                        int height, int64_t* out) {
+  if (!out || nfeatures <= 0 || nlevels < 1 || nlevels > kMaxLevels || !(scaleFactor > 1.0f)) return B2S_ERR_BAD_ARG;
+  b2s_extractor h;
+  h.nfeatures = nfeatures;
+  h.nlevels = nlevels;
+  h.iniTh = 20;
+  h.minTh = 7;
+  h.scaleFactor = scaleFactor;
+  h.maxW = max_width;
+  h.maxH = max_height;
+  h.maxBatch = 1;
+  h.device = 0;
+  init_tables(&h);
+  size_buffers(&h);
+  std::vector<int16_t> rxOfs, ryOfs;
+  std::vector<uint32_t> rxAlpha, ryBeta, info;
+  const int rc = plan_geometry(&h, width, height, rxOfs, rxAlpha, ryOfs, ryBeta, info);
+  const ExtractGeom& g = h.geom;
+  const int64_t head[8] = {(int64_t)h.candCapAlloc, g.totalCandCap, (int64_t)h.cellAlloc, g.totalCells, (int64_t)h.bmWordsAlloc,
+                           kCellsListCap, kCellsMaxCols, kFastCellCap};
+  for (int k = 0; k < 8; k++) out[k] = head[k];
+  for (int l = 0; l < nlevels; l++) {
+    const LevelGeom& L = g.lv[l];
+    const int64_t v[8] = {L.w, L.h, L.nCols, L.nRows, L.wCell, L.hCell, L.candCap, L.cellsPerCta};
+    for (int k = 0; k < 8; k++) out[8 + 8 * l + k] = v[k];
+  }
+  return rc;
+}
+
 extern "C" int b2s_extractor_create(int nfeatures, float scaleFactor, int nlevels, int iniThFAST, int minThFAST,
                                     int max_width, int max_height, int max_batch, int device, b2s_extractor** out) {
   if (!out) return B2S_ERR_BAD_ARG;
@@ -1407,61 +1554,15 @@ extern "C" int b2s_extractor_create(int nfeatures, float scaleFactor, int nlevel
   h->maxH = max_height;
   h->maxBatch = max_batch;
   h->device = device;
-  // scale tables and per-level quotas — src/ORBextractor.cc:500-554
-  h->scale.resize(nlevels);
-  h->sigma2.resize(nlevels);
-  h->scale[0] = 1.0f;
-  h->sigma2[0] = 1.0f;
-  for (int i = 1; i < nlevels; i++) {
-    h->scale[i] = (float)(h->scale[i - 1] * h->scaleFactor);
-    h->sigma2[i] = h->scale[i] * h->scale[i];
-  }
-  h->invScale.resize(nlevels);
-  h->invSigma2.resize(nlevels);
-  for (int i = 0; i < nlevels; i++) {
-    h->invScale[i] = 1.0f / h->scale[i];
-    h->invSigma2[i] = 1.0f / h->sigma2[i];
-  }
-  h->nFeat.resize(nlevels);
-  {
-    float factor = (float)(1.0f / h->scaleFactor);
-    float nDesired = nfeatures * (1 - factor) / (1 - (float)pow((double)factor, (double)nlevels));
-    int sum = 0;
-    for (int l = 0; l < nlevels - 1; l++) {
-      h->nFeat[l] = cv_roundf(nDesired);
-      sum += h->nFeat[l];
-      nDesired *= factor;
-    }
-    h->nFeat[nlevels - 1] = std::max(nfeatures - sum, 0);
-  }
+  init_tables(h);
   if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess ||
       cudaStreamCreateWithFlags(&h->stream2, cudaStreamNonBlocking) != cudaSuccess) {
     set_error("cudaStreamCreate failed");
     delete h;
     return B2S_ERR_CUDA;
   }
-  // compute sizes without touching the device: replicate the size arithmetic
-  size_t pyrBytes = 0, candCap = 0, selCap = 0, rx = 0, ry = 0;
-  for (int l = 0; l < nlevels; l++) {
-    const int w = cv_roundf((float)max_width * h->invScale[l]), hh = cv_roundf((float)max_height * h->invScale[l]);
-    pyrBytes += align_up(align_up((size_t)w, 16) * hh, 256);
-    candCap += align_up((size_t)std::min(65535, std::max(1024, (w * hh) / 10)), 64);
-    selCap += align_up((size_t)std::max(h->nFeat[l] + 4, 64), 8);
-    if (l > 0) {
-      rx += w;
-      ry += hh;
-    }
-  }
-  // slack so that smaller images with different rounding still fit
-  pyrBytes += 4096;
-  candCap += 64 * nlevels;
-  selCap += 64 * nlevels;
-  h->pyrBytesAlloc = pyrBytes;
-  h->candCapAlloc = candCap;
-  h->selCapAlloc = selCap;
-  h->rxAlloc = rx + 16;
-  h->ryAlloc = ry + 16;
-  h->outCap = nfeatures + 4 * nlevels + 16;
+  size_buffers(h);
+  const size_t candCap = h->candCapAlloc, selCap = h->selCapAlloc, pyrBytes = h->pyrBytesAlloc;
   DeviceBuffers& d = h->d;
   const size_t B = (size_t)max_batch;
   cudaError_t e = cudaSuccess;
@@ -1471,16 +1572,7 @@ extern "C" int b2s_extractor_create(int nfeatures, float scaleFactor, int nlevel
   A((void**)&d.pyr, B * pyrBytes);
   A((void**)&d.blur, B * pyrBytes);
   A((void**)&d.score, B * pyrBytes);
-  {
-    size_t bw = 0;  // per level: rows padded to 32, 4 words per 128 columns
-    for (int l = 0; l < nlevels; l++) {
-      const int w = cv_roundf((float)max_width * h->invScale[l]), hh = cv_roundf((float)max_height * h->invScale[l]);
-      bw += (size_t)(div_up(w + 1, 128) * 4) * (size_t)(div_up(hh + 1, 32) * 32);
-    }
-    h->bmWordsAlloc = bw + 1024;
-  }
   A((void**)&d.bitmap, B * h->bmWordsAlloc * 4);
-  h->tileTabAlloc = (size_t)nlevels * (size_t)(div_up(max_width, 32) + div_up(max_height, 32) + 8);
   A((void**)&d.tileDx, h->tileTabAlloc * 2);
   A((void**)&d.tileDy, h->tileTabAlloc * 2);
   if (max_batch > 1) A((void**)&d.raw, B * (size_t)max_width * max_height + 64);  // dense upload staging (batch path)
@@ -1493,7 +1585,6 @@ extern "C" int b2s_extractor_create(int nfeatures, float scaleFactor, int nlevel
   A((void**)&d.selXYR, B * selCap * 8);
   A((void**)&d.selCount, B * kMaxLevels * 4);
   A((void**)&d.status, 4);
-  h->cellAlloc = (size_t)(div_up(max_width, 28) + 2) * (size_t)(div_up(max_height, 28) + 2) * 4 + 64;
   A((void**)&d.cellInfo, h->cellAlloc * 4);
   A((void**)&d.fbList, B * h->cellAlloc * sizeof(uint2));
   A((void**)&d.fbCount, B * 4);  // one counter per possible first image of a chunk (chunks of a batch run on two streams)

@@ -22,7 +22,9 @@ struct LevelGeom {
   int N;                  // mnFeaturesPerLevel[level]
   int nIni;               // quadtree roots (:719)
   float hX;               // root width (:722)
-  int candCap, candOff;   // candidate capacity / offset (entries) inside one image's candidate arrays
+  int candCap, candOff;   // candidate capacity (the level's exact maximum, cand_bound) / offset (entries) inside one
+                          // image's candidate arrays
+  int cellsPerCta, nChunks;  // k_cells: cell columns per CTA (their NMS maxima always fit its list) and CTAs per row
   int nodeCap, selOff;    // quadtree node capacity / offset of the level's selected keypoints
   float scale;            // mvScaleFactor[level]
   float kpsize;           // (float)(int)(PATCH_SIZE*scale) (:1175,1189)
@@ -79,6 +81,9 @@ int tile_build(b2s_extractor* h);  // tensor maps + resize ownership tables for 
 int tile_run(b2s_extractor* h, int bBase, int batch, cudaStream_t st);
 int launch_fast_fallback(const ExtractGeom& g, const DeviceBuffers& d, const uint2* fbList, const int32_t* fbCount, int gridCtas,
                          cudaStream_t st);  // extractor.cu
+constexpr int kCellsListCap = 8192;  // k_cells: NMS maxima one CTA collects in shared memory (extractor_tile.cu)
+constexpr int kCellsMaxCols = 64;    // k_cells: cell columns one CTA owns at most
+constexpr int kFastCellCap = 1024;   // k_fast_cells_list: maxima of one cell it keeps in shared memory (extractor.cu)
 }  // namespace b2s
 
 struct b2s_extractor {

@@ -57,8 +57,8 @@ struct TileSmem {
   uint16_t candList[CAND_CAP];              // interior pixels with M > iniThFAST (offset into scoreP)
   alignas(8) unsigned long long bar;        // mbarrier of the tile load
   int nPass, nCand;
-  uint32_t rzB[32];                         // per destination row of the tile: vertical weights b0 | b1 << 16
-  int16_t rzO0[32], rzO1[32];               // ... and the box rows of its two source rows
+  uint32_t rzB[TH + 2];                     // per destination row of the tile: vertical weights b0 | b1 << 16
+  int16_t rzO0[TH + 2], rzO1[TH + 2];       // ... and the box rows of its two source rows
   uint8_t colFlag[TW], rowFlag[TH];         // per interior column / row: bit0 = in the FAST band, bit1 = the left / upper
                                             // neighbour is in the same cell, bit2 = the right / lower neighbour is
 };
@@ -444,7 +444,9 @@ __global__ void __launch_bounds__(TILE_THREADS) k_tile(const __grid_constant__ C
     const LevelGeom& D = g.lv[a.level + 1];
     const int16_t* tdx = a.tileDx + L.tdxOff;
     const int16_t* tdy = a.tileDy + L.tdyOff;
-    const int dx0 = tdx[tx], nw = tdx[tx + 1] - dx0, dy0 = tdy[ty], nh = tdy[ty + 1] - dy0;  // nw <= 108, nh <= 28
+    const int dx0 = tdx[tx], nw = tdx[tx + 1] - dx0, dy0 = tdy[ty], nh = tdy[ty + 1] - dy0;
+    // (nw <= TW and nh <= TH + 1: tile_build refuses scale factors so close to 1 that a tile would own more; at 1.1 a
+    // tile owns up to 117 columns)
     if (tid < nh) {  // row parameters once per tile
       const int dy = dy0 + tid;
       const int sy = a.ryOfs[D.ryOff + dy];
@@ -457,7 +459,8 @@ __global__ void __launch_bounds__(TILE_THREADS) k_tile(const __grid_constant__ C
     // column, h = S[sx] * a0 + S[sx + 1] * a1 (>> 4 as the vertical stage wants it); the buffer reuses the blur's
     // horizontal sums (the blur is finished: barrier above)
     uint16_t* hb = S.blurH;  // [row of the box][destination column], pitch RZP
-    constexpr int RZP = 112;
+    constexpr int RZP = TW + 2;  // >= nw; box rows <= HY + TH, so the rows fit the blur's horizontal-sum buffer
+    static_assert((HY + TH) * RZP + TW + 1 < BH * TW, "resize rows fit blurH");
     {
       const int rowLo = nh > 0 ? S.rzO0[0] : 0, rowHi = nh > 0 ? S.rzO1[nh - 1] : -1;  // box rows
       const int c = tid & 127;
@@ -510,10 +513,13 @@ __global__ void __launch_bounds__(TILE_THREADS) k_tile(const __grid_constant__ C
 // minThFAST; a cell falls back to minThFAST only if it has no maximum above iniThFAST.
 // The detectable areas of a level's cells tile [19, maxBorderX-3) x [19, maxBorderY-3) without gaps (cell j owns
 // x in [19 + j*wCell, 19 + (j+1)*wCell)); cells the reference skips (:1099, :1116) own no pixel of that band.
-// The strip is swept 4 pixels per load with a SWAR threshold test; only pixels above minThFAST reach the NMS.
+// A row of cells is split by column range over L.nChunks CTAs of L.cellsPerCta cells: a strict 3x3 maximum of a cell
+// occupies at most one pixel of each 2x2 block, so one CTA collects at most cellsPerCta * ceil(wCell/2) * ceil(hCell/2)
+// <= CL_CAP maxima whatever the texture (build_geometry picks cellsPerCta).  The emission order does not matter: the
+// quadtree orders candidates by candKey.
 // ------------------------------------------------------------------------------------------------
-constexpr int CL_CAP = 8192;  // NMS survivors of one row of cells (a level-0 KITTI row: ~39 k pixels, survivors <= 1/4)
-constexpr int CL_MAXCOLS = 320;
+constexpr int CL_CAP = kCellsListCap;
+constexpr int CL_MAXCOLS = kCellsMaxCols;
 
 __global__ void __launch_bounds__(256) k_cells(const __grid_constant__ ExtractGeom g, const uint8_t* __restrict__ score,
                                                const uint32_t* __restrict__ bitmap, uint32_t* __restrict__ candXY,
@@ -525,21 +531,24 @@ __global__ void __launch_bounds__(256) k_cells(const __grid_constant__ ExtractGe
   __shared__ int sN, sBase, sEmit, sTotal;
   const int tid = threadIdx.x;
   const int b = blockIdx.y;
-  int l = 0, ci = blockIdx.x;
-  while (l < g.nlevels && ci >= g.lv[l].nRows) ci -= g.lv[l++].nRows;
+  int l = 0, k0 = blockIdx.x;  // CTA index -> (level, row of cells, column chunk)
+  while (l < g.nlevels && k0 >= g.lv[l].nRows * g.lv[l].nChunks) {
+    k0 -= g.lv[l].nRows * g.lv[l].nChunks;
+    l++;
+  }
   if (l >= g.nlevels) return;
   const LevelGeom& L = g.lv[l];
+  const int ci = k0 / L.nChunks, chunk = k0 - ci * L.nChunks;
+  const int cj0 = chunk * L.cellsPerCta, nc = min(L.nCols - cj0, L.cellsPerCta);  // cell columns [cj0, cj0 + nc)
   const int iniY = kMinBorder + ci * L.hCell;
   if (iniY >= L.maxBY - 3) return;  // :1099
   const int maxY = min(iniY + L.hCell + 6, L.maxBY);
   if (maxY - iniY < 7) return;
   const int ay0 = iniY + 3, ay1 = maxY - 3;          // detectable rows of this row of cells
   const int ax0 = kMinBorder + 3, ax1 = L.maxBX - 3;  // detectable columns of the level
-  if (ax1 <= ax0 || L.nCols > CL_MAXCOLS) {
-    if (L.nCols > CL_MAXCOLS && tid == 0) atomicOr(status, 1);
-    return;
-  }
-  for (int k = tid; k < L.nCols; k += 256) {
+  if (ax1 <= ax0) return;
+  const int x0 = ax0 + cj0 * L.wCell, x1 = min(ax1, ax0 + (cj0 + nc) * L.wCell);  // this CTA's detectable columns
+  for (int k = tid; k < nc; k += 256) {
     cellAll[k] = 0;
     cellHi[k] = 0;
   }
@@ -553,19 +562,22 @@ __global__ void __launch_bounds__(256) k_cells(const __grid_constant__ ExtractGe
   const int iniTh = g.iniTh;
   // the tile kernel left one bit per pixel: "maximum of its cell above minThFAST" (row = tilesX*4 words; per 64 pixels an
   // even-pixel word and an odd-pixel word)
+  // (this CTA reads the words of the 64-pixel groups that overlap [x0, x1) and keeps the bits inside it)
   const int bmPitch = L.tilesX * 4, ah = ay1 - ay0;
-  const uint32_t* bm = bitmap + (size_t)b * g.bmWords + L.bmOff + (size_t)ay0 * bmPitch;
-  for (int k = tid; k < bmPitch * ah; k += 256) {
-    uint32_t bits = bm[k];
+  const int wLo = (x0 >> 6) * 2, nw = x1 > x0 ? ((x1 - 1) >> 6) * 2 + 2 - wLo : 0;
+  const uint32_t* bm = bitmap + (size_t)b * g.bmWords + L.bmOff + (size_t)ay0 * bmPitch + wLo;
+  for (int k = tid; k < nw * ah; k += 256) {
+    const int r = k / nw, wi = k - r * nw;
+    uint32_t bits = bm[(size_t)r * bmPitch + wi];
     if (!bits) continue;
-    const int r = k / bmPitch, wi = k - r * bmPitch;
-    const int xBase = (wi >> 1) * 64 + (wi & 1);
+    const int xBase = ((wLo + wi) >> 1) * 64 + (wi & 1);
     while (bits) {
       const int bi = __ffs(bits) - 1;
       bits &= bits - 1;
       const int x = xBase + 2 * bi;
+      if (x < x0 || x >= x1) continue;
       const int M = img[(size_t)(ay0 + r) * pitch + x];
-      const int cj = (x - ax0) / wCell;
+      const int cj = (x - ax0) / wCell - cj0;
       const int slot = atomicAdd(&sN, 1);
       if (slot < CL_CAP) list[slot] = (uint32_t)x | ((uint32_t)r << 13) | ((uint32_t)M << 19);
       atomicAdd(&cellAll[cj], 1);
@@ -573,20 +585,22 @@ __global__ void __launch_bounds__(256) k_cells(const __grid_constant__ ExtractGe
     }
   }
   __syncthreads();
-  if (tid < 32) {  // candidates this row of cells emits: per cell the maxima above iniThFAST if it has any, else all
+  if (tid < 32) {  // candidates these cells emit: per cell the maxima above iniThFAST if it has any, else all
     int t = 0;
-    for (int k = tid; k < L.nCols; k += 32) t += cellHi[k] > 0 ? cellHi[k] : cellAll[k];
+    for (int k = tid; k < nc; k += 32) t += cellHi[k] > 0 ? cellHi[k] : cellAll[k];
     t = warp_reduce_sum(t);
     if (tid == 0) {
       sTotal = t;
       sBase = t ? atomicAdd(&candCount[b * kMaxLevels + l], t) : 0;
+      // (neither can happen: CL_CAP and candCap hold the geometric maximum; kept so that a sizing bug is an error)
       if (sN > CL_CAP || (t && sBase + t > L.candCap)) atomicOr(status, 1);
     }
   }
   __syncthreads();
-  // cells of this row without a maximum above iniThFAST: the minThFAST pass re-does them (k_fast_cells_list)
-  for (int cj = tid; cj < L.nCols; cj += 256) {
-    if (cellHi[cj] > 0 || kMinBorder + cj * wCell >= L.maxBX - 6) continue;
+  // cells without a maximum above iniThFAST: the minThFAST pass re-does them (k_fast_cells_list)
+  for (int c = tid; c < nc; c += 256) {
+    const int cj = cj0 + c;
+    if (cellHi[c] > 0 || kMinBorder + cj * wCell >= L.maxBX - 6) continue;
     const int slot = atomicAdd(fbCount, 1);
     fbList[slot] = make_uint2((uint32_t)(bAbs + b), (uint32_t)(L.cellStart + ci * L.nCols + cj));
   }
@@ -597,7 +611,7 @@ __global__ void __launch_bounds__(256) k_cells(const __grid_constant__ ExtractGe
     const uint32_t e = list[k];
     const int x = e & 0x1fff, r = (e >> 13) & 0x3f, M = e >> 19;
     const int cj = (x - ax0) / wCell;
-    if (cellHi[cj] > 0 && M <= iniTh) continue;  // :1132-1139
+    if (cellHi[cj - cj0] > 0 && M <= iniTh) continue;  // :1132-1139
     const int slot = sBase + atomicAdd(&sEmit, 1);
     if (slot >= L.candCap) continue;
     // kp.pt += (j*wCell, i*hCell) (:1150-1151) -> coordinates relative to the 16-pixel border
@@ -691,6 +705,22 @@ int tile_build(b2s_extractor* h) {
     }
   }
   g.bmWords = bmWords;
+  // k_tile resizes with one thread per destination column a tile owns (at most TW) and keeps TH + 2 rows of parameters
+  for (int l = 0; l + 1 < g.nlevels; l++) {
+    const LevelGeom& L = g.lv[l];
+    for (int t = 0; t < L.tilesX; t++)
+      if (tdx[L.tdxOff + t + 1] - tdx[L.tdxOff + t] > TW) {
+        set_error("scale factor %.6f is too close to 1: a 128-column tile of level %d owns more than 128 columns of level %d",
+                  h->scaleFactor, l, l + 1);
+        return B2S_ERR_BAD_ARG;
+      }
+    for (int t = 0; t < L.tilesY; t++)
+      if (tdy[L.tdyOff + t + 1] - tdy[L.tdyOff + t] > TH + 2) {
+        set_error("scale factor %.6f is too close to 1: a 32-row tile of level %d owns more than 34 rows of level %d",
+                  h->scaleFactor, l, l + 1);
+        return B2S_ERR_BAD_ARG;
+      }
+  }
   if ((size_t)bmWords > h->bmWordsAlloc) {
     set_error("NMS bitmap (%u words per image) exceeds its allocation", bmWords);
     return B2S_ERR_BAD_ARG;
@@ -739,9 +769,9 @@ int tile_run(b2s_extractor* h, int bBase, int batch, cudaStream_t st) {
   uint2* fbList = d.fbList + (size_t)bBase * g.totalCells;
   int32_t* fbCount = d.fbCount + bBase;
   B2S_CUDA(cudaMemsetAsync(fbCount, 0, 4, st));
-  int cellRows = 0;
-  for (int l = 0; l < g.nlevels; l++) cellRows += g.lv[l].nRows;
-  k_cells<<<dim3(cellRows, batch), 256, 0, st>>>(
+  int cellCtas = 0;
+  for (int l = 0; l < g.nlevels; l++) cellCtas += g.lv[l].nRows * g.lv[l].nChunks;
+  k_cells<<<dim3(cellCtas, batch), 256, 0, st>>>(
       g, d.score + (size_t)bBase * g.pyrBytes, d.bitmap + (size_t)bBase * g.bmWords, d.candXY + (size_t)bBase * g.totalCandCap,
       d.candKey + (size_t)bBase * g.totalCandCap, d.candResp + (size_t)bBase * g.totalCandCap,
       d.candCount + (size_t)bBase * kMaxLevels, d.status, fbList, fbCount, bBase);

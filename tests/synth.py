@@ -35,6 +35,105 @@ def synth_image(w, h, seed, blocks=True):
     return np.clip(base, 0, 255).astype(np.uint8)
 
 
+TEXTURES = ("noise", "saltpepper", "dark", "bright", "checker2", "checker3", "checker4", "checker5", "checker6", "corner",
+            "fallback", "dense")
+
+
+def level_sizes(W, H, scale_factor, nlevels):
+    """(w, h) of every pyramid level as the extractor rounds them: cvRound(W * mvInvScaleFactor[l]) in float32, with
+    mvScaleFactor[l] = (float)(mvScaleFactor[l-1] * (double)scaleFactor) (src/ORBextractor.cc:500-520, :1680-1682)."""
+    sf = np.float64(np.float32(scale_factor))
+    s, out = np.float32(1.0), []
+    for l in range(nlevels):
+        if l:
+            s = np.float32(np.float64(s) * sf)
+        inv = np.float32(1.0) / s
+        out.append((int(np.rint(np.float32(W) * inv)), int(np.rint(np.float32(H) * inv))))
+    return out
+
+
+def grid_ok(w, h):
+    """The 30-px cell grid of a level exists (nCols, nRows >= 1) and its width is >= height / 2 (quadtree roots)."""
+    width, height = np.float32(w - 32), np.float32(h - 32)
+    return int(width / np.float32(30)) >= 1 and int(height / np.float32(30)) >= 1 and round(float(width / height)) >= 1
+
+
+def residue_shapes(scale_factor=1.2, nlevels=8):
+    """A small set of image sizes such that, over all of them, some level's width is 0, 1 and 127 mod 128 (the tile
+    width) and some level's height is 0, 1 and 31 mod 32 (the tile height).  Returns [(W, H)] and the residues covered."""
+    shapes, xs, ys = [], set(), set()
+    want_x, want_y = {0, 1, 127}, {0, 1, 31}
+    W, H = 640, 480
+    for Wc in range(640, 1100):
+        lv = level_sizes(Wc, H, scale_factor, nlevels)
+        got = {w % 128 for w, _ in lv} & (want_x - xs)
+        if got:
+            shapes.append((Wc, H))
+            xs |= {w % 128 for w, _ in lv} & want_x
+        if xs == want_x:
+            break
+    for Hc in range(400, 700):
+        lv = level_sizes(W, Hc, scale_factor, nlevels)
+        got = {h % 32 for _, h in lv} & (want_y - ys)
+        if got:
+            shapes.append((W, Hc))
+            ys |= {h % 32 for _, h in lv} & want_y
+        if ys == want_y:
+            break
+    return shapes, xs, ys
+
+
+def synth_texture(kind, w, h, seed):
+    """Extractor stress textures: uniform noise 0..255 (dense candidates), salt-and-pepper 0/255, dark 0..30 and bright
+    225..255 noise (FAST's p - t < 0 and p + t > 255 lanes), checkerboards of period 2..6, one isolated corner on a
+    constant image, and weak noise with strong noise only in the first 30 columns after the border (every other level-0
+    cell has no maximum above iniThFAST and goes through the minThFAST pass)."""
+    rng = np.random.RandomState(seed)
+    if kind == "noise":
+        return rng.randint(0, 256, size=(h, w)).astype(np.uint8)
+    if kind == "saltpepper":
+        return (rng.randint(0, 2, size=(h, w)) * 255).astype(np.uint8)
+    if kind == "dark":
+        return rng.randint(0, 31, size=(h, w)).astype(np.uint8)
+    if kind == "bright":
+        return (225 + rng.randint(0, 31, size=(h, w))).astype(np.uint8)
+    if kind.startswith("checker"):
+        p = int(kind[7:])
+        yy, xx = np.mgrid[0:h, 0:w]
+        return np.where((xx // p + yy // p) % 2 == 0, 40, 210).astype(np.uint8)
+    if kind == "corner":
+        img = np.full((h, w), 90, np.uint8)
+        img[h // 2:, w // 2:] = 180
+        return img
+    if kind == "dense":  # a 2 x 7 tile on which 56 % of all pixels are FAST corners at threshold 20
+        tile = np.array([[8, 214], [84, 9], [201, 3], [103, 31], [90, 160], [135, 41], [132, 109]], np.uint8)
+        return np.tile(tile, (h // 7 + 1, w // 2 + 1))[:h, :w].copy()
+    if kind == "fallback":
+        img = (100 + rng.randint(0, 18, size=(h, w))).astype(np.uint8)
+        img[:, 19:49] = rng.randint(0, 256, size=(h, 30))
+        return img
+    raise ValueError(kind)
+
+
+_CIRCLE = ((0, 3), (1, 3), (2, 2), (3, 1), (3, 0), (3, -1), (2, -2), (1, -3), (0, -3), (-1, -3), (-2, -2), (-3, -1), (-3, 0),
+           (-3, 1), (-2, 2), (-1, 3))
+
+
+def fast_strength(img):
+    """FAST-9/16 arc strength of every pixel (0 on the 3-pixel rim): M = max over the 16 arcs of 9 circle pixels of
+    min |I_k - p| with one sign; a pixel is a corner at threshold t iff M > t."""
+    a = img.astype(np.int32)
+    h, w = a.shape
+    c = a[3:h - 3, 3:w - 3]
+    ring = np.stack([a[3 + dy:h - 3 + dy, 3 + dx:w - 3 + dx] for dx, dy in _CIRCLE])
+    ring = np.concatenate([ring, ring[:8]])
+    bright = np.max([ring[s:s + 9].min(axis=0) for s in range(16)], axis=0) - c
+    dark = c - np.min([ring[s:s + 9].max(axis=0) for s in range(16)], axis=0)
+    M = np.zeros((h, w), np.int32)
+    M[3:h - 3, 3:w - 3] = np.maximum(np.maximum(bright, dark), 0)
+    return M
+
+
 def synth_stereo(w, h, seed):
     left = synth_image(w, h, seed)
     rng = np.random.RandomState(seed + 100003)

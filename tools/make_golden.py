@@ -38,6 +38,11 @@ img = synth_image(1241, 376, 3)
 k, d = o.extractor(2000, 1.2, 8, 20, 7)(img)
 np.savez_compressed(os.path.join(out, "extract_1241x376_seed3.npz"), n=len(k), kps_sha=sha(k), desc_sha=sha(d),
                     kps_head=k[:64], desc_head=d[:64], image_sha=sha(img))
+# extractor on uniform noise (dense candidates) at iniThFAST 12 / minThFAST 7: full arrays
+from synth import synth_texture  # noqa: E402
+img = synth_texture("noise", 640, 480, 3)
+k, d = o.extractor(1000, 1.2, 8, 12, 7)(img)
+np.savez_compressed(os.path.join(out, "extract_640x480_noise_12_7.npz"), kps=k, desc=d, image_sha=sha(img))
 # SearchByBoW
 for nodes in (100, 1):
     A, nA, vA, aA, B, nB, aB = synth_descriptors(2000, seed=1234 + nodes, n_nodes=nodes)
