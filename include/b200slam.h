@@ -615,6 +615,55 @@ int b2s_optimize_sim3(b2s_sim3opt_solver* h, int batch, const b2s_sim3_problem* 
 /* Device time (CUDA events on the solver's stream: upload, kernel, download) of the last call and its LM trials. */
 float b2s_sim3opt_last_ms(const b2s_sim3opt_solver* h, long long* lm_trials);
 
+/* ------------------------------------------------------------------ monocular initialisation */
+/* Initializer::Initialize (src/Initializer.cc:68-231) with the minimal sets drawn by the caller (:132-168): normalise
+ * both keypoint sets, score `iterations` homographies and fundamental matrices (ComputeH21 / ComputeF21 by Jacobi SVD,
+ * CheckHomography / CheckFundamental), keep the first strict maximum of each, pick H when SH/(SH+SF) > 0.40 and
+ * reconstruct the chosen model only (ReconstructH: 8 motion hypotheses, ReconstructF: 4) with minParallax = 1 and
+ * minTriangulated = 50.  The cv::Mat arithmetic follows OpenCV's (float storage, double accumulators in gemm / dot /
+ * norm, float scaling); DESIGN §7 lists it.  One call runs a batch of independent problems with no host synchronisation
+ * between the stages; every score is a serial float sum in match order, so two calls give bit-identical outputs and a
+ * batch equals its problems run one by one. */
+typedef struct {
+  int32_t n1, n2;             /* keypoints of the reference frame (1) and the current frame (2) */
+  const float* kp1;           /* n1 x 2: mvKeysUn[i].pt of frame 1 */
+  const float* kp2;           /* n2 x 2 */
+  const int32_t* matches12;   /* n1: vMatches12, the frame-2 keypoint matched to frame-1 keypoint i, or < 0 */
+  float K[9];                 /* mK, row-major */
+  float sigma;
+  int32_t iterations;         /* mMaxIterations */
+  const int32_t* sets;        /* iterations x 8: mvSets, indices into the matches compacted in frame-1 order */
+} b2s_init_problem;
+typedef struct {
+  int32_t ret;                /* Initialize's return value */
+  int32_t model;              /* 1: homography (RH > 0.40), 2: fundamental matrix */
+  int32_t rt_state;           /* R21 / t21: 1 written, -1 emptied (ReconstructF's failure after DecomposeE), 0 untouched */
+  float R21[9], t21[3];
+  float* p3d;                 /* n1 x 3: vP3D, written only when ret != 0 */
+  uint8_t* triangulated;      /* n1: vbTriangulated, written only when ret != 0 */
+  uint8_t* inliers_h;         /* optional, n_matches: the best homography's inlier flags */
+  uint8_t* inliers_f;         /* optional, n_matches: the best fundamental matrix's inlier flags */
+  int32_t n_matches;          /* matched frame-1 keypoints (the compacted match list's length) */
+  int32_t best_h_iter, best_f_iter; /* -1 when no iteration scored above 0 */
+  float SH, SF, RH;
+  float H21[9], F21[9];       /* the best hypotheses (zero when none) */
+  int32_t n_hyp;              /* motion hypotheses checked: 8 (H), 4 (F), 0 (ReconstructH's singular-value early-out) */
+  int32_t n_good[8];          /* CheckRT's return value per hypothesis */
+  float parallax[8];          /* CheckRT's parallax per hypothesis, degrees */
+} b2s_init_result;
+typedef struct b2s_init_solver b2s_init_solver;
+/* max_keys keypoints per frame (<= 16384), max_iterations per problem, max_batch problems per call. */
+int b2s_init_create(int max_keys, int max_iterations, int max_batch, int device, b2s_init_solver** out);
+void b2s_init_destroy(b2s_init_solver* h);
+/* n1, n2 > max_keys, iterations > max_iterations or batch > max_batch: B2S_ERR_CAPACITY.  batch < 1, sigma <= 0,
+ * iterations < 1, n1 or n2 < 1, a null array, fewer than 8 matches, a match index outside [0, n2), a set index outside
+ * [0, n_matches) or repeated within its set: B2S_ERR_BAD_ARG.  Nothing is written unless every problem is valid.  Where
+ * neither model scored above 0 the reference would multiply an empty matrix; here the call returns 0 for that problem
+ * with n_hyp = 0 and R21, t21, p3d and triangulated untouched. */
+int b2s_initialize(b2s_init_solver* h, int batch, const b2s_init_problem* p, b2s_init_result* r);
+/* Device time (CUDA events on the solver's stream: upload, kernels, download) of the last call. */
+float b2s_init_last_ms(const b2s_init_solver* h);
+
 #ifdef __cplusplus
 }
 #endif

@@ -113,6 +113,20 @@ class _Sim3Result(ctypes.Structure):
                 ("n_trials", ctypes.c_int32)]
 
 
+class _InitProblem(ctypes.Structure):  # b2s_init_problem
+    _fields_ = [("n1", ctypes.c_int32), ("n2", ctypes.c_int32), ("kp1", _vp), ("kp2", _vp), ("matches12", _vp),
+                ("K", ctypes.c_float * 9), ("sigma", ctypes.c_float), ("iterations", ctypes.c_int32), ("sets", _vp)]
+
+
+class _InitResult(ctypes.Structure):  # b2s_init_result
+    _fields_ = [("ret", ctypes.c_int32), ("model", ctypes.c_int32), ("rt_state", ctypes.c_int32),
+                ("R21", ctypes.c_float * 9), ("t21", ctypes.c_float * 3), ("p3d", _vp), ("triangulated", _vp),
+                ("inliers_h", _vp), ("inliers_f", _vp), ("n_matches", ctypes.c_int32), ("best_h_iter", ctypes.c_int32),
+                ("best_f_iter", ctypes.c_int32), ("SH", ctypes.c_float), ("SF", ctypes.c_float),
+                ("RH", ctypes.c_float), ("H21", ctypes.c_float * 9), ("F21", ctypes.c_float * 9),
+                ("n_hyp", ctypes.c_int32), ("n_good", ctypes.c_int32 * 8), ("parallax", ctypes.c_float * 8)]
+
+
 class _GbaResult(ctypes.Structure):
     _fields_ = [("Tcw_out", _vp), ("points_out", _vp), ("point_included", _vp), ("trace", _vp),
                 ("chi2_final", ctypes.c_double), ("n_trials", ctypes.c_int)]
@@ -211,6 +225,13 @@ def lib():
             L.b2s_optimize_sim3.argtypes = [_vp, ctypes.c_int, _vp, _vp]
             L.b2s_sim3opt_last_ms.restype = ctypes.c_float
             L.b2s_sim3opt_last_ms.argtypes = [_vp, _vp]
+        if hasattr(L, "b2s_init_create"):
+            L.b2s_init_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+            L.b2s_init_destroy.argtypes = [_vp]
+            L.b2s_init_destroy.restype = None
+            L.b2s_initialize.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+            L.b2s_init_last_ms.restype = ctypes.c_float
+            L.b2s_init_last_ms.argtypes = [_vp]
         _lib = L
     return _lib
 
@@ -1113,4 +1134,73 @@ class Sim3Optimizer:
             out["S12"] = np.array(res[i].S12_out.v[:], np.float64)
             out["n_inliers"] = res[i].n_inliers
             out["n_trials"] = res[i].n_trials
+        return outs
+
+
+class MonoInitializer:
+    """Mirror of ORB_SLAM2::Initializer::Initialize (src/Initializer.cc:68-231) with the minimal sets given
+    (b2s_initialize): H and F RANSAC over the sets, the model choice and the two-view reconstruction.  A batch of
+    independent problems runs in one call."""
+
+    def __init__(self, max_keys=4096, max_iterations=300, max_batch=64, device=0):
+        self._h = _vp()
+        _check(lib().b2s_init_create(max_keys, max_iterations, max_batch, device, ctypes.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().b2s_init_destroy(self._h)
+            self._h = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def last_ms(self):
+        """Device time of the last call (CUDA events: upload, kernels, download)."""
+        return float(lib().b2s_init_last_ms(self._h))
+
+    def Initialize(self, d):
+        """d: kp1 (n1 x 2, mvKeysUn of the reference frame), kp2 (n2 x 2), matches12 (n1, -1: unmatched), K (3 x 3),
+        sigma, sets (iterations x 8, indices into the matches compacted in frame-1 order).  Returns ret, model (1: H,
+        2: F), rt_state (1 written, -1 emptied, 0 untouched), R21 (3 x 3), t21 (3), p3d (n1 x 3) and triangulated (n1)
+        (None unless ret), n_matches, SH, SF, RH, best_h_iter, best_f_iter, H21, F21 (3 x 3), inliers_h, inliers_f
+        (n_matches, bool), n_good and parallax (per motion hypothesis checked)."""
+        return self.InitializeBatch([d])[0]
+
+    def InitializeBatch(self, ds):
+        keep, probs, outs = [], (_InitProblem * len(ds))(), []
+        res = (_InitResult * len(ds))()
+        for i, d in enumerate(ds):
+            a = dict(kp1=np.ascontiguousarray(d["kp1"], np.float32).reshape(-1, 2),
+                     kp2=np.ascontiguousarray(d["kp2"], np.float32).reshape(-1, 2),
+                     matches12=np.ascontiguousarray(d["matches12"], np.int32).reshape(-1),
+                     sets=np.ascontiguousarray(d["sets"], np.int32).reshape(-1, 8))
+            keep.append(a)
+            P = probs[i]
+            P.n1, P.n2, P.iterations = len(a["kp1"]), len(a["kp2"]), len(a["sets"])
+            for k in a:
+                setattr(P, k, a[k].ctypes.data)
+            P.K[:] = [float(v) for v in np.asarray(d["K"], np.float32).reshape(9)]
+            P.sigma = float(d["sigma"])
+            nm = int((a["matches12"] >= 0).sum())
+            out = dict(p3d=np.zeros((P.n1, 3), np.float32), triangulated=np.zeros(P.n1, np.uint8),
+                       inliers_h=np.zeros(max(nm, 1), np.uint8), inliers_f=np.zeros(max(nm, 1), np.uint8))
+            outs.append(out)
+            for k in out:
+                setattr(res[i], k, out[k].ctypes.data)
+        _check(lib().b2s_initialize(self._h, len(ds), probs, res))
+        for r, out in zip(res, outs):
+            n = r.n_matches
+            out.update(ret=r.ret, model=r.model, rt_state=r.rt_state, n_matches=n, SH=np.float32(r.SH),
+                       SF=np.float32(r.SF), RH=np.float32(r.RH), best_h_iter=r.best_h_iter, best_f_iter=r.best_f_iter,
+                       R21=np.array(r.R21[:], np.float32).reshape(3, 3), t21=np.array(r.t21[:], np.float32),
+                       H21=np.array(r.H21[:], np.float32).reshape(3, 3), F21=np.array(r.F21[:], np.float32).reshape(3, 3),
+                       n_good=np.array(r.n_good[:r.n_hyp], np.int32), parallax=np.array(r.parallax[:r.n_hyp], np.float32))
+            out["inliers_h"] = out["inliers_h"][:n].astype(bool)
+            out["inliers_f"] = out["inliers_f"][:n].astype(bool)
+            out["triangulated"] = out["triangulated"].astype(bool)
+            if not r.ret:
+                out["p3d"] = out["triangulated"] = None
         return outs
