@@ -664,6 +664,55 @@ int b2s_initialize(b2s_init_solver* h, int batch, const b2s_init_problem* p, b2s
 /* Device time (CUDA events on the solver's stream: upload, kernels, download) of the last call. */
 float b2s_init_last_ms(const b2s_init_solver* h);
 
+/* ------------------------------------------------------------------ Sim3 RANSAC (loop-closure candidates) */
+/* Sim3Solver::iterate (src/Sim3Solver.cc:199-285) with the minimal sets drawn by the caller: for each set, Horn's closed
+ * form (ComputeSim3 :309-448: centroids, the 4 x 4 float Jacobi eigen, Rodrigues, scale, T12 and T21), CheckInliers in
+ * both directions with the thresholds (size_t)(9.210 * sigma2), then the reference's scan: the best model replaced on
+ * >=, an immediate return when an iteration has more than min_inliers inliers.  The solver state the reference keeps
+ * across calls (mnIterations, mnBestInliers, the best model) goes in and comes out, so the ABI is stateless.  The
+ * cv::Mat arithmetic follows OpenCV's; DESIGN §7 lists it.  One call runs a batch of independent solvers with no host
+ * synchronisation between stages; inlier counts are integers, so a batch equals its problems run one by one. */
+typedef struct {
+  int32_t n;                  /* N: the correspondences the constructor kept (:78-127), in vpMatched12 order */
+  const float* X1c;           /* n x 3: mvX3Dc1, Rcw1*Xw + tcw1 as the caller's cv::Mat expression produced it */
+  const float* X2c;           /* n x 3: mvX3Dc2 */
+  const float* sigma2_1;      /* n: pKF1->mvLevelSigma2[octave]; the threshold is (size_t)(9.210 * sigma2) */
+  const float* sigma2_2;      /* n: pKF2->mvLevelSigma2[octave] */
+  float K1[4], K2[4];         /* fx, fy, cx, cy of mK1 / mK2 */
+  int32_t fix_scale;          /* mbFixScale */
+  int32_t min_inliers;        /* mRansacMinInliers */
+  int32_t max_its;            /* mRansacMaxIts after SetRansacParameters */
+  int32_t iterations_done;    /* mnIterations on entry */
+  int32_t best_inliers;       /* mnBestInliers on entry */
+  int32_t k;                  /* minimal sets given: the iterations this call may run (<= max_its - iterations_done) */
+  const int32_t* sets;        /* k x 3: indices into [0, n), in draw order; not read when n < min_inliers */
+} b2s_sim3solver_problem;
+typedef struct {
+  int32_t returned;           /* 1: iterate returned mBestT12 (an iteration had more than min_inliers inliers) */
+  float T12[16];              /* the returned T12, row-major 4 x 4, when returned */
+  int32_t best_changed;       /* 1: an iteration of this call replaced the best model; R, t and s hold the new one */
+  float R[9], t[3], s;        /* mBestRotation, mBestTranslation (3 x 1), mBestScale: written only when best_changed */
+  uint8_t* inliers;           /* n: vbInliers in compacted order (entry i is vpMatched12[mvnIndices1[i]]); 0 unless
+                                 returned */
+  int32_t n_inliers;          /* nInliers: 0 unless returned */
+  int32_t no_more;            /* bNoMore */
+  int32_t iterations_used;    /* sets consumed by this call */
+  int32_t iterations_done;    /* mnIterations after the call */
+  int32_t best_inliers;       /* mnBestInliers after the call */
+} b2s_sim3solver_result;
+typedef struct b2s_sim3solver b2s_sim3solver;
+/* max_matches correspondences (<= 65536) and max_sets sets per problem, max_batch problems per call. */
+int b2s_sim3solver_create(int max_matches, int max_sets, int max_batch, int device, b2s_sim3solver** out);
+void b2s_sim3solver_destroy(b2s_sim3solver* h);
+/* n > max_matches, k > max_sets or batch > max_batch: B2S_ERR_CAPACITY.  batch < 1, a null array, n < 0, max_its < 1,
+ * iterations_done < 0, best_inliers < 0, k < 0 or k > max_its - iterations_done, a sigma2 that is negative or not
+ * finite, n < 3 where an iteration would run (n >= min_inliers and k > 0), a set index outside [0, n) or repeated within
+ * its set: B2S_ERR_BAD_ARG.  Nothing is written unless every problem is valid.  Where n < min_inliers the call returns
+ * no_more = 1 and consumes no set, as the reference does before it draws. */
+int b2s_sim3solver_iterate(b2s_sim3solver* h, int batch, const b2s_sim3solver_problem* p, b2s_sim3solver_result* r);
+/* Device time (CUDA events on the solver's stream: upload, kernels, download) of the last call. */
+float b2s_sim3solver_last_ms(const b2s_sim3solver* h);
+
 #ifdef __cplusplus
 }
 #endif

@@ -127,6 +127,20 @@ class _InitResult(ctypes.Structure):  # b2s_init_result
                 ("n_hyp", ctypes.c_int32), ("n_good", ctypes.c_int32 * 8), ("parallax", ctypes.c_float * 8)]
 
 
+class _Sim3SolverProblem(ctypes.Structure):  # b2s_sim3solver_problem
+    _fields_ = [("n", ctypes.c_int32), ("X1c", _vp), ("X2c", _vp), ("sigma2_1", _vp), ("sigma2_2", _vp),
+                ("K1", ctypes.c_float * 4), ("K2", ctypes.c_float * 4), ("fix_scale", ctypes.c_int32),
+                ("min_inliers", ctypes.c_int32), ("max_its", ctypes.c_int32), ("iterations_done", ctypes.c_int32),
+                ("best_inliers", ctypes.c_int32), ("k", ctypes.c_int32), ("sets", _vp)]
+
+
+class _Sim3SolverResult(ctypes.Structure):  # b2s_sim3solver_result
+    _fields_ = [("returned", ctypes.c_int32), ("T12", ctypes.c_float * 16), ("best_changed", ctypes.c_int32),
+                ("R", ctypes.c_float * 9), ("t", ctypes.c_float * 3), ("s", ctypes.c_float), ("inliers", _vp),
+                ("n_inliers", ctypes.c_int32), ("no_more", ctypes.c_int32), ("iterations_used", ctypes.c_int32),
+                ("iterations_done", ctypes.c_int32), ("best_inliers", ctypes.c_int32)]
+
+
 class _GbaResult(ctypes.Structure):
     _fields_ = [("Tcw_out", _vp), ("points_out", _vp), ("point_included", _vp), ("trace", _vp),
                 ("chi2_final", ctypes.c_double), ("n_trials", ctypes.c_int)]
@@ -232,6 +246,13 @@ def lib():
             L.b2s_initialize.argtypes = [_vp, ctypes.c_int, _vp, _vp]
             L.b2s_init_last_ms.restype = ctypes.c_float
             L.b2s_init_last_ms.argtypes = [_vp]
+        if hasattr(L, "b2s_sim3solver_create"):
+            L.b2s_sim3solver_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+            L.b2s_sim3solver_destroy.argtypes = [_vp]
+            L.b2s_sim3solver_destroy.restype = None
+            L.b2s_sim3solver_iterate.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+            L.b2s_sim3solver_last_ms.restype = ctypes.c_float
+            L.b2s_sim3solver_last_ms.argtypes = [_vp]
         _lib = L
     return _lib
 
@@ -1204,3 +1225,161 @@ class MonoInitializer:
             if not r.ret:
                 out["p3d"] = out["triangulated"] = None
         return outs
+
+
+def sim3_ransac_max_its(n, probability=0.99, min_inliers=6, max_iterations=300):
+    """Sim3Solver::SetRansacParameters (src/Sim3Solver.cc:143-196) on the host: the mRansacMaxIts it leaves for n
+    correspondences.  epsilon = min_inliers / n is a float; the iteration count ceil(log(1-p) / log(1-epsilon^3)) is
+    double, converted to int as x86 converts (NaN and out-of-range values become INT_MIN); min_inliers == n gives 1; the
+    result is max(1, min(count, max_iterations))."""
+    import math
+
+    def log(x):  # C's log, with its IEEE special cases
+        return math.log(x) if 0 < x < math.inf else (-math.inf if x == 0 else (x if x > 0 else math.nan))
+
+    with np.errstate(all="ignore"):
+        if min_inliers == n:
+            it = 1
+        else:
+            eps = float(np.float32(min_inliers) / np.float32(n))
+            c = float(np.float64(log(1 - probability)) / np.float64(log(1 - math.pow(eps, 3))))
+            it = math.ceil(c) if math.isfinite(c) and -2 ** 31 <= math.ceil(c) < 2 ** 31 else -2 ** 31
+    return max(1, min(it, max_iterations))
+
+
+class Sim3Solver:
+    """Mirror of ORB_SLAM2::Sim3Solver (src/Sim3Solver.cc) for one loop candidate, with the minimal sets drawn by the
+    caller (b2s_sim3solver_iterate).  The constructor takes what the reference's constructor keeps: X1c / X2c (n x 3,
+    mvX3Dc1 / mvX3Dc2), sigma2_1 / sigma2_2 (n, mvLevelSigma2 of each keypoint's octave), K1 / K2 (fx, fy, cx, cy) and
+    fix_scale; the object keeps mnIterations, mnBestInliers and the best model across calls as the reference does.
+    `iterate` and `find` run on the device; `iterate_batch` runs the calls of many solvers in one launch sequence."""
+
+    def __init__(self, X1c, X2c, sigma2_1, sigma2_2, K1, K2, fix_scale=True, max_matches=None, max_sets=300,
+                 device=0, _handle=None):
+        self.X1c = np.ascontiguousarray(X1c, np.float32).reshape(-1, 3)
+        self.X2c = np.ascontiguousarray(X2c, np.float32).reshape(-1, 3)
+        self.sigma2_1 = np.ascontiguousarray(sigma2_1, np.float32).reshape(-1)
+        self.sigma2_2 = np.ascontiguousarray(sigma2_2, np.float32).reshape(-1)
+        self.K1 = [float(v) for v in np.asarray(K1, np.float32).reshape(4)]
+        self.K2 = [float(v) for v in np.asarray(K2, np.float32).reshape(4)]
+        self.fix_scale = bool(fix_scale)
+        self.N = len(self.X1c)
+        self.iterations = 0
+        self.best_inliers = 0
+        self.R = self.t = self.s = None
+        self.set_ransac_parameters()
+        self._own = _handle is None
+        self._h = _handle._h if _handle is not None else _vp()
+        if self._own:
+            _check(lib().b2s_sim3solver_create(max(3, max_matches or self.N), max_sets, 1, device,
+                                               ctypes.byref(self._h)))
+
+    def close(self):
+        if self._own and self._h:
+            lib().b2s_sim3solver_destroy(self._h)
+        self._h = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def last_ms(self):
+        """Device time of the last call (CUDA events: upload, kernels, download)."""
+        return float(lib().b2s_sim3solver_last_ms(self._h))
+
+    def set_ransac_parameters(self, probability=0.99, min_inliers=6, max_iterations=300):
+        """SetRansacParameters: resets the iteration count, keeps the best inlier count."""
+        self.min_inliers = int(min_inliers)
+        self.max_its = sim3_ransac_max_its(self.N, probability, min_inliers, max_iterations)
+        self.iterations = 0
+
+    def sets_needed(self, n_iterations):
+        """How many minimal sets iterate(n_iterations) may consume: 0 when N < min_inliers (the reference draws
+        nothing), else min(n_iterations, max_its - iterations)."""
+        if self.N < self.min_inliers:
+            return 0
+        return max(0, min(int(n_iterations), self.max_its - self.iterations))
+
+    def iterate(self, n_iterations, sets):
+        """iterate(n_iterations) with its minimal sets (at least sets_needed(n_iterations) rows of 3 indices into
+        [0, N), in draw order; the extra rows are ignored).  Returns a dict: T12 (4 x 4, or None for the empty matrix),
+        no_more, inliers (N, compacted order), n_inliers, iterations_used."""
+        return Sim3Solver.iterate_batch([self], [n_iterations], [sets])[0]
+
+    def find(self, sets):
+        """find(): iterate(mRansacMaxIts)."""
+        return self.iterate(self.max_its, sets)
+
+    @staticmethod
+    def iterate_batch(solvers, n_iterations, sets, handle=None):
+        """One iterate call per solver, all in one device call (on `handle`, a Sim3SolverBatch, or the first solver's
+        handle)."""
+        h = handle._h if handle is not None else solvers[0]._h
+        probs = (_Sim3SolverProblem * len(solvers))()
+        res = (_Sim3SolverResult * len(solvers))()
+        keep, outs = [], []
+        for i, (sv, nit, st) in enumerate(zip(solvers, n_iterations, sets)):
+            k = sv.sets_needed(nit)
+            st = np.ascontiguousarray(np.asarray(st, np.int32).reshape(-1, 3)[:k])
+            if len(st) < k:
+                raise ValueError("iterate: %d sets given, %d needed" % (len(st), k))
+            keep.append(st)
+            P = probs[i]
+            P.n, P.X1c, P.X2c = sv.N, sv.X1c.ctypes.data, sv.X2c.ctypes.data
+            P.sigma2_1, P.sigma2_2 = sv.sigma2_1.ctypes.data, sv.sigma2_2.ctypes.data
+            P.K1[:], P.K2[:] = sv.K1, sv.K2
+            P.fix_scale, P.min_inliers, P.max_its = int(sv.fix_scale), sv.min_inliers, sv.max_its
+            P.iterations_done, P.best_inliers, P.k, P.sets = sv.iterations, sv.best_inliers, k, st.ctypes.data
+            out = np.zeros(max(sv.N, 1), np.uint8)
+            outs.append(out)
+            res[i].inliers = out.ctypes.data
+        _check(lib().b2s_sim3solver_iterate(h, len(solvers), probs, res))
+        ret = []
+        for sv, r, out in zip(solvers, res, outs):
+            sv.iterations, sv.best_inliers = r.iterations_done, r.best_inliers
+            if r.best_changed:
+                sv.R = np.array(r.R[:], np.float32).reshape(3, 3)
+                sv.t = np.array(r.t[:], np.float32).reshape(3, 1)
+                sv.s = np.float32(r.s)
+            ret.append(dict(T12=np.array(r.T12[:], np.float32).reshape(4, 4) if r.returned else None,
+                            no_more=bool(r.no_more), inliers=out[:sv.N].astype(bool), n_inliers=r.n_inliers,
+                            iterations_used=r.iterations_used))
+        return ret
+
+    def GetEstimatedRotation(self):
+        return None if self.R is None else self.R.copy()
+
+    def GetEstimatedTranslation(self):
+        return None if self.t is None else self.t.copy()
+
+    def GetEstimatedScale(self):
+        return self.s
+
+
+class Sim3SolverBatch:
+    """A device handle sized for batched Sim3Solver.iterate_batch calls (max_matches per solver, max_sets per call,
+    max_batch solvers)."""
+
+    def __init__(self, max_matches=4096, max_sets=300, max_batch=64, device=0):
+        self._h = _vp()
+        _check(lib().b2s_sim3solver_create(max_matches, max_sets, max_batch, device, ctypes.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().b2s_sim3solver_destroy(self._h)
+            self._h = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def last_ms(self):
+        return float(lib().b2s_sim3solver_last_ms(self._h))
+
+    def solver(self, *args, **kw):
+        """A Sim3Solver on this handle (Sim3Solver's constructor arguments)."""
+        return Sim3Solver(*args, _handle=self, **kw)
