@@ -713,6 +713,64 @@ int b2s_sim3solver_iterate(b2s_sim3solver* h, int batch, const b2s_sim3solver_pr
 /* Device time (CUDA events on the solver's stream: upload, kernels, download) of the last call. */
 float b2s_sim3solver_last_ms(const b2s_sim3solver* h);
 
+/* ---------------------------------------------------------------------------------------------------------------------
+ * EPnP RANSAC for relocalisation candidates: PnPsolver::iterate (src/PnPsolver.cc:240-363) with the minimal sets drawn
+ * by the caller.  Each iteration runs compute_pose (EPnP: control points, barycentric coordinates, the 12 x 12 SVD of
+ * MtM, three beta approximations with 5 Gauss-Newton steps each) on its 4 correspondences and CheckInliers over all n;
+ * then the reference's scan: the best model replaced on >, and on an iteration with at least min_inliers inliers a
+ * Refine (compute_pose on the best mask's correspondences) that returns when it keeps more than min_inliers inliers.
+ * The loop runs until iterations_done reaches max_its and at least the caller's nIterations times (its condition is
+ * ||), so a call that does not return early runs exactly k iterations.  The solver state the reference keeps across
+ * calls (mnIterations, mnBestInliers, mBestTcw, mvbBestInliers) goes in and comes out, so the ABI is stateless.  The
+ * arithmetic is the reference's double precision with OpenCV's C API (cvMulTransposed, cvSVD, cvInvert, cvSolve) as
+ * OpenCV computes it; DESIGN §7 lists it.  One call runs a batch of independent solvers with no host synchronisation
+ * between stages; a batch equals its problems run one by one. */
+typedef struct {
+  int32_t n;                  /* N: the correspondences the constructor kept (:120-168), in vpMapPointMatches order */
+  const float* P3Dw;          /* n x 3: mvP3Dw */
+  const float* P2D;           /* n x 2: mvP2D (undistorted keypoints) */
+  const float* sigma2;        /* n: mvSigma2, F.mvLevelSigma2[octave]; mvMaxError = sigma2 * th2 in float */
+  float fu, fv, uc, vc;       /* F.fx, F.fy, F.cx, F.cy */
+  float th2;                  /* SetRansacParameters' th2 */
+  int32_t min_inliers;        /* mRansacMinInliers after SetRansacParameters */
+  int32_t max_its;            /* mRansacMaxIts after SetRansacParameters */
+  int32_t min_set;            /* mRansacMinSet: must be 4 */
+  int32_t iterations_done;    /* mnIterations on entry */
+  int32_t best_inliers;       /* mnBestInliers on entry */
+  const float* best_Tcw;      /* 16: mBestTcw on entry, row-major (any values while best_inliers == 0) */
+  const uint8_t* best_mask;   /* n: mvbBestInliers on entry (any values while best_inliers == 0) */
+  int32_t k;                  /* minimal sets given: the iterations this call runs unless it returns early,
+                                 max(nIterations, max_its - iterations_done); 0 when n < min_inliers */
+  const int32_t* sets;        /* k x 4: indices into [0, n), in draw order; not read when n < min_inliers */
+} b2s_pnpsolver_problem;
+typedef struct {
+  int32_t returned;           /* 1: iterate returned a pose (no_more = 0: a Refine succeeded, Tcw is mRefinedTcw;
+                                 no_more = 1: the loop ended with best_inliers >= min_inliers, Tcw is mBestTcw) */
+  float Tcw[16];              /* the returned pose, row-major 4 x 4, when returned */
+  uint8_t* inliers;           /* n: vbInliers in compacted order (mvbRefinedInliers or mvbBestInliers); 0 unless
+                                 returned */
+  int32_t n_inliers;          /* nInliers: 0 unless returned */
+  int32_t no_more;            /* bNoMore */
+  int32_t iterations_used;    /* sets consumed by this call */
+  int32_t iterations_done;    /* mnIterations after the call */
+  int32_t best_inliers;       /* mnBestInliers after the call */
+  int32_t best_changed;       /* 1: an iteration of this call replaced the best model */
+  float best_Tcw[16];         /* mBestTcw after the call (the entry value when best_changed is 0) */
+  uint8_t* best_mask;         /* n: mvbBestInliers after the call (the entry value when best_changed is 0) */
+} b2s_pnpsolver_result;
+typedef struct b2s_pnpsolver b2s_pnpsolver;
+/* max_matches correspondences (<= 65536) and max_sets sets per problem, max_batch (<= 65535) problems per call. */
+int b2s_pnpsolver_create(int max_matches, int max_sets, int max_batch, int device, b2s_pnpsolver** out);
+void b2s_pnpsolver_destroy(b2s_pnpsolver* h);
+/* n > max_matches, k > max_sets or batch > max_batch: B2S_ERR_CAPACITY.  batch < 1, a null array, n < 0, max_its < 1,
+ * min_set != 4, iterations_done < 0, best_inliers < 0 or > n, k < 0, k < max_its - iterations_done where n >=
+ * min_inliers (the loop cannot stop before max_its), a sigma2 that is negative or not finite, a set index outside
+ * [0, n) or repeated within its set: B2S_ERR_BAD_ARG.  Nothing is written unless every problem is valid.  Where
+ * n < min_inliers the call returns no_more = 1 and consumes no set, as the reference does before it draws. */
+int b2s_pnpsolver_iterate(b2s_pnpsolver* h, int batch, const b2s_pnpsolver_problem* p, b2s_pnpsolver_result* r);
+/* Device time (CUDA events on the solver's stream: upload, kernels, download) of the last call. */
+float b2s_pnpsolver_last_ms(const b2s_pnpsolver* h);
+
 #ifdef __cplusplus
 }
 #endif

@@ -141,6 +141,21 @@ class _Sim3SolverResult(ctypes.Structure):  # b2s_sim3solver_result
                 ("iterations_done", ctypes.c_int32), ("best_inliers", ctypes.c_int32)]
 
 
+class _PnPsolverProblem(ctypes.Structure):  # b2s_pnpsolver_problem
+    _fields_ = [("n", ctypes.c_int32), ("P3Dw", _vp), ("P2D", _vp), ("sigma2", _vp), ("fu", ctypes.c_float),
+                ("fv", ctypes.c_float), ("uc", ctypes.c_float), ("vc", ctypes.c_float), ("th2", ctypes.c_float),
+                ("min_inliers", ctypes.c_int32), ("max_its", ctypes.c_int32), ("min_set", ctypes.c_int32),
+                ("iterations_done", ctypes.c_int32), ("best_inliers", ctypes.c_int32), ("best_Tcw", _vp),
+                ("best_mask", _vp), ("k", ctypes.c_int32), ("sets", _vp)]
+
+
+class _PnPsolverResult(ctypes.Structure):  # b2s_pnpsolver_result
+    _fields_ = [("returned", ctypes.c_int32), ("Tcw", ctypes.c_float * 16), ("inliers", _vp),
+                ("n_inliers", ctypes.c_int32), ("no_more", ctypes.c_int32), ("iterations_used", ctypes.c_int32),
+                ("iterations_done", ctypes.c_int32), ("best_inliers", ctypes.c_int32), ("best_changed", ctypes.c_int32),
+                ("best_Tcw", ctypes.c_float * 16), ("best_mask", _vp)]
+
+
 class _GbaResult(ctypes.Structure):
     _fields_ = [("Tcw_out", _vp), ("points_out", _vp), ("point_included", _vp), ("trace", _vp),
                 ("chi2_final", ctypes.c_double), ("n_trials", ctypes.c_int)]
@@ -253,6 +268,13 @@ def lib():
             L.b2s_sim3solver_iterate.argtypes = [_vp, ctypes.c_int, _vp, _vp]
             L.b2s_sim3solver_last_ms.restype = ctypes.c_float
             L.b2s_sim3solver_last_ms.argtypes = [_vp]
+        if hasattr(L, "b2s_pnpsolver_create"):
+            L.b2s_pnpsolver_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+            L.b2s_pnpsolver_destroy.argtypes = [_vp]
+            L.b2s_pnpsolver_destroy.restype = None
+            L.b2s_pnpsolver_iterate.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+            L.b2s_pnpsolver_last_ms.restype = ctypes.c_float
+            L.b2s_pnpsolver_last_ms.argtypes = [_vp]
         _lib = L
     return _lib
 
@@ -1227,24 +1249,55 @@ class MonoInitializer:
         return outs
 
 
+def _c_log(x):
+    """C's log, with its IEEE special cases."""
+    import math
+    return math.log(x) if 0 < x < math.inf else (-math.inf if x == 0 else (x if x > 0 else math.nan))
+
+
+def _x86_int(x):
+    """A float or double converted to int as x86 converts it (truncation; NaN and out-of-range values become
+    INT_MIN)."""
+    import math
+    return int(x) if math.isfinite(x) and -2 ** 31 <= math.trunc(x) < 2 ** 31 else -2 ** 31
+
+
+def _ransac_iterations(probability, epsilon, power):
+    """ceil(log(1-p) / log(1-pow(epsilon, power))) in double, converted to int as x86 converts it."""
+    import math
+    with np.errstate(all="ignore"):
+        c = float(np.float64(_c_log(1 - probability)) / np.float64(_c_log(1 - math.pow(epsilon, power))))
+    return _x86_int(math.ceil(c) if math.isfinite(c) else c)
+
+
 def sim3_ransac_max_its(n, probability=0.99, min_inliers=6, max_iterations=300):
     """Sim3Solver::SetRansacParameters (src/Sim3Solver.cc:143-196) on the host: the mRansacMaxIts it leaves for n
     correspondences.  epsilon = min_inliers / n is a float; the iteration count ceil(log(1-p) / log(1-epsilon^3)) is
     double, converted to int as x86 converts (NaN and out-of-range values become INT_MIN); min_inliers == n gives 1; the
     result is max(1, min(count, max_iterations))."""
-    import math
-
-    def log(x):  # C's log, with its IEEE special cases
-        return math.log(x) if 0 < x < math.inf else (-math.inf if x == 0 else (x if x > 0 else math.nan))
-
     with np.errstate(all="ignore"):
         if min_inliers == n:
             it = 1
         else:
-            eps = float(np.float32(min_inliers) / np.float32(n))
-            c = float(np.float64(log(1 - probability)) / np.float64(log(1 - math.pow(eps, 3))))
-            it = math.ceil(c) if math.isfinite(c) and -2 ** 31 <= math.ceil(c) < 2 ** 31 else -2 ** 31
+            it = _ransac_iterations(probability, float(np.float32(min_inliers) / np.float32(n)), 3)
     return max(1, min(it, max_iterations))
+
+
+def pnp_ransac_parameters(n, probability=0.99, min_inliers=8, max_iterations=300, min_set=4, epsilon=0.4):
+    """PnPsolver::SetRansacParameters (src/PnPsolver.cc:181-230) on the host: (mRansacMinInliers, mRansacMaxIts) for n
+    correspondences.  min_inliers is raised to (int)(n*epsilon) (a float product, converted as x86 converts) and to
+    min_set; epsilon is raised to the float min_inliers / n; the iteration count is ceil(log(1-p) / log(1-epsilon^3)) in
+    double (3, although the minimal set is 4), 1 when min_inliers == n; the result is max(1, min(count,
+    max_iterations)).  The reference's defaults."""
+    with np.errstate(all="ignore"):
+        eps = np.float32(epsilon)
+        m = _x86_int(float(np.float32(n) * eps))
+        m = max(m, int(min_inliers), int(min_set))
+        q = np.float32(m) / np.float32(n) if n else np.float32(np.inf)
+        if eps < q:
+            eps = q
+        it = 1 if m == n else _ransac_iterations(probability, float(eps), 3)
+    return m, max(1, min(it, int(max_iterations)))
 
 
 class Sim3Solver:
@@ -1383,3 +1436,130 @@ class Sim3SolverBatch:
     def solver(self, *args, **kw):
         """A Sim3Solver on this handle (Sim3Solver's constructor arguments)."""
         return Sim3Solver(*args, _handle=self, **kw)
+
+
+class PnPsolver:
+    """Mirror of ORB_SLAM2::PnPsolver (src/PnPsolver.cc) for one relocalisation candidate, with the minimal sets drawn by
+    the caller (b2s_pnpsolver_iterate).  The constructor takes what the reference's constructor keeps: P3Dw (n x 3,
+    mvP3Dw), P2D (n x 2, mvP2D), sigma2 (n, mvLevelSigma2 of each keypoint's octave) and K (fx, fy, cx, cy); the object
+    keeps mnIterations, mnBestInliers, mBestTcw and mvbBestInliers across calls as the reference does.  `iterate` and
+    `find` run on the device; `iterate_batch` runs the calls of many solvers in one launch sequence."""
+
+    def __init__(self, P3Dw, P2D, sigma2, K, max_matches=None, max_sets=300, device=0, _handle=None):
+        self.P3Dw = np.ascontiguousarray(P3Dw, np.float32).reshape(-1, 3)
+        self.P2D = np.ascontiguousarray(P2D, np.float32).reshape(-1, 2)
+        self.sigma2 = np.ascontiguousarray(sigma2, np.float32).reshape(-1)
+        self.K = [float(v) for v in np.asarray(K, np.float32).reshape(4)]
+        self.N = len(self.P3Dw)
+        self.iterations = 0
+        self.best_inliers = 0
+        self.best_Tcw = np.eye(4, dtype=np.float32)
+        self.best_mask = np.zeros(max(self.N, 1), np.uint8)
+        self.set_ransac_parameters()
+        self._own = _handle is None
+        self._h = _handle._h if _handle is not None else _vp()
+        if self._own:
+            _check(lib().b2s_pnpsolver_create(max(4, max_matches or self.N), max_sets, 1, device, ctypes.byref(self._h)))
+
+    def close(self):
+        if self._own and self._h:
+            lib().b2s_pnpsolver_destroy(self._h)
+        self._h = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def last_ms(self):
+        """Device time of the last call (CUDA events: upload, kernels, download)."""
+        return float(lib().b2s_pnpsolver_last_ms(self._h))
+
+    def set_ransac_parameters(self, probability=0.99, min_inliers=8, max_iterations=300, min_set=4, epsilon=0.4,
+                              th2=5.991):
+        """SetRansacParameters with the reference's defaults.  Like the reference it resets neither the iteration
+        count nor the best model.  Only min_set = 4 is supported (the device rejects any other)."""
+        self.min_inliers, self.max_its = pnp_ransac_parameters(self.N, probability, min_inliers, max_iterations,
+                                                               min_set, epsilon)
+        self.min_set = int(min_set)
+        self.th2 = float(np.float32(th2))
+
+    def sets_needed(self, n_iterations):
+        """How many minimal sets iterate(n_iterations) may consume: 0 when N < min_inliers (the reference draws
+        nothing), else max(n_iterations, max_its - iterations): the loop runs while either bound is not reached."""
+        if self.N < self.min_inliers:
+            return 0
+        return max(0, int(n_iterations), self.max_its - self.iterations)
+
+    def iterate(self, n_iterations, sets):
+        """iterate(n_iterations) with its minimal sets (at least sets_needed(n_iterations) rows of 4 indices into
+        [0, N), in draw order; the extra rows are ignored).  Returns a dict: Tcw (4 x 4, or None for the empty matrix),
+        no_more, inliers (N, compacted order), n_inliers, iterations_used."""
+        return PnPsolver.iterate_batch([self], [n_iterations], [sets])[0]
+
+    def find(self, sets):
+        """find(): iterate(mRansacMaxIts)."""
+        return self.iterate(self.max_its, sets)
+
+    @staticmethod
+    def iterate_batch(solvers, n_iterations, sets, handle=None):
+        """One iterate call per solver, all in one device call (on `handle`, a PnPsolverBatch, or the first solver's
+        handle)."""
+        h = handle._h if handle is not None else solvers[0]._h
+        probs = (_PnPsolverProblem * len(solvers))()
+        res = (_PnPsolverResult * len(solvers))()
+        keep, outs = [], []
+        for i, (sv, nit, st) in enumerate(zip(solvers, n_iterations, sets)):
+            k = sv.sets_needed(nit)
+            st = np.ascontiguousarray(np.asarray(st, np.int32).reshape(-1, 4)[:k])
+            if len(st) < k:
+                raise ValueError("iterate: %d sets given, %d needed" % (len(st), k))
+            tcw = np.ascontiguousarray(sv.best_Tcw, np.float32)
+            keep += [st, tcw]
+            P = probs[i]
+            P.n, P.P3Dw, P.P2D, P.sigma2 = sv.N, sv.P3Dw.ctypes.data, sv.P2D.ctypes.data, sv.sigma2.ctypes.data
+            P.fu, P.fv, P.uc, P.vc, P.th2 = sv.K + [sv.th2]
+            P.min_inliers, P.max_its, P.min_set = sv.min_inliers, sv.max_its, sv.min_set
+            P.iterations_done, P.best_inliers = sv.iterations, sv.best_inliers
+            P.best_Tcw, P.best_mask, P.k, P.sets = tcw.ctypes.data, sv.best_mask.ctypes.data, k, st.ctypes.data
+            out, bm = np.zeros(max(sv.N, 1), np.uint8), np.zeros(max(sv.N, 1), np.uint8)
+            outs.append((out, bm))
+            res[i].inliers, res[i].best_mask = out.ctypes.data, bm.ctypes.data
+        _check(lib().b2s_pnpsolver_iterate(h, len(solvers), probs, res))
+        ret = []
+        for sv, r, (out, bm) in zip(solvers, res, outs):
+            sv.iterations, sv.best_inliers = r.iterations_done, r.best_inliers
+            sv.best_Tcw = np.array(r.best_Tcw[:], np.float32).reshape(4, 4)
+            sv.best_mask = bm
+            ret.append(dict(Tcw=np.array(r.Tcw[:], np.float32).reshape(4, 4) if r.returned else None,
+                            no_more=bool(r.no_more), inliers=out[:sv.N].astype(bool), n_inliers=r.n_inliers,
+                            iterations_used=r.iterations_used))
+        return ret
+
+
+class PnPsolverBatch:
+    """A device handle sized for batched PnPsolver.iterate_batch calls (max_matches per solver, max_sets per call,
+    max_batch solvers)."""
+
+    def __init__(self, max_matches=4096, max_sets=300, max_batch=64, device=0):
+        self._h = _vp()
+        _check(lib().b2s_pnpsolver_create(max_matches, max_sets, max_batch, device, ctypes.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().b2s_pnpsolver_destroy(self._h)
+            self._h = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def last_ms(self):
+        return float(lib().b2s_pnpsolver_last_ms(self._h))
+
+    def solver(self, *args, **kw):
+        """A PnPsolver on this handle (PnPsolver's constructor arguments)."""
+        return PnPsolver(*args, _handle=self, **kw)

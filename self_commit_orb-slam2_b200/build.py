@@ -18,7 +18,7 @@ NVCC_FLAGS = GENCODE + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-
 # extractor/matcher/keyframe database: bit-exact float arithmetic, never contract a*b+c; LocalBA is FP64 with a 1e-5 bar
 # -> FMA allowed; the essential graph differentiates numerically (delta = 1e-9 amplifies last-bit differences ~5e8 times)
 NO_FMAD = {"extractor.cu", "extractor_tile.cu", "matcher.cu", "common.cu", "kfdb.cu", "essential.cu", "sim3opt.cu",
-            "initializer.cu", "sim3solver.cu"}
+            "initializer.cu", "sim3solver.cu", "pnpsolver.cu"}
 
 
 def _newer(target, sources):
@@ -46,6 +46,8 @@ def _deps_of(src):
         deps.append(os.path.join(CSRC, "sim3.cuh"))
     if base in ("gba.cu", "essential.cu"):
         deps.append(os.path.join(CSRC, "chol.cuh"))
+    if base in ("initializer.cu", "pnpsolver.cu"):
+        deps.append(os.path.join(CSRC, "jacobi.cuh"))
     if base == "extractor.cu":
         deps.append(os.path.join(ROOT, "data", "orb_pattern_31.inc"))
     return deps
@@ -98,6 +100,9 @@ def build_oracle(force=False):
     # the Sim3 RANSAC's CPU restatement (oracle/sim3solver.mk)
     subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "sim3solver.mk"] + (["-B"] if force else []) +
                           ["liborb_sim3solver.so"])
+    # the EPnP RANSAC's CPU restatement (oracle/pnpsolver.mk)
+    subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "pnpsolver.mk"] + (["-B"] if force else []) +
+                          ["liborb_pnpsolver.so"])
     return ORACLE_LIB
 
 
@@ -115,6 +120,7 @@ def build_oracle_ref():
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "sim3opt.mk", "sim3opt-ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "init.mk", "init-ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "sim3solver.mk", "sim3solver-ref", "REF=" + ref])
+    subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "pnpsolver.mk", "pnpsolver-ref", "REF=" + ref])
     return os.path.join(ORACLE_DIR, "_ref")
 
 

@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "jacobi.cuh"
 
 namespace b2s {
 namespace ini {
@@ -67,130 +68,6 @@ struct Ptrs {
 };
 
 // ------------------------------------------------------------------------------------------------ OpenCV arithmetic
-__device__ __forceinline__ unsigned rng_next(uint64_t& state) {
-  state = (uint64_t)(unsigned)state * 4164903690u + (unsigned)(state >> 32);
-  return (unsigned)state;
-}
-
-// JacobiSVDImpl_<float> (oracle/init.cpp jacobi_svd): At n rows of m, W n, Vt n x n (row stride n), n1 rows of At
-// normalised / completed.  NMAX bounds n.
-template <int NMAX>
-__device__ void jacobi_svd(float* At, int astep, float* Wout, float* Vt, int m, int n, int n1) {
-  const double minval = FLT_MIN;
-  const float eps = FLT_EPSILON * 2;
-  double W[NMAX];
-  const int max_iter = m > 30 ? m : 30;
-  for (int i = 0; i < n; i++) {
-    double sd = 0;
-    for (int k = 0; k < m; k++) {
-      const float t = At[i * astep + k];
-      sd += (double)t * t;
-    }
-    W[i] = sd;
-    for (int k = 0; k < n; k++) Vt[i * n + k] = 0;
-    Vt[i * n + i] = 1;
-  }
-  for (int iter = 0; iter < max_iter; iter++) {
-    bool changed = false;
-    for (int i = 0; i < n - 1; i++)
-      for (int j = i + 1; j < n; j++) {
-        float *Ai = At + i * astep, *Aj = At + j * astep;
-        double a = W[i], p = 0, b = W[j];
-        for (int k = 0; k < m; k++) p += (double)Ai[k] * Aj[k];
-        if (fabs(p) <= eps * sqrt((double)a * b)) continue;
-        p *= 2;
-        const double beta = a - b, gamma = hypot(p, beta);
-        float c, s;
-        if (beta < 0) {
-          const double delta = (gamma - beta) * 0.5;
-          s = (float)sqrt(delta / gamma);
-          c = (float)(p / (gamma * s * 2));
-        } else {
-          c = (float)sqrt((gamma + beta) / (gamma * 2));
-          s = (float)(p / (gamma * c * 2));
-        }
-        a = b = 0;
-        for (int k = 0; k < m; k++) {
-          const float t0 = c * Ai[k] + s * Aj[k];
-          const float t1 = -s * Ai[k] + c * Aj[k];
-          Ai[k] = t0;
-          Aj[k] = t1;
-          a += (double)t0 * t0;
-          b += (double)t1 * t1;
-        }
-        W[i] = a;
-        W[j] = b;
-        changed = true;
-        float *Vi = Vt + i * n, *Vj = Vt + j * n;
-        for (int k = 0; k < n; k++) {
-          const float t0 = c * Vi[k] + s * Vj[k];
-          const float t1 = -s * Vi[k] + c * Vj[k];
-          Vi[k] = t0;
-          Vj[k] = t1;
-        }
-      }
-    if (!changed) break;
-  }
-  for (int i = 0; i < n; i++) {
-    double sd = 0;
-    for (int k = 0; k < m; k++) {
-      const float t = At[i * astep + k];
-      sd += (double)t * t;
-    }
-    W[i] = sqrt(sd);
-  }
-  for (int i = 0; i < n - 1; i++) {
-    int j = i;
-    for (int k = i + 1; k < n; k++)
-      if (W[j] < W[k]) j = k;
-    if (i != j) {
-      const double w = W[i];
-      W[i] = W[j];
-      W[j] = w;
-      for (int k = 0; k < m; k++) {
-        const float x = At[i * astep + k];
-        At[i * astep + k] = At[j * astep + k];
-        At[j * astep + k] = x;
-      }
-      for (int k = 0; k < n; k++) {
-        const float x = Vt[i * n + k];
-        Vt[i * n + k] = Vt[j * n + k];
-        Vt[j * n + k] = x;
-      }
-    }
-  }
-  for (int i = 0; i < n; i++) Wout[i] = (float)W[i];
-  uint64_t rng = 0x12345678;
-  for (int i = 0; i < n1; i++) {
-    double sd = i < n ? W[i] : 0;
-    for (int ii = 0; ii < 100 && sd <= minval; ii++) {
-      const float val0 = (float)(1. / m);
-      for (int k = 0; k < m; k++) At[i * astep + k] = (rng_next(rng) & 256) != 0 ? val0 : -val0;
-      for (int it2 = 0; it2 < 2; it2++)
-        for (int j = 0; j < i; j++) {
-          sd = 0;
-          for (int k = 0; k < m; k++) sd += At[i * astep + k] * At[j * astep + k];
-          float asum = 0;
-          for (int k = 0; k < m; k++) {
-            const float t = (float)(At[i * astep + k] - sd * At[j * astep + k]);
-            At[i * astep + k] = t;
-            asum += fabsf(t);
-          }
-          asum = asum > eps * 100 ? 1 / asum : 0;
-          for (int k = 0; k < m; k++) At[i * astep + k] *= asum;
-        }
-      sd = 0;
-      for (int k = 0; k < m; k++) {
-        const float t = At[i * astep + k];
-        sd += (double)t * t;
-      }
-      sd = sqrt(sd);
-    }
-    const float s = (float)(sd > minval ? 1 / sd : 0.);
-    for (int k = 0; k < m; k++) At[i * astep + k] *= s;
-  }
-}
-
 // SVD::compute of a square 3 x 3 (u, w, vt) or, with want_u = false, vt of a 4 x 4 (Triangulate)
 template <int N>
 __device__ void svd_square(const float* A, float* w, float* u, float* vt, bool want_u) {
