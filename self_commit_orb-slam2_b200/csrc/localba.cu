@@ -1131,7 +1131,9 @@ __device__ void control_end(const BaPtrs& p, int w, int nCta) {
     st.needBuild = 1;
     st.errCurrent = 0;  // levels and kernels change: the stored weights are void
   } else {
-    st.doOutlier = 2;  // final outlier test (:921-958); it also runs when round 2 is skipped
+    // final outlier test (:921-958); it also runs when round 2 is skipped.  3: skipped because its2 == 0, so ba_run
+    // replaces chi2Final by the chi2 of round 2's active set
+    st.doOutlier = (st.round == 0 && !stop) ? 3 : 2;
     st.active = 0;
   }
 }
@@ -2066,6 +2068,17 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
     if (s.st[w].pairsOverflow) {
       set_error("b2s_local_ba: window %d: covisibility pair list exceeds its capacity of %d", w, d.capPairs);
       return B2S_ERR_CAPACITY;
+    }
+  // round 2 skipped (its2 == 0): the optimiser still ends with round 2's active set, the edges the final test keeps
+  // without robust kernels, so chi2_final is their plain chi2 (as when round 2 runs, or has no edge left: k_local_ba)
+  for (int w = 0; w < batch; w++)
+    if (s.st[w].doOutlier == 3) {
+      std::vector<double> c2((size_t)probs[w].n_edges);
+      B2S_CUDA(cudaMemcpy(c2.data(), d.chi2 + (size_t)w * d.capE, c2.size() * 8, cudaMemcpyDeviceToHost));
+      double chi = 0;
+      for (size_t e = 0; e < c2.size(); e++)
+        if (!s.eOutlier[(size_t)w * d.capE + e]) chi += c2[e];
+      s.st[w].chi2Final = chi;
     }
   ba_for_windows(batch, [&](int w) {
     const b2s_ba_problem& P = probs[w];

@@ -87,6 +87,27 @@ def call_local_ba(fn, d, stop=None, its1=5, its2=10):
     return out
 
 
+def call_ref_local_ba(fn, d, stop=None):
+    """ref_local_ba / adp_local_ba (oracle/ref_optimizer_glue.cpp) for any window.  The glue's keyframe 0 is the triggering
+    keyframe with mnId 0, which the reference keeps fixed (src/Optimizer.cc:722), so the glue takes only windows whose
+    keyframe 0 is fixed.  A window whose current keyframe is free (every LocalBA after the map's first keyframe) goes in
+    behind one extra keyframe: a fixed pKF with mnId 0 and no observation.  Its vertex has no edge, so g2o leaves it out of
+    the optimisation (initializeOptimization activates only vertices with an edge at the level), and keyframe k of the
+    window becomes the free local keyframe with mnId k + 1.  Returns the result of the window as given."""
+    if d["fixed"][0]:
+        return call_local_ba(fn, d, stop)
+    e = dict(d)
+    e["n_kf"], e["n_local"] = d["n_kf"] + 1, d["n_local"] + 1
+    e["Tcw"] = np.concatenate([np.eye(4, dtype=np.float32).reshape(1, 16), np.asarray(d["Tcw"], np.float32).reshape(-1, 16)])
+    e["fixed"] = np.concatenate([[1], d["fixed"]]).astype(np.uint8)
+    e["edges"] = np.array(d["edges"], copy=True)
+    e["edges"]["kf"] += 1
+    out = call_local_ba(fn, e, stop)
+    if out is not None:
+        out["Tcw"] = np.ascontiguousarray(out["Tcw"][1:])
+    return out
+
+
 class Oracle:
     def __init__(self, L):
         self.L = L

@@ -177,25 +177,37 @@ def synth_descriptors(n, seed=1234, match_frac=0.7, max_flips=40, n_nodes=100):
     return A, nodeA, validA, angA, B, nodeB, angB
 
 
-def synth_local_ba(n_kf=50, n_fixed=10, n_mp=5000, obs_per_mp=6, seed=42, mono_frac=0.0, outlier_frac=0.03):
+def _path_position(n_kf, revisit):
+    """Position of every keyframe along the path (metres): a straight forward path, or with `revisit` one that runs
+    twice over the same ground, so that keyframes k and k + ceil(n_kf / 2) see the same points."""
+    k = np.arange(n_kf)
+    return k % -(-n_kf // 2) if revisit else k
+
+
+def synth_local_ba(n_kf=50, n_fixed=10, n_mp=5000, obs_per_mp=6, seed=42, mono_frac=0.0, outlier_frac=0.03,
+                   fix_first=True, revisit=False):
     """KITTI-shaped LocalBA window (SURVEY §8d): forward path, stereo edges, 3 % gross outliers.
 
     Returns dict with float32 arrays exactly as Converter would hand them over.
-    Keyframes [0, n_kf-n_fixed) are local (free, except index 0 which plays mnId==0 only if fix_first),
-    the last n_fixed are fixed cameras.
+    Keyframes [0, n_kf-n_fixed) are local: free, except keyframe 0 when fix_first (it plays the map's first keyframe,
+    mnId == 0); the last n_fixed are fixed cameras.  A point is observed by the obs_per_mp keyframes that see it and lie
+    nearest its anchor keyframe along the path; with `revisit` the path passes twice over the same ground, so the
+    covisibility graph is not banded (see _path_position).  The defaults reproduce the windows of earlier versions bit for
+    bit.
     """
     rng = np.random.RandomState(seed)
     fx = fy = 718.856
     cx, cy, bf = 607.1928, 185.2157, 386.1448
     W, H = 1241, 376
     n_local = n_kf - n_fixed
+    pos = _path_position(n_kf, revisit)
     # true poses: camera moves along +z, 1 m spacing, small yaw jitter. Tcw = [R | -R*c]
     Tcw_true = np.zeros((n_kf, 4, 4))
     for k in range(n_kf):
         yaw = np.deg2rad(rng.uniform(-2, 2))
         c, s = np.cos(yaw), np.sin(yaw)
         R = np.array([[c, 0, -s], [0, 1, 0], [s, 0, c]])
-        center = np.array([rng.uniform(-0.1, 0.1), rng.uniform(-0.05, 0.05), 1.0 * k])
+        center = np.array([rng.uniform(-0.1, 0.1), rng.uniform(-0.05, 0.05), 1.0 * pos[k]])
         Tcw_true[k, :3, :3] = R
         Tcw_true[k, :3, 3] = -R @ center
         Tcw_true[k, 3, 3] = 1
@@ -221,7 +233,7 @@ def synth_local_ba(n_kf=50, n_fixed=10, n_mp=5000, obs_per_mp=6, seed=42, mono_f
                 uu = fx * Xk[0] / Xk[2] + cx
                 vv = fy * Xk[1] / Xk[2] + cy
                 if 0 < uu < W and 0 < vv < H:
-                    vis.append((abs(k - ka), k, uu, vv, Xk[2]))
+                    vis.append((abs(int(pos[k]) - int(pos[ka])), k, uu, vv, Xk[2]))
             if len(vis) >= obs_per_mp:
                 break
         vis.sort()
@@ -246,7 +258,8 @@ def synth_local_ba(n_kf=50, n_fixed=10, n_mp=5000, obs_per_mp=6, seed=42, mono_f
     pts0 = pts_true + rng.normal(0, 0.05, pts_true.shape)
     fixed = np.zeros(n_kf, np.uint8)
     fixed[n_local:] = 1
-    fixed[0] = 1  # plays the role of mnId==0
+    if fix_first:
+        fixed[0] = 1  # plays the role of mnId==0
     edge_dt = np.dtype([("kf", "i4"), ("mp", "i4"), ("obs", "f4", 3), ("inv_sigma2", "f4")])
     E = np.zeros(len(edges), edge_dt)
     for i, (k, m, a, b_, c_, w) in enumerate(edges):
@@ -494,21 +507,23 @@ def synth_voc_features(voc, n=2000, seed=5):
     return f
 
 
-def synth_local_ba_fast(n_kf=50, n_fixed=10, n_mp=5000, obs_per_mp=6, seed=42, mono_frac=0.0, outlier_frac=0.03):
+def synth_local_ba_fast(n_kf=50, n_fixed=10, n_mp=5000, obs_per_mp=6, seed=42, mono_frac=0.0, outlier_frac=0.03,
+                        fix_first=True, revisit=False):
     """Vectorised variant of synth_local_ba (same construction: KITTI-shaped forward path, points in the frustum of an
     anchor keyframe, the obs_per_mp observing keyframes nearest to it, noise ~ 1.2^octave, gross outliers, perturbed
-    initial state) for callers that need many different windows quickly (bench.py).  Not stream-compatible with
-    synth_local_ba: the parity tests keep that one."""
+    initial state, the same fix_first and revisit options) for callers that need many different windows quickly
+    (bench.py).  Not stream-compatible with synth_local_ba: the parity tests keep that one."""
     rng = np.random.RandomState(seed)
     fx = fy = 718.856
     cx, cy, bf = 607.1928, 185.2157, 386.1448
     W, H = 1241, 376
     n_local = n_kf - n_fixed
+    pos = _path_position(n_kf, revisit)
     yaw = np.deg2rad(rng.uniform(-2, 2, n_kf))
     c, s = np.cos(yaw), np.sin(yaw)
     R = np.zeros((n_kf, 3, 3))
     R[:, 0, 0] = c; R[:, 0, 2] = -s; R[:, 1, 1] = 1; R[:, 2, 0] = s; R[:, 2, 2] = c
-    center = np.stack([rng.uniform(-0.1, 0.1, n_kf), rng.uniform(-0.05, 0.05, n_kf), 1.0 * np.arange(n_kf)], 1)
+    center = np.stack([rng.uniform(-0.1, 0.1, n_kf), rng.uniform(-0.05, 0.05, n_kf), 1.0 * pos], 1)
     t = -np.einsum("kij,kj->ki", R, center)
     pts = np.zeros((n_mp, 3))
     chosen = np.full((n_mp, obs_per_mp), -1, np.int64)
@@ -529,7 +544,7 @@ def synth_local_ba_fast(n_kf=50, n_fixed=10, n_mp=5000, obs_per_mp=6, seed=42, m
         vv = fy * Xk[..., 1] / np.where(zz > 0, zz, 1) + cy
         vis = (zz >= 2.0) & (uu > 0) & (uu < W) & (vv > 0) & (vv < H)
         ok = vis.sum(1) >= obs_per_mp
-        dist = np.where(vis, np.abs(np.arange(n_kf)[None] - ka[:, None]), 10 ** 6)
+        dist = np.where(vis, np.abs(pos[None] - pos[ka][:, None]), 10 ** 6)
         near = np.sort(np.argsort(dist, 1, kind="stable")[:, :obs_per_mp], 1)
         pts[todo[ok]] = Xw[ok]
         chosen[todo[ok]] = near[ok]
@@ -562,7 +577,8 @@ def synth_local_ba_fast(n_kf=50, n_fixed=10, n_mp=5000, obs_per_mp=6, seed=42, m
     pts0 = pts + rng.normal(0, 0.05, pts.shape)
     fixed = np.zeros(n_kf, np.uint8)
     fixed[n_local:] = 1
-    fixed[0] = 1
+    if fix_first:
+        fixed[0] = 1
     edge_dt = np.dtype([("kf", "i4"), ("mp", "i4"), ("obs", "f4", 3), ("inv_sigma2", "f4")])
     E = np.zeros(ne, edge_dt)
     E["kf"] = kf

@@ -16,7 +16,7 @@ import os
 import numpy as np
 import pytest
 
-from oracle_binding import call_local_ba, call_pose_optimization
+from oracle_binding import call_local_ba, call_pose_optimization, call_ref_local_ba
 from synth import synth_local_ba, synth_pose_problem
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -41,12 +41,15 @@ def libs():
 
 @pytest.mark.parametrize("kw", [dict(n_kf=8, n_fixed=2, n_mp=200, obs_per_mp=4, seed=5),
                                 dict(n_kf=12, n_fixed=3, n_mp=600, obs_per_mp=5, seed=7, mono_frac=0.4),
-                                dict(n_kf=50, n_fixed=10, n_mp=5000, obs_per_mp=6, seed=42)])
+                                dict(n_kf=50, n_fixed=10, n_mp=5000, obs_per_mp=6, seed=42),
+                                # a free current keyframe; behind the unobserved first keyframe of call_ref_local_ba the
+                                # adapter's window has 128 keyframes, 126 of them free, and it grows its handle to 128
+                                dict(n_kf=127, n_fixed=1, n_mp=1500, obs_per_mp=4, seed=128, fix_first=False)])
 def test_local_bundle_adjustment_signature(libs, kw):
     ref, adp = libs
     d = synth_local_ba(**kw)
-    want = call_local_ba(ref.ref_local_ba, d)
-    got = call_local_ba(adp.adp_local_ba, d)
+    want = call_ref_local_ba(ref.ref_local_ba, d)
+    got = call_ref_local_ba(adp.adp_local_ba, d)
     assert np.array_equal(got["outlier"], want["outlier"])  # the same observations are erased
     assert _close(got["Tcw"], want["Tcw"], d["Tcw"][:d["n_local"]])
     assert _close(got["points"], want["points"], d["points"])
