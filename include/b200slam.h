@@ -771,6 +771,77 @@ int b2s_pnpsolver_iterate(b2s_pnpsolver* h, int batch, const b2s_pnpsolver_probl
 /* Device time (CUDA events on the solver's stream: upload, kernels, download) of the last call. */
 float b2s_pnpsolver_last_ms(const b2s_pnpsolver* h);
 
+/* ---------------------------------------------------------------------------------------------------------------------
+ * Covisibility graph update: KeyFrame::UpdateConnections (src/KeyFrame.cc:386-507) for a batch of keyframes, with the
+ * AddConnection (:159-178) and UpdateBestCovisibles (:185-209) it calls on the partners.  A batch gives exactly the state
+ * that calling the reference on its members one after another gives.  Keyframes are dense table indices in ascending
+ * mnId, which stands for the reference's pointer order (map iteration and the pair sort's tie-break, DESIGN §2).  The
+ * state goes in and comes out, so the ABI is stateless.  Everything is an integer; the result is exact.
+ *
+ * The table must hold every member and every keyframe that observes one of their non-bad points.  Connection maps and
+ * ordered lists name table indices; the entry state of a keyframe that is neither a member nor such an observer is
+ * never read, so it may be passed empty. */
+typedef struct {
+  int32_t n_kf;
+  const uint64_t* kf_id;          /* n_kf: mnId, strictly ascending */
+  const int32_t* map_off;         /* n_kf + 1: mConnectedKeyFrameWeights on entry, CSR */
+  const int32_t* map_kf;          /* keyframe indices, strictly ascending within a row */
+  const int32_t* map_w;           /* weights */
+  const int32_t* list_off;        /* n_kf + 1: mvpOrderedConnectedKeyFrames on entry, CSR */
+  const int32_t* list_kf;
+  const int32_t* list_w;          /* mvOrderedWeights on entry */
+  const uint8_t* first_connection;/* n_kf: mbFirstConnection */
+  const int32_t* parent;          /* n_kf: mpParent's index, -1 for NULL */
+  int32_t n_mp;
+  const uint8_t* mp_bad;          /* n_mp: MapPoint::isBad() */
+  const int32_t* obs_off;         /* n_mp + 1: the observers of each point (GetObservations' keys), CSR */
+  const int32_t* obs_kf;          /* keyframe indices, strictly ascending within a row */
+  int32_t batch;                  /* calls, in call order */
+  const int32_t* member;          /* batch: the keyframe of each call (repeats allowed) */
+  const int32_t* slot_off;        /* batch + 1: each call's mvpMapPoints, CSR */
+  const int32_t* slot_mp;         /* map-point index, -1 for NULL, in feature order */
+} b2s_covis_problem;
+/* Rows of the CSR outputs are packed in row order; row i spans [off[i], off[i + 1]). */
+typedef struct {
+  uint8_t* changed;               /* n_kf: 1 when a call of the batch wrote the keyframe's connection state */
+  int32_t* parent;                /* n_kf: mpParent after the batch */
+  uint8_t* first_connection;      /* n_kf: mbFirstConnection after the batch */
+  int32_t* map_off;               /* n_kf + 1: the final connection map of each changed keyframe (other rows empty) */
+  int32_t* map_kf;                /* map_cap */
+  int32_t* map_w;
+  int32_t map_cap;
+  int32_t* list_off;              /* n_kf + 1: the final ordered list of each changed keyframe (other rows empty) */
+  int32_t* list_kf;               /* list_cap */
+  int32_t* list_w;
+  int32_t list_cap;
+  int32_t* child_pairs;           /* 2 x batch: the (parent, child) pairs AddChild added, in call order */
+  int32_t n_pairs;
+  int32_t* start_off;             /* batch + 1: each call's GetVectorCovisibleKeyFrames() just before the call */
+  int32_t* start_kf;              /* start_cap */
+  int32_t start_cap;
+  int32_t* after_off;             /* batch + 1: each call's connection map right after the call (the counter it
+                                     computed, or the unchanged map when the counter was empty) */
+  int32_t* after_kf;              /* after_cap */
+  int32_t* after_w;
+  int32_t after_cap;
+  int32_t map_need, list_need, start_need, after_need; /* entries the four CSRs need (written on B2S_ERR_CAPACITY too) */
+} b2s_covis_result;
+typedef struct b2s_covis b2s_covis;
+/* Per call: up to max_kf keyframes, max_mp map points, max_obs observations, max_slots slots over the batch, max_conn
+ * entries in the entry maps (and in each of the device's output areas), max_batch calls.  The handle keeps
+ * max_batch x max_kf x 28 bytes of scratch. */
+int b2s_covis_create(int max_kf, int max_mp, int max_obs, int max_slots, int max_conn, int max_batch, int device,
+                     b2s_covis** out);
+void b2s_covis_destroy(b2s_covis* h);
+/* A problem beyond the handle's capacities, or outputs that do not fit the handle's max_conn: B2S_ERR_CAPACITY; outputs
+ * beyond the caller's caps: B2S_ERR_CAPACITY with the *_need fields written.  A null array, batch < 1, n_kf < 1, ids not
+ * strictly ascending, offsets that are not a CSR, an index out of range (a member, a map or list entry, a parent, an
+ * observer, a slot), or a map or observer row that is not strictly ascending: B2S_ERR_BAD_ARG.  Nothing else is written
+ * unless the call succeeds. */
+int b2s_update_connections(b2s_covis* h, const b2s_covis_problem* p, b2s_covis_result* r);
+/* Device time (CUDA events on the handle's stream: upload, kernels, download) of the last call. */
+float b2s_covis_last_ms(const b2s_covis* h);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,0 +1,2 @@
+// <opencv2/core/core.hpp> for the in-place build of src/KeyFrame.cc only (oracle/covis.mk)
+#include "../../../refshim_cv_keyframe.h"

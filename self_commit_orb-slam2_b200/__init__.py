@@ -156,6 +156,22 @@ class _PnPsolverResult(ctypes.Structure):  # b2s_pnpsolver_result
                 ("best_Tcw", ctypes.c_float * 16), ("best_mask", _vp)]
 
 
+class _CovisProblem(ctypes.Structure):  # b2s_covis_problem
+    _fields_ = [("n_kf", ctypes.c_int32), ("kf_id", _vp), ("map_off", _vp), ("map_kf", _vp), ("map_w", _vp),
+                ("list_off", _vp), ("list_kf", _vp), ("list_w", _vp), ("first_connection", _vp), ("parent", _vp),
+                ("n_mp", ctypes.c_int32), ("mp_bad", _vp), ("obs_off", _vp), ("obs_kf", _vp), ("batch", ctypes.c_int32),
+                ("member", _vp), ("slot_off", _vp), ("slot_mp", _vp)]
+
+
+class _CovisResult(ctypes.Structure):  # b2s_covis_result
+    _fields_ = [("changed", _vp), ("parent", _vp), ("first_connection", _vp), ("map_off", _vp), ("map_kf", _vp),
+                ("map_w", _vp), ("map_cap", ctypes.c_int32), ("list_off", _vp), ("list_kf", _vp), ("list_w", _vp),
+                ("list_cap", ctypes.c_int32), ("child_pairs", _vp), ("n_pairs", ctypes.c_int32), ("start_off", _vp),
+                ("start_kf", _vp), ("start_cap", ctypes.c_int32), ("after_off", _vp), ("after_kf", _vp),
+                ("after_w", _vp), ("after_cap", ctypes.c_int32), ("map_need", ctypes.c_int32),
+                ("list_need", ctypes.c_int32), ("start_need", ctypes.c_int32), ("after_need", ctypes.c_int32)]
+
+
 class _GbaResult(ctypes.Structure):
     _fields_ = [("Tcw_out", _vp), ("points_out", _vp), ("point_included", _vp), ("trace", _vp),
                 ("chi2_final", ctypes.c_double), ("n_trials", ctypes.c_int)]
@@ -275,6 +291,13 @@ def lib():
             L.b2s_pnpsolver_iterate.argtypes = [_vp, ctypes.c_int, _vp, _vp]
             L.b2s_pnpsolver_last_ms.restype = ctypes.c_float
             L.b2s_pnpsolver_last_ms.argtypes = [_vp]
+        if hasattr(L, "b2s_covis_create"):
+            L.b2s_covis_create.argtypes = [ctypes.c_int] * 7 + [_vp]
+            L.b2s_covis_destroy.argtypes = [_vp]
+            L.b2s_covis_destroy.restype = None
+            L.b2s_update_connections.argtypes = [_vp, _vp, _vp]
+            L.b2s_covis_last_ms.restype = ctypes.c_float
+            L.b2s_covis_last_ms.argtypes = [_vp]
         _lib = L
     return _lib
 
@@ -1563,3 +1586,105 @@ class PnPsolverBatch:
     def solver(self, *args, **kw):
         """A PnPsolver on this handle (PnPsolver's constructor arguments)."""
         return PnPsolver(*args, _handle=self, **kw)
+
+
+# ------------------------------------------------------------------------------------------ covisibility graph update
+_COVIS_ARRAYS = [("kf_id", np.uint64), ("map_off", np.int32), ("map_kf", np.int32), ("map_w", np.int32),
+                 ("list_off", np.int32), ("list_kf", np.int32), ("list_w", np.int32), ("first_connection", np.uint8),
+                 ("parent", np.int32), ("mp_bad", np.uint8), ("obs_off", np.int32), ("obs_kf", np.int32),
+                 ("member", np.int32), ("slot_off", np.int32), ("slot_mp", np.int32)]
+
+
+def covis_problem(d):
+    """(b2s_covis_problem, the contiguous arrays it points into) from a problem dict with the fields of
+    b2s_covis_problem (arrays; n_kf, n_mp and batch follow from kf_id, mp_bad and member)."""
+    arr = {k: np.ascontiguousarray(d[k], t) for k, t in _COVIS_ARRAYS}
+    p = _CovisProblem(n_kf=len(arr["kf_id"]), n_mp=len(arr["mp_bad"]), batch=len(arr["member"]))
+    for k, _ in _COVIS_ARRAYS:
+        setattr(p, k, arr[k].ctypes.data_as(_vp))
+    return p, arr
+
+
+def covis_call(call, d, cap, extra=None):
+    """Runs `call(problem, result)` (b2s_update_connections or a checker with its signature) with output capacities
+    `cap` and returns (status, raw result dict).  `extra`: arrays a checker fills beside the result."""
+    p, keep = covis_problem(d)
+    n, B = p.n_kf, p.batch
+    o = {"changed": np.zeros(n, np.uint8), "parent": np.zeros(n, np.int32), "first_connection": np.zeros(n, np.uint8),
+         "map_off": np.zeros(n + 1, np.int32), "map_kf": np.zeros(cap, np.int32), "map_w": np.zeros(cap, np.int32),
+         "list_off": np.zeros(n + 1, np.int32), "list_kf": np.zeros(cap, np.int32), "list_w": np.zeros(cap, np.int32),
+         "child_pairs": np.zeros(2 * B, np.int32), "start_off": np.zeros(B + 1, np.int32),
+         "start_kf": np.zeros(cap, np.int32), "after_off": np.zeros(B + 1, np.int32),
+         "after_kf": np.zeros(cap, np.int32), "after_w": np.zeros(cap, np.int32)}
+    r = _CovisResult(map_cap=cap, list_cap=cap, start_cap=cap, after_cap=cap)
+    for k, v in o.items():
+        setattr(r, k, v.ctypes.data_as(_vp))
+    rc = call(ctypes.byref(p), ctypes.byref(r))
+    o["n_pairs"] = r.n_pairs
+    o["need"] = (r.map_need, r.list_need, r.start_need, r.after_need)
+    return rc, o
+
+
+def covis_state(d, o):
+    """The final state of every keyframe from a raw result: rows of unchanged keyframes are their entry rows.  Returns
+    a dict: changed, parent, first_connection, map / list CSRs (off, kf, w) for all keyframes, pairs (n_pairs x 2),
+    start (off, kf) and after (off, kf, w) per call."""
+    n = len(d["kf_id"])
+    out = {"changed": o["changed"].copy(), "parent": o["parent"].copy(),
+           "first_connection": o["first_connection"].copy()}
+    for name, cols in (("map", ("kf", "w")), ("list", ("kf", "w"))):
+        off_in, off_out = np.asarray(d[name + "_off"]), o[name + "_off"]
+        rows = {c: [] for c in cols}
+        for t in range(n):
+            for c in cols:
+                src = o[name + "_" + c][off_out[t]:off_out[t + 1]] if o["changed"][t] else \
+                    np.asarray(d[name + "_" + c])[off_in[t]:off_in[t + 1]]
+                rows[c].append(np.asarray(src, np.int32))
+        lens = np.array([len(x) for x in rows[cols[0]]], np.int64)
+        out[name + "_off"] = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
+        for c in cols:
+            out[name + "_" + c] = np.concatenate(rows[c]) if n else np.zeros(0, np.int32)
+    out["pairs"] = o["child_pairs"][:2 * o["n_pairs"]].reshape(-1, 2).copy()
+    ns, na = o["start_off"][-1], o["after_off"][-1]
+    out["start_off"], out["start_kf"] = o["start_off"].copy(), o["start_kf"][:ns].copy()
+    out["after_off"], out["after_kf"], out["after_w"] = o["after_off"].copy(), o["after_kf"][:na].copy(), \
+        o["after_w"][:na].copy()
+    return out
+
+
+class Covisibility:
+    """KeyFrame::UpdateConnections for a batch of keyframes (b2s_update_connections), stateless: the problem dict
+    holds the keyframe table with its connection state on entry, the map points the members see and the batch (the
+    fields of b2s_covis_problem, as arrays); the result is a dict with the state after the batch (covis_state)."""
+
+    def __init__(self, max_kf=8192, max_mp=1 << 17, max_obs=1 << 20, max_slots=1 << 17, max_conn=1 << 20,
+                 max_batch=256, device=0):
+        self.max_conn = max_conn
+        self._h = _vp()
+        _check(lib().b2s_covis_create(max_kf, max_mp, max_obs, max_slots, max_conn, max_batch, device,
+                                      ctypes.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().b2s_covis_destroy(self._h)
+            self._h = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def last_ms(self):
+        """Device time of the last call (CUDA events: upload, kernels, download)."""
+        return float(lib().b2s_covis_last_ms(self._h))
+
+    def raw(self, d, cap=None):
+        """(status, raw result dict) with output capacities `cap` (default: the handle's max_conn, always enough)."""
+        return covis_call(lambda p, r: lib().b2s_update_connections(self._h, p, r), d,
+                          self.max_conn if cap is None else cap)
+
+    def UpdateConnections(self, d):
+        rc, o = self.raw(d)
+        _check(rc)
+        return covis_state(d, o)

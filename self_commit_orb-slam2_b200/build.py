@@ -103,6 +103,9 @@ def build_oracle(force=False):
     # the EPnP RANSAC's CPU restatement (oracle/pnpsolver.mk)
     subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "pnpsolver.mk"] + (["-B"] if force else []) +
                           ["liborb_pnpsolver.so"])
+    # the covisibility update's CPU restatement (oracle/covis.mk)
+    subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "covis.mk"] + (["-B"] if force else []) +
+                          ["liborb_covis.so"])
     return ORACLE_LIB
 
 
@@ -121,6 +124,7 @@ def build_oracle_ref():
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "init.mk", "init-ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "sim3solver.mk", "sim3solver-ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "pnpsolver.mk", "pnpsolver-ref", "REF=" + ref])
+    subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "covis.mk", "covis-ref", "REF=" + ref])
     return os.path.join(ORACLE_DIR, "_ref")
 
 
