@@ -842,6 +842,65 @@ int b2s_update_connections(b2s_covis* h, const b2s_covis_problem* p, b2s_covis_r
 /* Device time (CUDA events on the handle's stream: upload, kernels, download) of the last call. */
 float b2s_covis_last_ms(const b2s_covis* h);
 
+/* ---------------------------------------------------------------------------------------------------------------------
+ * Keyframe culling: LocalMapping::KeyFrameCulling (src/LocalMapping.cc:873-956) for a batch of independent local maps,
+ * with the effects on map points of the KeyFrame::SetBadFlag (src/KeyFrame.cc:599-722) it calls on each redundant
+ * keyframe: MapPoint::EraseObservation (src/MapPoint.cc:170-200) on every non-NULL slot, and MapPoint::SetBadFlag
+ * (:217-234) with the EraseMapPointMatch it makes on the remaining observers.  The local keyframes are decided in list
+ * order, each from the state the earlier culls left.  The state goes in and comes out, so the ABI is stateless.  The
+ * work is integer counting and one double-precision compare per keyframe (nRedundant > 0.9 * nMPs); the result is
+ * exact.  The spanning tree, the covisibility graph and the map / database erasure that SetBadFlag also performs are
+ * left to the caller, which calls the reference's SetBadFlag on the culled and deferred keyframes in list order.
+ *
+ * The graph need not be consistent: a slot whose point does not list the keyframe, the same point in two slots and bad
+ * points that still list observers are modelled as the reference treats them. */
+typedef struct {
+  int32_t n_kf;                   /* the keyframe table: every local keyframe and every observer of a point */
+  const uint64_t* kf_id;          /* n_kf: mnId (0 is never culled) */
+  const uint8_t* not_erase;       /* n_kf: mbNotErase */
+  const float* th_depth;          /* n_kf: mThDepth */
+  int32_t n_mp;
+  const uint8_t* mp_bad;          /* n_mp: MapPoint::mbBad on entry */
+  const int32_t* mp_nobs;         /* n_mp: MapPoint::nObs on entry (Observations(): a stereo observation counts 2) */
+  const int32_t* obs_off;         /* n_mp + 1: mObservations, CSR */
+  const int32_t* obs_kf;          /* keyframe table index, strictly ascending within a row */
+  const int32_t* obs_idx;         /* the observation's index in that keyframe (>= 0) */
+  const int32_t* obs_octave;      /* that keyframe's mvKeysUn[idx].octave */
+  const uint8_t* obs_stereo;      /* that keyframe's mvuRight[idx] >= 0 */
+  int32_t n_local;
+  const int32_t* local_kf;        /* n_local: GetVectorCovisibleKeyFrames() of the current keyframe, distinct indices */
+  const int32_t* slot_off;        /* n_local + 1: each local keyframe's mvpMapPoints, CSR */
+  const int32_t* slot_mp;         /* map-point index, -1 for NULL */
+  const int32_t* slot_octave;     /* mvKeysUn[i].octave */
+  const float* slot_depth;        /* mvDepth[i] (read only when monocular is 0) */
+  int32_t monocular;              /* LocalMapping::mbMonocular */
+} b2s_culling_problem;
+enum { B2S_CULL_SKIPPED = 0, B2S_CULL_KEPT = 1, B2S_CULL_CULLED = 2, B2S_CULL_DEFERRED = 3 };
+typedef struct {
+  uint8_t* verdict;               /* n_local: B2S_CULL_SKIPPED (mnId 0), _KEPT, _CULLED, or _DEFERRED (redundant, but
+                                     mbNotErase: SetBadFlag only sets mbToBeErased) */
+  int32_t* n_mps;                 /* n_local: nMPs (0 when skipped) */
+  int32_t* n_redundant;           /* n_local: nRedundantObservations (0 when skipped) */
+  uint8_t* mp_bad;                /* n_mp: mbBad after the call */
+  int32_t* mp_nobs;               /* n_mp: nObs after the call */
+  uint8_t* obs_alive;             /* obs_off[n_mp]: 1 while the observation is still in mObservations */
+  int32_t* slot_mp;               /* slot_off[n_local]: the local keyframes' slots after the call (-1: NULL) */
+  int32_t n_culled;               /* keyframes with verdict B2S_CULL_CULLED */
+} b2s_culling_result;
+typedef struct b2s_culling b2s_culling;
+/* Per problem: up to max_kf keyframes, max_mp map points, max_obs observations, max_local local keyframes and max_slots
+ * slots; up to max_batch problems per call.  Device memory is sized by each call's totals and kept for the next. */
+int b2s_culling_create(int max_kf, int max_mp, int max_obs, int max_local, int max_slots, int max_batch, int device,
+                       b2s_culling** out);
+void b2s_culling_destroy(b2s_culling* h);
+/* A problem beyond the handle's capacities, or batch > max_batch: B2S_ERR_CAPACITY.  A null array, batch < 1, a negative
+ * count, offsets that are not a CSR, an index out of range (an observer, a local keyframe, a slot), an observer row that
+ * is not strictly ascending, a repeated local keyframe, a negative obs_idx, or an obs_idx beyond the slot row of an
+ * observer that is a local keyframe: B2S_ERR_BAD_ARG.  Nothing is written unless every problem is valid. */
+int b2s_keyframe_culling(b2s_culling* h, int batch, const b2s_culling_problem* p, b2s_culling_result* r);
+/* Device time (CUDA events on the handle's stream: upload, kernels, download) of the last call. */
+float b2s_culling_last_ms(const b2s_culling* h);
+
 #ifdef __cplusplus
 }
 #endif

@@ -172,6 +172,19 @@ class _CovisResult(ctypes.Structure):  # b2s_covis_result
                 ("list_need", ctypes.c_int32), ("start_need", ctypes.c_int32), ("after_need", ctypes.c_int32)]
 
 
+class _CullingProblem(ctypes.Structure):  # b2s_culling_problem
+    _fields_ = [("n_kf", ctypes.c_int32), ("kf_id", _vp), ("not_erase", _vp), ("th_depth", _vp), ("n_mp", ctypes.c_int32),
+                ("mp_bad", _vp), ("mp_nobs", _vp), ("obs_off", _vp), ("obs_kf", _vp), ("obs_idx", _vp),
+                ("obs_octave", _vp), ("obs_stereo", _vp), ("n_local", ctypes.c_int32), ("local_kf", _vp),
+                ("slot_off", _vp), ("slot_mp", _vp), ("slot_octave", _vp), ("slot_depth", _vp),
+                ("monocular", ctypes.c_int32)]
+
+
+class _CullingResult(ctypes.Structure):  # b2s_culling_result
+    _fields_ = [("verdict", _vp), ("n_mps", _vp), ("n_redundant", _vp), ("mp_bad", _vp), ("mp_nobs", _vp),
+                ("obs_alive", _vp), ("slot_mp", _vp), ("n_culled", ctypes.c_int32)]
+
+
 class _GbaResult(ctypes.Structure):
     _fields_ = [("Tcw_out", _vp), ("points_out", _vp), ("point_included", _vp), ("trace", _vp),
                 ("chi2_final", ctypes.c_double), ("n_trials", ctypes.c_int)]
@@ -298,6 +311,13 @@ def lib():
             L.b2s_update_connections.argtypes = [_vp, _vp, _vp]
             L.b2s_covis_last_ms.restype = ctypes.c_float
             L.b2s_covis_last_ms.argtypes = [_vp]
+        if hasattr(L, "b2s_culling_create"):
+            L.b2s_culling_create.argtypes = [ctypes.c_int] * 7 + [_vp]
+            L.b2s_culling_destroy.argtypes = [_vp]
+            L.b2s_culling_destroy.restype = None
+            L.b2s_keyframe_culling.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+            L.b2s_culling_last_ms.restype = ctypes.c_float
+            L.b2s_culling_last_ms.argtypes = [_vp]
         _lib = L
     return _lib
 
@@ -1688,3 +1708,87 @@ class Covisibility:
         rc, o = self.raw(d)
         _check(rc)
         return covis_state(d, o)
+
+
+# ------------------------------------------------------------------------------------------------- keyframe culling
+_CULL_ARRAYS = [("kf_id", np.uint64), ("not_erase", np.uint8), ("th_depth", np.float32), ("mp_bad", np.uint8),
+                ("mp_nobs", np.int32), ("obs_off", np.int32), ("obs_kf", np.int32), ("obs_idx", np.int32),
+                ("obs_octave", np.int32), ("obs_stereo", np.uint8), ("local_kf", np.int32), ("slot_off", np.int32),
+                ("slot_mp", np.int32), ("slot_octave", np.int32), ("slot_depth", np.float32)]
+VERDICT_SKIPPED, VERDICT_KEPT, VERDICT_CULLED, VERDICT_DEFERRED = range(4)  # B2S_CULL_*
+
+
+def culling_problem(d):
+    """(b2s_culling_problem, the contiguous arrays it points into) from a problem dict with the fields of
+    b2s_culling_problem (arrays; n_kf, n_mp and n_local follow from kf_id, mp_bad and local_kf; monocular a bool)."""
+    arr = {k: np.ascontiguousarray(d[k], t) for k, t in _CULL_ARRAYS}
+    p = _CullingProblem(n_kf=len(arr["kf_id"]), n_mp=len(arr["mp_bad"]), n_local=len(arr["local_kf"]),
+                        monocular=1 if d["monocular"] else 0)
+    for k, _ in _CULL_ARRAYS:
+        setattr(p, k, arr[k].ctypes.data_as(_vp))
+    return p, arr
+
+
+def culling_outputs(d):
+    """(b2s_culling_result, its zeroed output arrays as a dict) sized for problem dict d."""
+    L, M = len(d["local_kf"]), len(d["mp_bad"])
+    o = {"verdict": np.zeros(L, np.uint8), "n_mps": np.zeros(L, np.int32), "n_redundant": np.zeros(L, np.int32),
+         "mp_bad": np.zeros(M, np.uint8), "mp_nobs": np.zeros(M, np.int32),
+         "obs_alive": np.zeros(int(np.asarray(d["obs_off"])[-1]), np.uint8),
+         "slot_mp": np.zeros(int(np.asarray(d["slot_off"])[-1]), np.int32)}
+    r = _CullingResult()
+    for k, v in o.items():
+        setattr(r, k, v.ctypes.data_as(_vp))
+    return r, o
+
+
+class KeyFrameCulling:
+    """LocalMapping::KeyFrameCulling for a batch of independent local maps (b2s_keyframe_culling), stateless: each
+    problem dict holds the keyframe table, the points with their observations and the local list with its slots (the
+    fields of b2s_culling_problem, as arrays); each result is a dict with the verdicts, the counts and the state after
+    the call (the fields of b2s_culling_result)."""
+
+    def __init__(self, max_kf=4096, max_mp=1 << 18, max_obs=1 << 21, max_local=512, max_slots=1 << 20, max_batch=256,
+                 device=0):
+        self._h = _vp()
+        _check(lib().b2s_culling_create(max_kf, max_mp, max_obs, max_local, max_slots, max_batch, device,
+                                        ctypes.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().b2s_culling_destroy(self._h)
+            self._h = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def last_ms(self):
+        """Device time of the last call (CUDA events: upload, kernels, download)."""
+        return float(lib().b2s_culling_last_ms(self._h))
+
+    def raw(self, ds):
+        """(status, [result dict per problem]) for a list of problem dicts; on an error the outputs stay zero."""
+        probs, keep, res, outs = [], [], [], []
+        for d in ds:
+            p, k = culling_problem(d)
+            r, o = culling_outputs(d)
+            probs.append(p)
+            keep.append(k)
+            res.append(r)
+            outs.append(o)
+        P = (_CullingProblem * len(ds))(*probs)
+        R = (_CullingResult * len(ds))(*res)
+        rc = lib().b2s_keyframe_culling(self._h, len(ds), P, R)
+        for o, r in zip(outs, R):
+            o["n_culled"] = r.n_culled
+        return rc, outs
+
+    def __call__(self, ds):
+        """The results of a list of problems, or of one problem dict."""
+        one = isinstance(ds, dict)
+        rc, outs = self.raw([ds] if one else ds)
+        _check(rc)
+        return outs[0] if one else outs

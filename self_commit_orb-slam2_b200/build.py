@@ -106,6 +106,9 @@ def build_oracle(force=False):
     # the covisibility update's CPU restatement (oracle/covis.mk)
     subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "covis.mk"] + (["-B"] if force else []) +
                           ["liborb_covis.so"])
+    # the keyframe culling's CPU restatement (oracle/culling.mk)
+    subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "culling.mk"] + (["-B"] if force else []) +
+                          ["liborb_culling.so"])
     return ORACLE_LIB
 
 
@@ -125,6 +128,7 @@ def build_oracle_ref():
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "sim3solver.mk", "sim3solver-ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "pnpsolver.mk", "pnpsolver-ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "covis.mk", "covis-ref", "REF=" + ref])
+    subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "culling.mk", "culling-ref", "REF=" + ref])
     return os.path.join(ORACLE_DIR, "_ref")
 
 

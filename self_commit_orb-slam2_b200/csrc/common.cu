@@ -46,6 +46,22 @@ int grow(DevBuf& b, size_t bytes) {
   b.bytes = bytes;
   return B2S_OK;
 }
+
+bool csr_ok(const int32_t* off, int rows, int64_t cap) {
+  if (!off || off[0] != 0) return false;
+  for (int i = 0; i < rows; i++)
+    if (off[i + 1] < off[i]) return false;
+  return off[rows] <= cap;
+}
+
+bool entries_ok(const int32_t* off, const int32_t* v, int rows, int lo, int hi, bool ascending) {
+  for (int r = 0; r < rows; r++)
+    for (int i = off[r]; i < off[r + 1]; i++) {
+      if (v[i] < lo || v[i] >= hi) return false;
+      if (ascending && i > off[r] && v[i] <= v[i - 1]) return false;
+    }
+  return true;
+}
 }  // namespace b2s
 
 extern "C" const char* b2s_last_error(void) { return b2s::g_last_error.c_str(); }

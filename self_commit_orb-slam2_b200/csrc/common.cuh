@@ -34,6 +34,11 @@ struct DevBuf {
 };
 int grow(DevBuf& b, size_t bytes);
 
+// Host-side checks of caller CSRs: off[0] == 0, non-decreasing, off[rows] <= cap.
+bool csr_ok(const int32_t* off, int rows, int64_t cap);
+// Every entry of the rows of a valid CSR in [lo, hi); each row strictly ascending when `ascending`.
+bool entries_ok(const int32_t* off, const int32_t* v, int rows, int lo, int hi, bool ascending);
+
 static inline int div_up(int a, int b) { return (a + b - 1) / b; }
 static inline size_t align_up(size_t a, size_t b) { return (a + b - 1) / b * b; }
 

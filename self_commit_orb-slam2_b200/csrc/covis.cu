@@ -312,23 +312,6 @@ __global__ void __launch_bounds__(kReplayWarps * 32) k_covis_replay(Args a) {
   }
 }
 
-bool csr_ok(const int32_t* off, int rows, int64_t cap) {
-  if (!off || off[0] != 0) return false;
-  for (int i = 0; i < rows; i++)
-    if (off[i + 1] < off[i]) return false;
-  return off[rows] <= cap;
-}
-
-// every entry in [0, hi); rows strictly ascending when `ascending`
-bool entries_ok(const int32_t* off, const int32_t* v, int rows, int lo, int hi, bool ascending) {
-  for (int r = 0; r < rows; r++)
-    for (int i = off[r]; i < off[r + 1]; i++) {
-      if (v[i] < lo || v[i] >= hi) return false;
-      if (ascending && i > off[r] && v[i] <= v[i - 1]) return false;
-    }
-  return true;
-}
-
 }  // namespace
 
 struct b2s_covis {
