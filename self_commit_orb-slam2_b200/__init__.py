@@ -217,107 +217,128 @@ def lib():
         L.b2s_extractor_get_timing.argtypes = [_vp, _vp, _vp]
         L.b2s_extractor_debug_level.argtypes = [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]
         L.b2s_extractor_debug_candidates.argtypes = [_vp, ctypes.c_int, ctypes.c_int, _vp, _vp, ctypes.c_int, _vp]
-        if hasattr(L, "b2s_matcher_create"):
-            L.b2s_matcher_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
-            L.b2s_matcher_destroy.argtypes = [_vp]
-            L.b2s_matcher_destroy.restype = None
-            L.b2s_matcher_launch_count.restype = ctypes.c_longlong
-            L.b2s_matcher_launch_count.argtypes = [_vp]
-            L.b2s_descriptor_distance.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp]
-            L.b2s_search_by_bow.argtypes = [_vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, ctypes.c_int,
-                                            ctypes.c_int, ctypes.c_float, ctypes.c_int, ctypes.c_int, _vp, _vp]
-            L.b2s_search_by_bow_batch.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp,
-                                                  _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_int,
-                                                  ctypes.c_int, _vp, _vp]
-            L.b2s_search_by_bow_device.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp,
-                                                   _vp, _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_float,
-                                                   ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]
-            L.b2s_search_by_projection_last.argtypes = [_vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+        L.b2s_matcher_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+        L.b2s_matcher_destroy.argtypes = [_vp]
+        L.b2s_matcher_destroy.restype = None
+        L.b2s_matcher_launch_count.restype = ctypes.c_longlong
+        L.b2s_matcher_launch_count.argtypes = [_vp]
+        L.b2s_descriptor_distance.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp]
+        L.b2s_search_by_bow.argtypes = [_vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, ctypes.c_int,
+                                        ctypes.c_int, ctypes.c_float, ctypes.c_int, ctypes.c_int, _vp, _vp]
+        L.b2s_search_by_bow_batch.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp,
+                                              _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_int,
+                                              ctypes.c_int, _vp, _vp]
+        L.b2s_search_by_bow_device.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp,
+                                               _vp, _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_float,
+                                               ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]
+        L.b2s_search_by_projection_last.argtypes = [_vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                                    ctypes.c_int, _vp, ctypes.c_float, ctypes.c_int, ctypes.c_int,
+                                                    ctypes.c_int, _vp, _vp]
+        L.b2s_search_by_projection_last_device.argtypes = [_vp, ctypes.c_int, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp,
+                                                           ctypes.c_int, _vp, ctypes.c_float, ctypes.c_int,
+                                                           ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]
+        L.b2s_search_by_projection_last_batch.argtypes = [_vp, ctypes.c_int, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp,
+                                                          ctypes.c_int, _vp, ctypes.c_float, ctypes.c_int,
+                                                          ctypes.c_int, ctypes.c_int, _vp, _vp]
+        L.b2s_search_by_projection_sequence.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp,
+                                                        ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                                         ctypes.c_int, _vp, ctypes.c_float, ctypes.c_int, ctypes.c_int,
                                                         ctypes.c_int, _vp, _vp]
-            L.b2s_search_by_projection_last_device.argtypes = [_vp, ctypes.c_int, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp,
-                                                               ctypes.c_int, _vp, ctypes.c_float, ctypes.c_int,
-                                                               ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]
-            L.b2s_search_by_projection_last_batch.argtypes = [_vp, ctypes.c_int, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp,
-                                                              ctypes.c_int, _vp, ctypes.c_float, ctypes.c_int,
-                                                              ctypes.c_int, ctypes.c_int, _vp, _vp]
-            L.b2s_search_by_projection_sequence.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp,
-                                                            ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float,
-                                                            ctypes.c_int, _vp, ctypes.c_float, ctypes.c_int, ctypes.c_int,
-                                                            ctypes.c_int, _vp, _vp]
-            L.b2s_track_queries_device.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_float,
-                                                   ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_int, _vp, _vp,
-                                                   _vp]
-            L.b2s_search_by_projection_map.argtypes = [_vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int,
-                                                       _vp, ctypes.c_float, ctypes.c_int, ctypes.c_float, _vp, _vp]
-        if hasattr(L, "b2s_ba_create"):
-            L.b2s_ba_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
-            L.b2s_ba_destroy.argtypes = [_vp]
-            L.b2s_ba_destroy.restype = None
-            L.b2s_ba_launch_count.restype = ctypes.c_longlong
-            L.b2s_ba_launch_count.argtypes = [_vp]
-            L.b2s_ba_last_kernel_ms.restype = ctypes.c_float
-            L.b2s_ba_last_kernel_ms.argtypes = [_vp, _vp]
-            L.b2s_local_ba.argtypes = [_vp, _vp, _vp, _vp]
-            L.b2s_ba_set_sm_budget.argtypes = [_vp, ctypes.c_int]
-            L.b2s_local_ba_batch.argtypes = [_vp, ctypes.c_int, _vp, _vp]
-            L.b2s_pose_optimization_batch.argtypes = [_vp, ctypes.c_int, _vp, _vp]
-        if hasattr(L, "b2s_gba_create"):
-            L.b2s_gba_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
-            L.b2s_gba_destroy.argtypes = [_vp]
-            L.b2s_gba_destroy.restype = None
-            L.b2s_global_ba.argtypes = [_vp, _vp, _vp, _vp]
-            L.b2s_gba_last_ms.restype = ctypes.c_float
-            L.b2s_gba_last_ms.argtypes = [_vp, _vp]
-        if hasattr(L, "b2s_eg_create"):
-            L.b2s_eg_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
-            L.b2s_eg_destroy.argtypes = [_vp]
-            L.b2s_eg_destroy.restype = None
-            L.b2s_optimize_essential_graph.argtypes = [_vp, _vp, _vp]
-            L.b2s_eg_last_ms.restype = ctypes.c_float
-            L.b2s_eg_last_ms.argtypes = [_vp, _vp]
-        if hasattr(L, "b2s_sim3opt_create"):
-            L.b2s_sim3opt_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
-            L.b2s_sim3opt_destroy.argtypes = [_vp]
-            L.b2s_sim3opt_destroy.restype = None
-            L.b2s_optimize_sim3.argtypes = [_vp, ctypes.c_int, _vp, _vp]
-            L.b2s_sim3opt_last_ms.restype = ctypes.c_float
-            L.b2s_sim3opt_last_ms.argtypes = [_vp, _vp]
-        if hasattr(L, "b2s_init_create"):
-            L.b2s_init_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
-            L.b2s_init_destroy.argtypes = [_vp]
-            L.b2s_init_destroy.restype = None
-            L.b2s_initialize.argtypes = [_vp, ctypes.c_int, _vp, _vp]
-            L.b2s_init_last_ms.restype = ctypes.c_float
-            L.b2s_init_last_ms.argtypes = [_vp]
-        if hasattr(L, "b2s_sim3solver_create"):
-            L.b2s_sim3solver_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
-            L.b2s_sim3solver_destroy.argtypes = [_vp]
-            L.b2s_sim3solver_destroy.restype = None
-            L.b2s_sim3solver_iterate.argtypes = [_vp, ctypes.c_int, _vp, _vp]
-            L.b2s_sim3solver_last_ms.restype = ctypes.c_float
-            L.b2s_sim3solver_last_ms.argtypes = [_vp]
-        if hasattr(L, "b2s_pnpsolver_create"):
-            L.b2s_pnpsolver_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
-            L.b2s_pnpsolver_destroy.argtypes = [_vp]
-            L.b2s_pnpsolver_destroy.restype = None
-            L.b2s_pnpsolver_iterate.argtypes = [_vp, ctypes.c_int, _vp, _vp]
-            L.b2s_pnpsolver_last_ms.restype = ctypes.c_float
-            L.b2s_pnpsolver_last_ms.argtypes = [_vp]
-        if hasattr(L, "b2s_covis_create"):
-            L.b2s_covis_create.argtypes = [ctypes.c_int] * 7 + [_vp]
-            L.b2s_covis_destroy.argtypes = [_vp]
-            L.b2s_covis_destroy.restype = None
-            L.b2s_update_connections.argtypes = [_vp, _vp, _vp]
-            L.b2s_covis_last_ms.restype = ctypes.c_float
-            L.b2s_covis_last_ms.argtypes = [_vp]
-        if hasattr(L, "b2s_culling_create"):
-            L.b2s_culling_create.argtypes = [ctypes.c_int] * 7 + [_vp]
-            L.b2s_culling_destroy.argtypes = [_vp]
-            L.b2s_culling_destroy.restype = None
-            L.b2s_keyframe_culling.argtypes = [_vp, ctypes.c_int, _vp, _vp]
-            L.b2s_culling_last_ms.restype = ctypes.c_float
-            L.b2s_culling_last_ms.argtypes = [_vp]
+        L.b2s_track_queries_device.argtypes = [_vp, ctypes.c_int, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_float,
+                                               ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_int, _vp, _vp,
+                                               _vp]
+        L.b2s_search_by_projection_map.argtypes = [_vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int,
+                                                   _vp, ctypes.c_float, ctypes.c_int, ctypes.c_float, _vp, _vp]
+        L.b2s_ba_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+        L.b2s_ba_destroy.argtypes = [_vp]
+        L.b2s_ba_destroy.restype = None
+        L.b2s_ba_launch_count.restype = ctypes.c_longlong
+        L.b2s_ba_launch_count.argtypes = [_vp]
+        L.b2s_ba_last_kernel_ms.restype = ctypes.c_float
+        L.b2s_ba_last_kernel_ms.argtypes = [_vp, _vp]
+        L.b2s_local_ba.argtypes = [_vp, _vp, _vp, _vp]
+        L.b2s_ba_set_sm_budget.argtypes = [_vp, ctypes.c_int]
+        L.b2s_local_ba_batch.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+        L.b2s_pose_optimization_batch.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+        L.b2s_gba_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+        L.b2s_gba_destroy.argtypes = [_vp]
+        L.b2s_gba_destroy.restype = None
+        L.b2s_global_ba.argtypes = [_vp, _vp, _vp, _vp]
+        L.b2s_gba_last_ms.restype = ctypes.c_float
+        L.b2s_gba_last_ms.argtypes = [_vp, _vp]
+        L.b2s_eg_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+        L.b2s_eg_destroy.argtypes = [_vp]
+        L.b2s_eg_destroy.restype = None
+        L.b2s_optimize_essential_graph.argtypes = [_vp, _vp, _vp]
+        L.b2s_eg_last_ms.restype = ctypes.c_float
+        L.b2s_eg_last_ms.argtypes = [_vp, _vp]
+        L.b2s_sim3opt_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+        L.b2s_sim3opt_destroy.argtypes = [_vp]
+        L.b2s_sim3opt_destroy.restype = None
+        L.b2s_optimize_sim3.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+        L.b2s_sim3opt_last_ms.restype = ctypes.c_float
+        L.b2s_sim3opt_last_ms.argtypes = [_vp, _vp]
+        L.b2s_init_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+        L.b2s_init_destroy.argtypes = [_vp]
+        L.b2s_init_destroy.restype = None
+        L.b2s_initialize.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+        L.b2s_init_last_ms.restype = ctypes.c_float
+        L.b2s_init_last_ms.argtypes = [_vp]
+        L.b2s_sim3solver_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+        L.b2s_sim3solver_destroy.argtypes = [_vp]
+        L.b2s_sim3solver_destroy.restype = None
+        L.b2s_sim3solver_iterate.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+        L.b2s_sim3solver_last_ms.restype = ctypes.c_float
+        L.b2s_sim3solver_last_ms.argtypes = [_vp]
+        L.b2s_pnpsolver_create.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp]
+        L.b2s_pnpsolver_destroy.argtypes = [_vp]
+        L.b2s_pnpsolver_destroy.restype = None
+        L.b2s_pnpsolver_iterate.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+        L.b2s_pnpsolver_last_ms.restype = ctypes.c_float
+        L.b2s_pnpsolver_last_ms.argtypes = [_vp]
+        L.b2s_covis_create.argtypes = [ctypes.c_int] * 7 + [_vp]
+        L.b2s_covis_destroy.argtypes = [_vp]
+        L.b2s_covis_destroy.restype = None
+        L.b2s_update_connections.argtypes = [_vp, _vp, _vp]
+        L.b2s_covis_last_ms.restype = ctypes.c_float
+        L.b2s_covis_last_ms.argtypes = [_vp]
+        L.b2s_culling_create.argtypes = [ctypes.c_int] * 7 + [_vp]
+        L.b2s_culling_destroy.argtypes = [_vp]
+        L.b2s_culling_destroy.restype = None
+        L.b2s_keyframe_culling.argtypes = [_vp, ctypes.c_int, _vp, _vp]
+        L.b2s_culling_last_ms.restype = ctypes.c_float
+        L.b2s_culling_last_ms.argtypes = [_vp]
+        L.b2s_frame_grid_create.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp]
+        L.b2s_frame_grid_create_device.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp]
+        L.b2s_frame_grid_destroy.argtypes = [_vp]
+        L.b2s_frame_grid_destroy.restype = None
+        L.b2s_frame_grid_size.argtypes = [_vp]
+        L.b2s_frame_grid_features_in_area.argtypes = [_vp, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_int,
+                                                      ctypes.c_int, _vp, ctypes.c_int, _vp]
+        L.b2s_search_by_projection_last_grid.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_float, ctypes.c_int,
+                                                         ctypes.c_int, ctypes.c_int, _vp, _vp]
+        L.b2s_search_by_projection_map_grid.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_float, ctypes.c_int,
+                                                        ctypes.c_float, _vp, _vp]
+        L.b2s_search_windows_grid.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]
+        L.b2s_vocabulary_create.argtypes = [_vp, ctypes.c_int, _vp]
+        L.b2s_vocabulary_destroy.argtypes = [_vp]
+        L.b2s_vocabulary_destroy.restype = None
+        L.b2s_bow_transform.argtypes = [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]
+        L.b2s_bow_transform_device.argtypes = [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp]
+        L.b2s_kfdb_create.argtypes = [ctypes.c_int, ctypes.c_int, _vp]
+        L.b2s_kfdb_destroy.argtypes = [_vp]
+        L.b2s_kfdb_destroy.restype = None
+        L.b2s_kfdb_add.argtypes = [_vp, ctypes.c_uint64, _vp, _vp, ctypes.c_int]
+        L.b2s_kfdb_erase.argtypes = [_vp, ctypes.c_uint64]
+        L.b2s_kfdb_clear.argtypes = [_vp]
+        L.b2s_kfdb_size.argtypes = [_vp, _vp]
+        L.b2s_kfdb_detect_loop_candidates.argtypes = [_vp, ctypes.c_uint64, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int,
+                                                      ctypes.c_float, _vp, _vp, ctypes.c_int, _vp]
+        L.b2s_kfdb_detect_relocalization_candidates.argtypes = [_vp, ctypes.c_uint64, _vp, _vp, ctypes.c_int, _vp, _vp,
+                                                                ctypes.c_int, _vp]
+        L.b2s_kfdb_keyframe_state.argtypes = [_vp, ctypes.c_uint64, _vp]
+        L.b2s_kfdb_last_query_ms.argtypes = [_vp]
+        L.b2s_kfdb_last_query_ms.restype = ctypes.c_float
         _lib = L
     return _lib
 
@@ -335,8 +356,28 @@ def device_count():
     return lib().b2s_device_count()
 
 
-class ORBextractor:
+class _Handle:
+    """Owns one C handle, `_h`, and destroys it with the entry point named by `_destroy` on close() or collection.  An
+    object whose `_own` is false borrows `_h` (from a *Batch handle) and never destroys it."""
+    _destroy = None
+    _h = None
+    _own = True
+
+    def close(self):
+        if self._own and self._h:
+            getattr(lib(), self._destroy)(self._h)
+        self._h = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class ORBextractor(_Handle):
     """Mirror of ORB_SLAM2::ORBextractor (include/ORBextractor.h:92-161)."""
+    _destroy = "b2s_extractor_destroy"
 
     def __init__(self, nfeatures, scaleFactor, nlevels, iniThFAST, minThFAST, max_width=1280, max_height=1024,
                  max_batch=1, device=0):
@@ -352,17 +393,6 @@ class ORBextractor:
         self.mvScaleFactor, self.mvInvScaleFactor, self.mvLevelSigma2, self.mvInvLevelSigma2 = s
         self.mnFeaturesPerLevel = nf
         self.mvImagePyramid = []
-
-    def close(self):
-        if self._h:
-            lib().b2s_extractor_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     # getters of include/ORBextractor.h:118-161
     def GetLevels(self):
@@ -465,8 +495,9 @@ class ORBextractor:
         return xy[:n.value].copy(), resp[:n.value].copy()
 
 
-class ORBmatcher:
+class ORBmatcher(_Handle):
     """Mirror of ORB_SLAM2::ORBmatcher (include/ORBmatcher.h:57-215) on flattened arrays."""
+    _destroy = "b2s_matcher_destroy"
     TH_HIGH, TH_LOW, HISTO_LENGTH = TH_HIGH, TH_LOW, HISTO_LENGTH
 
     def __init__(self, nnratio=0.6, checkOri=True, max_features=4096, max_batch=1, device=0):
@@ -474,17 +505,6 @@ class ORBmatcher:
         self.mbCheckOrientation = bool(checkOri)
         self._h = _vp()
         _check(lib().b2s_matcher_create(max_features, max_batch, device, ctypes.byref(self._h)))
-
-    def close(self):
-        if self._h:
-            lib().b2s_matcher_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def launch_count(self):
         return lib().b2s_matcher_launch_count(self._h)
@@ -684,27 +704,16 @@ class _VocDesc(ctypes.Structure):
                 ("leaf_flag", ctypes.c_void_p), ("desc", ctypes.c_void_p), ("weight", ctypes.c_void_p)]
 
 
-class FrameGrid:
+class FrameGrid(_Handle):
     """Frame::AssignFeaturesToGrid / GetFeaturesInArea (src/Frame.cc:461-491, 741-852) kept on the device: build once per
     frame, then run several projection matchers that upload only their queries (SURVEY §8f rank 4)."""
+    _destroy = "b2s_frame_grid_destroy"
 
     def __init__(self, matcher, kpx=None, kpy=None, octave=None, angle=None, uright=None, desc=None, geom=None,
                  inv_level_sigma2=None, d_kps_ptr=None, d_desc_ptr=None, d_uright_ptr=None, nf=None, stream=0):
         self.matcher = matcher
         self._h = _vp()
         L = lib()
-        L.b2s_frame_grid_create.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp]
-        L.b2s_frame_grid_create_device.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp]
-        L.b2s_frame_grid_destroy.argtypes = [_vp]
-        L.b2s_frame_grid_destroy.restype = None
-        L.b2s_frame_grid_size.argtypes = [_vp]
-        L.b2s_frame_grid_features_in_area.argtypes = [_vp, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_int,
-                                                      ctypes.c_int, _vp, ctypes.c_int, _vp]
-        L.b2s_search_by_projection_last_grid.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_float, ctypes.c_int,
-                                                         ctypes.c_int, ctypes.c_int, _vp, _vp]
-        L.b2s_search_by_projection_map_grid.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_float, ctypes.c_int,
-                                                        ctypes.c_float, _vp, _vp]
-        L.b2s_search_windows_grid.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]
         g, sf = ORBmatcher.frame_geom(geom)
         is2 = None if inv_level_sigma2 is None else np.ascontiguousarray(inv_level_sigma2, np.float32)
         if d_kps_ptr is not None:
@@ -718,17 +727,6 @@ class FrameGrid:
             _check(L.b2s_frame_grid_create(matcher._h, _p(a[0]), _p(a[1]), _p(a[2]), _p(a[3]), _p(a[4]), _p(a[5]), len(a[0]),
                                            ctypes.byref(g), _p(is2), ctypes.byref(self._h)))
         self.n = lib().b2s_frame_grid_size(self._h)
-
-    def close(self):
-        if self._h:
-            lib().b2s_frame_grid_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def GetFeaturesInArea(self, x, y, r, minLevel=-1, maxLevel=-1):
         out = np.zeros(max(self.n, 1), np.int32)
@@ -767,32 +765,16 @@ class FrameGrid:
         return na.value, best, bd
 
 
-class ORBVocabulary:
+class ORBVocabulary(_Handle):
     """Mirror of ORBVocabulary::transform (DBoW2 TemplatedVocabulary.h:1127-1256) on a flattened vocabulary."""
+    _destroy = "b2s_vocabulary_destroy"
 
     def __init__(self, k, L, parent, leaf_flag, desc, weight, device=0):
         self._h = _vp()
         self._keep = [np.ascontiguousarray(parent, np.int32), np.ascontiguousarray(leaf_flag, np.uint8),
                       np.ascontiguousarray(desc, np.uint8), np.ascontiguousarray(weight, np.float64)]
         d = _VocDesc(k, L, len(self._keep[0]), *[a.ctypes.data for a in self._keep])
-        L_ = lib()
-        L_.b2s_vocabulary_create.argtypes = [_vp, ctypes.c_int, _vp]
-        L_.b2s_vocabulary_destroy.argtypes = [_vp]
-        L_.b2s_vocabulary_destroy.restype = None
-        L_.b2s_bow_transform.argtypes = [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]
-        L_.b2s_bow_transform_device.argtypes = [_vp, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp]
-        _check(L_.b2s_vocabulary_create(ctypes.byref(d), device, ctypes.byref(self._h)))
-
-    def close(self):
-        if self._h:
-            lib().b2s_vocabulary_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        _check(lib().b2s_vocabulary_create(ctypes.byref(d), device, ctypes.byref(self._h)))
 
     def transform_features(self, features, levelsup=4):
         """Per feature (word_id, weight, node_id)."""
@@ -831,42 +813,17 @@ class _KfdbCovis(ctypes.Structure):
     _fields_ = [("ids", _vp), ("n", _vp), ("n_rows", ctypes.c_int32)]
 
 
-class KeyFrameDatabase:
+class KeyFrameDatabase(_Handle):
     """Mirror of ORB_SLAM2::KeyFrameDatabase (include/KeyFrameDatabase.h) on the device (b2s_kfdb_*).
 
     A BowVector is (words, values): ascending uint32 word ids and their float64 values.  `covis` is the
     GetBestCovisibilityKeyFrames(10) table at query time, (ids [n_rows, 10] uint64, n [n_rows] int32) indexed by keyframe
     id, or None.  The Detect* methods return the candidate keyframe ids in the reference's order."""
+    _destroy = "b2s_kfdb_destroy"
 
     def __init__(self, n_words, device=0):
         self._h = _vp()
-        L = lib()
-        L.b2s_kfdb_create.argtypes = [ctypes.c_int, ctypes.c_int, _vp]
-        L.b2s_kfdb_destroy.argtypes = [_vp]
-        L.b2s_kfdb_destroy.restype = None
-        L.b2s_kfdb_add.argtypes = [_vp, ctypes.c_uint64, _vp, _vp, ctypes.c_int]
-        L.b2s_kfdb_erase.argtypes = [_vp, ctypes.c_uint64]
-        L.b2s_kfdb_clear.argtypes = [_vp]
-        L.b2s_kfdb_size.argtypes = [_vp, _vp]
-        L.b2s_kfdb_detect_loop_candidates.argtypes = [_vp, ctypes.c_uint64, _vp, _vp, ctypes.c_int, _vp, ctypes.c_int,
-                                                      ctypes.c_float, _vp, _vp, ctypes.c_int, _vp]
-        L.b2s_kfdb_detect_relocalization_candidates.argtypes = [_vp, ctypes.c_uint64, _vp, _vp, ctypes.c_int, _vp, _vp,
-                                                                ctypes.c_int, _vp]
-        L.b2s_kfdb_keyframe_state.argtypes = [_vp, ctypes.c_uint64, _vp]
-        L.b2s_kfdb_last_query_ms.argtypes = [_vp]
-        L.b2s_kfdb_last_query_ms.restype = ctypes.c_float
-        _check(L.b2s_kfdb_create(int(n_words), device, ctypes.byref(self._h)))
-
-    def close(self):
-        if self._h:
-            lib().b2s_kfdb_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        _check(lib().b2s_kfdb_create(int(n_words), device, ctypes.byref(self._h)))
 
     @staticmethod
     def _bow(words, values):
@@ -926,23 +883,13 @@ class KeyFrameDatabase:
         return float(lib().b2s_kfdb_last_query_ms(self._h))
 
 
-class Optimizer:
+class Optimizer(_Handle):
     """Mirror of ORB_SLAM2::Optimizer::LocalBundleAdjustment (include/Optimizer.h:112) on a flattened window."""
+    _destroy = "b2s_ba_destroy"
 
     def __init__(self, max_kf=64, max_mp=8192, max_edges=65536, max_batch=1, device=0):
         self._h = _vp()
         _check(lib().b2s_ba_create(max_kf, max_mp, max_edges, max_batch, device, ctypes.byref(self._h)))
-
-    def close(self):
-        if self._h:
-            lib().b2s_ba_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def launch_count(self):
         return lib().b2s_ba_launch_count(self._h)
@@ -1059,25 +1006,15 @@ class Optimizer:
         return self.run_prepared_ba(self.prepare_ba_batch(ds, its1, its2))
 
 
-class GlobalOptimizer:
+class GlobalOptimizer(_Handle):
     """Mirror of ORB_SLAM2::Optimizer::BundleAdjustment (include/Optimizer.h, src/Optimizer.cc:86-341), the body of
     GlobalBundleAdjustemnt, on a flattened map (b2s_global_ba).  The handle's capacities bound the problem sizes; the
     reduced-system storage grows with the maps it is given."""
+    _destroy = "b2s_gba_destroy"
 
     def __init__(self, max_kf=2048, max_mp=262144, max_edges=1 << 21, device=0):
         self._h = _vp()
         _check(lib().b2s_gba_create(max_kf, max_mp, max_edges, device, ctypes.byref(self._h)))
-
-    def close(self):
-        if self._h:
-            lib().b2s_gba_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def last_ms(self):
         """(ms, trials): device time of the last call (its stream segments between the host's LM decisions, CUDA
@@ -1110,25 +1047,15 @@ class GlobalOptimizer:
         return out
 
 
-class EssentialGraphOptimizer:
+class EssentialGraphOptimizer(_Handle):
     """Mirror of ORB_SLAM2::Optimizer::OptimizeEssentialGraph (src/Optimizer.cc:1017-1339) on a flattened pose graph
     (b2s_optimize_essential_graph).  The handle's capacities bound the problem sizes; the factorisation's tile storage
     grows with the graphs it is given."""
+    _destroy = "b2s_eg_destroy"
 
     def __init__(self, max_kf=4096, max_edges=1 << 17, max_mp=1 << 22, device=0):
         self._h = _vp()
         _check(lib().b2s_eg_create(max_kf, max_edges, max_mp, device, ctypes.byref(self._h)))
-
-    def close(self):
-        if self._h:
-            lib().b2s_eg_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def last_ms(self):
         """(ms, trials): device time of the last call (CUDA events) and the LM trials it ran."""
@@ -1158,24 +1085,14 @@ class EssentialGraphOptimizer:
         return out
 
 
-class Sim3Optimizer:
+class Sim3Optimizer(_Handle):
     """Mirror of ORB_SLAM2::Optimizer::OptimizeSim3 (src/Optimizer.cc:1364-1590) on flattened correspondences
     (b2s_optimize_sim3).  A batch of independent problems runs in one launch."""
+    _destroy = "b2s_sim3opt_destroy"
 
     def __init__(self, max_matches=4096, max_batch=64, device=0):
         self._h = _vp()
         _check(lib().b2s_sim3opt_create(max_matches, max_batch, device, ctypes.byref(self._h)))
-
-    def close(self):
-        if self._h:
-            lib().b2s_sim3opt_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def last_ms(self):
         """(ms, trials): device time of the last call (CUDA events) and the LM trials of all its problems."""
@@ -1223,25 +1140,15 @@ class Sim3Optimizer:
         return outs
 
 
-class MonoInitializer:
+class MonoInitializer(_Handle):
     """Mirror of ORB_SLAM2::Initializer::Initialize (src/Initializer.cc:68-231) with the minimal sets given
     (b2s_initialize): H and F RANSAC over the sets, the model choice and the two-view reconstruction.  A batch of
     independent problems runs in one call."""
+    _destroy = "b2s_init_destroy"
 
     def __init__(self, max_keys=4096, max_iterations=300, max_batch=64, device=0):
         self._h = _vp()
         _check(lib().b2s_init_create(max_keys, max_iterations, max_batch, device, ctypes.byref(self._h)))
-
-    def close(self):
-        if self._h:
-            lib().b2s_init_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def last_ms(self):
         """Device time of the last call (CUDA events: upload, kernels, download)."""
@@ -1343,12 +1250,13 @@ def pnp_ransac_parameters(n, probability=0.99, min_inliers=8, max_iterations=300
     return m, max(1, min(it, int(max_iterations)))
 
 
-class Sim3Solver:
+class Sim3Solver(_Handle):
     """Mirror of ORB_SLAM2::Sim3Solver (src/Sim3Solver.cc) for one loop candidate, with the minimal sets drawn by the
     caller (b2s_sim3solver_iterate).  The constructor takes what the reference's constructor keeps: X1c / X2c (n x 3,
     mvX3Dc1 / mvX3Dc2), sigma2_1 / sigma2_2 (n, mvLevelSigma2 of each keypoint's octave), K1 / K2 (fx, fy, cx, cy) and
     fix_scale; the object keeps mnIterations, mnBestInliers and the best model across calls as the reference does.
     `iterate` and `find` run on the device; `iterate_batch` runs the calls of many solvers in one launch sequence."""
+    _destroy = "b2s_sim3solver_destroy"
 
     def __init__(self, X1c, X2c, sigma2_1, sigma2_2, K1, K2, fix_scale=True, max_matches=None, max_sets=300,
                  device=0, _handle=None):
@@ -1369,17 +1277,6 @@ class Sim3Solver:
         if self._own:
             _check(lib().b2s_sim3solver_create(max(3, max_matches or self.N), max_sets, 1, device,
                                                ctypes.byref(self._h)))
-
-    def close(self):
-        if self._own and self._h:
-            lib().b2s_sim3solver_destroy(self._h)
-        self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def last_ms(self):
         """Device time of the last call (CUDA events: upload, kernels, download)."""
@@ -1454,24 +1351,14 @@ class Sim3Solver:
         return self.s
 
 
-class Sim3SolverBatch:
+class Sim3SolverBatch(_Handle):
     """A device handle sized for batched Sim3Solver.iterate_batch calls (max_matches per solver, max_sets per call,
     max_batch solvers)."""
+    _destroy = "b2s_sim3solver_destroy"
 
     def __init__(self, max_matches=4096, max_sets=300, max_batch=64, device=0):
         self._h = _vp()
         _check(lib().b2s_sim3solver_create(max_matches, max_sets, max_batch, device, ctypes.byref(self._h)))
-
-    def close(self):
-        if self._h:
-            lib().b2s_sim3solver_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def last_ms(self):
         return float(lib().b2s_sim3solver_last_ms(self._h))
@@ -1481,12 +1368,13 @@ class Sim3SolverBatch:
         return Sim3Solver(*args, _handle=self, **kw)
 
 
-class PnPsolver:
+class PnPsolver(_Handle):
     """Mirror of ORB_SLAM2::PnPsolver (src/PnPsolver.cc) for one relocalisation candidate, with the minimal sets drawn by
     the caller (b2s_pnpsolver_iterate).  The constructor takes what the reference's constructor keeps: P3Dw (n x 3,
     mvP3Dw), P2D (n x 2, mvP2D), sigma2 (n, mvLevelSigma2 of each keypoint's octave) and K (fx, fy, cx, cy); the object
     keeps mnIterations, mnBestInliers, mBestTcw and mvbBestInliers across calls as the reference does.  `iterate` and
     `find` run on the device; `iterate_batch` runs the calls of many solvers in one launch sequence."""
+    _destroy = "b2s_pnpsolver_destroy"
 
     def __init__(self, P3Dw, P2D, sigma2, K, max_matches=None, max_sets=300, device=0, _handle=None):
         self.P3Dw = np.ascontiguousarray(P3Dw, np.float32).reshape(-1, 3)
@@ -1503,17 +1391,6 @@ class PnPsolver:
         self._h = _handle._h if _handle is not None else _vp()
         if self._own:
             _check(lib().b2s_pnpsolver_create(max(4, max_matches or self.N), max_sets, 1, device, ctypes.byref(self._h)))
-
-    def close(self):
-        if self._own and self._h:
-            lib().b2s_pnpsolver_destroy(self._h)
-        self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def last_ms(self):
         """Device time of the last call (CUDA events: upload, kernels, download)."""
@@ -1581,24 +1458,14 @@ class PnPsolver:
         return ret
 
 
-class PnPsolverBatch:
+class PnPsolverBatch(_Handle):
     """A device handle sized for batched PnPsolver.iterate_batch calls (max_matches per solver, max_sets per call,
     max_batch solvers)."""
+    _destroy = "b2s_pnpsolver_destroy"
 
     def __init__(self, max_matches=4096, max_sets=300, max_batch=64, device=0):
         self._h = _vp()
         _check(lib().b2s_pnpsolver_create(max_matches, max_sets, max_batch, device, ctypes.byref(self._h)))
-
-    def close(self):
-        if self._h:
-            lib().b2s_pnpsolver_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def last_ms(self):
         return float(lib().b2s_pnpsolver_last_ms(self._h))
@@ -1672,10 +1539,11 @@ def covis_state(d, o):
     return out
 
 
-class Covisibility:
+class Covisibility(_Handle):
     """KeyFrame::UpdateConnections for a batch of keyframes (b2s_update_connections), stateless: the problem dict
     holds the keyframe table with its connection state on entry, the map points the members see and the batch (the
     fields of b2s_covis_problem, as arrays); the result is a dict with the state after the batch (covis_state)."""
+    _destroy = "b2s_covis_destroy"
 
     def __init__(self, max_kf=8192, max_mp=1 << 17, max_obs=1 << 20, max_slots=1 << 17, max_conn=1 << 20,
                  max_batch=256, device=0):
@@ -1683,17 +1551,6 @@ class Covisibility:
         self._h = _vp()
         _check(lib().b2s_covis_create(max_kf, max_mp, max_obs, max_slots, max_conn, max_batch, device,
                                       ctypes.byref(self._h)))
-
-    def close(self):
-        if self._h:
-            lib().b2s_covis_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def last_ms(self):
         """Device time of the last call (CUDA events: upload, kernels, download)."""
@@ -1742,28 +1599,18 @@ def culling_outputs(d):
     return r, o
 
 
-class KeyFrameCulling:
+class KeyFrameCulling(_Handle):
     """LocalMapping::KeyFrameCulling for a batch of independent local maps (b2s_keyframe_culling), stateless: each
     problem dict holds the keyframe table, the points with their observations and the local list with its slots (the
     fields of b2s_culling_problem, as arrays); each result is a dict with the verdicts, the counts and the state after
     the call (the fields of b2s_culling_result)."""
+    _destroy = "b2s_culling_destroy"
 
     def __init__(self, max_kf=4096, max_mp=1 << 18, max_obs=1 << 21, max_local=512, max_slots=1 << 20, max_batch=256,
                  device=0):
         self._h = _vp()
         _check(lib().b2s_culling_create(max_kf, max_mp, max_obs, max_local, max_slots, max_batch, device,
                                         ctypes.byref(self._h)))
-
-    def close(self):
-        if self._h:
-            lib().b2s_culling_destroy(self._h)
-            self._h = _vp()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def last_ms(self):
         """Device time of the last call (CUDA events: upload, kernels, download)."""

@@ -1,4 +1,4 @@
-// common.cu — error text, device selection, version for libb200slam.so
+// common.cu — error text, device selection, buffers and stage handles, input checks, version for libb200slam.so
 #include <stdarg.h>
 
 #include "common.cuh"
@@ -47,6 +47,55 @@ int grow(DevBuf& b, size_t bytes) {
   return B2S_OK;
 }
 
+int grow(HostBuf& b, size_t bytes) {
+  if (bytes == 0) bytes = 16;
+  if (b.bytes >= bytes) return B2S_OK;
+  if (b.p) cudaFreeHost(b.p);
+  b.p = nullptr;
+  b.bytes = 0;
+  B2S_CUDA(cudaMallocHost(&b.p, bytes));
+  b.bytes = bytes;
+  return B2S_OK;
+}
+
+void Stage::open(int dev) {
+  device = dev;
+  if (error == cudaSuccess) error = cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
+  if (error == cudaSuccess) error = cudaEventCreate(&ev[0]);
+  if (error == cudaSuccess) error = cudaEventCreate(&ev[1]);
+}
+
+void Stage::alloc_bytes(void** p, size_t bytes, bool pinned) {
+  if (error != cudaSuccess) return;
+  error = pinned ? cudaMallocHost(p, bytes) : cudaMalloc(p, bytes);
+  if (error == cudaSuccess) (pinned ? pinnedAllocs : devAllocs).push_back(*p);
+}
+
+int Stage::begin() {
+  B2S_CUDA(cudaEventRecord(ev[0], stream));
+  return B2S_OK;
+}
+
+int Stage::finish() {
+  B2S_CUDA(cudaEventRecord(ev[1], stream));
+  B2S_CUDA(cudaStreamSynchronize(stream));
+  B2S_CUDA(cudaGetLastError());
+  float ms = 0.f;
+  B2S_CUDA(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+  lastMs = ms;
+  return B2S_OK;
+}
+
+void Stage::close() {
+  cudaSetDevice(device);
+  if (stream) cudaStreamSynchronize(stream);
+  for (void* p : devAllocs) cudaFree(p);
+  for (void* p : pinnedAllocs) cudaFreeHost(p);
+  for (cudaEvent_t e : ev)
+    if (e) cudaEventDestroy(e);
+  if (stream) cudaStreamDestroy(stream);
+}
+
 bool csr_ok(const int32_t* off, int rows, int64_t cap) {
   if (!off || off[0] != 0) return false;
   for (int i = 0; i < rows; i++)
@@ -59,6 +108,21 @@ bool entries_ok(const int32_t* off, const int32_t* v, int rows, int lo, int hi, 
     for (int i = off[r]; i < off[r + 1]; i++) {
       if (v[i] < lo || v[i] >= hi) return false;
       if (ascending && i > off[r] && v[i] <= v[i - 1]) return false;
+    }
+  return true;
+}
+
+bool sets_ok(const int32_t* sets, int k, int width, int n, int* set, int* entry) {
+  for (int j = 0; j < k; j++)
+    for (int l = 0; l < width; l++) {
+      const int32_t* row = sets + (size_t)j * width;
+      bool dup = false;
+      for (int m = 0; m < l; m++) dup |= row[m] == row[l];
+      if (row[l] < 0 || row[l] >= n || dup) {
+        *set = j;
+        *entry = l;
+        return false;
+      }
     }
   return true;
 }

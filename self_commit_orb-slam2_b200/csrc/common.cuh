@@ -6,6 +6,7 @@
 #include <string.h>
 
 #include <string>
+#include <vector>
 
 #include "../../include/b200slam.h"
 
@@ -26,18 +27,72 @@ void set_error(const char* fmt, ...);
 
 int select_device(int device);  // returns B2S_OK / B2S_ERR_NO_DEVICE
 
-// Device buffer grown on demand.  grow() reallocates when `bytes` exceeds the capacity, without keeping the contents
-// (cudaFree synchronises the device); returns B2S_OK or a B2S_CUDA error.
+// Device buffer grown on demand, freed by its destructor.  grow() reallocates when `bytes` exceeds the capacity, without
+// keeping the contents (cudaFree synchronises the device); returns B2S_OK or a B2S_CUDA error.
 struct DevBuf {
   void* p = nullptr;
   size_t bytes = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() {
+    if (p) cudaFree(p);
+  }
 };
 int grow(DevBuf& b, size_t bytes);
+// Its pinned host counterpart (cudaMallocHost), with the same grow().
+struct HostBuf {
+  void* p = nullptr;
+  size_t bytes = 0;
+  HostBuf() = default;
+  HostBuf(const HostBuf&) = delete;
+  HostBuf& operator=(const HostBuf&) = delete;
+  ~HostBuf() {
+    if (p) cudaFreeHost(p);
+  }
+};
+int grow(HostBuf& b, size_t bytes);
+
+// The host side every device stage's handle shares (the handle struct derives from it): its device, a non-blocking
+// stream, the two events around the timed segment of a call and that segment's device time, and the buffers allocated
+// for the handle's lifetime.
+//   create:  open(device), then alloc / alloc_pinned for each buffer; `error` holds the first failure, after which
+//            every later open / alloc does nothing, so a create function checks it once at the end.
+//   a call:  begin() before the timed segment, finish() after it (waits for the stream, reads lastMs).
+//   destroy: close(), then delete the handle; buffers the handle holds itself (DevBuf, HostBuf) are freed by their
+//            destructors after close() has synchronised the stream.
+struct Stage {
+  int device = 0;
+  cudaStream_t stream = nullptr;
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  float lastMs = 0.f;
+  cudaError_t error = cudaSuccess;
+  std::vector<void*> devAllocs, pinnedAllocs;
+
+  void open(int dev);
+  template <class T>
+  void alloc(T*& p, size_t bytes) {
+    alloc_bytes(reinterpret_cast<void**>(&p), bytes, false);
+  }
+  template <class T>
+  void alloc_pinned(T*& p, size_t bytes) {
+    alloc_bytes(reinterpret_cast<void**>(&p), bytes, true);
+  }
+  int begin();   // records ev[0] on the stream
+  int finish();  // records ev[1], waits for the stream, checks for a launch error and sets lastMs
+  void close();  // sets the device, waits for the stream, frees the recorded buffers, destroys the events and stream
+
+ private:
+  void alloc_bytes(void** p, size_t bytes, bool pinned);
+};
 
 // Host-side checks of caller CSRs: off[0] == 0, non-decreasing, off[rows] <= cap.
 bool csr_ok(const int32_t* off, int rows, int64_t cap);
 // Every entry of the rows of a valid CSR in [lo, hi); each row strictly ascending when `ascending`.
 bool entries_ok(const int32_t* off, const int32_t* v, int rows, int lo, int hi, bool ascending);
+// k minimal sets of `width` indices each (row-major): true when every entry is in [0, n) and differs from the earlier
+// entries of its row, else false with the first bad (set, entry) written to *set / *entry.
+bool sets_ok(const int32_t* sets, int k, int width, int n, int* set, int* entry);
 
 static inline int div_up(int a, int b) { return (a + b - 1) / b; }
 static inline size_t align_up(size_t a, size_t b) { return (a + b - 1) / b * b; }

@@ -314,11 +314,8 @@ __global__ void __launch_bounds__(kReplayWarps * 32) k_covis_replay(Args a) {
 
 }  // namespace
 
-struct b2s_covis {
-  int maxKf, maxMp, maxObs, maxSlots, maxConn, maxBatch, device;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  float lastMs = 0.f;
+struct b2s_covis : b2s::Stage {
+  int maxKf, maxMp, maxObs, maxSlots, maxConn, maxBatch;
   int* dIn = nullptr;     // the packed problem
   int* hIn = nullptr;     // its pinned staging copy
   size_t inCap = 0;
@@ -345,19 +342,17 @@ extern "C" int b2s_covis_create(int max_kf, int max_mp, int max_obs, int max_slo
   h->maxSlots = max_slots;
   h->maxConn = max_conn;
   h->maxBatch = max_batch;
-  h->device = device;
   const size_t K = max_kf, B = max_batch, C = max_conn, KB = K * B;
   h->inCap = 2 * (K + 1) + 4 * C + 2 * K + 2 * (size_t)max_mp + 1 + max_obs + 2 * B + 1 + max_slots;
   h->smallCap = 1 + (K + 1) + (B + 1) + 5 * K + 4 * B;
   // hist, cnt kf/w, str kf/w, ev pos/k: 7 x KB; cntN, strN: 2B; evCnt, evStart, cur, bound: 4(K+1); small; 7 areas of C
   const size_t scr = 7 * KB + 2 * B + 4 * (K + 1) + h->smallCap + 7 * C;
-  cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[0]);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[1]);
-  if (e == cudaSuccess) e = cudaMalloc(&h->dIn, h->inCap * 4);
-  if (e == cudaSuccess) e = cudaMallocHost(&h->hIn, h->inCap * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&h->dScr, scr * 4);
-  if (e == cudaSuccess) e = cudaMallocHost(&h->hSmall, h->smallCap * 4);
+  h->open(device);
+  h->alloc(h->dIn, h->inCap * 4);
+  h->alloc_pinned(h->hIn, h->inCap * 4);
+  h->alloc(h->dScr, scr * 4);
+  h->alloc_pinned(h->hSmall, h->smallCap * 4);
+  cudaError_t e = h->error;
   if (e == cudaSuccess) e = cudaMemset(h->dScr, 0, KB * 4);  // hist
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e != cudaSuccess) {
@@ -400,14 +395,7 @@ extern "C" int b2s_covis_create(int max_kf, int max_mp, int max_obs, int max_slo
 
 extern "C" void b2s_covis_destroy(b2s_covis* h) {
   if (!h) return;
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  if (h->dIn) cudaFree(h->dIn);
-  if (h->dScr) cudaFree(h->dScr);
-  if (h->hIn) cudaFreeHost(h->hIn);
-  if (h->hSmall) cudaFreeHost(h->hSmall);
-  for (cudaEvent_t ev : h->ev)
-    if (ev) cudaEventDestroy(ev);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  h->close();
   delete h;
 }
 
@@ -508,7 +496,8 @@ extern "C" int b2s_update_connections(b2s_covis* h, const b2s_covis_problem* p, 
   a.afterN = small(B);
   a.pair = small(B);
 
-  B2S_CUDA(cudaEventRecord(h->ev[0], s));
+  int rc = h->begin();
+  if (rc != B2S_OK) return rc;
   B2S_CUDA(cudaMemcpyAsync(h->dIn, h->hIn, o * 4, cudaMemcpyHostToDevice, s));
   k_covis_count<<<B, kCountThreads, 0, s>>>(a);
   k_covis_group<<<1, kGroupThreads, 0, s>>>(a);
@@ -531,12 +520,7 @@ extern "C" int b2s_update_connections(b2s_covis* h, const b2s_covis_problem* p, 
     h->hArea[i].resize((size_t)len);
     if (len) B2S_CUDA(cudaMemcpyAsync(h->hArea[i].data(), areas[i], (size_t)len * 4, cudaMemcpyDeviceToHost, s));
   }
-  B2S_CUDA(cudaEventRecord(h->ev[1], s));
-  B2S_CUDA(cudaStreamSynchronize(s));
-  B2S_CUDA(cudaGetLastError());
-  float ms = 0.f;
-  B2S_CUDA(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
-  h->lastMs = ms;
+  if ((rc = h->finish()) != B2S_OK) return rc;
 
   const int *changed = at(a.changed), *parent = at(a.parent), *first = at(a.first), *mapN = at(a.mapN),
             *listN = at(a.listN), *startN = at(a.startN), *afterN = at(a.afterN), *pair = at(a.pair);

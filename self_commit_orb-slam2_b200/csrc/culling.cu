@@ -177,27 +177,10 @@ __global__ void __launch_bounds__(kThreads) k_cull_walk(Args a) {
   if (tid == 0) a.nCulled[b] = culled;
 }
 
-struct HostBuf {  // pinned staging grown on demand
-  int* p = nullptr;
-  size_t n = 0;
-  int grow(size_t want) {
-    if (want <= n) return B2S_OK;
-    if (p) cudaFreeHost(p);
-    p = nullptr;
-    n = 0;
-    B2S_CUDA(cudaMallocHost(&p, want * 4));
-    n = want;
-    return B2S_OK;
-  }
-};
-
 }  // namespace
 
-struct b2s_culling {
-  int maxKf, maxMp, maxObs, maxLocal, maxSlots, maxBatch, device;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  float lastMs = 0.f;
+struct b2s_culling : b2s::Stage {
+  int maxKf, maxMp, maxObs, maxLocal, maxSlots, maxBatch;
   DevBuf dIn, dOut;  // the packed problems; outputs and scratch
   HostBuf hIn, hOut;
 };
@@ -218,12 +201,9 @@ extern "C" int b2s_culling_create(int max_kf, int max_mp, int max_obs, int max_l
   h->maxLocal = max_local;
   h->maxSlots = max_slots;
   h->maxBatch = max_batch;
-  h->device = device;
-  cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[0]);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[1]);
-  if (e != cudaSuccess) {
-    set_error("b2s_culling_create: %s", cudaGetErrorString(e));
+  h->open(device);
+  if (h->error != cudaSuccess) {
+    set_error("b2s_culling_create: %s", cudaGetErrorString(h->error));
     b2s_culling_destroy(h);
     return B2S_ERR_CUDA;
   }
@@ -233,14 +213,7 @@ extern "C" int b2s_culling_create(int max_kf, int max_mp, int max_obs, int max_l
 
 extern "C" void b2s_culling_destroy(b2s_culling* h) {
   if (!h) return;
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  if (h->dIn.p) cudaFree(h->dIn.p);
-  if (h->dOut.p) cudaFree(h->dOut.p);
-  if (h->hIn.p) cudaFreeHost(h->hIn.p);
-  if (h->hOut.p) cudaFreeHost(h->hOut.p);
-  for (cudaEvent_t ev : h->ev)
-    if (ev) cudaEventDestroy(ev);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  h->close();
   delete h;
 }
 
@@ -347,12 +320,12 @@ extern "C" int b2s_keyframe_culling(b2s_culling* h, int batch, const b2s_culling
   const size_t outN = 3 * L + 2 * M + O + S + B, scrN = 2 * L + K;
   int rc = grow(h->dIn, inN * 4);
   if (rc == B2S_OK) rc = grow(h->dOut, (outN + scrN) * 4);
-  if (rc == B2S_OK) rc = h->hIn.grow(inN);
-  if (rc == B2S_OK) rc = h->hOut.grow(outN);
+  if (rc == B2S_OK) rc = grow(h->hIn, inN * 4);
+  if (rc == B2S_OK) rc = grow(h->hOut, outN * 4);
   if (rc != B2S_OK) return rc;
 
   // pack: one upload
-  int* q = h->hIn.p;
+  int* q = static_cast<int*>(h->hIn.p);
   int* dIn = static_cast<int*>(h->dIn.p);
   size_t o = 0;
   auto take = [&](size_t n) {
@@ -422,20 +395,15 @@ extern "C" int b2s_keyframe_culling(b2s_culling* h, int batch, const b2s_culling
   a.cntR = dOut + take(L);
   a.localPos = dOut + take(K);
 
-  B2S_CUDA(cudaEventRecord(h->ev[0], s));
+  if ((rc = h->begin()) != B2S_OK) return rc;
   B2S_CUDA(cudaMemcpyAsync(dIn, q, inN * 4, cudaMemcpyHostToDevice, s));
   if (L) k_cull_count<<<(unsigned)L, kThreads, 0, s>>>(a);
   k_cull_walk<<<batch, kThreads, 0, s>>>(a);
   B2S_CUDA(cudaGetLastError());
   B2S_CUDA(cudaMemcpyAsync(h->hOut.p, dOut, outN * 4, cudaMemcpyDeviceToHost, s));
-  B2S_CUDA(cudaEventRecord(h->ev[1], s));
-  B2S_CUDA(cudaStreamSynchronize(s));
-  B2S_CUDA(cudaGetLastError());
-  float ms = 0.f;
-  B2S_CUDA(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
-  h->lastMs = ms;
+  if ((rc = h->finish()) != B2S_OK) return rc;
 
-  const int* ho = h->hOut.p;
+  const int* ho = static_cast<const int*>(h->hOut.p);
   auto at = [&](const int* d) { return ho + (d - dOut); };
   const int *verdict = at(a.verdict), *nM = at(a.nM), *nR = at(a.nR), *bad = at(a.bad), *nobs = at(a.nobs),
             *alive = at(a.alive), *slot = at(a.slot), *nCulled = at(a.nCulled);

@@ -225,13 +225,9 @@ using namespace b2s;
 using namespace b2s::eg;
 
 // ================================================================================================ host side
-struct b2s_eg_solver {
-  int maxKf, maxE, maxMp, device;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  float lastMs = 0.f;
+struct b2s_eg_solver : b2s::Stage {
+  int maxKf, maxE, maxMp;
   long long lastTrials = 0;
-  std::vector<void*> allocs;
   // capacity-sized
   int *ei = nullptr, *ej = nullptr, *pidx = nullptr, *vOff = nullptr, *vList = nullptr, *bOff = nullptr, *bList = nullptr,
       *envT = nullptr, *ref = nullptr, *fail = nullptr;
@@ -291,17 +287,9 @@ extern "C" int b2s_eg_create(int max_kf, int max_edges, int max_mp, int device, 
   int rc = select_device(device);
   if (rc != B2S_OK) return rc;
   b2s_eg_solver* h = new b2s_eg_solver();
-  h->maxKf = max_kf; h->maxE = max_edges; h->maxMp = max_mp; h->device = device;
-  cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[0]);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[1]);
-  auto A = [&](void* pp, size_t bytes) {
-    void** p = (void**)pp;
-    if (e == cudaSuccess) {
-      e = cudaMalloc(p, bytes);
-      if (e == cudaSuccess) h->allocs.push_back(*p);
-    }
-  };
+  h->maxKf = max_kf; h->maxE = max_edges; h->maxMp = max_mp;
+  h->open(device);
+  auto A = [h](auto* p, size_t bytes) { h->alloc(*p, bytes); };
   const size_t K = max_kf, E = max_edges, M = max_mp;
   const size_t npPad = ((K * 7 + TS - 1) / TS) * TS, nT = npPad / TS;
   A(&h->ei, E * 4); A(&h->ej, E * 4); A(&h->meas, E * SD * 8); A(&h->err, E * 7 * 8); A(&h->chi2, E * 8);
@@ -312,8 +300,9 @@ extern "C" int b2s_eg_create(int max_kf, int max_edges, int max_mp, int device, 
   A(&h->tmp, std::max(E, npPad) * 8); A(&h->linv, nT * TT * 8);
   A(&h->P, M * 12); A(&h->Pout, M * 12); A(&h->ref, M * 4);
   A(&h->part, RED_BLOCKS * 8); A(&h->scal, 4 * 8); A(&h->fail, 4);
-  if (e == cudaSuccess) e = cudaMallocHost(&h->hScal, 4 * 8);
-  if (e == cudaSuccess) e = cudaMallocHost(&h->hFail, 4);
+  h->alloc_pinned(h->hScal, 4 * 8);
+  h->alloc_pinned(h->hFail, 4);
+  cudaError_t e = h->error;
   if (e == cudaSuccess) e = set_smem_limits();
   if (e != cudaSuccess) {
     set_error("b2s_eg_create: %s", cudaGetErrorString(e));
@@ -326,15 +315,7 @@ extern "C" int b2s_eg_create(int max_kf, int max_edges, int max_mp, int device, 
 
 extern "C" void b2s_eg_destroy(b2s_eg_solver* h) {
   if (!h) return;
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  for (void* p : h->allocs) cudaFree(p);
-  if (h->tiles.p) cudaFree(h->tiles.p);
-  if (h->rows.p) cudaFree(h->rows.p);
-  if (h->hScal) cudaFreeHost(h->hScal);
-  if (h->hFail) cudaFreeHost(h->hFail);
-  for (cudaEvent_t ev : h->ev)
-    if (ev) cudaEventDestroy(ev);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  h->close();
   delete h;
 }
 

@@ -441,13 +441,9 @@ using namespace b2s;
 using namespace b2s::gba;
 
 // ================================================================================================ host side
-struct b2s_gba_solver {
-  int maxKf, maxMp, maxE, device;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  float lastMs = 0.f;
+struct b2s_gba_solver : b2s::Stage {
+  int maxKf, maxMp, maxE;
   long long lastTrials = 0;
-  std::vector<void*> allocs;
   // capacity-sized
   int *eKf = nullptr, *eMp = nullptr, *pidx = nullptr, *ptBeg = nullptr, *ptEnd = nullptr, *kfBeg = nullptr,
       *kfEnd = nullptr, *kfEdge = nullptr, *kfVal = nullptr, *envBlk = nullptr, *envT = nullptr;
@@ -518,17 +514,9 @@ extern "C" int b2s_gba_create(int max_kf, int max_mp, int max_edges, int device,
   int rc = select_device(device);
   if (rc != B2S_OK) return rc;
   b2s_gba_solver* h = new b2s_gba_solver();
-  h->maxKf = max_kf; h->maxMp = max_mp; h->maxE = max_edges; h->device = device;
-  cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[0]);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[1]);
-  auto A = [&](void* pp, size_t bytes) {
-    void** p = (void**)pp;
-    if (e == cudaSuccess) {
-      e = cudaMalloc(p, bytes);
-      if (e == cudaSuccess) h->allocs.push_back(*p);
-    }
-  };
+  h->maxKf = max_kf; h->maxMp = max_mp; h->maxE = max_edges;
+  h->open(device);
+  auto A = [h](auto* p, size_t bytes) { h->alloc(*p, bytes); };
   const size_t K = max_kf, M = max_mp, E = max_edges;
   A(&h->eKf, E * 4); A(&h->eMp, E * 4); A(&h->eObs, E * 12); A(&h->eW, E * 4);
   A(&h->kfKey, E * 4); A(&h->kfKeyS, E * 4); A(&h->kfVal, E * 4); A(&h->kfEdge, E * 4);
@@ -539,8 +527,9 @@ extern "C" int b2s_gba_create(int max_kf, int max_mp, int max_edges, int device,
   A(&h->X, M * 12); A(&h->pts, M * 24); A(&h->ptsT, M * 24); A(&h->ptBeg, M * 4); A(&h->ptEnd, M * 4);
   A(&h->Hll, M * 72); A(&h->Dinv, M * 72); A(&h->db, M * 24); A(&h->pairCnt, (M + 1) * 8); A(&h->pairOff, (M + 1) * 8);
   A(&h->part, RED_BLOCKS * 8); A(&h->scal, 4 * 8); A(&h->fail, 4);
-  if (e == cudaSuccess) e = cudaMallocHost(&h->hScal, 4 * 8);
-  if (e == cudaSuccess) e = cudaMallocHost(&h->hFail, 4);
+  h->alloc_pinned(h->hScal, 4 * 8);
+  h->alloc_pinned(h->hFail, 4);
+  cudaError_t e = h->error;
   if (e == cudaSuccess) e = set_smem_limits();
   if (e != cudaSuccess) {
     set_error("b2s_gba_create: %s", cudaGetErrorString(e));
@@ -553,18 +542,7 @@ extern "C" int b2s_gba_create(int max_kf, int max_mp, int max_edges, int device,
 
 extern "C" void b2s_gba_destroy(b2s_gba_solver* h) {
   if (!h) return;
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  for (void* p : h->allocs) cudaFree(p);
-  DevBuf* bufs[] = {&h->pairKey, &h->pairKeyS, &h->pairVal, &h->pairValS, &h->pairRec, &h->pairRecS,
-                                 &h->uKey, &h->runLen, &h->blkBeg, &h->nRuns, &h->cubTmp, &h->tiles, &h->linv,
-                                 &h->bvec, &h->xvec, &h->rhs, &h->ybuf, &h->tmp, &h->rows};
-  for (auto* b : bufs)
-    if (b->p) cudaFree(b->p);
-  if (h->hScal) cudaFreeHost(h->hScal);
-  if (h->hFail) cudaFreeHost(h->hFail);
-  for (cudaEvent_t ev : h->ev)
-    if (ev) cudaEventDestroy(ev);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  h->close();
   delete h;
 }
 

@@ -599,11 +599,8 @@ using namespace b2s;
 using namespace b2s::ini;
 
 // ================================================================================================ host side
-struct b2s_init_solver {
-  int maxKeys, maxIters, maxBatch, device;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  float lastMs = 0.f;
+struct b2s_init_solver : b2s::Stage {
+  int maxKeys, maxIters, maxBatch;
   Prob* prob = nullptr;
   float *kp1 = nullptr, *kp2 = nullptr, *pn1 = nullptr, *pn2 = nullptr, *hyp = nullptr, *score = nullptr;
   int *m12 = nullptr, *sets = nullptr, *mt = nullptr;
@@ -630,30 +627,28 @@ extern "C" int b2s_init_create(int max_keys, int max_iterations, int max_batch, 
   h->maxKeys = max_keys;
   h->maxIters = max_iterations;
   h->maxBatch = max_batch;
-  h->device = device;
   const size_t B = max_batch, NK = (size_t)max_keys * B, IT = (size_t)max_iterations * B;
   const size_t W = (size_t)((max_keys + 31) / 32) * 2 * IT;
-  cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[0]);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[1]);
-  if (e == cudaSuccess) e = cudaMalloc(&h->prob, B * sizeof(Prob));
-  if (e == cudaSuccess) e = cudaMalloc(&h->kp1, NK * 2 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->kp2, NK * 2 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->pn1, NK * 2 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->pn2, NK * 2 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->m12, NK * sizeof(int));
-  if (e == cudaSuccess) e = cudaMalloc(&h->mt, NK * 2 * sizeof(int));
-  if (e == cudaSuccess) e = cudaMalloc(&h->sets, IT * 8 * sizeof(int));
-  if (e == cudaSuccess) e = cudaMalloc(&h->hyp, IT * 2 * 18 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->score, IT * 2 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->inl, W * sizeof(uint32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&h->st, B * sizeof(St));
-  if (e == cudaSuccess) e = cudaMalloc(&h->p3dh, NK * 8 * 3 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->goodh, NK * 8);
-  if (e == cudaSuccess) e = cudaMalloc(&h->p3d, NK * 3 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->tri, NK);
-  if (e == cudaSuccess) e = cudaMalloc(&h->inlH, NK);
-  if (e == cudaSuccess) e = cudaMalloc(&h->inlF, NK);
+  h->open(device);
+  h->alloc(h->prob, B * sizeof(Prob));
+  h->alloc(h->kp1, NK * 2 * sizeof(float));
+  h->alloc(h->kp2, NK * 2 * sizeof(float));
+  h->alloc(h->pn1, NK * 2 * sizeof(float));
+  h->alloc(h->pn2, NK * 2 * sizeof(float));
+  h->alloc(h->m12, NK * sizeof(int));
+  h->alloc(h->mt, NK * 2 * sizeof(int));
+  h->alloc(h->sets, IT * 8 * sizeof(int));
+  h->alloc(h->hyp, IT * 2 * 18 * sizeof(float));
+  h->alloc(h->score, IT * 2 * sizeof(float));
+  h->alloc(h->inl, W * sizeof(uint32_t));
+  h->alloc(h->st, B * sizeof(St));
+  h->alloc(h->p3dh, NK * 8 * 3 * sizeof(float));
+  h->alloc(h->goodh, NK * 8);
+  h->alloc(h->p3d, NK * 3 * sizeof(float));
+  h->alloc(h->tri, NK);
+  h->alloc(h->inlH, NK);
+  h->alloc(h->inlF, NK);
+  cudaError_t e = h->error;
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(k_init_checkrt, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_KEYS * sizeof(float));
   if (e != cudaSuccess) {
@@ -667,14 +662,7 @@ extern "C" int b2s_init_create(int max_keys, int max_iterations, int max_batch, 
 
 extern "C" void b2s_init_destroy(b2s_init_solver* h) {
   if (!h) return;
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  for (void* q : {(void*)h->prob, (void*)h->kp1, (void*)h->kp2, (void*)h->pn1, (void*)h->pn2, (void*)h->m12,
-                  (void*)h->mt, (void*)h->sets, (void*)h->hyp, (void*)h->score, (void*)h->inl, (void*)h->st,
-                  (void*)h->p3dh, (void*)h->goodh, (void*)h->p3d, (void*)h->tri, (void*)h->inlH, (void*)h->inlF})
-    if (q) cudaFree(q);
-  for (cudaEvent_t ev : h->ev)
-    if (ev) cudaEventDestroy(ev);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  h->close();
   delete h;
 }
 
@@ -714,16 +702,11 @@ extern "C" int b2s_initialize(b2s_init_solver* h, int batch, const b2s_init_prob
       set_error("b2s_initialize: problem %d has %d matches (at least 8)", i, n);
       return B2S_ERR_BAD_ARG;
     }
-    for (int it = 0; it < q.iterations; it++)
-      for (int j = 0; j < 8; j++) {
-        const int s = q.sets[8 * it + j];
-        bool dup = false;
-        for (int l = 0; l < j; l++) dup |= q.sets[8 * it + l] == s;
-        if (s < 0 || s >= n || dup) {
-          set_error("b2s_initialize: problem %d: set %d entry %d = %d (n_matches = %d)", i, it, j, s, n);
-          return B2S_ERR_BAD_ARG;
-        }
-      }
+    int it, j;
+    if (!sets_ok(q.sets, q.iterations, 8, n, &it, &j)) {
+      set_error("b2s_initialize: problem %d: set %d entry %d = %d (n_matches = %d)", i, it, j, q.sets[8 * it + j], n);
+      return B2S_ERR_BAD_ARG;
+    }
     nm[(size_t)i] = n;
   }
   B2S_CUDA(cudaSetDevice(h->device));
@@ -770,7 +753,8 @@ extern "C" int b2s_initialize(b2s_init_solver* h, int batch, const b2s_init_prob
   h->hInlH.resize(o1);
   h->hInlF.resize(o1);
 
-  B2S_CUDA(cudaEventRecord(h->ev[0], s));
+  int rc = h->begin();
+  if (rc != B2S_OK) return rc;
   B2S_CUDA(cudaMemcpyAsync(h->prob, h->hProb.data(), (size_t)batch * sizeof(Prob), cudaMemcpyHostToDevice, s));
   B2S_CUDA(cudaMemcpyAsync(h->kp1, h->hKp1.data(), o1 * 2 * sizeof(float), cudaMemcpyHostToDevice, s));
   B2S_CUDA(cudaMemcpyAsync(h->kp2, h->hKp2.data(), o2 * 2 * sizeof(float), cudaMemcpyHostToDevice, s));
@@ -792,9 +776,7 @@ extern "C" int b2s_initialize(b2s_init_solver* h, int batch, const b2s_init_prob
   B2S_CUDA(cudaMemcpyAsync(h->hTri.data(), h->tri, o1, cudaMemcpyDeviceToHost, s));
   B2S_CUDA(cudaMemcpyAsync(h->hInlH.data(), h->inlH, o1, cudaMemcpyDeviceToHost, s));
   B2S_CUDA(cudaMemcpyAsync(h->hInlF.data(), h->inlF, o1, cudaMemcpyDeviceToHost, s));
-  B2S_CUDA(cudaEventRecord(h->ev[1], s));
-  B2S_CUDA(cudaStreamSynchronize(s));
-  B2S_CUDA(cudaGetLastError());
+  if ((rc = h->finish()) != B2S_OK) return rc;
 
   for (int i = 0; i < batch; i++) {
     const St& S = h->hSt[(size_t)i];
@@ -825,8 +807,5 @@ extern "C" int b2s_initialize(b2s_init_solver* h, int batch, const b2s_init_prob
       R.parallax[k] = S.par[k];
     }
   }
-  float ms = 0.f;
-  B2S_CUDA(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
-  h->lastMs = ms;
   return B2S_OK;
 }

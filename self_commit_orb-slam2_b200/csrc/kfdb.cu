@@ -326,11 +326,8 @@ size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
 
 using namespace b2s;
 
-struct b2s_kfdb {
-  int n_words = 0, device = 0;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  float last_ms = 0.0f;
+struct b2s_kfdb : b2s::Stage {
+  int n_words = 0;
   // BowVector pool: [0, pool_tail) holds the vectors of live and erased keyframes; pool_live entries are live
   uint32_t* d_pw = nullptr;
   double* d_pv = nullptr;
@@ -477,7 +474,7 @@ int query(b2s_kfdb* db, int loop, uint64_t qid, const uint32_t* words, const dou
   *n_out = 0;
   int rc = check_bow(db, words, values, n, fn);
   if (rc != B2S_OK) return rc;
-  db->last_ms = 0.0f;
+  db->lastMs = 0.0f;
   const int n_live = (int)db->live.size();
   if (n == 0 || n_live == 0) return B2S_OK;  // no keyframe shares a word: nothing is touched
   B2S_CUDA(cudaSetDevice(db->device));
@@ -514,7 +511,7 @@ int query(b2s_kfdb* db, int loop, uint64_t qid, const uint32_t* words, const dou
   }
   unsigned char* d = db->d_stage;
   B2S_CUDA(cudaMemcpyAsync(d, h, total, cudaMemcpyHostToDevice, db->stream));
-  B2S_CUDA(cudaEventRecord(db->ev0, db->stream));
+  if ((rc = db->begin()) != B2S_OK) return rc;
   k_kfdb_match<<<div_up(n_live, kMatchWarps), kMatchWarps * 32, (size_t)n * 12, db->stream>>>(
       db->d_pw, db->d_pv, db->d_live, n_live, reinterpret_cast<const uint32_t*>(d + o_qw),
       reinterpret_cast<const double*>(d + o_qv), n, reinterpret_cast<const uint64_t*>(d + o_conn), n_conn, loop,
@@ -525,11 +522,11 @@ int query(b2s_kfdb* db, int loop, uint64_t qid, const uint32_t* words, const dou
       reinterpret_cast<const uint64_t*>(d + o_cid), reinterpret_cast<const int32_t*>(d + o_cn), n_rows, db->d_state,
       db->state_cap, db->d_order, db->d_acc, db->d_best, db->d_first_pos, db->d_out);
   B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaEventRecord(db->ev1, db->stream));
+  B2S_CUDA(cudaEventRecord(db->ev[1], db->stream));  // the kernels only: the download is not timed
   const int n_dl = 1 + std::min(cap, n_live);
   B2S_CUDA(cudaMemcpyAsync(db->h_out, db->d_out, (size_t)n_dl * 4, cudaMemcpyDeviceToHost, db->stream));
   B2S_CUDA(cudaStreamSynchronize(db->stream));
-  B2S_CUDA(cudaEventElapsedTime(&db->last_ms, db->ev0, db->ev1));
+  B2S_CUDA(cudaEventElapsedTime(&db->lastMs, db->ev[0], db->ev[1]));
   const int cnt = db->h_out[0];
   *n_out = cnt;
   if (cnt > cap) {
@@ -544,16 +541,13 @@ int query(b2s_kfdb* db, int loop, uint64_t qid, const uint32_t* words, const dou
 
 extern "C" void b2s_kfdb_destroy(b2s_kfdb* db) {
   if (!db) return;
-  cudaSetDevice(db->device);
-  if (db->stream) cudaStreamSynchronize(db->stream);
+  db->close();
+  // the buffers that keep their contents when they grow are the database's own
   free_live_scratch(db);
   void* p[] = {db->d_pw, db->d_pv, db->d_state, db->d_first_pos, db->d_stage};
   for (void* x : p)
     if (x) cudaFree(x);
   if (db->h_stage) cudaFreeHost(db->h_stage);
-  if (db->ev0) cudaEventDestroy(db->ev0);
-  if (db->ev1) cudaEventDestroy(db->ev1);
-  if (db->stream) cudaStreamDestroy(db->stream);
   delete db;
 }
 
@@ -565,15 +559,14 @@ extern "C" int b2s_kfdb_create(int n_words, int device, b2s_kfdb** out) {
   *out = nullptr;
   int rc = select_device(device);
   if (rc != B2S_OK) return rc;
-  B2S_CUDA(cudaFuncSetAttribute(k_kfdb_match, cudaFuncAttributeMaxDynamicSharedMemorySize, B2S_KFDB_MAX_WORDS * 12));
   b2s_kfdb* db = new b2s_kfdb();
   db->n_words = n_words;
-  db->device = device;
-  cudaError_t e = cudaStreamCreateWithFlags(&db->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaEventCreate(&db->ev0);
-  if (e == cudaSuccess) e = cudaEventCreate(&db->ev1);
+  db->open(device);
+  cudaError_t e = db->error;
   if (e == cudaSuccess) e = cudaMalloc(&db->d_pw, (size_t)kPoolMin * 4);
   if (e == cudaSuccess) e = cudaMalloc(&db->d_pv, (size_t)kPoolMin * 8);
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(k_kfdb_match, cudaFuncAttributeMaxDynamicSharedMemorySize, B2S_KFDB_MAX_WORDS * 12);
   if (e != cudaSuccess) {
     set_error("b2s_kfdb_create: %s", cudaGetErrorString(e));
     b2s_kfdb_destroy(db);
@@ -684,4 +677,4 @@ extern "C" int b2s_kfdb_keyframe_state(b2s_kfdb* db, uint64_t kf_id, b2s_kfdb_st
   return B2S_OK;
 }
 
-extern "C" float b2s_kfdb_last_query_ms(const b2s_kfdb* db) { return db ? db->last_ms : 0.0f; }
+extern "C" float b2s_kfdb_last_query_ms(const b2s_kfdb* db) { return db ? db->lastMs : 0.0f; }

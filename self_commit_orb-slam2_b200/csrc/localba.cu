@@ -1780,7 +1780,6 @@ extern "C" void b2s_ba_destroy(b2s_ba_solver* h) {
   cudaSetDevice(h->device);
   pose_scratch_free(h->pose);
   for (void* p : h->allocs) cudaFree(p);
-  cudaFree(h->pairRec.p);
   for (void* p : h->hostAllocs) cudaFreeHost(p);
   for (auto& e : h->evLm)
     if (e) cudaEventDestroy(e);

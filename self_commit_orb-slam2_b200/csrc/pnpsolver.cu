@@ -693,11 +693,8 @@ using namespace b2s;
 using namespace b2s::pnp;
 
 // ================================================================================================ host side
-struct b2s_pnpsolver {
-  int maxMatches, maxSets, maxBatch, device;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  float lastMs = 0.f;
+struct b2s_pnpsolver : b2s::Stage {
+  int maxMatches, maxSets, maxBatch;
   Prob* prob = nullptr;
   float *P3Dw = nullptr, *P2D = nullptr, *sig = nullptr, *bestTcw = nullptr;
   int *sets = nullptr, *cnt = nullptr, *idx = nullptr;
@@ -726,31 +723,28 @@ extern "C" int b2s_pnpsolver_create(int max_matches, int max_sets, int max_batch
   h->maxMatches = max_matches;
   h->maxSets = max_sets;
   h->maxBatch = max_batch;
-  h->device = device;
   const size_t B = max_batch, NM = (size_t)max_matches * B, NS = (size_t)max_sets * B;
   const size_t WPB = (size_t)((max_matches + 31) / 32) * B, W = (size_t)((max_matches + 31) / 32) * NS;
-  cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[0]);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[1]);
-  if (e == cudaSuccess) e = cudaMalloc(&h->prob, B * sizeof(Prob));
-  if (e == cudaSuccess) e = cudaMalloc(&h->P3Dw, NM * 3 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->P2D, NM * 2 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->sig, NM * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->bestTcw, B * 16 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->bestIn, NM);
-  if (e == cudaSuccess) e = cudaMalloc(&h->sets, NS * 4 * sizeof(int));
-  if (e == cudaSuccess) e = cudaMalloc(&h->hyp, NS * HYP * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc(&h->cnt, NS * sizeof(int));
-  if (e == cudaSuccess) e = cudaMalloc(&h->mask, W * sizeof(uint32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&h->carried, WPB * sizeof(uint32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&h->refined, WPB * sizeof(uint32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&h->scratch, NM * SCR * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc(&h->idx, NM * sizeof(int));
-  if (e == cudaSuccess) e = cudaMalloc(&h->st, B * sizeof(St));
-  if (e == cudaSuccess) e = cudaMalloc(&h->inl, NM);
-  if (e == cudaSuccess) e = cudaMalloc(&h->bestOut, NM);
-  if (e != cudaSuccess) {
-    set_error("b2s_pnpsolver_create: %s", cudaGetErrorString(e));
+  h->open(device);
+  h->alloc(h->prob, B * sizeof(Prob));
+  h->alloc(h->P3Dw, NM * 3 * sizeof(float));
+  h->alloc(h->P2D, NM * 2 * sizeof(float));
+  h->alloc(h->sig, NM * sizeof(float));
+  h->alloc(h->bestTcw, B * 16 * sizeof(float));
+  h->alloc(h->bestIn, NM);
+  h->alloc(h->sets, NS * 4 * sizeof(int));
+  h->alloc(h->hyp, NS * HYP * sizeof(double));
+  h->alloc(h->cnt, NS * sizeof(int));
+  h->alloc(h->mask, W * sizeof(uint32_t));
+  h->alloc(h->carried, WPB * sizeof(uint32_t));
+  h->alloc(h->refined, WPB * sizeof(uint32_t));
+  h->alloc(h->scratch, NM * SCR * sizeof(double));
+  h->alloc(h->idx, NM * sizeof(int));
+  h->alloc(h->st, B * sizeof(St));
+  h->alloc(h->inl, NM);
+  h->alloc(h->bestOut, NM);
+  if (h->error != cudaSuccess) {
+    set_error("b2s_pnpsolver_create: %s", cudaGetErrorString(h->error));
     b2s_pnpsolver_destroy(h);
     return B2S_ERR_CUDA;
   }
@@ -760,14 +754,7 @@ extern "C" int b2s_pnpsolver_create(int max_matches, int max_sets, int max_batch
 
 extern "C" void b2s_pnpsolver_destroy(b2s_pnpsolver* h) {
   if (!h) return;
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  for (void* q : {(void*)h->prob, (void*)h->P3Dw, (void*)h->P2D, (void*)h->sig, (void*)h->bestTcw, (void*)h->bestIn,
-                  (void*)h->sets, (void*)h->hyp, (void*)h->cnt, (void*)h->mask, (void*)h->carried, (void*)h->refined,
-                  (void*)h->scratch, (void*)h->idx, (void*)h->st, (void*)h->inl, (void*)h->bestOut})
-    if (q) cudaFree(q);
-  for (cudaEvent_t ev : h->ev)
-    if (ev) cudaEventDestroy(ev);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  h->close();
   delete h;
 }
 
@@ -809,17 +796,11 @@ extern "C" int b2s_pnpsolver_iterate(b2s_pnpsolver* h, int batch, const b2s_pnps
       nb += q.best_mask[c] != 0;
     }
     if (q.best_inliers > 0 && nb != q.best_inliers) return pnp_bad(i, "best_mask does not hold best_inliers entries");
-    if (run)
-      for (int j = 0; j < q.k; j++)
-        for (int l = 0; l < 4; l++) {
-          const int s = q.sets[4 * j + l];
-          bool dup = false;
-          for (int m = 0; m < l; m++) dup |= q.sets[4 * j + m] == s;
-          if (s < 0 || s >= q.n || dup) {
-            set_error("b2s_pnpsolver_iterate: problem %d: set %d entry %d = %d (n = %d)", i, j, l, s, q.n);
-            return B2S_ERR_BAD_ARG;
-          }
-        }
+    int j, l;
+    if (run && !sets_ok(q.sets, q.k, 4, q.n, &j, &l)) {
+      set_error("b2s_pnpsolver_iterate: problem %d: set %d entry %d = %d (n = %d)", i, j, l, q.sets[4 * j + l], q.n);
+      return B2S_ERR_BAD_ARG;
+    }
   }
   B2S_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
@@ -874,7 +855,8 @@ extern "C" int b2s_pnpsolver_iterate(b2s_pnpsolver* h, int batch, const b2s_pnps
   h->hInl.resize(on);
   h->hBestOut.resize(on);
 
-  B2S_CUDA(cudaEventRecord(h->ev[0], s));
+  int rc = h->begin();
+  if (rc != B2S_OK) return rc;
   B2S_CUDA(cudaMemcpyAsync(h->prob, h->hProb.data(), (size_t)batch * sizeof(Prob), cudaMemcpyHostToDevice, s));
   B2S_CUDA(cudaMemcpyAsync(h->bestTcw, h->hBestTcw.data(), (size_t)batch * 16 * sizeof(float), cudaMemcpyHostToDevice,
                            s));
@@ -898,9 +880,7 @@ extern "C" int b2s_pnpsolver_iterate(b2s_pnpsolver* h, int batch, const b2s_pnps
     B2S_CUDA(cudaMemcpyAsync(h->hInl.data(), h->inl, on, cudaMemcpyDeviceToHost, s));
     B2S_CUDA(cudaMemcpyAsync(h->hBestOut.data(), h->bestOut, on, cudaMemcpyDeviceToHost, s));
   }
-  B2S_CUDA(cudaEventRecord(h->ev[1], s));
-  B2S_CUDA(cudaStreamSynchronize(s));
-  B2S_CUDA(cudaGetLastError());
+  if ((rc = h->finish()) != B2S_OK) return rc;
 
   for (int i = 0; i < batch; i++) {
     const St& S = h->hSt[(size_t)i];
@@ -920,8 +900,5 @@ extern "C" int b2s_pnpsolver_iterate(b2s_pnpsolver* h, int batch, const b2s_pnps
     R.best_changed = S.bestChanged;
     memcpy(R.best_Tcw, S.bestTcw, sizeof(R.best_Tcw));
   }
-  float ms = 0.f;
-  B2S_CUDA(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
-  h->lastMs = ms;
   return B2S_OK;
 }

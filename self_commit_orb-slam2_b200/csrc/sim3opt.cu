@@ -336,11 +336,8 @@ using namespace b2s;
 using namespace b2s::s3o;
 
 // ================================================================================================ host side
-struct b2s_sim3opt_solver {
-  int maxN, maxBatch, device;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  float lastMs = 0.f;
+struct b2s_sim3opt_solver : b2s::Stage {
+  int maxN, maxBatch;
   long long lastTrials = 0;
   Prob* prob = nullptr;
   float* in = nullptr;
@@ -365,17 +362,15 @@ extern "C" int b2s_sim3opt_create(int max_matches, int max_batch, int device, b2
   b2s_sim3opt_solver* h = new b2s_sim3opt_solver();
   h->maxN = max_matches;
   h->maxBatch = max_batch;
-  h->device = device;
   const size_t M = (size_t)max_matches * max_batch, B = max_batch;
-  cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[0]);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[1]);
-  if (e == cudaSuccess) e = cudaMalloc(&h->prob, B * sizeof(Prob));
-  if (e == cudaSuccess) e = cudaMalloc(&h->in, M * IN * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->scr, M * 2 * ES * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc(&h->keep, M);
-  if (e == cudaSuccess) e = cudaMalloc(&h->Sout, B * 8 * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc(&h->outI, B * OUT_I * sizeof(int));
+  h->open(device);
+  h->alloc(h->prob, B * sizeof(Prob));
+  h->alloc(h->in, M * IN * sizeof(float));
+  h->alloc(h->scr, M * 2 * ES * sizeof(double));
+  h->alloc(h->keep, M);
+  h->alloc(h->Sout, B * 8 * sizeof(double));
+  h->alloc(h->outI, B * OUT_I * sizeof(int));
+  cudaError_t e = h->error;
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(k_optimize_sim3, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_N);
   if (e != cudaSuccess) {
@@ -389,12 +384,7 @@ extern "C" int b2s_sim3opt_create(int max_matches, int max_batch, int device, b2
 
 extern "C" void b2s_sim3opt_destroy(b2s_sim3opt_solver* h) {
   if (!h) return;
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  for (void* q : {(void*)h->prob, (void*)h->in, (void*)h->scr, (void*)h->keep, (void*)h->Sout, (void*)h->outI})
-    if (q) cudaFree(q);
-  for (cudaEvent_t ev : h->ev)
-    if (ev) cudaEventDestroy(ev);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  h->close();
   delete h;
 }
 
@@ -468,7 +458,8 @@ extern "C" int b2s_optimize_sim3(b2s_sim3opt_solver* h, int batch, const b2s_sim
   h->hOutI.resize((size_t)batch * OUT_I);
   h->hKeep.resize(std::max<size_t>(total, 1));
 
-  B2S_CUDA(cudaEventRecord(h->ev[0], s));
+  int rc = h->begin();
+  if (rc != B2S_OK) return rc;
   B2S_CUDA(cudaMemcpyAsync(h->prob, h->hProb.data(), (size_t)batch * sizeof(Prob), cudaMemcpyHostToDevice, s));
   if (total) B2S_CUDA(cudaMemcpyAsync(h->in, h->hIn.data(), total * IN * sizeof(float), cudaMemcpyHostToDevice, s));
   Ptrs a = {h->prob, h->in, h->scr, h->keep, h->Sout, h->outI};
@@ -478,9 +469,7 @@ extern "C" int b2s_optimize_sim3(b2s_sim3opt_solver* h, int batch, const b2s_sim
   B2S_CUDA(cudaMemcpyAsync(h->hSout.data(), h->Sout, (size_t)batch * 8 * sizeof(double), cudaMemcpyDeviceToHost, s));
   B2S_CUDA(cudaMemcpyAsync(h->hOutI.data(), h->outI, (size_t)batch * OUT_I * sizeof(int), cudaMemcpyDeviceToHost, s));
   if (total) B2S_CUDA(cudaMemcpyAsync(h->hKeep.data(), h->keep, total, cudaMemcpyDeviceToHost, s));
-  B2S_CUDA(cudaEventRecord(h->ev[1], s));
-  B2S_CUDA(cudaStreamSynchronize(s));
-  B2S_CUDA(cudaGetLastError());
+  if ((rc = h->finish()) != B2S_OK) return rc;
 
   long long trials = 0;
   for (int i = 0; i < batch; i++) {
@@ -497,9 +486,6 @@ extern "C" int b2s_optimize_sim3(b2s_sim3opt_solver* h, int batch, const b2s_sim
     }
     trials += o[1];
   }
-  float ms = 0.f;
-  B2S_CUDA(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
-  h->lastMs = ms;
   h->lastTrials = trials;
   return B2S_OK;
 }

@@ -387,11 +387,8 @@ using namespace b2s;
 using namespace b2s::s3s;
 
 // ================================================================================================ host side
-struct b2s_sim3solver {
-  int maxMatches, maxSets, maxBatch, device;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  float lastMs = 0.f;
+struct b2s_sim3solver : b2s::Stage {
+  int maxMatches, maxSets, maxBatch;
   Prob* prob = nullptr;
   float *X1 = nullptr, *X2 = nullptr, *sig1 = nullptr, *sig2 = nullptr, *hyp = nullptr;
   int *sets = nullptr, *cnt = nullptr;
@@ -418,25 +415,22 @@ extern "C" int b2s_sim3solver_create(int max_matches, int max_sets, int max_batc
   h->maxMatches = max_matches;
   h->maxSets = max_sets;
   h->maxBatch = max_batch;
-  h->device = device;
   const size_t B = max_batch, NM = (size_t)max_matches * B, NS = (size_t)max_sets * B;
   const size_t W = (size_t)((max_matches + 31) / 32) * NS;
-  cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[0]);
-  if (e == cudaSuccess) e = cudaEventCreate(&h->ev[1]);
-  if (e == cudaSuccess) e = cudaMalloc(&h->prob, B * sizeof(Prob));
-  if (e == cudaSuccess) e = cudaMalloc(&h->X1, NM * 3 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->X2, NM * 3 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->sig1, NM * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->sig2, NM * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->sets, NS * 3 * sizeof(int));
-  if (e == cudaSuccess) e = cudaMalloc(&h->hyp, NS * HYP * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->cnt, NS * sizeof(int));
-  if (e == cudaSuccess) e = cudaMalloc(&h->mask, W * sizeof(uint32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&h->st, B * sizeof(St));
-  if (e == cudaSuccess) e = cudaMalloc(&h->inl, NM);
-  if (e != cudaSuccess) {
-    set_error("b2s_sim3solver_create: %s", cudaGetErrorString(e));
+  h->open(device);
+  h->alloc(h->prob, B * sizeof(Prob));
+  h->alloc(h->X1, NM * 3 * sizeof(float));
+  h->alloc(h->X2, NM * 3 * sizeof(float));
+  h->alloc(h->sig1, NM * sizeof(float));
+  h->alloc(h->sig2, NM * sizeof(float));
+  h->alloc(h->sets, NS * 3 * sizeof(int));
+  h->alloc(h->hyp, NS * HYP * sizeof(float));
+  h->alloc(h->cnt, NS * sizeof(int));
+  h->alloc(h->mask, W * sizeof(uint32_t));
+  h->alloc(h->st, B * sizeof(St));
+  h->alloc(h->inl, NM);
+  if (h->error != cudaSuccess) {
+    set_error("b2s_sim3solver_create: %s", cudaGetErrorString(h->error));
     b2s_sim3solver_destroy(h);
     return B2S_ERR_CUDA;
   }
@@ -446,13 +440,7 @@ extern "C" int b2s_sim3solver_create(int max_matches, int max_sets, int max_batc
 
 extern "C" void b2s_sim3solver_destroy(b2s_sim3solver* h) {
   if (!h) return;
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  for (void* q : {(void*)h->prob, (void*)h->X1, (void*)h->X2, (void*)h->sig1, (void*)h->sig2, (void*)h->sets,
-                  (void*)h->hyp, (void*)h->cnt, (void*)h->mask, (void*)h->st, (void*)h->inl})
-    if (q) cudaFree(q);
-  for (cudaEvent_t ev : h->ev)
-    if (ev) cudaEventDestroy(ev);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  h->close();
   delete h;
 }
 
@@ -487,17 +475,11 @@ extern "C" int b2s_sim3solver_iterate(b2s_sim3solver* h, int batch, const b2s_si
         set_error("b2s_sim3solver_iterate: problem %d: sigma2 of correspondence %d is negative or not finite", i, c);
         return B2S_ERR_BAD_ARG;
       }
-    if (run)
-      for (int j = 0; j < q.k; j++)
-        for (int l = 0; l < 3; l++) {
-          const int s = q.sets[3 * j + l];
-          bool dup = false;
-          for (int m = 0; m < l; m++) dup |= q.sets[3 * j + m] == s;
-          if (s < 0 || s >= q.n || dup) {
-            set_error("b2s_sim3solver_iterate: problem %d: set %d entry %d = %d (n = %d)", i, j, l, s, q.n);
-            return B2S_ERR_BAD_ARG;
-          }
-        }
+    int j, l;
+    if (run && !sets_ok(q.sets, q.k, 3, q.n, &j, &l)) {
+      set_error("b2s_sim3solver_iterate: problem %d: set %d entry %d = %d (n = %d)", i, j, l, q.sets[3 * j + l], q.n);
+      return B2S_ERR_BAD_ARG;
+    }
   }
   B2S_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
@@ -545,7 +527,8 @@ extern "C" int b2s_sim3solver_iterate(b2s_sim3solver* h, int batch, const b2s_si
   h->hSt.resize((size_t)batch);
   h->hInl.resize(on);
 
-  B2S_CUDA(cudaEventRecord(h->ev[0], s));
+  int rc = h->begin();
+  if (rc != B2S_OK) return rc;
   B2S_CUDA(cudaMemcpyAsync(h->prob, h->hProb.data(), (size_t)batch * sizeof(Prob), cudaMemcpyHostToDevice, s));
   if (on) {
     B2S_CUDA(cudaMemcpyAsync(h->X1, h->hX1.data(), on * 3 * sizeof(float), cudaMemcpyHostToDevice, s));
@@ -563,9 +546,7 @@ extern "C" int b2s_sim3solver_iterate(b2s_sim3solver* h, int batch, const b2s_si
   B2S_CUDA(cudaGetLastError());
   B2S_CUDA(cudaMemcpyAsync(h->hSt.data(), h->st, (size_t)batch * sizeof(St), cudaMemcpyDeviceToHost, s));
   if (on) B2S_CUDA(cudaMemcpyAsync(h->hInl.data(), h->inl, on, cudaMemcpyDeviceToHost, s));
-  B2S_CUDA(cudaEventRecord(h->ev[1], s));
-  B2S_CUDA(cudaStreamSynchronize(s));
-  B2S_CUDA(cudaGetLastError());
+  if ((rc = h->finish()) != B2S_OK) return rc;
 
   for (int i = 0; i < batch; i++) {
     const St& S = h->hSt[(size_t)i];
@@ -587,8 +568,5 @@ extern "C" int b2s_sim3solver_iterate(b2s_sim3solver* h, int batch, const b2s_si
     R.iterations_done = S.doneAfter;
     R.best_inliers = S.bestAfter;
   }
-  float ms = 0.f;
-  B2S_CUDA(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
-  h->lastMs = ms;
   return B2S_OK;
 }
