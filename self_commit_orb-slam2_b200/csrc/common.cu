@@ -47,6 +47,11 @@ int grow(DevBuf& b, size_t bytes) {
   return B2S_OK;
 }
 
+void swap(DevBuf& a, DevBuf& b) {
+  std::swap(a.p, b.p);
+  std::swap(a.bytes, b.bytes);
+}
+
 int grow(HostBuf& b, size_t bytes) {
   if (bytes == 0) bytes = 16;
   if (b.bytes >= bytes) return B2S_OK;

@@ -40,6 +40,8 @@ struct DevBuf {
   }
 };
 int grow(DevBuf& b, size_t bytes);
+// Exchanges two buffers: a buffer whose contents must survive a reallocation is filled in a new one, then swapped in.
+void swap(DevBuf& a, DevBuf& b);
 // Its pinned host counterpart (cudaMallocHost), with the same grow().
 struct HostBuf {
   void* p = nullptr;

@@ -1135,26 +1135,26 @@ static int run_pipeline(b2s_extractor* h, const DeviceBuffers& d, int batch, b2s
   const bool tm = allowTiming && h->timing != 0;
   if (tm) {
     if (h->evPending) b2s_extractor_timing_collect(h);
-    cudaEventRecord(h->ev[0], st);
+    cudaEventRecord(h->stageEv[0], st);
   }
   // fused front end: per level one tile kernel (TMA-staged tile -> FAST strength map, blur, level l+1), then the per-cell
   // NMS / threshold rules.  `d` may be a slice of the handle's buffers: pass its image offset.
   const int bBase = (int)((size_t)(d.pyr - h->d.pyr) / g.pyrBytes);
   const int rc = tile_run(h, bBase, batch, st);
   if (rc != B2S_OK) return rc;
-  if (tm) cudaEventRecord(h->ev[1], st);
+  if (tm) cudaEventRecord(h->stageEv[1], st);
   int capMax = 0;
   for (int l = 0; l < g.nlevels; l++) capMax = std::max(capMax, g.lv[l].nodeCap);
   const size_t qsm = quadtree_smem_bytes(capMax);
   k_quadtree<<<dim3(g.nlevels, batch), 256, qsm, st>>>(g, capMax, d.candXY, d.candKey, d.candResp, d.candNode, d.candQ,
                                                        d.candCount, d.selXYR, d.selCount, d.status);
   h->launches++;
-  if (tm) cudaEventRecord(h->ev[2], st);
+  if (tm) cudaEventRecord(h->stageEv[2], st);
   k_orient_describe<<<dim3(div_up(g.totalSelCap, 8), batch), 256, 0, st>>>(g, d.pyr, d.blur, d.selXYR, d.selCount, dKps,
                                                                            dDesc, dCounts, cap, d.status);
   h->launches++;
   if (tm) {
-    cudaEventRecord(h->ev[3], st);
+    cudaEventRecord(h->stageEv[3], st);
     h->evPending = 1;
   }
   B2S_CUDA(cudaGetLastError());
@@ -1163,11 +1163,12 @@ static int run_pipeline(b2s_extractor* h, const DeviceBuffers& d, int batch, b2s
 
 static void b2s_extractor_timing_collect(b2s_extractor* h) {
   if (!h->evPending) return;
-  static const int kSlot[3] = {1, 2, 4};  // stage slot of the span ev[k] -> ev[k + 1]: tiles + cells, quadtree, describe
-  if (cudaEventSynchronize(h->ev[3]) != cudaSuccess) return;
+  // stage slot of the span stageEv[k] -> stageEv[k + 1]: tiles + cells, quadtree, describe
+  static const int kSlot[3] = {1, 2, 4};
+  if (cudaEventSynchronize(h->stageEv[3]) != cudaSuccess) return;
   for (int k = 0; k < 3; k++) {
     float ms = 0;
-    if (cudaEventElapsedTime(&ms, h->ev[k], h->ev[k + 1]) == cudaSuccess) h->stageMs[kSlot[k]] += ms;
+    if (cudaEventElapsedTime(&ms, h->stageEv[k], h->stageEv[k + 1]) == cudaSuccess) h->stageMs[kSlot[k]] += ms;
   }
   h->timedCalls++;
   h->evPending = 0;
@@ -1403,8 +1404,8 @@ using namespace b2s;
 extern "C" int b2s_extractor_set_timing(b2s_extractor* h, int enable) {
   if (!h) return B2S_ERR_BAD_ARG;
   B2S_CUDA(cudaSetDevice(h->device));
-  if (enable && !h->ev[0])
-    for (int k = 0; k < 4; k++) B2S_CUDA(cudaEventCreate(&h->ev[k]));
+  if (enable && !h->stageEv[0])
+    for (int k = 0; k < 4; k++) B2S_CUDA(cudaEventCreate(&h->stageEv[k]));
   b2s_extractor_timing_collect(h);
   h->timing = enable;
   for (int k = 0; k < 5; k++) h->stageMs[k] = 0;
@@ -1553,53 +1554,50 @@ extern "C" int b2s_extractor_create(int nfeatures, float scaleFactor, int nlevel
   h->maxW = max_width;
   h->maxH = max_height;
   h->maxBatch = max_batch;
-  h->device = device;
   init_tables(h);
-  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&h->stream2, cudaStreamNonBlocking) != cudaSuccess) {
+  h->open(device);
+  if (h->error == cudaSuccess) h->error = cudaStreamCreateWithFlags(&h->stream2, cudaStreamNonBlocking);
+  if (h->error != cudaSuccess) {
     set_error("cudaStreamCreate failed");
-    delete h;
+    b2s_extractor_destroy(h);
     return B2S_ERR_CUDA;
   }
   size_buffers(h);
   const size_t candCap = h->candCapAlloc, selCap = h->selCapAlloc, pyrBytes = h->pyrBytesAlloc;
   DeviceBuffers& d = h->d;
   const size_t B = (size_t)max_batch;
-  cudaError_t e = cudaSuccess;
-  auto A = [&](void** p, size_t bytes) {
-    if (e == cudaSuccess) e = cudaMalloc(p, bytes);
-  };
-  A((void**)&d.pyr, B * pyrBytes);
-  A((void**)&d.blur, B * pyrBytes);
-  A((void**)&d.score, B * pyrBytes);
-  A((void**)&d.bitmap, B * h->bmWordsAlloc * 4);
-  A((void**)&d.tileDx, h->tileTabAlloc * 2);
-  A((void**)&d.tileDy, h->tileTabAlloc * 2);
-  if (max_batch > 1) A((void**)&d.raw, B * (size_t)max_width * max_height + 64);  // dense upload staging (batch path)
-  A((void**)&d.candXY, B * candCap * 4);
-  A((void**)&d.candKey, B * candCap * 4);
-  A((void**)&d.candResp, B * candCap);
-  A((void**)&d.candNode, B * candCap * 2);
-  A((void**)&d.candQ, B * candCap);
-  A((void**)&d.candCount, B * kMaxLevels * 4);
-  A((void**)&d.selXYR, B * selCap * 8);
-  A((void**)&d.selCount, B * kMaxLevels * 4);
-  A((void**)&d.status, 4);
-  A((void**)&d.cellInfo, h->cellAlloc * 4);
-  A((void**)&d.fbList, B * h->cellAlloc * sizeof(uint2));
-  A((void**)&d.fbCount, B * 4);  // one counter per possible first image of a chunk (chunks of a batch run on two streams)
-  A((void**)&d.rxOfs, h->rxAlloc * 2);
-  A((void**)&d.rxAlpha, h->rxAlloc * 4);
-  A((void**)&d.ryOfs, h->ryAlloc * 2);
-  A((void**)&d.ryBeta, h->ryAlloc * 4);
-  A((void**)&d.outKps, B * h->outCap * sizeof(b2s_keypoint));
-  A((void**)&d.outDesc, B * h->outCap * 32);
-  A((void**)&d.outCounts, B * 4);
+  h->alloc(d.pyr, B * pyrBytes);
+  h->alloc(d.blur, B * pyrBytes);
+  h->alloc(d.score, B * pyrBytes);
+  h->alloc(d.bitmap, B * h->bmWordsAlloc * 4);
+  h->alloc(d.tileDx, h->tileTabAlloc * 2);
+  h->alloc(d.tileDy, h->tileTabAlloc * 2);
+  if (max_batch > 1) h->alloc(d.raw, B * (size_t)max_width * max_height + 64);  // dense upload staging (batch path)
+  h->alloc(d.candXY, B * candCap * 4);
+  h->alloc(d.candKey, B * candCap * 4);
+  h->alloc(d.candResp, B * candCap);
+  h->alloc(d.candNode, B * candCap * 2);
+  h->alloc(d.candQ, B * candCap);
+  h->alloc(d.candCount, B * kMaxLevels * 4);
+  h->alloc(d.selXYR, B * selCap * 8);
+  h->alloc(d.selCount, B * kMaxLevels * 4);
+  h->alloc(d.status, 4);
+  h->alloc(d.cellInfo, h->cellAlloc * 4);
+  h->alloc(d.fbList, B * h->cellAlloc * sizeof(uint2));
+  h->alloc(d.fbCount, B * 4);  // one counter per possible first image of a chunk (chunks of a batch run on two streams)
+  h->alloc(d.rxOfs, h->rxAlloc * 2);
+  h->alloc(d.rxAlpha, h->rxAlloc * 4);
+  h->alloc(d.ryOfs, h->ryAlloc * 2);
+  h->alloc(d.ryBeta, h->ryAlloc * 4);
+  h->alloc(d.outKps, B * h->outCap * sizeof(b2s_keypoint));
+  h->alloc(d.outDesc, B * h->outCap * 32);
+  h->alloc(d.outCounts, B * 4);
+  h->alloc_pinned(h->hKps, B * h->outCap * sizeof(b2s_keypoint));
+  h->alloc_pinned(h->hDesc, B * h->outCap * 32);
+  h->alloc_pinned(h->hCounts, B * 4);
+  h->alloc_pinned(h->hStatus, 4);
+  cudaError_t e = h->error;
   if (e == cudaSuccess) e = cudaMemset(d.status, 0, 4);
-  if (e == cudaSuccess) e = cudaMallocHost((void**)&h->hKps, B * h->outCap * sizeof(b2s_keypoint));
-  if (e == cudaSuccess) e = cudaMallocHost((void**)&h->hDesc, B * h->outCap * 32);
-  if (e == cudaSuccess) e = cudaMallocHost((void**)&h->hCounts, B * 4);
-  if (e == cudaSuccess) e = cudaMallocHost((void**)&h->hStatus, 4);
   if (e == cudaSuccess) {
     int capMax = 0;
     for (int l = 0; l < nlevels; l++) capMax = std::max(capMax, (int)align_up((size_t)std::max(h->nFeat[l] + 4, 64), 8));
@@ -1622,23 +1620,10 @@ extern "C" int b2s_extractor_create(int nfeatures, float scaleFactor, int nlevel
 
 extern "C" void b2s_extractor_destroy(b2s_extractor* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
-  DeviceBuffers& d = h->d;
-  void* ptrs[] = {d.pyr, d.blur, d.candXY, d.candKey, d.candResp, d.candNode, d.candQ, d.candCount, d.selXYR,
-                  d.selCount, d.status, d.rxOfs, d.rxAlpha, d.ryOfs, d.ryBeta, d.outKps, d.outDesc, d.outCounts, d.cellInfo,
-                  d.raw, d.score, d.tileDx, d.tileDy, d.bitmap, d.fbList, d.fbCount};
-  for (void* p : ptrs)
-    if (p) cudaFree(p);
-  if (h->hKps) cudaFreeHost(h->hKps);
-  if (h->hDesc) cudaFreeHost(h->hDesc);
-  if (h->hCounts) cudaFreeHost(h->hCounts);
-  if (h->hStatus) cudaFreeHost(h->hStatus);
-  if (h->dStereoSad) cudaFree(h->dStereoSad);
-  if (h->dStereoU) cudaFree(h->dStereoU);
-  if (h->dStereoD) cudaFree(h->dStereoD);
-  if (h->dStereoN) cudaFree(h->dStereoN);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  h->close();
   if (h->stream2) cudaStreamDestroy(h->stream2);
+  for (cudaEvent_t e : h->stageEv)
+    if (e) cudaEventDestroy(e);
   delete h;
 }
 
@@ -1848,17 +1833,15 @@ extern "C" int b2s_extractor_debug_candidates(b2s_extractor* h, int b, int level
 extern "C" int b2s_debug_sincosf(const float* in, int n, float* s, float* c) {
   int rc = select_device(0);
   if (rc != B2S_OK) return rc;
-  float *din, *ds, *dc;
-  B2S_CUDA(cudaMalloc(&din, (size_t)n * 4));
-  B2S_CUDA(cudaMalloc(&ds, (size_t)n * 4));
-  B2S_CUDA(cudaMalloc(&dc, (size_t)n * 4));
-  B2S_CUDA(cudaMemcpy(din, in, (size_t)n * 4, cudaMemcpyHostToDevice));
-  k_sincos_test<<<div_up(n, 256), 256>>>(din, n, ds, dc);
-  B2S_CUDA(cudaMemcpy(s, ds, (size_t)n * 4, cudaMemcpyDeviceToHost));
-  B2S_CUDA(cudaMemcpy(c, dc, (size_t)n * 4, cudaMemcpyDeviceToHost));
-  cudaFree(din);
-  cudaFree(ds);
-  cudaFree(dc);
+  DevBuf din, ds, dc;
+  rc = grow(din, (size_t)n * 4);
+  if (rc == B2S_OK) rc = grow(ds, (size_t)n * 4);
+  if (rc == B2S_OK) rc = grow(dc, (size_t)n * 4);
+  if (rc != B2S_OK) return rc;
+  B2S_CUDA(cudaMemcpy(din.p, in, (size_t)n * 4, cudaMemcpyHostToDevice));
+  k_sincos_test<<<div_up(n, 256), 256>>>((const float*)din.p, n, (float*)ds.p, (float*)dc.p);
+  B2S_CUDA(cudaMemcpy(s, ds.p, (size_t)n * 4, cudaMemcpyDeviceToHost));
+  B2S_CUDA(cudaMemcpy(c, dc.p, (size_t)n * 4, cudaMemcpyDeviceToHost));
   return B2S_OK;
 }
 
@@ -1871,16 +1854,12 @@ static int stereo_launch(b2s_extractor* h, int first_left, int first_right, int 
   StereoParams sp;
   for (int l = 0; l < kMaxLevels; l++) sp.invScale[l] = l < h->nlevels ? h->invScale[l] : 0.f;
   sp.bf = bf; sp.mb = mb; sp.firstLeft = first_left; sp.firstRight = first_right; sp.cap = cap;
-  if ((size_t)n_pairs * cap > h->stereoCap) {
-    if (h->dStereoSad) cudaFree(h->dStereoSad);
-    h->dStereoSad = nullptr;
-    h->stereoCap = 0;
-    B2S_CUDA(cudaMalloc((void**)&h->dStereoSad, (size_t)n_pairs * cap * 4));
-    h->stereoCap = (size_t)n_pairs * cap;
-  }
+  const int rc = grow(h->dStereoSad, (size_t)n_pairs * cap * 4);
+  if (rc != B2S_OK) return rc;
+  int32_t* sad = (int32_t*)h->dStereoSad.p;
   k_stereo_match<<<dim3(div_up(cap, ST_WARPS), n_pairs), ST_WARPS * 32, 0, st>>>(g, sp, h->d.pyr, d_kps, d_desc, d_counts,
-                                                                               d_uright, d_depth, h->dStereoSad);
-  k_stereo_cull<<<n_pairs, 1024, 0, st>>>(sp, d_counts, d_uright, d_depth, h->dStereoSad, d_nmatched);
+                                                                               d_uright, d_depth, sad);
+  k_stereo_cull<<<n_pairs, 1024, 0, st>>>(sp, d_counts, d_uright, d_depth, sad, d_nmatched);
   h->launches += 2;
   B2S_CUDA(cudaGetLastError());
   return B2S_OK;
@@ -1912,27 +1891,19 @@ extern "C" int b2s_stereo_match(b2s_extractor* h, int first_left, int first_righ
   B2S_CUDA(cudaSetDevice(h->device));
   const int cap = h->lastCap;
   const size_t need = (size_t)n_pairs * cap;
-  if (need > h->stereoOutCap) {
-    if (h->dStereoU) cudaFree(h->dStereoU);
-    if (h->dStereoD) cudaFree(h->dStereoD);
-    if (h->dStereoN) cudaFree(h->dStereoN);
-    h->dStereoU = h->dStereoD = nullptr;
-    h->dStereoN = nullptr;
-    h->stereoOutCap = 0;
-    B2S_CUDA(cudaMalloc((void**)&h->dStereoU, need * 4));
-    B2S_CUDA(cudaMalloc((void**)&h->dStereoD, need * 4));
-    B2S_CUDA(cudaMalloc((void**)&h->dStereoN, (size_t)h->maxBatch * 4));
-    h->stereoOutCap = need;
-  }
-  cudaStream_t st = h->stream;
-  int rc = stereo_launch(h, first_left, first_right, n_pairs, h->d.outKps, h->d.outDesc, h->d.outCounts, cap, bf, mb,
-                         h->dStereoU, h->dStereoD, h->dStereoN, st);
+  int rc = grow(h->dStereoU, need * 4);
+  if (rc == B2S_OK) rc = grow(h->dStereoD, need * 4);
+  if (rc == B2S_OK) rc = grow(h->dStereoN, (size_t)h->maxBatch * 4);
   if (rc != B2S_OK) return rc;
-  B2S_CUDA(cudaMemcpy2DAsync(uright, (size_t)cap_out * 4, h->dStereoU, (size_t)cap * 4, (size_t)cap * 4, n_pairs,
+  cudaStream_t st = h->stream;
+  rc = stereo_launch(h, first_left, first_right, n_pairs, h->d.outKps, h->d.outDesc, h->d.outCounts, cap, bf, mb,
+                     (float*)h->dStereoU.p, (float*)h->dStereoD.p, (int32_t*)h->dStereoN.p, st);
+  if (rc != B2S_OK) return rc;
+  B2S_CUDA(cudaMemcpy2DAsync(uright, (size_t)cap_out * 4, h->dStereoU.p, (size_t)cap * 4, (size_t)cap * 4, n_pairs,
                              cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaMemcpy2DAsync(depth, (size_t)cap_out * 4, h->dStereoD, (size_t)cap * 4, (size_t)cap * 4, n_pairs,
+  B2S_CUDA(cudaMemcpy2DAsync(depth, (size_t)cap_out * 4, h->dStereoD.p, (size_t)cap * 4, (size_t)cap * 4, n_pairs,
                              cudaMemcpyDeviceToHost, st));
-  if (n_matched) B2S_CUDA(cudaMemcpyAsync(n_matched, h->dStereoN, (size_t)n_pairs * 4, cudaMemcpyDeviceToHost, st));
+  if (n_matched) B2S_CUDA(cudaMemcpyAsync(n_matched, h->dStereoN.p, (size_t)n_pairs * 4, cudaMemcpyDeviceToHost, st));
   B2S_CUDA(cudaStreamSynchronize(st));
   return B2S_OK;
 }

@@ -86,10 +86,10 @@ constexpr int kCellsMaxCols = 64;    // k_cells: cell columns one CTA owns at mo
 constexpr int kFastCellCap = 1024;   // k_fast_cells_list: maxima of one cell it keeps in shared memory (extractor.cu)
 }  // namespace b2s
 
-struct b2s_extractor {
+struct b2s_extractor : b2s::Stage {
   int nfeatures, nlevels, iniTh, minTh;
   double scaleFactor;
-  int maxW, maxH, maxBatch, device;
+  int maxW, maxH, maxBatch;
   int numSMs = 0;  // multiprocessors of `device` (grid of the persistent kernels)
   std::vector<float> scale, invScale, sigma2, invSigma2;
   std::vector<int> nFeat;
@@ -99,12 +99,9 @@ struct b2s_extractor {
   b2s::ExtractGeom geom;
   b2s::DeviceBuffers d;
   size_t pyrBytesAlloc = 0, candCapAlloc = 0, selCapAlloc = 0, rxAlloc = 0, ryAlloc = 0, cellAlloc = 0;
-  cudaStream_t stream = nullptr, stream2 = nullptr;
+  cudaStream_t stream2 = nullptr;
   // stereo matching scratch + bookkeeping of the last host-buffer batch extraction (b2s_stereo_match)
-  int32_t* dStereoSad = nullptr;
-  size_t stereoCap = 0, stereoOutCap = 0;
-  float *dStereoU = nullptr, *dStereoD = nullptr;
-  int32_t* dStereoN = nullptr;
+  b2s::DevBuf dStereoSad, dStereoU, dStereoD, dStereoN;
   int lastCap = 0, lastBatch = 0;
   // pinned staging for the host-buffer entry points
   b2s_keypoint* hKps = nullptr;
@@ -120,7 +117,7 @@ struct b2s_extractor {
   // optional per-stage CUDA-event timing (bench.py roofline): resize chain, FAST, quadtree, blur, describe; events
   // around the tile front end, the quadtree and the description (resize chain and blur are part of the tile front end)
   int timing = 0;
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+  cudaEvent_t stageEv[4] = {nullptr, nullptr, nullptr, nullptr};
   double stageMs[5] = {0, 0, 0, 0, 0};
   long long timedCalls = 0;
   int evPending = 0;

@@ -328,80 +328,63 @@ using namespace b2s;
 
 struct b2s_kfdb : b2s::Stage {
   int n_words = 0;
-  // BowVector pool: [0, pool_tail) holds the vectors of live and erased keyframes; pool_live entries are live
-  uint32_t* d_pw = nullptr;
-  double* d_pv = nullptr;
+  // BowVector pool (uint32_t words, double values): [0, pool_tail) holds the vectors of live and erased keyframes;
+  // pool_live entries are live
+  DevBuf d_pw, d_pv;
   int64_t pool_cap = 0, pool_tail = 0, pool_live = 0;
   std::vector<LiveRec> live;  // in add order (= the order of every inverted list)
   bool live_dirty = true;
   std::vector<int32_t> slot_of_id;  // -1: not in the database
-  // per-id query state and dedupe scratch, grown on demand
-  b2s_kfdb_state* d_state = nullptr;
-  int32_t* d_first_pos = nullptr;
+  // per-id query state (b2s_kfdb_state) and dedupe scratch (int32_t), grown on demand
+  DevBuf d_state, d_first_pos;
   int state_cap = 0;
-  // per-live-keyframe scratch
+  // per-live-keyframe scratch: LiveRec, SlotRec, int32_t order / best, float acc; int32_t count + ids out
   int live_cap = 0;
-  LiveRec* d_live = nullptr;
-  SlotRec* d_rec = nullptr;
-  int32_t *d_order = nullptr, *d_best = nullptr, *d_out = nullptr;
-  float* d_acc = nullptr;
+  DevBuf d_live, d_rec, d_order, d_best, d_acc, d_out;
+  HostBuf h_out;
   // one upload per query: query words + values, connected ids, covisibility table
-  size_t stage_cap = 0;
-  unsigned char *h_stage = nullptr, *d_stage = nullptr;
-  int32_t* h_out = nullptr;
-  int h_out_cap = 0;
+  HostBuf h_stage;
+  DevBuf d_stage;
 };
 
 namespace {
 
-void free_live_scratch(b2s_kfdb* db) {
-  void* p[] = {db->d_live, db->d_rec, db->d_order, db->d_best, db->d_out, db->d_acc};
-  for (void* x : p)
-    if (x) cudaFree(x);
-  db->d_live = nullptr; db->d_rec = nullptr; db->d_order = db->d_best = db->d_out = nullptr; db->d_acc = nullptr;
-  if (db->h_out) cudaFreeHost(db->h_out);
-  db->h_out = nullptr;
-  db->live_cap = db->h_out_cap = 0;
-}
-
 int ensure_live_cap(b2s_kfdb* db, int n) {
   if (n <= db->live_cap) return B2S_OK;
   const int cap = std::max(n, std::max(2 * db->live_cap, 256));
-  free_live_scratch(db);
-  B2S_CUDA(cudaMalloc(&db->d_live, (size_t)cap * sizeof(LiveRec)));
-  B2S_CUDA(cudaMalloc(&db->d_rec, (size_t)cap * sizeof(SlotRec)));
-  B2S_CUDA(cudaMalloc(&db->d_order, (size_t)cap * 4));
-  B2S_CUDA(cudaMalloc(&db->d_best, (size_t)cap * 4));
-  B2S_CUDA(cudaMalloc(&db->d_acc, (size_t)cap * 4));
-  B2S_CUDA(cudaMalloc(&db->d_out, (size_t)(cap + 1) * 4));
-  B2S_CUDA(cudaMallocHost(&db->h_out, (size_t)(cap + 1) * 4));
-  db->live_cap = db->h_out_cap = cap;
+  db->live_cap = 0;  // until every buffer has grown
   db->live_dirty = true;
+  int rc = grow(db->d_live, (size_t)cap * sizeof(LiveRec));
+  if (rc == B2S_OK) rc = grow(db->d_rec, (size_t)cap * sizeof(SlotRec));
+  if (rc == B2S_OK) rc = grow(db->d_order, (size_t)cap * 4);
+  if (rc == B2S_OK) rc = grow(db->d_best, (size_t)cap * 4);
+  if (rc == B2S_OK) rc = grow(db->d_acc, (size_t)cap * 4);
+  if (rc == B2S_OK) rc = grow(db->d_out, (size_t)(cap + 1) * 4);
+  if (rc == B2S_OK) rc = grow(db->h_out, (size_t)(cap + 1) * 4);
+  if (rc != B2S_OK) return rc;
+  db->live_cap = cap;
   return B2S_OK;
 }
 
 int ensure_state_cap(b2s_kfdb* db, int n) {
   if (n <= db->state_cap) return B2S_OK;
   const int cap = (int)std::min<int64_t>(INT32_MAX, std::max<int64_t>(n, std::max<int64_t>(2 * (int64_t)db->state_cap, 1024)));
-  b2s_kfdb_state* s = nullptr;
-  int32_t* f = nullptr;
-  B2S_CUDA(cudaMalloc(&s, (size_t)cap * sizeof(b2s_kfdb_state)));
-  cudaError_t e = cudaMalloc(&f, (size_t)cap * 4);
-  if (e == cudaSuccess) e = cudaMemsetAsync(s, 0, (size_t)cap * sizeof(b2s_kfdb_state), db->stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(f, 0x7f, (size_t)cap * 4, db->stream);
+  // new arrays, then swapped in: the old ones are freed on return, or kept if anything fails
+  DevBuf s, f;
+  cudaError_t e = cudaSuccess;
+  if (grow(s, (size_t)cap * sizeof(b2s_kfdb_state)) != B2S_OK || grow(f, (size_t)cap * 4) != B2S_OK)
+    e = cudaErrorMemoryAllocation;
+  if (e == cudaSuccess) e = cudaMemsetAsync(s.p, 0, (size_t)cap * sizeof(b2s_kfdb_state), db->stream);
+  if (e == cudaSuccess) e = cudaMemsetAsync(f.p, 0x7f, (size_t)cap * 4, db->stream);
   if (e == cudaSuccess && db->state_cap)
-    e = cudaMemcpyAsync(s, db->d_state, (size_t)db->state_cap * sizeof(b2s_kfdb_state), cudaMemcpyDeviceToDevice, db->stream);
+    e = cudaMemcpyAsync(s.p, db->d_state.p, (size_t)db->state_cap * sizeof(b2s_kfdb_state), cudaMemcpyDeviceToDevice, db->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(db->stream);
   if (e != cudaSuccess) {
-    cudaFree(s);
-    if (f) cudaFree(f);
     set_error("b2s_kfdb: state arrays for %d ids: %s", cap, cudaGetErrorString(e));
     return B2S_ERR_CUDA;
   }
-  if (db->d_state) cudaFree(db->d_state);
-  if (db->d_first_pos) cudaFree(db->d_first_pos);
-  db->d_state = s;
-  db->d_first_pos = f;
+  swap(db->d_state, s);
+  swap(db->d_first_pos, f);
   db->state_cap = cap;
   return B2S_OK;
 }
@@ -409,10 +392,10 @@ int ensure_state_cap(b2s_kfdb* db, int n) {
 // Moves the live vectors to the front of a new pool with room for `extra` more entries.
 int compact_pool(b2s_kfdb* db, int64_t extra) {
   const int64_t cap = std::max(kPoolMin, 2 * (db->pool_live + extra));
-  uint32_t* nw = nullptr;
-  double* nv = nullptr;
-  B2S_CUDA(cudaMalloc(&nw, (size_t)cap * 4));
-  cudaError_t e = cudaMalloc(&nv, (size_t)cap * 8);
+  // a new pool, then swapped in as in ensure_state_cap
+  DevBuf nw, nv, from;
+  cudaError_t e = cudaSuccess;
+  if (grow(nw, (size_t)cap * 4) != B2S_OK || grow(nv, (size_t)cap * 8) != B2S_OK) e = cudaErrorMemoryAllocation;
   std::vector<LiveRec> moved(db->live);
   int64_t off = 0;
   for (LiveRec& r : moved) {
@@ -420,26 +403,22 @@ int compact_pool(b2s_kfdb* db, int64_t extra) {
     off += r.n;
   }
   const int n = (int)moved.size();
-  LiveRec* d_from = nullptr;
-  if (e == cudaSuccess && n) e = cudaMalloc(&d_from, (size_t)2 * n * sizeof(LiveRec));
+  if (e == cudaSuccess && n && grow(from, (size_t)2 * n * sizeof(LiveRec)) != B2S_OK) e = cudaErrorMemoryAllocation;
+  LiveRec* d_from = (LiveRec*)from.p;
   if (e == cudaSuccess && n) e = cudaMemcpyAsync(d_from, db->live.data(), (size_t)n * sizeof(LiveRec), cudaMemcpyHostToDevice, db->stream);
   if (e == cudaSuccess && n) e = cudaMemcpyAsync(d_from + n, moved.data(), (size_t)n * sizeof(LiveRec), cudaMemcpyHostToDevice, db->stream);
   if (e == cudaSuccess && n) {
-    k_kfdb_move<<<n, 128, 0, db->stream>>>(db->d_pw, db->d_pv, d_from, d_from + n, nw, nv);
+    k_kfdb_move<<<n, 128, 0, db->stream>>>((const uint32_t*)db->d_pw.p, (const double*)db->d_pv.p, d_from, d_from + n,
+                                           (uint32_t*)nw.p, (double*)nv.p);
     e = cudaGetLastError();
   }
   if (e == cudaSuccess) e = cudaStreamSynchronize(db->stream);
-  if (d_from) cudaFree(d_from);
   if (e != cudaSuccess) {
-    cudaFree(nw);
-    if (nv) cudaFree(nv);
     set_error("b2s_kfdb: pool compaction: %s", cudaGetErrorString(e));
     return B2S_ERR_CUDA;
   }
-  if (db->d_pw) cudaFree(db->d_pw);
-  if (db->d_pv) cudaFree(db->d_pv);
-  db->d_pw = nw;
-  db->d_pv = nv;
+  swap(db->d_pw, nw);
+  swap(db->d_pv, nv);
   db->pool_cap = cap;
   db->pool_tail = off;
   db->live.swap(moved);
@@ -480,24 +459,18 @@ int query(b2s_kfdb* db, int loop, uint64_t qid, const uint32_t* words, const dou
   B2S_CUDA(cudaSetDevice(db->device));
   if ((rc = ensure_live_cap(db, n_live)) != B2S_OK) return rc;
   if (db->live_dirty) {
-    B2S_CUDA(cudaMemcpyAsync(db->d_live, db->live.data(), (size_t)n_live * sizeof(LiveRec), cudaMemcpyHostToDevice, db->stream));
+    B2S_CUDA(cudaMemcpyAsync(db->d_live.p, db->live.data(), (size_t)n_live * sizeof(LiveRec), cudaMemcpyHostToDevice,
+                             db->stream));
     db->live_dirty = false;
   }
   const int n_rows = covis ? covis->n_rows : 0;
   const size_t o_qv = 0, o_qw = align16(o_qv + (size_t)n * 8), o_conn = align16(o_qw + (size_t)n * 4),
                o_cid = align16(o_conn + (size_t)n_conn * 8), o_cn = align16(o_cid + (size_t)n_rows * 10 * 8),
                total = align16(o_cn + (size_t)n_rows * 4);
-  if (total > db->stage_cap) {
-    const size_t c = std::max(total, 2 * db->stage_cap);
-    if (db->h_stage) cudaFreeHost(db->h_stage);
-    if (db->d_stage) cudaFree(db->d_stage);
-    db->h_stage = db->d_stage = nullptr;
-    db->stage_cap = 0;
-    B2S_CUDA(cudaMallocHost(&db->h_stage, c));
-    B2S_CUDA(cudaMalloc(&db->d_stage, c));
-    db->stage_cap = c;
-  }
-  unsigned char* h = db->h_stage;
+  if (db->h_stage.bytes < total) rc = grow(db->h_stage, std::max(total, 2 * db->h_stage.bytes));
+  if (rc == B2S_OK && db->d_stage.bytes < total) rc = grow(db->d_stage, std::max(total, 2 * db->d_stage.bytes));
+  if (rc != B2S_OK) return rc;
+  unsigned char* h = (unsigned char*)db->h_stage.p;
   memcpy(h + o_qv, values, (size_t)n * 8);
   memcpy(h + o_qw, words, (size_t)n * 4);
   if (n_conn) {
@@ -509,31 +482,35 @@ int query(b2s_kfdb* db, int loop, uint64_t qid, const uint32_t* words, const dou
     memcpy(h + o_cid, covis->ids, (size_t)n_rows * 10 * 8);
     memcpy(h + o_cn, covis->n, (size_t)n_rows * 4);
   }
-  unsigned char* d = db->d_stage;
+  unsigned char* d = (unsigned char*)db->d_stage.p;
   B2S_CUDA(cudaMemcpyAsync(d, h, total, cudaMemcpyHostToDevice, db->stream));
+  const LiveRec* live = (const LiveRec*)db->d_live.p;
+  SlotRec* rec = (SlotRec*)db->d_rec.p;
+  b2s_kfdb_state* state = (b2s_kfdb_state*)db->d_state.p;
   if ((rc = db->begin()) != B2S_OK) return rc;
   k_kfdb_match<<<div_up(n_live, kMatchWarps), kMatchWarps * 32, (size_t)n * 12, db->stream>>>(
-      db->d_pw, db->d_pv, db->d_live, n_live, reinterpret_cast<const uint32_t*>(d + o_qw),
+      (const uint32_t*)db->d_pw.p, (const double*)db->d_pv.p, live, n_live, reinterpret_cast<const uint32_t*>(d + o_qw),
       reinterpret_cast<const double*>(d + o_qv), n, reinterpret_cast<const uint64_t*>(d + o_conn), n_conn, loop,
-      (unsigned long long)qid, db->d_state, db->d_rec);
+      (unsigned long long)qid, state, rec);
   B2S_CUDA(cudaGetLastError());
   k_kfdb_finish<<<1, kFinThreads, 0, db->stream>>>(
-      db->d_live, n_live, db->d_rec, n, loop, (unsigned long long)qid, min_score,
-      reinterpret_cast<const uint64_t*>(d + o_cid), reinterpret_cast<const int32_t*>(d + o_cn), n_rows, db->d_state,
-      db->state_cap, db->d_order, db->d_acc, db->d_best, db->d_first_pos, db->d_out);
+      live, n_live, rec, n, loop, (unsigned long long)qid, min_score, reinterpret_cast<const uint64_t*>(d + o_cid),
+      reinterpret_cast<const int32_t*>(d + o_cn), n_rows, state, db->state_cap, (int32_t*)db->d_order.p,
+      (float*)db->d_acc.p, (int32_t*)db->d_best.p, (int32_t*)db->d_first_pos.p, (int32_t*)db->d_out.p);
   B2S_CUDA(cudaGetLastError());
   B2S_CUDA(cudaEventRecord(db->ev[1], db->stream));  // the kernels only: the download is not timed
   const int n_dl = 1 + std::min(cap, n_live);
-  B2S_CUDA(cudaMemcpyAsync(db->h_out, db->d_out, (size_t)n_dl * 4, cudaMemcpyDeviceToHost, db->stream));
+  B2S_CUDA(cudaMemcpyAsync(db->h_out.p, db->d_out.p, (size_t)n_dl * 4, cudaMemcpyDeviceToHost, db->stream));
   B2S_CUDA(cudaStreamSynchronize(db->stream));
   B2S_CUDA(cudaEventElapsedTime(&db->lastMs, db->ev[0], db->ev[1]));
-  const int cnt = db->h_out[0];
+  const int32_t* hout = (const int32_t*)db->h_out.p;
+  const int cnt = hout[0];
   *n_out = cnt;
   if (cnt > cap) {
     set_error("%s: %d candidates, cap %d", fn, cnt, cap);
     return B2S_ERR_CAPACITY;
   }
-  for (int i = 0; i < cnt; i++) out_ids[i] = (uint64_t)db->h_out[1 + i];
+  for (int i = 0; i < cnt; i++) out_ids[i] = (uint64_t)hout[1 + i];
   return B2S_OK;
 }
 
@@ -542,12 +519,6 @@ int query(b2s_kfdb* db, int loop, uint64_t qid, const uint32_t* words, const dou
 extern "C" void b2s_kfdb_destroy(b2s_kfdb* db) {
   if (!db) return;
   db->close();
-  // the buffers that keep their contents when they grow are the database's own
-  free_live_scratch(db);
-  void* p[] = {db->d_pw, db->d_pv, db->d_state, db->d_first_pos, db->d_stage};
-  for (void* x : p)
-    if (x) cudaFree(x);
-  if (db->h_stage) cudaFreeHost(db->h_stage);
   delete db;
 }
 
@@ -563,8 +534,8 @@ extern "C" int b2s_kfdb_create(int n_words, int device, b2s_kfdb** out) {
   db->n_words = n_words;
   db->open(device);
   cudaError_t e = db->error;
-  if (e == cudaSuccess) e = cudaMalloc(&db->d_pw, (size_t)kPoolMin * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&db->d_pv, (size_t)kPoolMin * 8);
+  if (e == cudaSuccess && (grow(db->d_pw, (size_t)kPoolMin * 4) != B2S_OK || grow(db->d_pv, (size_t)kPoolMin * 8) != B2S_OK))
+    e = cudaErrorMemoryAllocation;
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(k_kfdb_match, cudaFuncAttributeMaxDynamicSharedMemorySize, B2S_KFDB_MAX_WORDS * 12);
   if (e != cudaSuccess) {
@@ -593,8 +564,8 @@ extern "C" int b2s_kfdb_add(b2s_kfdb* db, uint64_t kf_id, const uint32_t* words,
   if ((rc = ensure_state_cap(db, id + 1)) != B2S_OK) return rc;
   if (db->pool_tail + n > db->pool_cap && (rc = compact_pool(db, n)) != B2S_OK) return rc;
   if (n) {
-    B2S_CUDA(cudaMemcpyAsync(db->d_pw + db->pool_tail, words, (size_t)n * 4, cudaMemcpyHostToDevice, db->stream));
-    B2S_CUDA(cudaMemcpyAsync(db->d_pv + db->pool_tail, values, (size_t)n * 8, cudaMemcpyHostToDevice, db->stream));
+    B2S_CUDA(cudaMemcpyAsync((uint32_t*)db->d_pw.p + db->pool_tail, words, (size_t)n * 4, cudaMemcpyHostToDevice, db->stream));
+    B2S_CUDA(cudaMemcpyAsync((double*)db->d_pv.p + db->pool_tail, values, (size_t)n * 8, cudaMemcpyHostToDevice, db->stream));
   }
   if (id >= (int)db->slot_of_id.size()) db->slot_of_id.resize((size_t)id + 1, -1);
   db->slot_of_id[id] = (int32_t)db->live.size();
@@ -635,7 +606,7 @@ extern "C" int b2s_kfdb_clear(b2s_kfdb* db) {
   db->pool_tail = db->pool_live = 0;
   db->live_dirty = true;
   if (db->state_cap) {
-    B2S_CUDA(cudaMemsetAsync(db->d_state, 0, (size_t)db->state_cap * sizeof(b2s_kfdb_state), db->stream));
+    B2S_CUDA(cudaMemsetAsync(db->d_state.p, 0, (size_t)db->state_cap * sizeof(b2s_kfdb_state), db->stream));
     B2S_CUDA(cudaStreamSynchronize(db->stream));
   }
   return B2S_OK;
@@ -672,7 +643,8 @@ extern "C" int b2s_kfdb_keyframe_state(b2s_kfdb* db, uint64_t kf_id, b2s_kfdb_st
   memset(state, 0, sizeof(*state));
   if (kf_id >= (uint64_t)db->state_cap) return B2S_OK;
   B2S_CUDA(cudaSetDevice(db->device));
-  B2S_CUDA(cudaMemcpyAsync(state, db->d_state + kf_id, sizeof(*state), cudaMemcpyDeviceToHost, db->stream));
+  B2S_CUDA(cudaMemcpyAsync(state, (const b2s_kfdb_state*)db->d_state.p + kf_id, sizeof(*state), cudaMemcpyDeviceToHost,
+                           db->stream));
   B2S_CUDA(cudaStreamSynchronize(db->stream));
   return B2S_OK;
 }

@@ -1667,23 +1667,20 @@ struct BaHostStage {  // pinned mirror of the uploaded per-window arrays (same s
   BaState* st = nullptr;
 };
 
-struct b2s_pose_scratch;
-static void pose_scratch_free(b2s_pose_scratch* s);
-struct b2s_ba_solver {
-  int maxKf, maxMp, maxE, maxBatch, device;
-  b2s_pose_scratch* pose = nullptr;  // PoseOptimization buffers (allocated on first use)
-  cudaStream_t stream = nullptr, stream2 = nullptr;
+// Stage::ev / lastMs time the persistent LM kernel of the last LocalBA batch (b2s_ba_last_kernel_ms).
+struct b2s_ba_solver : b2s::Stage {
+  int maxKf, maxMp, maxE, maxBatch;
+  cudaStream_t stream2 = nullptr;  // forwards the abort flag while the LM kernel runs on `stream`
   long long launches = 0;
   BaPtrs d;
-  std::vector<void*> allocs, hostAllocs;
   BaHostStage hs;
   size_t smemBytes = 0;
   int numSMs = 0;
-  cudaEvent_t evLm[2] = {nullptr, nullptr};  // around the persistent LM kernel of the last batch (b2s_ba_last_kernel_ms)
-  float lastLmMs = 0.f;
   long long lastTrials = 0;
   int smBudget = 0;  // CTAs (= SMs) one LocalBA batch may occupy; 0 = all (b2s_ba_set_sm_budget)
   DevBuf pairRec;    // d.pairRec: batch x d.capPairs records, grown by ba_run when a window needs more
+  // PoseOptimization buffers, grown on first use
+  DevBuf poFrames, poPoseInit, poPoseOut, poErr, poChi2, poXw, poObs, poInvS, poLevel, poOutlier, poNInl, poNTr, poTrace;
 };
 
 extern "C" int b2s_ba_create(int max_kf, int max_mp, int max_edges, int max_batch, int device, b2s_ba_solver** out) {
@@ -1695,7 +1692,7 @@ extern "C" int b2s_ba_create(int max_kf, int max_mp, int max_edges, int max_batc
   int rc = select_device(device);
   if (rc != B2S_OK) return rc;
   b2s_ba_solver* h = new b2s_ba_solver();
-  h->maxKf = max_kf; h->maxMp = max_mp; h->maxE = max_edges; h->maxBatch = max_batch; h->device = device;
+  h->maxKf = max_kf; h->maxMp = max_mp; h->maxE = max_edges; h->maxBatch = max_batch;
   cudaDeviceGetAttribute(&h->numSMs, cudaDevAttrMultiProcessorCount, device);
   BaPtrs& d = h->d;
   memset(&d, 0, sizeof(d));
@@ -1706,24 +1703,12 @@ extern "C" int b2s_ba_create(int max_kf, int max_mp, int max_edges, int max_batc
   d.capBlk = max_kf * (max_kf + 1) / 2;
   d.capPairs = 8 * max_edges;
   const size_t B = max_batch;
-  cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
+  h->open(device);
+  cudaError_t& e = h->error;
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->stream2, cudaStreamNonBlocking);
-  auto A = [&](void* pp, size_t bytes) {
-    void** p = (void**)pp;
-    if (e == cudaSuccess) {
-      e = cudaMalloc(p, bytes);
-      if (e == cudaSuccess) {
-        h->allocs.push_back(*p);
-        e = cudaMemset(*p, 0, bytes);
-      }
-    }
-  };
-  auto HA = [&](void* pp, size_t bytes) {
-    void** p = (void**)pp;
-    if (e == cudaSuccess) {
-      e = cudaMallocHost(p, bytes);
-      if (e == cudaSuccess) h->hostAllocs.push_back(*p);
-    }
+  auto A = [h](auto* p, size_t bytes) {  // zero-filled
+    h->alloc(*p, bytes);
+    if (h->error == cudaSuccess) h->error = cudaMemset(*p, 0, bytes);
   };
   A(&d.win, B * sizeof(BaWin)); A(&d.st, B * sizeof(BaState));
   A(&d.pose, B * max_kf * POSE_STRIDE * 8); A(&d.poseBak, B * max_kf * POSE_STRIDE * 8);
@@ -1750,15 +1735,15 @@ extern "C" int b2s_ba_create(int max_kf, int max_mp, int max_edges, int max_batc
   const size_t mapLen = std::max(B, (size_t)h->numSMs);
   A(&d.ctaMap, mapLen * 4); A(&d.winCtas, B * 4);
   BaHostStage& s = h->hs;
-  HA(&s.ctaMap, mapLen * 4); HA(&s.winCtas, B * 4);
-  HA(&s.pose, B * max_kf * POSE_STRIDE * 8); HA(&s.pts, B * max_mp * 3 * 8);
-  HA(&s.pidx, B * max_kf * 4); HA(&s.freeKf, B * max_kf * 4);
-  HA(&s.eKf, B * max_edges * 4); HA(&s.eMp, B * max_edges * 4);
-  HA(&s.mpStart, B * (max_mp + 1) * 4); HA(&s.kfStart, B * (max_kf + 1) * 4);
-  HA(&s.mpEdges, B * max_edges * 4); HA(&s.kfEdges, B * max_edges * 4);
-  HA(&s.eObs, B * max_edges * 12); HA(&s.eW, B * max_edges * 4);
-  HA(&s.eSt, B * max_edges); HA(&s.eOutlier, B * max_edges);
-  HA(&s.win, B * sizeof(BaWin)); HA(&s.st, B * sizeof(BaState));
+  h->alloc_pinned(s.ctaMap, mapLen * 4); h->alloc_pinned(s.winCtas, B * 4);
+  h->alloc_pinned(s.pose, B * max_kf * POSE_STRIDE * 8); h->alloc_pinned(s.pts, B * max_mp * 3 * 8);
+  h->alloc_pinned(s.pidx, B * max_kf * 4); h->alloc_pinned(s.freeKf, B * max_kf * 4);
+  h->alloc_pinned(s.eKf, B * max_edges * 4); h->alloc_pinned(s.eMp, B * max_edges * 4);
+  h->alloc_pinned(s.mpStart, B * (max_mp + 1) * 4); h->alloc_pinned(s.kfStart, B * (max_kf + 1) * 4);
+  h->alloc_pinned(s.mpEdges, B * max_edges * 4); h->alloc_pinned(s.kfEdges, B * max_edges * 4);
+  h->alloc_pinned(s.eObs, B * max_edges * 12); h->alloc_pinned(s.eW, B * max_edges * 4);
+  h->alloc_pinned(s.eSt, B * max_edges); h->alloc_pinned(s.eOutlier, B * max_edges);
+  h->alloc_pinned(s.win, B * sizeof(BaWin)); h->alloc_pinned(s.st, B * sizeof(BaState));
   if (e == cudaSuccess && grow(h->pairRec, B * (size_t)d.capPairs * 16) != B2S_OK) e = cudaErrorMemoryAllocation;
   d.pairRec = (int4*)h->pairRec.p;
   h->smemBytes = (size_t)((CHOL_BS + 1) * CHOL_PP + (size_t)(d.ldS + 8) * CHOL_PP + 2 * d.ldS) * 8 + (size_t)(d.ldS + 8 + max_kf) * 4;
@@ -1777,13 +1762,7 @@ extern "C" int b2s_ba_create(int max_kf, int max_mp, int max_edges, int max_batc
 
 extern "C" void b2s_ba_destroy(b2s_ba_solver* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
-  pose_scratch_free(h->pose);
-  for (void* p : h->allocs) cudaFree(p);
-  for (void* p : h->hostAllocs) cudaFreeHost(p);
-  for (auto& e : h->evLm)
-    if (e) cudaEventDestroy(e);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  h->close();
   if (h->stream2) cudaStreamDestroy(h->stream2);
   delete h;
 }
@@ -1966,7 +1945,7 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
     maxE = std::max(maxE, P.n_edges); maxMp = std::max(maxMp, P.n_mp); maxFree = std::max(maxFree, nFree[w]);
     maxPairs = std::max(maxPairs, pairBound[w]);
   }
-  // the pair list of every window fits: grow it before anything is enqueued (cudaFree synchronises the device)
+  // the pair list of every window fits: grow it before anything is enqueued (a reallocation synchronises the device)
   if (maxPairs > INT_MAX) {
     set_error("b2s_local_ba: a window may have %lld covisibility pairs (at most %d)", maxPairs, INT_MAX);
     return B2S_ERR_CAPACITY;
@@ -2012,11 +1991,7 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
   B2S_CUDA(cudaMemsetAsync(d.blkNZ, 0, nb * 4, st));
   k_block_order<<<batch, 256, 0, st>>>(d);
   // ---- the whole LM loop of every window: persistent cooperative launches, all CTAs of a launch co-resident
-  if (!h->evLm[0]) {
-    B2S_CUDA(cudaEventCreate(&h->evLm[0]));
-    B2S_CUDA(cudaEventCreate(&h->evLm[1]));
-  }
-  B2S_CUDA(cudaEventRecord(h->evLm[0], st));
+  B2S_CUDA(cudaEventRecord(h->ev[0], st));
   // the attribute is per FUNCTION, not per handle: another solver handle (different capacities) may have set a smaller
   // limit since this one was created, which makes the cooperative launch fail with "too many blocks"
   if (h->smemBytes > 48 * 1024)
@@ -2033,7 +2008,7 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
     c0 += grid;
   }
   h->launches += 5;
-  B2S_CUDA(cudaEventRecord(h->evLm[1], st));
+  B2S_CUDA(cudaEventRecord(h->ev[1], st));
   // asynchronous abort (LocalMapping::InsertKeyFrame sets mbAbortBA): forward the flag while the kernel runs
   if (stop) {
     bool sent = false;
@@ -2055,7 +2030,7 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
   B2S_CUDA(cudaMemcpyAsync(s.st, d.st, nb * sizeof(BaState), cudaMemcpyDeviceToHost, st));
   B2S_CUDA(cudaStreamSynchronize(st));
   B2S_CUDA(cudaGetLastError());
-  cudaEventElapsedTime(&h->lastLmMs, h->evLm[0], h->evLm[1]);
+  cudaEventElapsedTime(&h->lastMs, h->ev[0], h->ev[1]);
   h->lastTrials = 0;
   for (int w = 0; w < batch; w++) h->lastTrials += s.st[w].lm.nTrials;
   for (int w = 0; w < batch; w++)
@@ -2103,7 +2078,7 @@ static int ba_run(b2s_ba_solver* h, int batch, const b2s_ba_problem* probs, cons
 extern "C" float b2s_ba_last_kernel_ms(const b2s_ba_solver* h, long long* lm_trials) {
   if (!h) return 0.f;
   if (lm_trials) *lm_trials = h->lastTrials;
-  return h->lastLmMs;
+  return h->lastMs;
 }
 
 extern "C" int b2s_local_ba(b2s_ba_solver* h, const b2s_ba_problem* p, const volatile uint8_t* stop, b2s_ba_result* r) {
@@ -2115,25 +2090,6 @@ extern "C" int b2s_local_ba_batch(b2s_ba_solver* h, int batch, const b2s_ba_prob
 
 
 // ================================================================================================ PoseOptimization host side
-struct b2s_pose_scratch {
-  size_t capE = 0;
-  int capF = 0;
-  PoFrame* dFrames = nullptr;
-  double *dPoseInit = nullptr, *dPoseOut = nullptr, *dErr = nullptr, *dChi2 = nullptr;
-  float *dXw = nullptr, *dObs = nullptr, *dInvS = nullptr;
-  uint8_t *dLevel = nullptr, *dOutlier = nullptr;
-  int *dNInl = nullptr, *dNTr = nullptr, *dTrace = nullptr;
-};
-
-static void pose_scratch_free(b2s_pose_scratch* s) {
-  if (!s) return;
-  void* ptrs[] = {s->dFrames, s->dPoseInit, s->dPoseOut, s->dErr, s->dChi2, s->dXw, s->dObs, s->dInvS, s->dLevel,
-                  s->dOutlier, s->dNInl, s->dNTr, s->dTrace};
-  for (void* p : ptrs)
-    if (p) cudaFree(p);
-  delete s;
-}
-
 extern "C" int b2s_pose_optimization_batch(b2s_ba_solver* h, int batch, const b2s_pose_problem* probs, b2s_pose_result* res) {
   if (!h || !probs || !res || batch < 1) {
     set_error("b2s_pose_optimization_batch: bad argument");
@@ -2176,48 +2132,45 @@ extern "C" int b2s_pose_optimization_batch(b2s_ba_solver* h, int batch, const b2
       }
     }
   }
-  if (!h->pose) h->pose = new b2s_pose_scratch();
-  b2s_pose_scratch* s = h->pose;
-  if (totalE + 1 > s->capE || batch > s->capF) {
-    pose_scratch_free(s);
-    h->pose = s = new b2s_pose_scratch();
-    s->capE = std::max<size_t>(totalE + 1, 4096) * 2;
-    s->capF = std::max(batch, 16) * 2;
-    cudaError_t e = cudaSuccess;
-    auto A = [&](void* pp, size_t bytes) {
-      if (e == cudaSuccess) e = cudaMalloc((void**)pp, bytes);
-    };
-    A(&s->dFrames, s->capF * sizeof(PoFrame)); A(&s->dPoseInit, (size_t)s->capF * POSE_STRIDE * 8); A(&s->dPoseOut, (size_t)s->capF * POSE_STRIDE * 8);
-    A(&s->dErr, s->capE * 24); A(&s->dChi2, s->capE * 8); A(&s->dXw, s->capE * 12); A(&s->dObs, s->capE * 12);
-    A(&s->dInvS, s->capE * 4); A(&s->dLevel, s->capE); A(&s->dOutlier, s->capE);
-    A(&s->dNInl, (size_t)s->capF * 4); A(&s->dNTr, (size_t)s->capF * 4); A(&s->dTrace, (size_t)s->capF * 256 * 4);
-    if (e != cudaSuccess) {
-      set_error("b2s_pose_optimization_batch: %s", cudaGetErrorString(e));
-      return B2S_ERR_CUDA;
-    }
-  }
-  B2S_CUDA(cudaMemcpyAsync(s->dFrames, frames.data(), batch * sizeof(PoFrame), cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(s->dPoseInit, poseInit.data(), (size_t)batch * POSE_STRIDE * 8, cudaMemcpyHostToDevice, st));
-  if (totalE) {
-    B2S_CUDA(cudaMemcpyAsync(s->dXw, Xw.data(), totalE * 12, cudaMemcpyHostToDevice, st));
-    B2S_CUDA(cudaMemcpyAsync(s->dObs, obs.data(), totalE * 12, cudaMemcpyHostToDevice, st));
-    B2S_CUDA(cudaMemcpyAsync(s->dInvS, invS.data(), totalE * 4, cudaMemcpyHostToDevice, st));
+  // a buffer short of this call's need grows to twice it (at least 4096 edges, 16 frames)
+  const size_t nE = totalE + 1, nF = batch, capE = std::max<size_t>(nE, 4096) * 2, capF = std::max<size_t>(nF, 16) * 2;
+  int rc = B2S_OK;
+  auto G = [&](DevBuf& b, size_t n, size_t cap, size_t elem) {
+    if (rc == B2S_OK && b.bytes < n * elem) rc = grow(b, cap * elem);
+  };
+  G(h->poFrames, nF, capF, sizeof(PoFrame)); G(h->poPoseInit, nF, capF, POSE_STRIDE * 8);
+  G(h->poPoseOut, nF, capF, POSE_STRIDE * 8);
+  G(h->poErr, nE, capE, 24); G(h->poChi2, nE, capE, 8); G(h->poXw, nE, capE, 12); G(h->poObs, nE, capE, 12);
+  G(h->poInvS, nE, capE, 4); G(h->poLevel, nE, capE, 1); G(h->poOutlier, nE, capE, 1);
+  G(h->poNInl, nF, capF, 4); G(h->poNTr, nF, capF, 4); G(h->poTrace, nF, capF, 256 * 4);
+  if (rc != B2S_OK) {
+    set_error("b2s_pose_optimization_batch: %s", g_last_error.c_str());
+    return rc;
   }
   PoPtrs pp;
-  pp.frames = s->dFrames; pp.poseInit = s->dPoseInit; pp.Xw = s->dXw; pp.obs = s->dObs; pp.invSigma2 = s->dInvS;
-  pp.err = s->dErr; pp.chi2 = s->dChi2; pp.level = s->dLevel; pp.outlier = s->dOutlier; pp.poseOut = s->dPoseOut;
-  pp.nInliers = s->dNInl; pp.nTrials = s->dNTr; pp.trace = s->dTrace;
+  pp.frames = (PoFrame*)h->poFrames.p; pp.poseInit = (double*)h->poPoseInit.p; pp.Xw = (float*)h->poXw.p;
+  pp.obs = (float*)h->poObs.p; pp.invSigma2 = (float*)h->poInvS.p; pp.err = (double*)h->poErr.p;
+  pp.chi2 = (double*)h->poChi2.p; pp.level = (uint8_t*)h->poLevel.p; pp.outlier = (uint8_t*)h->poOutlier.p;
+  pp.poseOut = (double*)h->poPoseOut.p; pp.nInliers = (int*)h->poNInl.p; pp.nTrials = (int*)h->poNTr.p;
+  pp.trace = (int*)h->poTrace.p;
+  B2S_CUDA(cudaMemcpyAsync(h->poFrames.p, frames.data(), batch * sizeof(PoFrame), cudaMemcpyHostToDevice, st));
+  B2S_CUDA(cudaMemcpyAsync(h->poPoseInit.p, poseInit.data(), (size_t)batch * POSE_STRIDE * 8, cudaMemcpyHostToDevice, st));
+  if (totalE) {
+    B2S_CUDA(cudaMemcpyAsync(h->poXw.p, Xw.data(), totalE * 12, cudaMemcpyHostToDevice, st));
+    B2S_CUDA(cudaMemcpyAsync(h->poObs.p, obs.data(), totalE * 12, cudaMemcpyHostToDevice, st));
+    B2S_CUDA(cudaMemcpyAsync(h->poInvS.p, invS.data(), totalE * 4, cudaMemcpyHostToDevice, st));
+  }
   k_pose_opt<<<batch, PO_T, 0, st>>>(pp);
   h->launches++;
   B2S_CUDA(cudaGetLastError());
   std::vector<double> poseOut((size_t)batch * POSE_STRIDE);
   std::vector<uint8_t> outl(totalE + 1);
   std::vector<int> nInl(batch), nTr(batch), trace((size_t)batch * 256);
-  B2S_CUDA(cudaMemcpyAsync(poseOut.data(), s->dPoseOut, (size_t)batch * POSE_STRIDE * 8, cudaMemcpyDeviceToHost, st));
-  if (totalE) B2S_CUDA(cudaMemcpyAsync(outl.data(), s->dOutlier, totalE, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaMemcpyAsync(nInl.data(), s->dNInl, (size_t)batch * 4, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaMemcpyAsync(nTr.data(), s->dNTr, (size_t)batch * 4, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaMemcpyAsync(trace.data(), s->dTrace, (size_t)batch * 256 * 4, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA(cudaMemcpyAsync(poseOut.data(), pp.poseOut, (size_t)batch * POSE_STRIDE * 8, cudaMemcpyDeviceToHost, st));
+  if (totalE) B2S_CUDA(cudaMemcpyAsync(outl.data(), pp.outlier, totalE, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA(cudaMemcpyAsync(nInl.data(), pp.nInliers, (size_t)batch * 4, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA(cudaMemcpyAsync(nTr.data(), pp.nTrials, (size_t)batch * 4, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA(cudaMemcpyAsync(trace.data(), pp.trace, (size_t)batch * 256 * 4, cudaMemcpyDeviceToHost, st));
   B2S_CUDA(cudaStreamSynchronize(st));
   for (int f = 0; f < batch; f++) {
     const b2s_pose_problem& P = probs[f];

@@ -1456,9 +1456,8 @@ __global__ void __launch_bounds__(32) k_grid_query(float x, float y, float r, in
 
 using namespace b2s;
 
-struct b2s_matcher {
-  int maxF, maxBatch, device;
-  cudaStream_t stream = nullptr;
+struct b2s_matcher : b2s::Stage {
+  int maxF, maxBatch;
   long long launches = 0;
   // device work buffers
   uint8_t *dDescA = nullptr, *dDescB = nullptr, *dValidA = nullptr, *dValidB = nullptr, *dOcc = nullptr, *dTaken = nullptr;
@@ -1468,13 +1467,12 @@ struct b2s_matcher {
   float *dAngA = nullptr, *dAngB = nullptr, *dKpx = nullptr, *dKpy = nullptr, *dURight = nullptr;
   uint32_t* dTopk = nullptr;
   ProjQuery* dQueries = nullptr;
-  b2s_keypoint* dKpsStage = nullptr;  // record staging of b2s_search_by_projection_last_batch (allocated on first use)
-  size_t kpsStageCap = 0;
-  // staging of b2s_search_by_projection_sequence: records of batch + 1 frames
-  uint8_t* dSeqDesc = nullptr;
-  float *dSeqDepth = nullptr, *dSeqT = nullptr;
-  int32_t* dSeqN = nullptr;
-  size_t seqCap = 0;
+  // record staging of b2s_search_by_projection_last_batch and b2s_search_by_projection_sequence (grown on first use)
+  DevBuf dKpsStage;
+  // the rest of the staging of b2s_search_by_projection_sequence: records of batch + 1 frames
+  DevBuf dSeqDesc, dSeqDepth, dSeqT, dSeqN;
+  // b2s_distinctive_descriptors: descriptors, point offsets and results
+  DevBuf dDistDesc, dDistOff, dDistBest;
 };
 
 extern "C" int b2s_matcher_create(int max_features, int max_batch, int device, b2s_matcher** out) {
@@ -1488,29 +1486,26 @@ extern "C" int b2s_matcher_create(int max_features, int max_batch, int device, b
   b2s_matcher* h = new b2s_matcher();
   h->maxF = max_features;
   h->maxBatch = max_batch;
-  h->device = device;
   const size_t F = (size_t)max_features * max_batch;
-  cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-  auto A = [&](void** p, size_t bytes) {
-    if (e == cudaSuccess) e = cudaMalloc(p, bytes);
-  };
-  A((void**)&h->dDescA, F * 32); A((void**)&h->dDescB, F * 32);
-  A((void**)&h->dValidA, F); A((void**)&h->dValidB, F); A((void**)&h->dOcc, F); A((void**)&h->dTaken, F);
-  A((void**)&h->dNodeA, F * 4); A((void**)&h->dNodeB, F * 4);
-  A((void**)&h->dNA, max_batch * 4); A((void**)&h->dNB, max_batch * 4);
-  A((void**)&h->dOrder, F * 4); A((void**)&h->dCandCnt, F * 4);
-  A((void**)&h->dMatch, F * 4); A((void**)&h->dBin, F * 4); A((void**)&h->dNMatches, max_batch * 4);
-  A((void**)&h->dOct, F * 4); A((void**)&h->dCellKey, F * 4);
-  A((void**)&h->dCellStart, (size_t)CELL_STRIDE * max_batch * 4);
-  A((void**)&h->dTopkIdx, F * TOPK * 4); A((void**)&h->dExtra, (size_t)max_batch * 4 * 4);
-  A((void**)&h->dHist, (size_t)max_batch * HISTO * 4);
-  A((void**)&h->dPush, F * 4);
-  A((void**)&h->dAngA, F * 4); A((void**)&h->dAngB, F * 4);
-  A((void**)&h->dKpx, F * 4); A((void**)&h->dKpy, F * 4); A((void**)&h->dURight, F * 4);
-  A((void**)&h->dTopk, F * TOPK * 4);
-  A((void**)&h->dQueries, F * 64);  // ProjQuery / MapQuery (56 B) or WinQuery (60 B)
-  if (e != cudaSuccess) {
-    set_error("b2s_matcher_create: %s", cudaGetErrorString(e));
+  h->open(device);
+  auto A = [h](auto* p, size_t bytes) { h->alloc(*p, bytes); };
+  A(&h->dDescA, F * 32); A(&h->dDescB, F * 32);
+  A(&h->dValidA, F); A(&h->dValidB, F); A(&h->dOcc, F); A(&h->dTaken, F);
+  A(&h->dNodeA, F * 4); A(&h->dNodeB, F * 4);
+  A(&h->dNA, max_batch * 4); A(&h->dNB, max_batch * 4);
+  A(&h->dOrder, F * 4); A(&h->dCandCnt, F * 4);
+  A(&h->dMatch, F * 4); A(&h->dBin, F * 4); A(&h->dNMatches, max_batch * 4);
+  A(&h->dOct, F * 4); A(&h->dCellKey, F * 4);
+  A(&h->dCellStart, (size_t)CELL_STRIDE * max_batch * 4);
+  A(&h->dTopkIdx, F * TOPK * 4); A(&h->dExtra, (size_t)max_batch * 4 * 4);
+  A(&h->dHist, (size_t)max_batch * HISTO * 4);
+  A(&h->dPush, F * 4);
+  A(&h->dAngA, F * 4); A(&h->dAngB, F * 4);
+  A(&h->dKpx, F * 4); A(&h->dKpy, F * 4); A(&h->dURight, F * 4);
+  A(&h->dTopk, F * TOPK * 4);
+  A(&h->dQueries, F * 64);  // ProjQuery / MapQuery (56 B) or WinQuery (60 B)
+  if (h->error != cudaSuccess) {
+    set_error("b2s_matcher_create: %s", cudaGetErrorString(h->error));
     b2s_matcher_destroy(h);
     return B2S_ERR_CUDA;
   }
@@ -1520,14 +1515,7 @@ extern "C" int b2s_matcher_create(int max_features, int max_batch, int device, b
 
 extern "C" void b2s_matcher_destroy(b2s_matcher* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
-  void* ptrs[] = {h->dDescA, h->dDescB, h->dValidA, h->dValidB, h->dOcc, h->dTaken, h->dNodeA, h->dNodeB, h->dNA, h->dNB,
-                  h->dOrder, h->dCandCnt, h->dMatch, h->dBin, h->dNMatches, h->dOct, h->dCellKey, h->dCellStart,
-                  h->dTopkIdx, h->dExtra, h->dHist, h->dPush, h->dAngA, h->dAngB, h->dKpx, h->dKpy, h->dURight, h->dTopk,
-                  h->dQueries, h->dKpsStage, h->dSeqDesc, h->dSeqDepth, h->dSeqT, h->dSeqN};
-  for (void* p : ptrs)
-    if (p) cudaFree(p);
-  if (h->stream) cudaStreamDestroy(h->stream);
+  h->close();
   delete h;
 }
 
@@ -1669,6 +1657,11 @@ struct b2s_frame_grid {
   float *kpx = nullptr, *kpy = nullptr, *ang = nullptr, *uright = nullptr;
   int32_t *oct = nullptr, *order = nullptr, *cellStart = nullptr, *cellKey = nullptr, *nB = nullptr, *qOut = nullptr;
   uint8_t* desc = nullptr;
+};
+
+// A grid of b2s_frame_grid_create*: the arrays above are its own buffers.
+struct OwnedGrid : b2s_frame_grid {
+  DevBuf own[11];
 };
 
 // The grid of a host-buffer search: it aliases the matcher's work buffers, owns nothing and is never passed to
@@ -1941,22 +1934,18 @@ extern "C" int b2s_search_by_projection_last_batch(b2s_matcher* h, int batch, co
   B2S_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = h->stream;
   const size_t FQ = (size_t)batch * capQ, FF = (size_t)batch * capF;
-  if (h->kpsStageCap < FF) {
-    if (h->dKpsStage) cudaFree(h->dKpsStage);
-    h->dKpsStage = nullptr;
-    h->kpsStageCap = 0;
-    B2S_CUDA(cudaMalloc((void**)&h->dKpsStage, FF * sizeof(b2s_keypoint)));
-    h->kpsStageCap = FF;
-  }
+  int rc = grow(h->dKpsStage, FF * sizeof(b2s_keypoint));
+  if (rc != B2S_OK) return rc;
+  const b2s_keypoint* dKps = (const b2s_keypoint*)h->dKpsStage.p;
   B2S_CUDA(cudaMemcpyAsync(h->dQueries, q, FQ * sizeof(ProjQuery), cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dKpsStage, kps, FF * sizeof(b2s_keypoint), cudaMemcpyHostToDevice, st));
+  B2S_CUDA(cudaMemcpyAsync(h->dKpsStage.p, kps, FF * sizeof(b2s_keypoint), cudaMemcpyHostToDevice, st));
   B2S_CUDA(cudaMemcpyAsync(h->dURight, uright, FF * 4, cudaMemcpyHostToDevice, st));
   B2S_CUDA(cudaMemcpyAsync(h->dDescB, desc, FF * 32, cudaMemcpyHostToDevice, st));
   B2S_CUDA(cudaMemcpyAsync(h->dNA, nq, (size_t)batch * 4, cudaMemcpyHostToDevice, st));
   B2S_CUDA(cudaMemcpyAsync(h->dNB, nf, (size_t)batch * 4, cudaMemcpyHostToDevice, st));
-  int rc = b2s_search_by_projection_last_device(h, batch, reinterpret_cast<const b2s_proj_query*>(h->dQueries), h->dNA, capQ,
-                                                h->dKpsStage, h->dURight, h->dDescB, h->dNB, capF, g, th, mode, th_high,
-                                                check_ori, h->dMatch, h->dNMatches, st);
+  rc = b2s_search_by_projection_last_device(h, batch, reinterpret_cast<const b2s_proj_query*>(h->dQueries), h->dNA, capQ,
+                                            dKps, h->dURight, h->dDescB, h->dNB, capF, g, th, mode, th_high, check_ori,
+                                            h->dMatch, h->dNMatches, st);
   if (rc != B2S_OK) return rc;
   B2S_CUDA(cudaMemcpyAsync(match_cur, h->dMatch, FF * 4, cudaMemcpyDeviceToHost, st));
   B2S_CUDA(cudaMemcpyAsync(nmatches, h->dNMatches, (size_t)batch * 4, cudaMemcpyDeviceToHost, st));
@@ -1981,32 +1970,27 @@ extern "C" int b2s_search_by_projection_sequence(b2s_matcher* h, int batch, cons
   B2S_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = h->stream;
   const size_t S = (size_t)(batch + 1) * cap, FF = (size_t)batch * cap;
-  if (h->seqCap < S) {
-    void* old[] = {h->dKpsStage, h->dSeqDesc, h->dSeqDepth, h->dSeqN, h->dSeqT};
-    for (void* p : old)
-      if (p) cudaFree(p);
-    h->dKpsStage = nullptr; h->dSeqDesc = nullptr; h->dSeqDepth = nullptr; h->dSeqN = nullptr; h->dSeqT = nullptr;
-    h->seqCap = 0; h->kpsStageCap = 0;
-    B2S_CUDA(cudaMalloc((void**)&h->dKpsStage, S * sizeof(b2s_keypoint)));
-    B2S_CUDA(cudaMalloc((void**)&h->dSeqDesc, S * 32));
-    B2S_CUDA(cudaMalloc((void**)&h->dSeqDepth, S * 4));
-    B2S_CUDA(cudaMalloc((void**)&h->dSeqN, (size_t)(h->maxBatch + 1) * 4));
-    B2S_CUDA(cudaMalloc((void**)&h->dSeqT, (size_t)h->maxBatch * 12 * 4));
-    h->seqCap = S;
-    h->kpsStageCap = S;
-  }
-  B2S_CUDA(cudaMemcpyAsync(h->dKpsStage, kps, S * sizeof(b2s_keypoint), cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dSeqDesc, desc, S * 32, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dSeqDepth, depth, S * 4, cudaMemcpyHostToDevice, st));
+  int rc = grow(h->dKpsStage, S * sizeof(b2s_keypoint));
+  if (rc == B2S_OK) rc = grow(h->dSeqDesc, S * 32);
+  if (rc == B2S_OK) rc = grow(h->dSeqDepth, S * 4);
+  if (rc == B2S_OK) rc = grow(h->dSeqN, (size_t)(h->maxBatch + 1) * 4);
+  if (rc == B2S_OK) rc = grow(h->dSeqT, (size_t)h->maxBatch * 12 * 4);
+  if (rc != B2S_OK) return rc;
+  const b2s_keypoint* dKps = (const b2s_keypoint*)h->dKpsStage.p;
+  const uint8_t* dDesc = (const uint8_t*)h->dSeqDesc.p;
+  const int32_t* dN = (const int32_t*)h->dSeqN.p;
+  B2S_CUDA(cudaMemcpyAsync(h->dKpsStage.p, kps, S * sizeof(b2s_keypoint), cudaMemcpyHostToDevice, st));
+  B2S_CUDA(cudaMemcpyAsync(h->dSeqDesc.p, desc, S * 32, cudaMemcpyHostToDevice, st));
+  B2S_CUDA(cudaMemcpyAsync(h->dSeqDepth.p, depth, S * 4, cudaMemcpyHostToDevice, st));
   B2S_CUDA(cudaMemcpyAsync(h->dURight, uright, FF * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dSeqN, n, (size_t)(batch + 1) * 4, cudaMemcpyHostToDevice, st));
-  B2S_CUDA(cudaMemcpyAsync(h->dSeqT, Tcl, (size_t)batch * 12 * 4, cudaMemcpyHostToDevice, st));
-  int rc = b2s_track_queries_device(h, batch, h->dKpsStage, h->dSeqDesc, h->dSeqDepth, h->dSeqN, cap, h->dSeqT, fx, fy, cx, cy,
-                                    has_obs, reinterpret_cast<b2s_proj_query*>(h->dQueries), h->dNA, st);
+  B2S_CUDA(cudaMemcpyAsync(h->dSeqN.p, n, (size_t)(batch + 1) * 4, cudaMemcpyHostToDevice, st));
+  B2S_CUDA(cudaMemcpyAsync(h->dSeqT.p, Tcl, (size_t)batch * 12 * 4, cudaMemcpyHostToDevice, st));
+  rc = b2s_track_queries_device(h, batch, dKps, dDesc, (const float*)h->dSeqDepth.p, dN, cap, (const float*)h->dSeqT.p, fx,
+                                fy, cx, cy, has_obs, reinterpret_cast<b2s_proj_query*>(h->dQueries), h->dNA, st);
   if (rc != B2S_OK) return rc;
   rc = b2s_search_by_projection_last_device(h, batch, reinterpret_cast<const b2s_proj_query*>(h->dQueries), h->dNA, cap,
-                                            h->dKpsStage + cap, h->dURight, h->dSeqDesc + (size_t)cap * 32, h->dSeqN + 1, cap,
-                                            g, th, mode, th_high, check_ori, h->dMatch, h->dNMatches, st);
+                                            dKps + cap, h->dURight, dDesc + (size_t)cap * 32, dN + 1, cap, g, th, mode, th_high,
+                                            check_ori, h->dMatch, h->dNMatches, st);
   if (rc != B2S_OK) return rc;
   B2S_CUDA(cudaMemcpyAsync(match_cur, h->dMatch, FF * 4, cudaMemcpyDeviceToHost, st));
   B2S_CUDA(cudaMemcpyAsync(nmatches, h->dNMatches, (size_t)batch * 4, cudaMemcpyDeviceToHost, st));
@@ -2128,10 +2112,7 @@ extern "C" int b2s_search_windows(b2s_matcher* h, const b2s_win_query* q, int nq
 extern "C" void b2s_frame_grid_destroy(b2s_frame_grid* gr) {
   if (!gr) return;
   cudaSetDevice(gr->device);
-  void* ptrs[] = {gr->kpx, gr->kpy, gr->ang, gr->uright, gr->oct, gr->order, gr->cellStart, gr->cellKey, gr->nB, gr->qOut, gr->desc};
-  for (void* p : ptrs)
-    if (p) cudaFree(p);
-  delete gr;
+  delete static_cast<OwnedGrid*>(gr);
 }
 
 static int grid_alloc(b2s_matcher* h, int nf, const b2s_frame_geom* g, const float* inv_level_sigma2, b2s_frame_grid** out) {
@@ -2141,22 +2122,24 @@ static int grid_alloc(b2s_matcher* h, int nf, const b2s_frame_geom* g, const flo
   }
   *out = nullptr;
   B2S_CUDA(cudaSetDevice(h->device));
-  b2s_frame_grid* gr = new b2s_frame_grid();
+  OwnedGrid* gr = new OwnedGrid();
   gr->owner = h;
   gr->device = h->device;
   gr->nf = nf;
   gr->pg = proj_geom(g, inv_level_sigma2);
   const size_t n = (size_t)std::max(nf, 1);
-  cudaError_t e = cudaSuccess;
-  auto A = [&](void** p, size_t bytes) {
-    if (e == cudaSuccess) e = cudaMalloc(p, bytes);
+  int k = 0, rc = B2S_OK;
+  auto A = [&](auto** p, size_t bytes) {  // array *p in the next of the grid's own buffers
+    DevBuf& b = gr->own[k++];
+    if (rc == B2S_OK) rc = grow(b, bytes);
+    *(void**)p = b.p;
   };
-  A((void**)&gr->kpx, n * 4); A((void**)&gr->kpy, n * 4); A((void**)&gr->ang, n * 4); A((void**)&gr->uright, n * 4);
-  A((void**)&gr->oct, n * 4); A((void**)&gr->order, n * 4); A((void**)&gr->cellKey, n * 4);
-  A((void**)&gr->cellStart, (GRID_COLS * GRID_ROWS + 2) * 4); A((void**)&gr->nB, 4); A((void**)&gr->qOut, (n + 1) * 4);
-  A((void**)&gr->desc, n * 32);
-  if (e != cudaSuccess) {
-    set_error("b2s_frame_grid_create: %s", cudaGetErrorString(e));
+  A(&gr->kpx, n * 4); A(&gr->kpy, n * 4); A(&gr->ang, n * 4); A(&gr->uright, n * 4);
+  A(&gr->oct, n * 4); A(&gr->order, n * 4); A(&gr->cellKey, n * 4);
+  A(&gr->cellStart, (GRID_COLS * GRID_ROWS + 2) * 4); A(&gr->nB, 4); A(&gr->qOut, (n + 1) * 4);
+  A(&gr->desc, n * 32);
+  if (rc != B2S_OK) {
+    set_error("b2s_frame_grid_create: %s", g_last_error.c_str());
     b2s_frame_grid_destroy(gr);
     return B2S_ERR_CUDA;
   }
@@ -2357,27 +2340,18 @@ extern "C" int b2s_search_for_triangulation(b2s_matcher* h, const b2s_kf_feature
 }
 
 // ---------------------------------------------------------------- DBoW2 vocabulary
-struct b2s_vocabulary {
-  int k = 0, L = 0, nNodes = 0, nWords = 0, device = 0;
-  cudaStream_t stream = nullptr;
+struct b2s_vocabulary : b2s::Stage {
+  int k = 0, L = 0, nNodes = 0, nWords = 0;
   int32_t *dChildStart = nullptr, *dChildCount = nullptr, *dCNode = nullptr, *dWordOf = nullptr;
   uint8_t* dCDesc = nullptr;
   double* dWeight = nullptr;
   // scratch of the host-buffer entry point
-  size_t cap = 0;
-  uint8_t* dFeat = nullptr;
-  int32_t *dWord = nullptr, *dNode = nullptr;
-  double* dW = nullptr;
+  DevBuf dFeat, dWord, dNode, dW;
 };
 
 extern "C" void b2s_vocabulary_destroy(b2s_vocabulary* v) {
   if (!v) return;
-  cudaSetDevice(v->device);
-  void* ptrs[] = {v->dChildStart, v->dChildCount, v->dCNode, v->dWordOf, v->dCDesc, v->dWeight, v->dFeat, v->dWord, v->dNode,
-                  v->dW};
-  for (void* p : ptrs)
-    if (p) cudaFree(p);
-  if (v->stream) cudaStreamDestroy(v->stream);
+  v->close();
   delete v;
 }
 
@@ -2411,11 +2385,11 @@ extern "C" int b2s_vocabulary_create(const b2s_vocabulary_desc* d, int device, b
     memcpy(&cDesc[(size_t)pos * 32], d->desc + (size_t)nid * 32, 32);
   }
   b2s_vocabulary* v = new b2s_vocabulary();
-  v->k = d->k; v->L = d->L; v->nNodes = N; v->nWords = nWords; v->device = device;
-  cudaError_t e = cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking);
-  auto A = [&](void* pp, size_t bytes, const void* src) {
-    if (e == cudaSuccess) e = cudaMalloc((void**)pp, bytes);
-    if (e == cudaSuccess) e = cudaMemcpy(*(void**)pp, src, bytes, cudaMemcpyHostToDevice);
+  v->k = d->k; v->L = d->L; v->nNodes = N; v->nWords = nWords;
+  v->open(device);
+  auto A = [v](auto** p, size_t bytes, const void* src) {
+    v->alloc(*p, bytes);
+    if (v->error == cudaSuccess) v->error = cudaMemcpy(*p, src, bytes, cudaMemcpyHostToDevice);
   };
   A(&v->dChildStart, (size_t)N * 4, start.data());
   A(&v->dChildCount, (size_t)N * 4, cnt.data());
@@ -2423,8 +2397,8 @@ extern "C" int b2s_vocabulary_create(const b2s_vocabulary_desc* d, int device, b
   A(&v->dCDesc, cDesc.size(), cDesc.data());
   A(&v->dWordOf, (size_t)N * 4, wordOf.data());
   A(&v->dWeight, (size_t)N * 8, d->weight);
-  if (e != cudaSuccess) {
-    set_error("b2s_vocabulary_create: %s", cudaGetErrorString(e));
+  if (v->error != cudaSuccess) {
+    set_error("b2s_vocabulary_create: %s", cudaGetErrorString(v->error));
     b2s_vocabulary_destroy(v);
     return B2S_ERR_CUDA;
   }
@@ -2457,26 +2431,20 @@ extern "C" int b2s_bow_transform(b2s_vocabulary* v, const uint8_t* features, int
   }
   if (n == 0) return B2S_OK;
   B2S_CUDA(cudaSetDevice(v->device));
-  if ((size_t)n > v->cap) {
-    void* ptrs[] = {v->dFeat, v->dWord, v->dNode, v->dW};
-    for (void* p : ptrs)
-      if (p) cudaFree(p);
-    v->dFeat = nullptr; v->dWord = nullptr; v->dNode = nullptr; v->dW = nullptr;
-    v->cap = 0;
-    const size_t c = std::max<size_t>(n, 4096);
-    B2S_CUDA(cudaMalloc((void**)&v->dFeat, c * 32));
-    B2S_CUDA(cudaMalloc((void**)&v->dWord, c * 4));
-    B2S_CUDA(cudaMalloc((void**)&v->dNode, c * 4));
-    B2S_CUDA(cudaMalloc((void**)&v->dW, c * 8));
-    v->cap = c;
-  }
-  cudaStream_t st = v->stream;
-  B2S_CUDA(cudaMemcpyAsync(v->dFeat, features, (size_t)n * 32, cudaMemcpyHostToDevice, st));
-  int rc = b2s_bow_transform_device(v, v->dFeat, n, levelsup, v->dWord, v->dW, v->dNode, st);
+  const size_t c = std::max<size_t>(n, 4096);
+  int rc = grow(v->dFeat, c * 32);
+  if (rc == B2S_OK) rc = grow(v->dWord, c * 4);
+  if (rc == B2S_OK) rc = grow(v->dNode, c * 4);
+  if (rc == B2S_OK) rc = grow(v->dW, c * 8);
   if (rc != B2S_OK) return rc;
-  B2S_CUDA(cudaMemcpyAsync(word_id, v->dWord, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-  if (weight) B2S_CUDA(cudaMemcpyAsync(weight, v->dW, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
-  B2S_CUDA(cudaMemcpyAsync(node_id, v->dNode, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+  cudaStream_t st = v->stream;
+  B2S_CUDA(cudaMemcpyAsync(v->dFeat.p, features, (size_t)n * 32, cudaMemcpyHostToDevice, st));
+  rc = b2s_bow_transform_device(v, (const uint8_t*)v->dFeat.p, n, levelsup, (int32_t*)v->dWord.p, (double*)v->dW.p,
+                                (int32_t*)v->dNode.p, st);
+  if (rc != B2S_OK) return rc;
+  B2S_CUDA(cudaMemcpyAsync(word_id, v->dWord.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+  if (weight) B2S_CUDA(cudaMemcpyAsync(weight, v->dW.p, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA(cudaMemcpyAsync(node_id, v->dNode.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
   B2S_CUDA(cudaStreamSynchronize(st));
   return B2S_OK;
 }
@@ -2492,12 +2460,14 @@ extern "C" int b2s_distinctive_descriptors(b2s_matcher* h, const uint8_t* desc, 
   if (total < 0 || (total && !desc)) return B2S_ERR_BAD_ARG;
   B2S_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = h->stream;
-  uint8_t* dDesc = nullptr;
-  int32_t *dOff = nullptr, *dBest = nullptr;
-  B2S_CUDA(cudaMalloc((void**)&dDesc, (size_t)std::max(total, 1) * 32));
-  cudaError_t e = cudaMalloc((void**)&dOff, (size_t)(n_points + 1) * 4);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&dBest, (size_t)n_points * 4);
-  if (e == cudaSuccess && total) e = cudaMemcpyAsync(dDesc, desc, (size_t)total * 32, cudaMemcpyHostToDevice, st);
+  int rc = grow(h->dDistDesc, (size_t)std::max(total, 1) * 32);
+  if (rc == B2S_OK) rc = grow(h->dDistOff, (size_t)(n_points + 1) * 4);
+  if (rc == B2S_OK) rc = grow(h->dDistBest, (size_t)n_points * 4);
+  if (rc != B2S_OK) return rc;
+  uint8_t* dDesc = (uint8_t*)h->dDistDesc.p;
+  int32_t *dOff = (int32_t*)h->dDistOff.p, *dBest = (int32_t*)h->dDistBest.p;
+  cudaError_t e = cudaSuccess;
+  if (total) e = cudaMemcpyAsync(dDesc, desc, (size_t)total * 32, cudaMemcpyHostToDevice, st);
   if (e == cudaSuccess) e = cudaMemcpyAsync(dOff, offsets, (size_t)(n_points + 1) * 4, cudaMemcpyHostToDevice, st);
   if (e == cudaSuccess) {
     k_distinctive<<<div_up(n_points, 8), 256, 0, st>>>(dDesc, dOff, n_points, dBest);
@@ -2506,9 +2476,6 @@ extern "C" int b2s_distinctive_descriptors(b2s_matcher* h, const uint8_t* desc, 
   }
   if (e == cudaSuccess) e = cudaMemcpyAsync(best_idx, dBest, (size_t)n_points * 4, cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  cudaFree(dDesc);
-  if (dOff) cudaFree(dOff);
-  if (dBest) cudaFree(dBest);
   if (e != cudaSuccess) {
     set_error("b2s_distinctive_descriptors: %s", cudaGetErrorString(e));
     return B2S_ERR_CUDA;

@@ -1,15 +1,28 @@
 """The handle lifecycle the device stages share (b2s::Stage in csrc/common.cuh, _Handle in the package): argument checks
-come before device selection, a failed create leaves *out NULL, destroy(NULL) and last_ms(NULL) are safe, and every
-Python handle can be closed twice."""
+come before device selection, a failed create leaves *out NULL, destroy(NULL) and a query of a NULL handle are safe,
+and every Python handle can be closed twice."""
 import ctypes
 
 import numpy as np
 import pytest
 
 vp = ctypes.c_void_p
+# a three-node vocabulary (k = 2, L = 1): parent, leaf flag, descriptor and weight of each node
+VOC = [np.array([-1, 0, 0], np.int32), np.array([0, 1, 1], np.uint8), np.zeros((3, 32), np.uint8), np.ones(3)]
 
-# create entry point, good capacities, a bad capacity set, destroy, last_ms (and whether it takes an lm_trials pointer)
+
+def _voc_desc(pkg):
+    return ctypes.byref(pkg._VocDesc(2, 1, len(VOC[0]), *[a.ctypes.data for a in VOC]))
+
+
+# create entry point, good capacities (an entry may be a function of the package), a bad capacity set, destroy, a query
+# that takes a NULL handle: last_ms or a count (and whether it takes an lm_trials pointer)
 STAGES = [
+    ("b2s_extractor_create", (500, 1.2, 8, 20, 7, 640, 480, 1), (500, 1.2, 8, 20, 7, 640, 480, 0),
+     "b2s_extractor_destroy", "b2s_extractor_launch_count", False),
+    ("b2s_matcher_create", (1000, 1), (0, 1), "b2s_matcher_destroy", "b2s_matcher_launch_count", False),
+    ("b2s_vocabulary_create", (_voc_desc,), (None,), "b2s_vocabulary_destroy", "b2s_vocabulary_words", False),
+    ("b2s_ba_create", (4, 16, 64, 1), (0, 16, 64, 1), "b2s_ba_destroy", "b2s_ba_last_kernel_ms", True),
     ("b2s_init_create", (64, 10, 1), (7, 10, 1), "b2s_init_destroy", "b2s_init_last_ms", False),
     ("b2s_sim3solver_create", (64, 10, 1), (2, 10, 1), "b2s_sim3solver_destroy", "b2s_sim3solver_last_ms", False),
     ("b2s_pnpsolver_create", (64, 10, 1), (3, 10, 1), "b2s_pnpsolver_destroy", "b2s_pnpsolver_last_ms", False),
@@ -25,15 +38,15 @@ STAGES = [
 IDS = [s[0][4:-7] for s in STAGES]
 
 
-def _create(L, name, caps, out):  # on device 0, with the signatures lib() declares
-    return getattr(L, name)(*caps, 0, ctypes.byref(out))
+def _create(pkg, name, caps, out):  # on device 0, with the signatures lib() declares
+    return getattr(pkg.lib(), name)(*[c(pkg) if callable(c) else c for c in caps], 0, ctypes.byref(out))
 
 
 @pytest.mark.parametrize("stage", STAGES, ids=IDS)
 def test_bad_capacity_is_checked_before_the_device(pkg, stage):
     create, _, bad, *_ = stage
     out = vp(1234)
-    assert _create(pkg.lib(), create, bad, out) == pkg.ERR_BAD_ARG
+    assert _create(pkg, create, bad, out) == pkg.ERR_BAD_ARG
 
 
 @pytest.mark.parametrize("stage", STAGES, ids=IDS)
@@ -42,7 +55,7 @@ def test_create_without_a_device(pkg, stage):
         pytest.skip("a CUDA device is present")
     create, good, *_ = stage
     out = vp(1234)
-    assert _create(pkg.lib(), create, good, out) == pkg.ERR_NO_DEVICE
+    assert _create(pkg, create, good, out) == pkg.ERR_NO_DEVICE
     assert not out.value
 
 
