@@ -339,6 +339,116 @@ int b2s_search_for_triangulation(b2s_matcher* h, const b2s_kf_features* kf1, con
 int b2s_distinctive_descriptors(b2s_matcher* h, const uint8_t* desc, const int32_t* offsets, int n_points,
                                 int32_t* best_idx);
 
+/* MapPoint::UpdateNormalAndDepth (src/MapPoint.cc:477-521) for a batch of map points, bit-identical to the reference.
+ * Nothing changes for a bad point or a point without observations.  Every other point sums, over its observers in
+ * std::map<KeyFrame*,size_t> order (keyframe address order; bad keyframes are not skipped), normali = Pos - Ow and
+ * normal = normal + normali/norm(normali); then dist = norm(Pos - Ow_ref), max = dist * scale_factors[octave of the
+ * reference keyframe's observation], min = max / scale_factors[n_levels-1] and normal = normal/n.  The OpenCV forms
+ * (DESIGN.md §7): norm of a 3 x 1 column sums the squares in double in order; the running sum is scaleAdd, normali * (float)(1/norm)
+ * + normal fused and rounded once; normal/n is convertTo with (float)(1./n).  The keyframe table must therefore be in
+ * the address order of the caller's keyframes: it fixes the order of the float sums. */
+typedef struct {
+  int32_t n_kf;                   /* the keyframe table, in address order */
+  const float* kf_center;         /* 3 * n_kf: GetCameraCenter() */
+  int32_t n_mp;
+  const float* mp_pos;            /* 3 * n_mp: mWorldPos */
+  const uint8_t* mp_bad;          /* n_mp: mbBad */
+  const int32_t* mp_ref;          /* n_mp: mpRefKF's table index; it must be one of the observers of every point that is
+                                     not bad and has observers (elsewhere it is not read) */
+  const int32_t* obs_off;         /* n_mp + 1: mObservations, CSR */
+  const int32_t* obs_kf;          /* keyframe table index, strictly ascending within a row */
+  const int32_t* obs_octave;      /* that keyframe's mvKeysUn[idx].octave, in [0, n_levels) */
+  const float* scale_factors;     /* n_levels: mvScaleFactors */
+  int32_t n_levels;               /* >= 1 */
+} b2s_normal_depth_problem;
+typedef struct {
+  float* normal;                  /* 3 * n_mp: mNormalVector (written for updated points only) */
+  float* min_dist;                /* n_mp: mfMinDistance (updated points only) */
+  float* max_dist;                /* n_mp: mfMaxDistance (updated points only) */
+  uint8_t* updated;               /* n_mp: 1 where the point was refreshed (not bad, observed) */
+} b2s_normal_depth_result;
+/* A null array, a negative count, n_levels < 1, offsets that are not a CSR, an index out of range, an observer row that
+ * is not strictly ascending, an octave outside [0, n_levels) or a reference keyframe that is not an observer:
+ * B2S_ERR_BAD_ARG, and nothing is written.  Device buffers grow on demand.  One launch (b2s_matcher_launch_count). */
+int b2s_update_normal_and_depth(b2s_matcher* h, const b2s_normal_depth_problem* p, b2s_normal_depth_result* r);
+
+/* Keyframe insertion: the association loop of LocalMapping::ProcessNewKeyFrame (src/LocalMapping.cc:217-249) and
+ * LocalMapping::MapPointCulling (:261-308) for a batch of independent problems, bit-identical to the reference.
+ *   Association: the current keyframe's slots in order; for a non-NULL point that is not bad, a point that does not list
+ *   the current keyframe gets AddObservation(cur, i) (nObs += 2 when mvuRight[i] >= 0, else 1), UpdateNormalAndDepth
+ *   (as b2s_update_normal_and_depth) and ComputeDistinctiveDescriptors (observers in map order, bad keyframes skipped;
+ *   as b2s_distinctive_descriptors); any other such slot appends the point to mlpRecentAddedMapPoints.  A point in two
+ *   slots is associated by the first and appended by the later ones.  The new observation takes the current keyframe's
+ *   table position in the point's observer row, which is what orders the float sums.  ComputeBoW, UpdateConnections and
+ *   Map::AddKeyFrame are left to the caller.
+ *   Culling: the recent list after those appends, in order, with nThObs = 2 (monocular) or 3: a bad point is erased; a
+ *   point with (float)mnFound/mnVisible < 0.25f is set bad and erased (mnVisible 0 does not cull); a point with
+ *   (int)mnId - (int)mnFirstKFid >= 2 (32-bit, wrapping) and nObs <= nThObs is set bad and erased; with a difference
+ *   >= 3 it is erased and stays good; otherwise it is kept.  A later entry of a point that an earlier entry set bad is
+ *   erased as bad.  MapPoint::SetBadFlag (:217-234) clears the point's observations and nulls the slot idx of each
+ *   observer, whatever point it holds; here that is seen in the current keyframe's slots, and the caller applies it to
+ *   the other observers (the points set bad are the entries with a B2S_KFI_CULLED_* verdict, in list order).
+ * The graph need not be consistent: duplicate slots, bad points in slots and repeated recent entries are modelled. */
+typedef struct {
+  int32_t n_kf;                   /* the keyframe table, in address order: the current keyframe and every observer */
+  const float* kf_center;         /* 3 * n_kf: GetCameraCenter() */
+  const uint8_t* kf_bad;          /* n_kf: isBad() (ComputeDistinctiveDescriptors skips bad observers) */
+  int32_t cur;                    /* the current keyframe's table index */
+  uint64_t cur_id;                /* its mnId */
+  int32_t n_slots;
+  const int32_t* slot_mp;         /* n_slots: mvpMapPoints, map-point index or -1 for NULL */
+  const uint8_t* slot_stereo;     /* n_slots: mvuRight[i] >= 0 */
+  const uint8_t* slot_desc;       /* 32 * n_slots: mDescriptors */
+  int32_t n_mp;
+  const float* mp_pos;            /* 3 * n_mp: mWorldPos */
+  const uint8_t* mp_bad;          /* n_mp: mbBad on entry */
+  const int32_t* mp_ref;          /* n_mp: mpRefKF's table index; it must be one of the point's observers on entry for
+                                     every point the call associates (elsewhere it is not read) */
+  const int32_t* mp_nobs;         /* n_mp: nObs on entry */
+  const int32_t* mp_found;        /* n_mp: mnFound */
+  const int32_t* mp_visible;      /* n_mp: mnVisible */
+  const int64_t* mp_first_kf;     /* n_mp: mnFirstKFid */
+  const int32_t* obs_off;         /* n_mp + 1: mObservations on entry, CSR */
+  const int32_t* obs_kf;          /* keyframe table index, strictly ascending within a row */
+  const int32_t* obs_idx;         /* index in that keyframe (< n_slots where it is the current keyframe) */
+  const int32_t* obs_octave;      /* that keyframe's mvKeysUn[idx].octave, in [0, n_levels) */
+  const uint8_t* obs_desc;        /* 32 per observation: that keyframe's mDescriptors.row(idx) */
+  int32_t n_recent;
+  const int32_t* recent;          /* n_recent: mlpRecentAddedMapPoints on entry, map-point indices */
+  const float* scale_factors;     /* n_levels: mvScaleFactors */
+  int32_t n_levels;               /* >= 1 */
+  int32_t monocular;              /* LocalMapping::mbMonocular */
+} b2s_kfinsert_problem;
+enum { B2S_KFI_KEPT = 0, B2S_KFI_BAD = 1, B2S_KFI_CULLED_RATIO = 2, B2S_KFI_CULLED_OBS = 3, B2S_KFI_RETIRED = 4 };
+typedef struct {
+  int32_t* mp_nobs;               /* n_mp: nObs after the call */
+  uint8_t* mp_bad;                /* n_mp: mbBad after the call */
+  int32_t* mp_added;              /* n_mp: the slot the association added as the current keyframe's observation, or -1;
+                                     that observation is live unless the point was set bad */
+  uint8_t* obs_alive;             /* obs_off[n_mp]: 1 while the entry observation is still in mObservations */
+  uint8_t* mp_updated;            /* n_mp: 1 where UpdateNormalAndDepth ran */
+  float* mp_normal;               /* 3 * n_mp: mNormalVector (updated points only) */
+  float* mp_min_dist;             /* n_mp: mfMinDistance (updated points only) */
+  float* mp_max_dist;             /* n_mp: mfMaxDistance (updated points only) */
+  int32_t* mp_desc;               /* n_mp: the observation whose descriptor became mDescriptor, as its position in the
+                                     point's observer row after the association; -1 where mDescriptor is unchanged */
+  int32_t* slot_mp;               /* n_slots: the current keyframe's slots after the call */
+  int32_t* list_mp;               /* n_recent + n_slots: the recent list after the association's appends */
+  uint8_t* list_verdict;          /* n_recent + n_slots: each entry's B2S_KFI_* verdict; the list after the call is
+                                     the B2S_KFI_KEPT entries in order */
+  int32_t n_list;                 /* entries of list_mp */
+  int32_t n_culled;               /* points set bad by the culling */
+} b2s_kfinsert_result;
+/* A null array, batch < 1, a negative count, n_levels < 1, offsets that are not a CSR, an index out of range, an
+ * observer row that is not strictly ascending, an octave outside [0, n_levels), an obs_idx < 0 (or >= n_slots for the
+ * current keyframe), or a point to associate whose reference keyframe is not an observer: B2S_ERR_BAD_ARG.  Nothing is
+ * written unless every problem is valid.  Device buffers grow on demand.  Two launches per call for the whole batch
+ * (b2s_matcher_launch_count). */
+int b2s_process_new_keyframe(b2s_matcher* h, int batch, const b2s_kfinsert_problem* p, b2s_kfinsert_result* r);
+/* Device time (CUDA events on the handle's stream: upload, kernels, download) of the last b2s_update_normal_and_depth or
+ * b2s_process_new_keyframe call. */
+float b2s_matcher_last_ms(const b2s_matcher* h);
+
 /* ------------------------------------------------------------------ DBoW2 vocabulary (SURVEY.md §8f rank 3) */
 /* TemplatedVocabulary<FORB>::transform (Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1127-1256) as used by
  * Frame::ComputeBoW / KeyFrame::ComputeBoW (src/Frame.cc:880-896, src/KeyFrame.cc, levelsup = 4): it produces the word

@@ -1,0 +1,2 @@
+// <opencv2/core/core.hpp> for the in-place build of src/LocalMapping.cc for the keyframe-insertion checkers (oracle/kfinsert.mk)
+#include "../../../refshim_cv_kfinsert.h"

@@ -1,0 +1,2 @@
+// <opencv2/opencv.hpp> for the in-place build of src/LocalMapping.cc for the keyframe-insertion checkers (oracle/kfinsert.mk)
+#include "../../refshim_cv_kfinsert.h"

@@ -185,6 +185,32 @@ class _CullingResult(ctypes.Structure):  # b2s_culling_result
                 ("obs_alive", _vp), ("slot_mp", _vp), ("n_culled", ctypes.c_int32)]
 
 
+class _NormalDepthProblem(ctypes.Structure):  # b2s_normal_depth_problem
+    _fields_ = [("n_kf", ctypes.c_int32), ("kf_center", _vp), ("n_mp", ctypes.c_int32), ("mp_pos", _vp),
+                ("mp_bad", _vp), ("mp_ref", _vp), ("obs_off", _vp), ("obs_kf", _vp), ("obs_octave", _vp),
+                ("scale_factors", _vp), ("n_levels", ctypes.c_int32)]
+
+
+class _NormalDepthResult(ctypes.Structure):  # b2s_normal_depth_result
+    _fields_ = [("normal", _vp), ("min_dist", _vp), ("max_dist", _vp), ("updated", _vp)]
+
+
+class _KfinsertProblem(ctypes.Structure):  # b2s_kfinsert_problem
+    _fields_ = [("n_kf", ctypes.c_int32), ("kf_center", _vp), ("kf_bad", _vp), ("cur", ctypes.c_int32),
+                ("cur_id", ctypes.c_uint64), ("n_slots", ctypes.c_int32), ("slot_mp", _vp), ("slot_stereo", _vp),
+                ("slot_desc", _vp), ("n_mp", ctypes.c_int32), ("mp_pos", _vp), ("mp_bad", _vp), ("mp_ref", _vp),
+                ("mp_nobs", _vp), ("mp_found", _vp), ("mp_visible", _vp), ("mp_first_kf", _vp), ("obs_off", _vp),
+                ("obs_kf", _vp), ("obs_idx", _vp), ("obs_octave", _vp), ("obs_desc", _vp),
+                ("n_recent", ctypes.c_int32), ("recent", _vp), ("scale_factors", _vp), ("n_levels", ctypes.c_int32),
+                ("monocular", ctypes.c_int32)]
+
+
+class _KfinsertResult(ctypes.Structure):  # b2s_kfinsert_result
+    _fields_ = [("mp_nobs", _vp), ("mp_bad", _vp), ("mp_added", _vp), ("obs_alive", _vp), ("mp_updated", _vp),
+                ("mp_normal", _vp), ("mp_min_dist", _vp), ("mp_max_dist", _vp), ("mp_desc", _vp), ("slot_mp", _vp),
+                ("list_mp", _vp), ("list_verdict", _vp), ("n_list", ctypes.c_int32), ("n_culled", ctypes.c_int32)]
+
+
 class _GbaResult(ctypes.Structure):
     _fields_ = [("Tcw_out", _vp), ("points_out", _vp), ("point_included", _vp), ("trace", _vp),
                 ("chi2_final", ctypes.c_double), ("n_trials", ctypes.c_int)]
@@ -308,6 +334,10 @@ def lib():
         L.b2s_keyframe_culling.argtypes = [_vp, ctypes.c_int, _vp, _vp]
         L.b2s_culling_last_ms.restype = ctypes.c_float
         L.b2s_culling_last_ms.argtypes = [_vp]
+        L.b2s_update_normal_and_depth.argtypes = [_vp, _vp, _vp]
+        L.b2s_matcher_last_ms.restype = ctypes.c_float
+        L.b2s_matcher_last_ms.argtypes = [_vp]
+        L.b2s_process_new_keyframe.argtypes = [_vp, ctypes.c_int, _vp, _vp]
         L.b2s_frame_grid_create.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp]
         L.b2s_frame_grid_create_device.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp, _vp]
         L.b2s_frame_grid_destroy.argtypes = [_vp]
@@ -670,6 +700,51 @@ class ORBmatcher(_Handle):
         L.b2s_distinctive_descriptors.argtypes = [_vp, _vp, _vp, ctypes.c_int, _vp]
         _check(L.b2s_distinctive_descriptors(self._h, _p(desc), _p(offsets), len(offsets) - 1, _p(best)))
         return best
+
+    def last_ms(self):
+        """Device time of the last UpdateNormalAndDepth or ProcessNewKeyFrame call (CUDA events: upload, kernels,
+        download)."""
+        return float(lib().b2s_matcher_last_ms(self._h))
+
+    def UpdateNormalAndDepth(self, d):
+        """MapPoint::UpdateNormalAndDepth (src/MapPoint.cc:477-521) for a batch of map points
+        (b2s_update_normal_and_depth).  d: a dict with the fields of b2s_normal_depth_problem as arrays (kf_center
+        (n_kf, 3), mp_pos (n_mp, 3), mp_bad, mp_ref, obs_off, obs_kf, obs_octave, scale_factors).  Returns a dict with
+        normal (n_mp, 3), min_dist, max_dist and updated; the entries of points not updated are 0."""
+        p, keep = normal_depth_problem(d)
+        M = p.n_mp
+        o = {"normal": np.zeros((M, 3), np.float32), "min_dist": np.zeros(M, np.float32),
+             "max_dist": np.zeros(M, np.float32), "updated": np.zeros(M, np.uint8)}
+        r = _NormalDepthResult(*[o[k].ctypes.data_as(_vp) for k in ("normal", "min_dist", "max_dist", "updated")])
+        _check(lib().b2s_update_normal_and_depth(self._h, ctypes.byref(p), ctypes.byref(r)))
+        return o
+
+    def ProcessNewKeyFrame(self, ds):
+        """ProcessNewKeyFrame's association and MapPointCulling (b2s_process_new_keyframe) for a list of independent
+        problem dicts (kfinsert_problem), or one; each result is a dict (kfinsert_outputs) trimmed to its list."""
+        one = isinstance(ds, dict)
+        rc, outs = self.raw_kfinsert([ds] if one else ds)
+        _check(rc)
+        return outs[0] if one else outs
+
+    def raw_kfinsert(self, ds):
+        """(status, [result dict per problem]); on an error the outputs stay as kfinsert_outputs made them."""
+        probs, keep, res, outs = [], [], [], []
+        for d in ds:
+            p, k = kfinsert_problem(d)
+            r, o = kfinsert_outputs(d)
+            probs.append(p)
+            keep.append(k)
+            res.append(r)
+            outs.append(o)
+        P = (_KfinsertProblem * len(ds))(*probs)
+        R = (_KfinsertResult * len(ds))(*res)
+        rc = lib().b2s_process_new_keyframe(self._h, len(ds), P, R)
+        for o, r in zip(outs, R):
+            o["n_list"], o["n_culled"] = r.n_list, r.n_culled
+            if rc == 0:
+                o["list_mp"], o["list_verdict"] = o["list_mp"][:r.n_list], o["list_verdict"][:r.n_list]
+        return rc, outs
 
     def SearchForTriangulation(self, kf1, kf2, F12, ex, ey, scale_factors, level_sigma2, only_stereo=False):
         """ORBmatcher::SearchForTriangulation (src/ORBmatcher.cc:810-1009). kf1/kf2: dicts with desc, node, has_mp, stereo,
@@ -1639,3 +1714,52 @@ class KeyFrameCulling(_Handle):
         rc, outs = self.raw([ds] if one else ds)
         _check(rc)
         return outs[0] if one else outs
+
+
+# ------------------------------------------------------------------------------------ keyframe insertion (ORBmatcher)
+_ND_ARRAYS = [("kf_center", np.float32), ("mp_pos", np.float32), ("mp_bad", np.uint8), ("mp_ref", np.int32),
+              ("obs_off", np.int32), ("obs_kf", np.int32), ("obs_octave", np.int32), ("scale_factors", np.float32)]
+_KFI_ARRAYS = [("kf_center", np.float32), ("kf_bad", np.uint8), ("slot_mp", np.int32), ("slot_stereo", np.uint8),
+               ("slot_desc", np.uint8), ("mp_pos", np.float32), ("mp_bad", np.uint8), ("mp_ref", np.int32),
+               ("mp_nobs", np.int32), ("mp_found", np.int32), ("mp_visible", np.int32), ("mp_first_kf", np.int64),
+               ("obs_off", np.int32), ("obs_kf", np.int32), ("obs_idx", np.int32), ("obs_octave", np.int32),
+               ("obs_desc", np.uint8), ("recent", np.int32), ("scale_factors", np.float32)]
+KFI_KEPT, KFI_BAD, KFI_CULLED_RATIO, KFI_CULLED_OBS, KFI_RETIRED = range(5)  # B2S_KFI_*
+
+
+def normal_depth_problem(d):
+    """(b2s_normal_depth_problem, the contiguous arrays it points into) from a dict with its fields as arrays."""
+    arr = {k: np.ascontiguousarray(d[k], t) for k, t in _ND_ARRAYS}
+    p = _NormalDepthProblem(n_kf=len(arr["kf_center"]), n_mp=len(arr["mp_bad"]),
+                            n_levels=len(arr["scale_factors"]))
+    for k, _ in _ND_ARRAYS:
+        setattr(p, k, arr[k].ctypes.data_as(_vp))
+    return p, arr
+
+
+def kfinsert_problem(d):
+    """(b2s_kfinsert_problem, the contiguous arrays it points into) from a problem dict with the fields of
+    b2s_kfinsert_problem (arrays: kf_center (n_kf, 3), slot_desc (n_slots, 32), mp_pos (n_mp, 3), obs_desc (n_obs, 32);
+    cur and cur_id ints; monocular a bool; the counts follow from the arrays)."""
+    arr = {k: np.ascontiguousarray(d[k], t) for k, t in _KFI_ARRAYS}
+    p = _KfinsertProblem(n_kf=len(arr["kf_center"]), cur=int(d["cur"]), cur_id=int(d["cur_id"]),
+                         n_slots=len(arr["slot_mp"]), n_mp=len(arr["mp_bad"]), n_recent=len(arr["recent"]),
+                         n_levels=len(arr["scale_factors"]), monocular=1 if d["monocular"] else 0)
+    for k, _ in _KFI_ARRAYS:
+        setattr(p, k, arr[k].ctypes.data_as(_vp))
+    return p, arr
+
+
+def kfinsert_outputs(d):
+    """(b2s_kfinsert_result, its output arrays as a dict) sized for problem dict d; entries the call does not write
+    (the normal, distances of points not updated) stay 0."""
+    M, S, R = len(d["mp_bad"]), len(d["slot_mp"]), len(d["recent"])
+    o = {"mp_nobs": np.zeros(M, np.int32), "mp_bad": np.zeros(M, np.uint8), "mp_added": np.zeros(M, np.int32),
+         "obs_alive": np.zeros(int(np.asarray(d["obs_off"])[-1]), np.uint8), "mp_updated": np.zeros(M, np.uint8),
+         "mp_normal": np.zeros((M, 3), np.float32), "mp_min_dist": np.zeros(M, np.float32),
+         "mp_max_dist": np.zeros(M, np.float32), "mp_desc": np.zeros(M, np.int32), "slot_mp": np.zeros(S, np.int32),
+         "list_mp": np.zeros(R + S, np.int32), "list_verdict": np.zeros(R + S, np.uint8)}
+    r = _KfinsertResult()
+    for k, v in o.items():
+        setattr(r, k, v.ctypes.data_as(_vp))
+    return r, o

@@ -18,7 +18,7 @@ NVCC_FLAGS = GENCODE + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-
 # extractor/matcher/keyframe database: bit-exact float arithmetic, never contract a*b+c; LocalBA is FP64 with a 1e-5 bar
 # -> FMA allowed; the essential graph differentiates numerically (delta = 1e-9 amplifies last-bit differences ~5e8 times)
 NO_FMAD = {"extractor.cu", "extractor_tile.cu", "matcher.cu", "common.cu", "kfdb.cu", "essential.cu", "sim3opt.cu",
-            "initializer.cu", "sim3solver.cu", "pnpsolver.cu"}
+            "initializer.cu", "sim3solver.cu", "pnpsolver.cu", "mappoint.cu"}
 
 
 def _newer(target, sources):
@@ -48,6 +48,9 @@ def _deps_of(src):
         deps.append(os.path.join(CSRC, "chol.cuh"))
     if base in ("initializer.cu", "pnpsolver.cu"):
         deps.append(os.path.join(CSRC, "jacobi.cuh"))
+    if base in ("matcher.cu", "mappoint.cu"):
+        deps.append(os.path.join(CSRC, "matcher.cuh"))
+        deps.append(os.path.join(CSRC, "distinctive.cuh"))
     if base == "extractor.cu":
         deps.append(os.path.join(ROOT, "data", "orb_pattern_31.inc"))
     return deps
@@ -109,6 +112,9 @@ def build_oracle(force=False):
     # the keyframe culling's CPU restatement (oracle/culling.mk)
     subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "culling.mk"] + (["-B"] if force else []) +
                           ["liborb_culling.so"])
+    # the keyframe insertion's CPU restatement (oracle/kfinsert.mk)
+    subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "kfinsert.mk"] + (["-B"] if force else []) +
+                          ["liborb_kfinsert.so"])
     return ORACLE_LIB
 
 
@@ -129,6 +135,7 @@ def build_oracle_ref():
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "pnpsolver.mk", "pnpsolver-ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "covis.mk", "covis-ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "culling.mk", "culling-ref", "REF=" + ref])
+    subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "kfinsert.mk", "kfinsert-ref", "REF=" + ref])
     return os.path.join(ORACLE_DIR, "_ref")
 
 

@@ -13,6 +13,8 @@
 #include <vector>
 
 #include "common.cuh"
+#include "distinctive.cuh"
+#include "matcher.cuh"
 
 namespace b2s {
 
@@ -1014,9 +1016,7 @@ __global__ void __launch_bounds__(128) k_bow_transform(const uint8_t* __restrict
 }
 
 // ------------------------------------------------------------------------------------------------
-// MapPoint::ComputeDistinctiveDescriptors (src/MapPoint.cc:359-440): one warp per map point.  For every observation i the
-// median (sorted row element floor(0.5*(N-1))) of its distances to all observations is read off a 257-bin histogram
-// built by the warp; the first row with the smallest median wins.
+// MapPoint::ComputeDistinctiveDescriptors (src/MapPoint.cc:359-440): one warp per map point (distinctive.cuh).
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_distinctive(const uint8_t* __restrict__ desc, const int32_t* __restrict__ offsets,
                                                      int nPoints, int32_t* __restrict__ bestIdx) {
@@ -1029,43 +1029,7 @@ __global__ void __launch_bounds__(256) k_distinctive(const uint8_t* __restrict__
     if (lane == 0) bestIdx[p] = -1;
     return;
   }
-  int* h = hist[wid];
-  const int kth = (int)(0.5 * (double)(N - 1));
-  int bestMedian = 0x7fffffff, best = 0;
-  for (int i = 0; i < N; i++) {
-    for (int b = lane; b < 257; b += 32) h[b] = 0;
-    __syncwarp();
-    const u256 di = ld_desc(desc, beg + i);
-    for (int j = lane; j < N; j += 32) atomicAdd(&h[(j == i) ? 0 : hamming256(di, ld_desc(desc, beg + j))], 1);
-    __syncwarp();
-    // smallest value v with #(distances <= v) > kth: warp scan over 257 bins (9 per lane)
-    int local[9], sum = 0;
-#pragma unroll
-    for (int t = 0; t < 9; t++) {
-      const int b = lane * 9 + t;
-      local[t] = (b < 257) ? h[b] : 0;
-      sum += local[t];
-    }
-    int incl = sum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int v = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += v;
-    }
-    int run = incl - sum, med = 0x7fffffff;
-#pragma unroll
-    for (int t = 0; t < 9; t++) {
-      run += local[t];
-      if (med == 0x7fffffff && run > kth && lane * 9 + t < 257) med = lane * 9 + t;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) med = min(med, __shfl_xor_sync(0xffffffffu, med, o));
-    if (med < bestMedian) {  // strict: the first minimum wins (:424-428)
-      bestMedian = med;
-      best = i;
-    }
-    __syncwarp();
-  }
+  const int best = distinctive_best(N, [&](int i) { return ld_desc(desc, beg + i); }, hist[wid], lane);
   if (lane == 0) bestIdx[p] = best;
 }
 
@@ -1455,25 +1419,6 @@ __global__ void __launch_bounds__(32) k_grid_query(float x, float y, float r, in
 }  // namespace b2s
 
 using namespace b2s;
-
-struct b2s_matcher : b2s::Stage {
-  int maxF, maxBatch;
-  long long launches = 0;
-  // device work buffers
-  uint8_t *dDescA = nullptr, *dDescB = nullptr, *dValidA = nullptr, *dValidB = nullptr, *dOcc = nullptr, *dTaken = nullptr;
-  int32_t *dNodeA = nullptr, *dNodeB = nullptr, *dNA = nullptr, *dNB = nullptr, *dOrder = nullptr, *dCandCnt = nullptr;
-  int32_t *dMatch = nullptr, *dBin = nullptr, *dNMatches = nullptr, *dOct = nullptr, *dCellKey = nullptr;
-  int32_t *dCellStart = nullptr, *dTopkIdx = nullptr, *dExtra = nullptr, *dHist = nullptr, *dPush = nullptr;
-  float *dAngA = nullptr, *dAngB = nullptr, *dKpx = nullptr, *dKpy = nullptr, *dURight = nullptr;
-  uint32_t* dTopk = nullptr;
-  ProjQuery* dQueries = nullptr;
-  // record staging of b2s_search_by_projection_last_batch and b2s_search_by_projection_sequence (grown on first use)
-  DevBuf dKpsStage;
-  // the rest of the staging of b2s_search_by_projection_sequence: records of batch + 1 frames
-  DevBuf dSeqDesc, dSeqDepth, dSeqT, dSeqN;
-  // b2s_distinctive_descriptors: descriptors, point offsets and results
-  DevBuf dDistDesc, dDistOff, dDistBest;
-};
 
 extern "C" int b2s_matcher_create(int max_features, int max_batch, int device, b2s_matcher** out) {
   if (!out || max_features < 1 || max_features > 65535 || max_batch < 1) {
