@@ -209,11 +209,30 @@ void orc_distinctive_descriptors(const uint8_t* desc, const int32_t* offsets, in
  * kps: level-0 coordinates as produced by the extractor; pyr*: dense level images (stride = width), lvlW/lvlH their
  * sizes; scale / inv_scale = mvScaleFactors / mvInvScaleFactors; mb = the baseline the reference sees at that point
  * (0 in this fork: it is assigned after the call, so maxD = +inf).  Outputs mvuRight / mvDepth (-1 = no match).
- * Returns the number of stereo matches that survive the cull. */
+ * Returns the number of stereo matches that survive the cull.
+ * orc_compute_stereo_matches_reason computes the same and, where reason is not NULL, writes per left keypoint the
+ * decision that settled it (ORC_ST_*). */
+enum {
+  ORC_ST_KEPT = 0,       /* matched and kept by the cull */
+  ORC_ST_KEPT_ZERO = 1,  /* kept, with disparity <= 0 replaced by 0.01 (bestuR = uL - 0.01 in double) */
+  ORC_ST_NO_ROW = 2,     /* the left row has no right keypoint in its band (or lies outside the image) */
+  ORC_ST_MAXU = 3,       /* maxU = uL - minD < 0 */
+  ORC_ST_NO_CAND = 4,    /* no right keypoint of the row passes the octave and u gates */
+  ORC_ST_HAMMING = 5,    /* best Hamming distance >= thOrbDist (75) */
+  ORC_ST_WINDOW = 6,     /* the 11x11 windows leave the pyramid level (the iniu / endu test, or a range OpenCV asserts on) */
+  ORC_ST_EDGE = 7,       /* SAD minimum at bestincR == +-L */
+  ORC_ST_DELTA = 8,      /* parabola offset outside [-1, 1] */
+  ORC_ST_DISPARITY = 9,  /* disparity outside [minD, maxD) */
+  ORC_ST_CULLED = 10     /* matched, then removed by the median cull (SAD >= 1.5f*1.4f*median) */
+};
 int orc_compute_stereo_matches(const orc_keypoint* kpsL, const uint8_t* descL, int nL, const orc_keypoint* kpsR,
                                const uint8_t* descR, int nR, const uint8_t* const* pyrL, const uint8_t* const* pyrR,
                                const int* lvlW, const int* lvlH, const float* scale, const float* inv_scale, int nlevels,
                                float mbf, float mb, float* uright, float* depth);
+int orc_compute_stereo_matches_reason(const orc_keypoint* kpsL, const uint8_t* descL, int nL, const orc_keypoint* kpsR,
+                                      const uint8_t* descR, int nR, const uint8_t* const* pyrL, const uint8_t* const* pyrR,
+                                      const int* lvlW, const int* lvlH, const float* scale, const float* inv_scale,
+                                      int nlevels, float mbf, float mb, float* uright, float* depth, int32_t* reason);
 
 /* ---------------- PoseOptimization (src/Optimizer.cc:363-605 + vendored g2o; SURVEY §8f rank 2) ---------------- */
 typedef struct {

@@ -13,12 +13,14 @@ namespace {
 const int TH_HIGH = 100, TH_LOW = 50;  // include/ORBmatcher.h:199-200
 }
 
-extern "C" int orc_compute_stereo_matches(const orc_keypoint* kpsL, const uint8_t* descL, int N, const orc_keypoint* kpsR,
-                                          const uint8_t* descR, int Nr, const uint8_t* const* pyrL,
-                                          const uint8_t* const* pyrR, const int* lvlW, const int* lvlH, const float* scale,
-                                          const float* inv_scale, int nlevels, float mbf, float mb, float* mvuRight,
-                                          float* mvDepth) {
+extern "C" int orc_compute_stereo_matches_reason(const orc_keypoint* kpsL, const uint8_t* descL, int N,
+                                                 const orc_keypoint* kpsR, const uint8_t* descR, int Nr,
+                                                 const uint8_t* const* pyrL, const uint8_t* const* pyrR, const int* lvlW,
+                                                 const int* lvlH, const float* scale, const float* inv_scale, int nlevels,
+                                                 float mbf, float mb, float* mvuRight, float* mvDepth, int32_t* reason) {
   (void)nlevels;
+  int32_t noReason = 0;  // where reason is NULL every write goes here
+  auto why = [&](int i) -> int32_t& { return reason ? reason[i] : noReason; };
   for (int i = 0; i < N; i++) {  // :1029-1030
     mvuRight[i] = -1.0f;
     mvDepth[i] = -1.0f;
@@ -45,19 +47,23 @@ extern "C" int orc_compute_stereo_matches(const orc_keypoint* kpsL, const uint8_
     const int levelL = kpL.octave;
     const float vL = kpL.y, uL = kpL.x;
     const int row = (int)vL;  // vRowIndices[vL]: float -> index conversion truncates
+    why(iL) = ORC_ST_NO_ROW;
     if (row < 0 || row >= nRows) continue;
     const std::vector<size_t>& vCandidates = vRowIndices[row];
     if (vCandidates.empty()) continue;
     const float minU = uL - maxD, maxU = uL - minD;
+    why(iL) = ORC_ST_MAXU;
     if (maxU < 0) continue;
     int bestDist = TH_HIGH;
     size_t bestIdxR = 0;
+    why(iL) = ORC_ST_NO_CAND;
     for (size_t iC = 0; iC < vCandidates.size(); iC++) {  // :1169-1219
       const size_t iR = vCandidates[iC];
       const orc_keypoint& kpR = kpsR[iR];
       if (kpR.octave < levelL - 1 || kpR.octave > levelL + 1) continue;
       const float uR = kpR.x;
       if (uR >= minU && uR <= maxU) {
+        why(iL) = ORC_ST_HAMMING;
         const int dist = orc_descriptor_distance(descL + (size_t)iL * 32, descR + iR * 32);
         if (dist < bestDist) {
           bestDist = dist;
@@ -82,6 +88,7 @@ extern "C" int orc_compute_stereo_matches(const orc_keypoint* kpsL, const uint8_
       float vDists[2 * 5 + 1];
       const float iniu = scaleduR0 + L - w;
       const float endu = scaleduR0 + L + w + 1;
+      why(iL) = ORC_ST_WINDOW;
       if (iniu < 0 || endu >= lw) continue;  // :1290
       // cv::Mat::rowRange/colRange would assert outside the image; guard the same accesses (never hit for real keypoints)
       if (cy - w < 0 || cy + w >= lh || cxL - w < 0 || cxL + w >= lw || cxR0 - L - w < 0) continue;
@@ -102,18 +109,23 @@ extern "C" int orc_compute_stereo_matches(const orc_keypoint* kpsL, const uint8_
         }
         vDists[L + incR] = dist;
       }
+      why(iL) = ORC_ST_EDGE;
       if (bestincR == -L || bestincR == L) continue;
       const float dist1 = vDists[L + bestincR - 1];
       const float dist2 = vDists[L + bestincR];
       const float dist3 = vDists[L + bestincR + 1];
       const float deltaR = (dist1 - dist3) / (2.0f * (dist1 + dist3 - 2.0f * dist2));
+      why(iL) = ORC_ST_DELTA;
       if (deltaR < -1 || deltaR > 1) continue;
       float bestuR = scale[kpL.octave] * ((float)scaleduR0 + (float)bestincR + deltaR);
       float disparity = (uL - bestuR);
+      why(iL) = ORC_ST_DISPARITY;
       if (disparity >= minD && disparity < maxD) {
+        why(iL) = ORC_ST_KEPT;
         if (disparity <= 0) {
           disparity = 0.01;
           bestuR = uL - 0.01;
+          why(iL) = ORC_ST_KEPT_ZERO;
         }
         mvDepth[iL] = mbf / disparity;
         mvuRight[iL] = bestuR;
@@ -130,7 +142,17 @@ extern "C" int orc_compute_stereo_matches(const orc_keypoint* kpsL, const uint8_
     if (vDistIdx[i].first < thDist) break;
     mvuRight[vDistIdx[i].second] = -1;
     mvDepth[vDistIdx[i].second] = -1;
+    why(vDistIdx[i].second) = ORC_ST_CULLED;
     kept--;
   }
   return kept;
+}
+
+extern "C" int orc_compute_stereo_matches(const orc_keypoint* kpsL, const uint8_t* descL, int N, const orc_keypoint* kpsR,
+                                          const uint8_t* descR, int Nr, const uint8_t* const* pyrL,
+                                          const uint8_t* const* pyrR, const int* lvlW, const int* lvlH, const float* scale,
+                                          const float* inv_scale, int nlevels, float mbf, float mb, float* mvuRight,
+                                          float* mvDepth) {
+  return orc_compute_stereo_matches_reason(kpsL, descL, N, kpsR, descR, Nr, pyrL, pyrR, lvlW, lvlH, scale, inv_scale,
+                                           nlevels, mbf, mb, mvuRight, mvDepth, nullptr);
 }

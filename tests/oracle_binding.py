@@ -278,8 +278,9 @@ class Oracle:
                                       P(best), P(bdist))
         return n, best, bdist
 
-    def compute_stereo_matches(self, exL, exR, kpsL, descL, kpsR, descR, bf, mb=0.0):
-        """exL / exR: OracleExtractor objects that just extracted the left / right image (their pyramids are used)."""
+    def compute_stereo_matches(self, exL, exR, kpsL, descL, kpsR, descR, bf, mb=0.0, reason=None):
+        """exL / exR: OracleExtractor objects that just extracted the left / right image (their pyramids are used).
+        reason: None, or an int32 array of len(kpsL) that receives each left keypoint's ORC_ST_* decision."""
         nl = exL.nlevels
         lv_l = [exL.level(l) for l in range(nl)]
         lv_r = [exR.level(l) for l in range(nl)]
@@ -292,10 +293,11 @@ class Oracle:
         kpsR, descR = np.ascontiguousarray(kpsR), np.ascontiguousarray(descR)
         ur = np.zeros(len(kpsL), np.float32)
         dp = np.zeros(len(kpsL), np.float32)
-        self.L.orc_compute_stereo_matches.argtypes = [vp, vp, ctypes.c_int, vp, vp, ctypes.c_int, vp, vp, vp, vp, vp, vp,
-                                                      ctypes.c_int, ctypes.c_float, ctypes.c_float, vp, vp]
-        n = self.L.orc_compute_stereo_matches(P(kpsL), P(descL), len(kpsL), P(kpsR), P(descR), len(kpsR), pl, pr, P(W), P(H),
-                                              P(sc), P(isc), nl, bf, mb, P(ur), P(dp))
+        fn = self.L.orc_compute_stereo_matches_reason
+        fn.argtypes = [vp, vp, ctypes.c_int, vp, vp, ctypes.c_int, vp, vp, vp, vp, vp, vp, ctypes.c_int, ctypes.c_float,
+                       ctypes.c_float, vp, vp, vp]
+        n = fn(P(kpsL), P(descL), len(kpsL), P(kpsR), P(descR), len(kpsR), pl, pr, P(W), P(H),
+                 P(sc), P(isc), nl, bf, mb, P(ur), P(dp), P(reason))
         return n, ur, dp
 
     def distinctive_descriptors(self, desc, offsets):
