@@ -132,6 +132,43 @@ int b2s_stereo_match_device(b2s_extractor* h, int first_left, int first_right, i
 int b2s_stereo_match(b2s_extractor* h, int first_left, int first_right, int n_pairs, float bf, float mb, float* uright,
                      float* depth, int cap_out, int32_t* n_matched);
 
+/* ------------------------------------------------------------------ undistortion and RGB-D depth (monocular / RGB-D) */
+/* The keypoint records of b2s_extract_batch_device are the distorted mvKeys.  These calls give the rest of an
+ * undistorted or RGB-D Frame on the device, in the record layouts the grid and matchers take:
+ *   K4 = fx, fy, cx, cy (host floats); dist = k1, k2, p1, p2 [, k3] (host floats), n_dist = 4 or 5 (src/Tracking.cc:115-127
+ *   builds 5 only when k3 != 0).
+ * The undistortion is cv::undistortPoints(pts, K, dist, noArray(), K) of OpenCV 4 (5 iterations, in double, each
+ * operation rounded on its own): bit-identical to cv2.undistortPoints 4.x.  OpenCV 3.2, which the reference was written
+ * against, lacks one branch: when an iteration's icdist < 0 (only for very strong barrel distortion far from the
+ * centre) OpenCV 4 returns the first normalised point and 3.2 keeps iterating.
+ * Refused arguments (B2S_ERR_BAD_ARG, nothing written): a null pointer, batch < 1 or > 65535, cap < 1, n_dist not 4 or 5,
+ * a non-finite K4 or dist entry, fx or fy == 0; for the depth call width or height < 1 and a pitch smaller than width*4
+ * or not a multiple of 4.  A null handle when no device is present: B2S_ERR_NO_DEVICE.
+ * Records: d_counts[b] (device) keypoints of image b at d_kps[b*cap ..].  The _device calls cannot check the counts
+ * before they launch: a count above cap is read as cap (the records past cap are ignored), a negative count as 0.  Only
+ * the first min(d_counts[b], cap) entries of each image's output are written; the rest are left untouched. */
+
+/* Frame::UndistortKeyPoints (src/Frame.cc:899-964): d_kps_un[b*cap + i] = d_kps[b*cap + i] with x, y undistorted
+ * (mvKeysUn).  When dist[0] (k1) == 0 the records are copied unchanged, as the reference does, even if p1, p2 or k3 are
+ * not 0.  d_kps_un may equal d_kps.  Asynchronous on `stream` (NULL = the handle's own stream). */
+int b2s_undistort_keypoints_device(b2s_extractor* h, const b2s_keypoint* d_kps, const int32_t* d_counts, int batch, int cap,
+                                   const float* K4, const float* dist, int n_dist, b2s_keypoint* d_kps_un, void* stream);
+/* cv::undistortPoints on n HOST points (xy: n x 2 floats; xy_out may equal xy), run on the handle's device; synchronous.
+ * Unlike the keypoint call it always undistorts, k1 == 0 included.  Frame::ComputeImageBounds (src/Frame.cc:967-1014) is
+ * this on the corners (0,0), (cols,0), (0,rows), (cols,rows) when k1 != 0, then mnMinX = min(c0.x, c2.x),
+ * mnMaxX = max(c1.x, c3.x), mnMinY = min(c0.y, c1.y), mnMaxY = max(c2.y, c3.y); else 0, cols, 0, rows. */
+int b2s_undistort_points(b2s_extractor* h, const float* xy, int n, const float* K4, const float* dist, int n_dist,
+                         float* xy_out);
+/* Frame::ComputeStereoFromRGBD (src/Frame.cc:1423-1461): d_depth holds `batch` float depth images (metres: the image
+ * after Tracking::GrabImageRGBD's convertTo; the unit conversion is the caller's) of width x height, image b at
+ * d_depth + b*height*depth_pitch_bytes bytes.  For keypoint i of image b: d = depth at row (int)kp.y, column (int)kp.x of
+ * the distorted record d_kps; if d > 0 (false for 0, negatives and NaN) d_depth_out = d and d_uright =
+ * d_kps_un.x - bf/d (float), else both -1.  A keypoint whose truncated position lies outside the depth image gets -1
+ * (the reference would read outside the image).  Outputs [batch][cap] like b2s_stereo_match_device.  Asynchronous. */
+int b2s_stereo_from_depth_device(b2s_extractor* h, const b2s_keypoint* d_kps, const b2s_keypoint* d_kps_un,
+                                 const int32_t* d_counts, int batch, int cap, const float* d_depth, size_t depth_pitch_bytes,
+                                 int width, int height, float bf, float* d_uright, float* d_depth_out, void* stream);
+
 /* ------------------------------------------------------------------ matcher */
 typedef struct b2s_matcher b2s_matcher;
 int b2s_matcher_create(int max_features, int max_batch, int device, b2s_matcher** out);

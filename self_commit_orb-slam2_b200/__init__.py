@@ -239,6 +239,11 @@ def lib():
         L.b2s_extract_batch_device.argtypes = [_vp, _vp, ctypes.c_size_t, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                                ctypes.c_int, _vp, _vp, _vp, ctypes.c_int, _vp]
         L.b2s_extractor_check.argtypes = [_vp]
+        L.b2s_undistort_keypoints_device.argtypes = [_vp, _vp, _vp, ctypes.c_int, ctypes.c_int, _vp, _vp, ctypes.c_int, _vp,
+                                                     _vp]
+        L.b2s_undistort_points.argtypes = [_vp, _vp, ctypes.c_int, _vp, _vp, ctypes.c_int, _vp]
+        L.b2s_stereo_from_depth_device.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int, ctypes.c_int, _vp, ctypes.c_size_t,
+                                                   ctypes.c_int, ctypes.c_int, ctypes.c_float, _vp, _vp, _vp]
         L.b2s_extractor_set_timing.argtypes = [_vp, ctypes.c_int]
         L.b2s_extractor_get_timing.argtypes = [_vp, _vp, _vp]
         L.b2s_extractor_debug_level.argtypes = [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]
@@ -382,6 +387,21 @@ def _p(a):
     return None if a is None else a.ctypes.data_as(_vp)
 
 
+def _dptr(t):
+    """Device address of a CUDA tensor (contiguous), or an address given as an int."""
+    if isinstance(t, int):
+        return _vp(t)
+    assert t.is_cuda and t.is_contiguous(), "expected a contiguous CUDA tensor"
+    return _vp(t.data_ptr())
+
+
+def _calib(K, dist):
+    """(fx, fy, cx, cy) and the distortion coefficients as float32 arrays, from a 3 x 3 camera matrix or four values."""
+    K = np.asarray(K, np.float32)
+    K4 = np.float32([K[0, 0], K[1, 1], K[0, 2], K[1, 2]]) if K.shape == (3, 3) else np.ascontiguousarray(K.reshape(4))
+    return K4, np.ascontiguousarray(np.asarray(dist, np.float32).reshape(-1))
+
+
 def device_count():
     return lib().b2s_device_count()
 
@@ -500,6 +520,44 @@ class ORBextractor(_Handle):
         _check(L.b2s_stereo_match_device(self._h, first_left, first_right, n_pairs, _vp(d_kps_ptr), _vp(d_desc_ptr),
                                          _vp(d_counts_ptr), cap, float(bf), float(mb), _vp(d_uright_ptr),
                                          _vp(d_depth_ptr), _vp(d_nmatched_ptr), _vp(stream)))
+
+    # monocular / RGB-D frames: Frame::UndistortKeyPoints, ComputeImageBounds, ComputeStereoFromRGBD (src/Frame.cc:899-1014,
+    # :1423-1461).  K: the 3 x 3 camera matrix or (fx, fy, cx, cy); dist: k1, k2, p1, p2 [, k3].  Device arguments are
+    # CUDA tensors (or device addresses); stream None = the handle's own stream.
+    def undistort_keypoints_device(self, kps, counts, batch, cap, K, dist, kps_un, stream=None):
+        """mvKeysUn of `batch` images of extractor records (kps: [batch, cap] records, counts: [batch] int32) into kps_un
+        (may be kps); k1 == 0 copies the records.  Asynchronous."""
+        K4, d = _calib(K, dist)
+        _check(lib().b2s_undistort_keypoints_device(self._h, _dptr(kps), _dptr(counts), int(batch), int(cap), _p(K4), _p(d),
+                                                    len(d), _dptr(kps_un), _vp(stream) if stream else None))
+
+    def stereo_from_depth_device(self, kps, kps_un, counts, batch, cap, depth, bf, uright, depth_out, stream=None):
+        """mvuRight / mvDepth ([batch, cap] float32 tensors) from depth: a float32 CUDA tensor [batch, height, width] in
+        metres whose rows may be padded.  Asynchronous."""
+        B, H, W = depth.shape
+        assert depth.is_cuda and depth.dtype.itemsize == 4 and depth.stride(2) == 1 and depth.stride(0) == H * depth.stride(1)
+        _check(lib().b2s_stereo_from_depth_device(self._h, _dptr(kps), _dptr(kps_un), _dptr(counts), int(batch), int(cap),
+                                                  _vp(depth.data_ptr()), depth.stride(1) * 4, W, H, float(bf), _dptr(uright),
+                                                  _dptr(depth_out), _vp(stream) if stream else None))
+
+    def undistort_points(self, xy, K, dist):
+        """cv::undistortPoints(xy, K, dist, noArray(), K) on host points (n x 2); always undistorts, k1 == 0 included."""
+        K4, d = _calib(K, dist)
+        pts = np.ascontiguousarray(np.asarray(xy, np.float32).reshape(-1, 2))
+        out = np.empty_like(pts)
+        _check(lib().b2s_undistort_points(self._h, _p(pts), len(pts), _p(K4), _p(d), len(d), _p(out)))
+        return out
+
+    def image_bounds(self, width, height, K, dist):
+        """Frame::ComputeImageBounds (src/Frame.cc:967-1014) as the mnMinX / mnMaxX / mnMinY / mnMaxY entries of a frame
+        geometry (the dict FrameGrid and the matchers take)."""
+        K4, d = _calib(K, dist)
+        if d[0] == 0:
+            b = np.float32([0, width, 0, height])
+        else:
+            c = self.undistort_points([[0, 0], [width, 0], [0, height], [width, height]], K4, d)
+            b = np.float32([min(c[0, 0], c[2, 0]), max(c[1, 0], c[3, 0]), min(c[0, 1], c[1, 1]), max(c[2, 1], c[3, 1])])
+        return dict(mnMinX=b[0], mnMaxX=b[1], mnMinY=b[2], mnMaxY=b[3])
 
     def check(self):
         _check(lib().b2s_extractor_check(self._h))

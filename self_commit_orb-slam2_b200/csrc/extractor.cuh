@@ -103,6 +103,7 @@ struct b2s_extractor : b2s::Stage {
   // stereo matching scratch + bookkeeping of the last host-buffer batch extraction (b2s_stereo_match)
   b2s::DevBuf dStereoSad, dStereoU, dStereoD, dStereoN;
   int lastCap = 0, lastBatch = 0;
+  b2s::DevBuf dUndistortXY;  // b2s_undistort_points (undistort.cu)
   // pinned staging for the host-buffer entry points
   b2s_keypoint* hKps = nullptr;
   uint8_t* hDesc = nullptr;
