@@ -168,6 +168,49 @@ int b2s_undistort_points(b2s_extractor* h, const float* xy, int n, const float* 
 int b2s_stereo_from_depth_device(b2s_extractor* h, const b2s_keypoint* d_kps, const b2s_keypoint* d_kps_un,
                                  const int32_t* d_counts, int batch, int cap, const float* d_depth, size_t depth_pitch_bytes,
                                  int width, int height, float bf, float* d_uright, float* d_depth_out, void* stream);
+/* Frame::ComputeStereoFromRGBD on the sensor's 16-bit depth, with GrabImageRGBD's convertTo(CV_32F, mDepthMapFactor)
+ * (src/Tracking.cc:334-338) folded in and done only at the keypoints (Frame reads the depth image nowhere else):
+ * depth_map_factor is the settings value (DepthMapFactor), turned into the multiplier as src/Tracking.cc:212-216 does
+ * (1 when |DepthMapFactor| < 1e-5, else 1.0f / DepthMapFactor).  The depth of a raw value is (float)raw * multiplier,
+ * rounded once: a u16 times a float is exact in double, so this is OpenCV's convertTo whatever precision it multiplies in.
+ * Then the rules of b2s_stereo_from_depth_device.  d_depth: `batch` images of width x height uint16, rows
+ * depth_row_bytes apart (a multiple of 2, >= width*2), image b at d_depth + b*height*depth_row_bytes bytes.  Refused
+ * as the float call, and for a non-finite depth_map_factor.  Asynchronous on `stream`. */
+int b2s_stereo_from_depth_u16_device(b2s_extractor* h, const b2s_keypoint* d_kps, const b2s_keypoint* d_kps_un,
+                                     const int32_t* d_counts, int batch, int cap, const uint16_t* d_depth,
+                                     size_t depth_row_bytes, int width, int height, float depth_map_factor, float bf,
+                                     float* d_uright, float* d_depth_out, void* stream);
+
+/* ------------------------------------------------------------------ frame ingest (colour to grey, stereo rectification) */
+/* Tracking::GrabImage* step 1 (src/Tracking.cc:252-278, 313-326, 371-384), optionally preceded by the stereo examples'
+ * cv::remap(src, dst, mapx, mapy, INTER_LINEAR) with CV_32FC1 maps (BORDER_CONSTANT 0; Examples/Stereo/stereo_euroc.cc,
+ * Examples/ROS/ORB_SLAM2/src/ros_stereo.cc).  `batch` images share one map pair (call once per camera).
+ *   Source: image b at d_src + b*src_image_bytes, rows src_row_bytes apart, src_width x src_height pixels of `channels`
+ *   (1, 3, 4) interleaved bytes.  rgb = mbRGB (Camera.RGB), ignored for 1 channel: it, not the data, says whether byte 0
+ *   is R (RGB2GRAY / RGBA2GRAY) or B (BGR2GRAY / BGRA2GRAY).  One channel is copied (the reference's pass-through).
+ *   Maps: both or neither; width x height floats, rows map_row_bytes apart (a multiple of 4, >= width*4).  Without maps
+ *   width and height must equal the source's.
+ *   Output: grey image b at d_out + b*out_image_bytes, rows out_row_bytes apart (the layout b2s_extract_batch_device
+ *   reads); bytes outside the width x height pixels are never written.
+ * Grey (OpenCV 4.x, exact on all 2^24 triples against cv2 4.13): Y = (9798 R + 19235 G + 3735 B + 16384) >> 15, alpha
+ * ignored.  Older OpenCV releases are believed to use the 14-bit form (4899, 9617, 1868, shift 14), which differs on
+ * 43,864 triples; whether OpenCV 3.2, which the reference was written against, does is not checked (DESIGN.md §2, deviation 9).
+ * Remap, per output pixel and channel: X = cvRound(mapx*32), Y = cvRound(mapy*32) (half to even; the x32 is exact);
+ * sx = X >> 5, sy = Y >> 5, ax = X & 31, ay = Y & 31; taps (sx, sy), (sx+1, sy), (sx, sy+1), (sx+1, sy+1) with weights
+ * (32-ax)(32-ay), ax(32-ay), (32-ax)ay, ax*ay; a tap outside the source contributes 0; dst = (sum + 512) >> 10.  This is
+ * OpenCV's Q15 table (every entry exact, so no sum correction) and equals cv2.remap byte for byte.  A NaN coordinate is
+ * outside the image (x86's cvRound gives INT_MIN; the device's round-to-int would give 0, so NaN is sent outside
+ * explicitly); +-inf and huge coordinates saturate outside.  A colour image is remapped channel by channel (alpha is
+ * skipped: it cannot reach the output) and converted to grey afterwards: remap and grey conversion do not commute.
+ * Refused (B2S_ERR_BAD_ARG, nothing written): a null handle, source or output, exactly one map, batch outside 1..65535,
+ * channels not 1, 3 or 4, a size below 1 or above 8192, a row pitch below the row's bytes, an image pitch below
+ * rows * row pitch, a map pitch not a multiple of 4 or below width*4, without maps an output size other than the
+ * source's.  A null handle when no device is present: B2S_ERR_NO_DEVICE.  Asynchronous on `stream` (NULL = the
+ * handle's own stream). */
+int b2s_prepare_images_device(b2s_extractor* h, const uint8_t* d_src, size_t src_row_bytes, size_t src_image_bytes,
+                              int batch, int src_width, int src_height, int channels, int rgb, const float* d_mapx,
+                              const float* d_mapy, size_t map_row_bytes, int width, int height, uint8_t* d_out,
+                              size_t out_row_bytes, size_t out_image_bytes, void* stream);
 
 /* ------------------------------------------------------------------ matcher */
 typedef struct b2s_matcher b2s_matcher;

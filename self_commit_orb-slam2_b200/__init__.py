@@ -244,6 +244,12 @@ def lib():
         L.b2s_undistort_points.argtypes = [_vp, _vp, ctypes.c_int, _vp, _vp, ctypes.c_int, _vp]
         L.b2s_stereo_from_depth_device.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int, ctypes.c_int, _vp, ctypes.c_size_t,
                                                    ctypes.c_int, ctypes.c_int, ctypes.c_float, _vp, _vp, _vp]
+        L.b2s_stereo_from_depth_u16_device.argtypes = [_vp, _vp, _vp, _vp, ctypes.c_int, ctypes.c_int, _vp, ctypes.c_size_t,
+                                                       ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, _vp, _vp,
+                                                       _vp]
+        L.b2s_prepare_images_device.argtypes = [_vp, _vp, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_int, ctypes.c_int,
+                                                ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp, ctypes.c_size_t,
+                                                ctypes.c_int, ctypes.c_int, _vp, ctypes.c_size_t, ctypes.c_size_t, _vp]
         L.b2s_extractor_set_timing.argtypes = [_vp, ctypes.c_int]
         L.b2s_extractor_get_timing.argtypes = [_vp, _vp, _vp]
         L.b2s_extractor_debug_level.argtypes = [_vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, _vp, _vp, _vp]
@@ -539,6 +545,47 @@ class ORBextractor(_Handle):
         _check(lib().b2s_stereo_from_depth_device(self._h, _dptr(kps), _dptr(kps_un), _dptr(counts), int(batch), int(cap),
                                                   _vp(depth.data_ptr()), depth.stride(1) * 4, W, H, float(bf), _dptr(uright),
                                                   _dptr(depth_out), _vp(stream) if stream else None))
+
+    def stereo_from_depth_u16_device(self, kps, kps_un, counts, batch, cap, depth, depth_map_factor, bf, uright, depth_out,
+                                     stream=None):
+        """stereo_from_depth_device on the sensor's raw depth: a uint16 CUDA tensor [batch, height, width] (rows may be
+        padded), converted at the keypoints with the multiplier Tracking derives from the settings' DepthMapFactor
+        (src/Tracking.cc:212-216).  Asynchronous."""
+        B, H, W = depth.shape
+        assert depth.is_cuda and depth.dtype.itemsize == 2 and depth.stride(2) == 1
+        assert B == 1 or depth.stride(0) == H * depth.stride(1), "depth: images must follow each other"
+        _check(lib().b2s_stereo_from_depth_u16_device(self._h, _dptr(kps), _dptr(kps_un), _dptr(counts), int(batch),
+                                                      int(cap), _vp(depth.data_ptr()), depth.stride(1) * 2, W, H,
+                                                      float(depth_map_factor), float(bf), _dptr(uright), _dptr(depth_out),
+                                                      _vp(stream) if stream else None))
+
+    def prepare_images_device(self, src, out, rgb=True, maps=None, stream=None):
+        """Tracking::GrabImage*'s colour-to-grey step (rgb = mbRGB), optionally preceded by the stereo examples'
+        cv::remap(INTER_LINEAR) with float maps: src is a uint8 CUDA tensor [B, H, W] or [B, H, W, C] (C = 3, 4) whose rows
+        and images may be padded; out a uint8 CUDA tensor [B, h, w] (padding allowed, never written); maps None or a pair
+        (mapx, mapy) of float32 CUDA tensors [h, w] shared by the batch.  Asynchronous."""
+        assert src.is_cuda and str(src.dtype) == "torch.uint8" and src.dim() in (3, 4), "src: uint8 CUDA [B, H, W(, C)]"
+        B, H, W = src.shape[:3]
+        C = 1 if src.dim() == 3 else src.shape[3]
+        assert src.stride(2) == C and (C == 1 or src.stride(3) == 1), "src: pixels must be dense within a row"
+        assert out.is_cuda and str(out.dtype) == "torch.uint8" and out.dim() == 3 and out.shape[0] == B and out.stride(2) == 1
+        h, w = out.shape[1:]
+        mx = my = None
+        mrow = 0
+        if maps is not None:
+            mx, my = maps
+            for m in (mx, my):
+                assert m.is_cuda and str(m.dtype) == "torch.float32" and tuple(m.shape) == (h, w)
+                assert m.stride(1) == 1 and m.stride(0) == mx.stride(0), "maps: dense rows, one pitch"
+            mrow = mx.stride(0) * 4
+        # the stride of a batch of one means nothing (numpy gives a new axis stride 0): that image pitch is rows * pitch
+        simg = src.stride(0) if B > 1 else H * src.stride(1)
+        oimg = out.stride(0) if B > 1 else h * out.stride(1)
+        _check(lib().b2s_prepare_images_device(self._h, _vp(src.data_ptr()), src.stride(1), simg, B, W, H, C,
+                                               1 if rgb else 0, _vp(mx.data_ptr()) if mx is not None else None,
+                                               _vp(my.data_ptr()) if my is not None else None, mrow, w, h,
+                                               _vp(out.data_ptr()), out.stride(1), oimg,
+                                               _vp(stream) if stream else None))
 
     def undistort_points(self, xy, K, dist):
         """cv::undistortPoints(xy, K, dist, noArray(), K) on host points (n x 2); always undistorts, k1 == 0 included."""

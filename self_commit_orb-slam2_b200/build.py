@@ -18,7 +18,7 @@ NVCC_FLAGS = GENCODE + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-
 # extractor/matcher/keyframe database: bit-exact float arithmetic, never contract a*b+c; LocalBA is FP64 with a 1e-5 bar
 # -> FMA allowed; the essential graph differentiates numerically (delta = 1e-9 amplifies last-bit differences ~5e8 times)
 NO_FMAD = {"extractor.cu", "extractor_tile.cu", "matcher.cu", "common.cu", "kfdb.cu", "essential.cu", "sim3opt.cu",
-            "initializer.cu", "sim3solver.cu", "pnpsolver.cu", "mappoint.cu", "undistort.cu"}
+            "initializer.cu", "sim3solver.cu", "pnpsolver.cu", "mappoint.cu", "undistort.cu", "ingest.cu"}
 
 
 def _newer(target, sources):
@@ -37,7 +37,7 @@ def _deps_of(src):
     the architecture and compiler flags."""
     base = os.path.basename(src)
     deps = [src, os.path.join(CSRC, "common.cuh"), os.path.join(ROOT, "include", "b200slam.h"), os.path.abspath(__file__)]
-    if base.startswith("extractor") or base == "undistort.cu":
+    if base.startswith("extractor") or base in ("undistort.cu", "ingest.cu"):
         deps.append(os.path.join(CSRC, "extractor.cuh"))
     if base in ("localba.cu", "gba.cu", "essential.cu", "sim3opt.cu"):
         deps.append(os.path.join(CSRC, "ba_math.cuh"))
@@ -118,6 +118,9 @@ def build_oracle(force=False):
     # the undistortion's CPU restatement (oracle/undistort.mk)
     subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "undistort.mk"] + (["-B"] if force else []) +
                           ["liborb_undistort.so"])
+    # the frame ingest's CPU restatement: grey conversion, remap, 16-bit depth (oracle/ingest.mk)
+    subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "-f", "ingest.mk"] + (["-B"] if force else []) +
+                          ["liborb_ingest.so"])
     return ORACLE_LIB
 
 

@@ -84,6 +84,19 @@ int launch_fast_fallback(const ExtractGeom& g, const DeviceBuffers& d, const uin
 constexpr int kCellsListCap = 8192;  // k_cells: NMS maxima one CTA collects in shared memory (extractor_tile.cu)
 constexpr int kCellsMaxCols = 64;    // k_cells: cell columns one CTA owns at most
 constexpr int kFastCellCap = 1024;   // k_fast_cells_list: maxima of one cell it keeps in shared memory (extractor.cu)
+
+// a refused call on the extractor handle (undistort.cu, ingest.cu): B2S_ERR_NO_DEVICE when it is refused for a null handle
+// and there is no device (no handle can exist then), else B2S_ERR_BAD_ARG
+inline int refuse(const b2s_extractor* h, const char* fn) {
+  int n = 0;
+  if (!h && (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0)) {
+    cudaGetLastError();
+    set_error("%s: no CUDA device available: libb200slam has no CPU fallback", fn);
+    return B2S_ERR_NO_DEVICE;
+  }
+  set_error("%s: bad argument", fn);
+  return B2S_ERR_BAD_ARG;
+}
 }  // namespace b2s
 
 struct b2s_extractor : b2s::Stage {

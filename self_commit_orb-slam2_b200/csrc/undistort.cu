@@ -67,10 +67,13 @@ __global__ void k_undistort_xy(float2* __restrict__ xy, int n, Undistort p) {
 
 // ComputeStereoFromRGBD: the depth at the distorted keypoint (coordinates truncated to int), mvuRight from the
 // undistorted x.  `d > 0` is false for 0, negatives and NaN.  A keypoint whose truncated position is outside the depth
-// image has no depth.
+// image has no depth.  T = float: metres; T = uint16_t: the sensor's raw depth, converted at the keypoint as
+// GrabImageRGBD's convertTo(CV_32F, factor) converts every pixel (src/Tracking.cc:334-338): the product of a u16 and a
+// float is exact in double, so the one float rounding of (float)raw * factor is OpenCV's result whatever its precision.
+template <typename T>
 __global__ void k_stereo_from_depth(const b2s_keypoint* __restrict__ kps, const b2s_keypoint* __restrict__ kpsUn,
                                     const int32_t* __restrict__ counts, int cap, const uint8_t* __restrict__ depth,
-                                    size_t pitch, size_t imgBytes, int width, int height, float bf,
+                                    size_t pitch, size_t imgBytes, int width, int height, float factor, float bf,
                                     float* __restrict__ uright, float* __restrict__ depthOut) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int b = blockIdx.y;
@@ -80,7 +83,12 @@ __global__ void k_stereo_from_depth(const b2s_keypoint* __restrict__ kps, const 
   float ur = -1.f, dd = -1.f;
   if (x > -1.f && x < (float)width && y > -1.f && y < (float)height) {
     const int u = (int)x, v = (int)y;
-    const float d = *reinterpret_cast<const float*>(depth + (size_t)b * imgBytes + (size_t)v * pitch + (size_t)u * 4);
+    const T raw = *reinterpret_cast<const T*>(depth + (size_t)b * imgBytes + (size_t)v * pitch + (size_t)u * sizeof(T));
+    float d;
+    if constexpr (sizeof(T) == 2)
+      d = __fmul_rn((float)raw, factor);
+    else
+      d = raw;
     if (d > 0) {
       dd = d;
       ur = __fsub_rn(kpsUn[r].x, __fdiv_rn(bf, d));
@@ -103,19 +111,6 @@ bool make_params(const float* K4, const float* dist, int n_dist, Undistort* p) {
   p->ify = 1. / p->fy;
   for (int i = 0; i < 5; i++) p->k[i] = i < n_dist ? (double)dist[i] : 0.;
   return true;
-}
-
-// a refused call: B2S_ERR_NO_DEVICE when it is refused for a null handle and there is no device (no handle can exist then),
-// else B2S_ERR_BAD_ARG
-int refuse(const b2s_extractor* h, const char* fn) {
-  int n = 0;
-  if (!h && (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0)) {
-    cudaGetLastError();
-    set_error("%s: no CUDA device available: libb200slam has no CPU fallback", fn);
-    return B2S_ERR_NO_DEVICE;
-  }
-  set_error("%s: bad argument", fn);
-  return B2S_ERR_BAD_ARG;
 }
 
 }  // namespace
@@ -166,10 +161,29 @@ extern "C" int b2s_stereo_from_depth_device(b2s_extractor* h, const b2s_keypoint
     return refuse(h, "b2s_stereo_from_depth_device");
   B2S_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
-  k_stereo_from_depth<<<dim3(div_up(cap, 128), batch), 128, 0, st>>>(d_kps, d_kps_un, d_counts, cap,
-                                                                     reinterpret_cast<const uint8_t*>(d_depth),
-                                                                     depth_pitch_bytes, depth_pitch_bytes * height, width,
-                                                                     height, bf, d_uright, d_depth_out);
+  k_stereo_from_depth<float><<<dim3(div_up(cap, 128), batch), 128, 0, st>>>(
+      d_kps, d_kps_un, d_counts, cap, reinterpret_cast<const uint8_t*>(d_depth), depth_pitch_bytes,
+      depth_pitch_bytes * height, width, height, 1.f, bf, d_uright, d_depth_out);
+  h->launches += 1;
+  B2S_CUDA(cudaGetLastError());
+  return B2S_OK;
+}
+
+extern "C" int b2s_stereo_from_depth_u16_device(b2s_extractor* h, const b2s_keypoint* d_kps, const b2s_keypoint* d_kps_un,
+                                                const int32_t* d_counts, int batch, int cap, const uint16_t* d_depth,
+                                                size_t depth_row_bytes, int width, int height, float depth_map_factor,
+                                                float bf, float* d_uright, float* d_depth_out, void* stream) {
+  if (!h || !d_kps || !d_kps_un || !d_counts || !d_depth || !d_uright || !d_depth_out || batch < 1 || batch > 65535 ||
+      cap < 1 || width < 1 || height < 1 || depth_row_bytes < (size_t)width * 2 || depth_row_bytes % 2 ||
+      !std::isfinite(depth_map_factor))
+    return refuse(h, "b2s_stereo_from_depth_u16_device");
+  // the Tracking constructor (src/Tracking.cc:212-216): float mDepthMapFactor; fabs(float) < 1e-5 compares in double
+  const float factor = (double)std::fabs(depth_map_factor) < 1e-5 ? 1.f : 1.0f / depth_map_factor;
+  B2S_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+  k_stereo_from_depth<uint16_t><<<dim3(div_up(cap, 128), batch), 128, 0, st>>>(
+      d_kps, d_kps_un, d_counts, cap, reinterpret_cast<const uint8_t*>(d_depth), depth_row_bytes, depth_row_bytes * height,
+      width, height, factor, bf, d_uright, d_depth_out);
   h->launches += 1;
   B2S_CUDA(cudaGetLastError());
   return B2S_OK;

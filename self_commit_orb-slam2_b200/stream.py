@@ -30,7 +30,8 @@ class StereoStream:
     def __init__(self, frames_per_step, width, height, nfeatures=2000, scale=1.2, nlevels=8, ini_th=20, min_th=7,
                  ba_problem=None, ba_every=5, device=0, rank=0, world=1, nnratio=0.7, ba_depth=1,
                  exchange="boundary", ba_problems=None, pose_problems=None, stereo=False, bf=386.1448, project=False,
-                 intrinsics=(718.856, 718.856, 607.1928, 185.2157), motion=None, ba_sms=64):
+                 intrinsics=(718.856, 718.856, 607.1928, 185.2157), motion=None, ba_sms=64, source_channels=1, rgb=True,
+                 rectify=None, source_size=None):
         """ba_problems: list of LocalBA windows (a step solves ceil(F / ba_every) of them, taken round-robin);
         pose_problems: list of per-frame PoseOptimization problems (F per step, round-robin); stereo: run
         Frame::ComputeStereoMatches for the F pairs of every step on the resident pyramids; project (needs stereo): also
@@ -38,7 +39,12 @@ class StereoStream:
         points moved by `motion` (Tcl, 3 x 4; default: 0.8 m forward with a small yaw, the KITTI-like case that takes the
         reference's forward branch, src/ORBmatcher.cc:1595-1598).  ba_sms: SMs one LocalBA batch may occupy (0 = all): the LM
         kernel shares the GPU with extraction and matching, and about half of the SMs gives the best stream throughput
-        (DESIGN.md §6)."""
+        (DESIGN.md §6).
+        Frame ingest (all off by default): source_channels (1, 3, 4) and rgb (mbRGB) say what a raw frame holds; rectify =
+        (left mapx, left mapy, right mapx, right mapy), float32 [height, width] each, the stereo examples'
+        initUndistortRectifyMap maps; source_size = the raw (width, height), default (width, height).  When colour or
+        rectification is asked for, upload / load_window take raw frames and every step first runs
+        b2s_prepare_images_device (left maps, then right maps) into the grey input of the extractor."""
         self.F, self.w, self.h = frames_per_step, width, height
         self.rank, self.world = rank, world
         self.dev = torch.device("cuda", device)
@@ -92,6 +98,25 @@ class StereoStream:
             self.g_desc = torch.zeros((world, self.G, cap, 32), dtype=torch.uint8, **z)
             self.g_counts = torch.zeros((world, self.G), dtype=torch.int32, **z)
         self.d_imgs = torch.zeros((2 * F, height, width), dtype=torch.uint8, **z)
+        self.src_c, self.rgb = int(source_channels), bool(rgb)
+        self.sw, self.sh = (width, height) if source_size is None else (int(source_size[0]), int(source_size[1]))
+        if self.src_c not in (1, 3, 4):
+            raise ValueError("source_channels must be 1, 3 or 4")
+        if rectify is None and (self.sw, self.sh) != (width, height):
+            raise ValueError("source_size differs from the output size: only rectification changes the size")
+        self.ingest = self.src_c != 1 or rectify is not None
+        self.maps = None
+        if self.ingest:  # raw frames: [2F, sh, sw] or [2F, sh, sw, C]
+            self.d_src = torch.zeros((2 * F, self.sh, self.sw) + ((self.src_c,) if self.src_c > 1 else ()),
+                                     dtype=torch.uint8, **z)
+            if rectify is not None:
+                if len(rectify) != 4:
+                    raise ValueError("rectify: (left mapx, left mapy, right mapx, right mapy)")
+                ms = [torch.as_tensor(m, dtype=torch.float32).to(self.dev).contiguous() for m in rectify]
+                for m in ms:
+                    if tuple(m.shape) != (height, width):
+                        raise ValueError("rectify: every map must be [height, width]")
+                self.maps = ((ms[0], ms[1]), (ms[2], ms[3]))
         if self.stereo:  # mvuRight / mvDepth per left feature, matches per pair
             self.ur = torch.zeros((F, cap), dtype=torch.float32, **z)
             self.dp_all = torch.zeros((1 + F, cap), dtype=torch.float32, **z)  # slot 0: depth of the shard's predecessor
@@ -168,19 +193,20 @@ class StereoStream:
     def upload(self, imgs_host):
         """imgs_host: uint8 [2F, h, w] (L_0..L_F-1, R_0..R_F-1), ideally pinned."""
         with torch.cuda.stream(self.stream):
-            self.d_imgs.copy_(imgs_host, non_blocking=True)
+            (self.d_src if self.ingest else self.d_imgs).copy_(imgs_host, non_blocking=True)
 
     def load_window(self, d_all, start):
         """d_all: device uint8 [2, D, h, w] (left / right images of D resident frames).  Copies frames start .. start+F-1
         (modulo D) into the step's input batch on the stream (device-to-device, part of the timed step)."""
         D, F = d_all.shape[1], self.F
+        dst = self.d_src if self.ingest else self.d_imgs  # raw frames [2, D, sh, sw(, C)] when ingesting
         with torch.cuda.stream(self.stream):
             done = 0
             while done < F:
                 a = (start + done) % D
                 n = min(F - done, D - a)
-                self.d_imgs[done:done + n].copy_(d_all[0, a:a + n], non_blocking=True)
-                self.d_imgs[F + done:F + done + n].copy_(d_all[1, a:a + n], non_blocking=True)
+                dst[done:done + n].copy_(d_all[0, a:a + n], non_blocking=True)
+                dst[F + done:F + done + n].copy_(d_all[1, a:a + n], non_blocking=True)
                 done += n
 
     def step_device(self, run_ba=True, pipelined=False):
@@ -275,6 +301,13 @@ class StereoStream:
     def _enqueue_extract_match(self):
         F, cap = self.F, self.cap
         st = self.stream.cuda_stream
+        if self.ingest:  # Tracking::GrabImageStereo's grey conversion, after the examples' rectification of each camera
+            if self.maps is None:
+                self.ex.prepare_images_device(self.d_src, self.d_imgs, rgb=self.rgb, stream=st)
+            else:
+                for side in range(2):
+                    self.ex.prepare_images_device(self.d_src[side * F:(side + 1) * F], self.d_imgs[side * F:(side + 1) * F],
+                                                  rgb=self.rgb, maps=self.maps[side], stream=st)
         self.ex.extract_batch_device(self.d_imgs.data_ptr(), self.w * self.h, 2 * F, self.w, self.h, self.w,
                                      self.kps[1:].data_ptr(), self.desc[1:].data_ptr(), self.counts[1:].data_ptr(), cap,
                                      stream=st)
@@ -320,6 +353,8 @@ class StereoStream:
     def step_host(self, imgs_host_np, run_ba=True, pipelined=False, img_ptrs=None):
         """imgs_host_np: numpy uint8 [2F, h, w] (or img_ptrs: 2F host addresses of dense h x w images, left images first).
         Returns (counts, nmatches, ba_out); everything ends up in host memory."""
+        if self.ingest:
+            raise ValueError("step_host takes grey images: a stream with source_channels or rectify ingests on the device")
         F, cap = self.F, self.cap
         if getattr(self, "_h_kps", None) is None:  # pinned result buffers, allocated once
             # slot 0 = the frame before the shard's first one (ring), slots 1..2F = this step's images: both sides of the
@@ -396,7 +431,7 @@ class StereoStream:
         return c
 
     def h2d_bytes_per_step(self):
-        b = 2 * self.F * self.w * self.h
+        b = 2 * self.F * self.sw * self.sh * self.src_c
         b += self.F * self.cap * (32 + 4 + 4 + 1) * 2  # descriptors, nodes, angles, valid for both sides of the matcher
         if self.project:  # records + depths of F + 1 frames, mvuRight of F, relative poses
             b += (self.F + 1) * self.cap * (KP_BYTES + 32 + 4) + self.F * self.cap * 4 + self.F * 48
