@@ -1,32 +1,23 @@
 #include "Initializer.h"
 
-#include <cstdio>
-#include <cstdlib>
 #include <mutex>
+
+#include "b2s_host.h"
 
 namespace ORB_SLAM2 {
 
 // Tracking's thread: one handle for the process, grown on demand
-static b2s_init_solver* g_initSolver = nullptr;
-static int g_initKeys = 0, g_initIterations = 0;
-static std::mutex g_initMutex;
+static b2s_host::Slot<b2s_init_solver, 2, b2s_init_destroy> g_init;
 
 int MonoInitializer::Initialize(const InitProblem& p, InitResult& out) {
-  std::lock_guard<std::mutex> lock(g_initMutex);
+  std::lock_guard<std::mutex> lock(g_init.mutex);
   const int n1 = (int)p.matches12.size(), n2 = (int)(p.kp2.size() / 2), it = (int)(p.sets.size() / 8);
-  const int keys = n1 > n2 ? n1 : n2;
-  if (!g_initSolver || keys > g_initKeys || it > g_initIterations) {
-    b2s_init_destroy(g_initSolver);
-    g_initSolver = nullptr;
-    g_initKeys = keys > 4096 ? keys : 4096;
-    g_initIterations = it > 200 ? it : 200;
-    const char* e = getenv("B2S_DEVICE");
-    const int rc = b2s_init_create(g_initKeys, g_initIterations, 1, e ? atoi(e) : 0, &g_initSolver);
-    if (rc != B2S_OK) {
-      fprintf(stderr, "MonoInitializer::Initialize: libb200slam error %d: %s\n", rc, b2s_last_error());
-      g_initSolver = nullptr;
-      return rc;
-    }
+  int rc = g_init.get({n1 > n2 ? n1 : n2, it}, {4096, 200}, [](const int* c, b2s_init_solver** h) {
+    return b2s_init_create(c[0], c[1], 1, b2s_host::device(), h);
+  });
+  if (rc != B2S_OK) {
+    b2s_host::report("MonoInitializer::Initialize", rc);
+    return rc;
   }
   b2s_init_problem q;
   q.n1 = n1;
@@ -44,9 +35,9 @@ int MonoInitializer::Initialize(const InitProblem& p, InitResult& out) {
   r.p3d = out.p3d.data();
   r.triangulated = out.triangulated.data();
   r.inliers_h = r.inliers_f = nullptr;
-  const int rc = b2s_initialize(g_initSolver, 1, &q, &r);
+  rc = b2s_initialize(g_init.h, 1, &q, &r);
   if (rc != B2S_OK) {
-    fprintf(stderr, "MonoInitializer::Initialize: libb200slam error %d: %s\n", rc, b2s_last_error());
+    b2s_host::report("MonoInitializer::Initialize", rc);
     return rc;
   }
   out.ret = r.ret != 0;

@@ -2,10 +2,10 @@
 
 #include <cmath>
 #include <cstdio>
-#include <cstdlib>
 #include <fstream>
 #include <sstream>
-#include <stdexcept>
+
+#include "b2s_host.h"
 
 namespace ORB_SLAM2 {
 
@@ -18,10 +18,9 @@ bool ORBVocabulary::load(int k, int L, const std::vector<int32_t>& parent, const
   b2s_vocabulary_desc d;
   d.k = k; d.L = L; d.n_nodes = (int32_t)parent.size();
   d.parent = parent.data(); d.leaf_flag = leafFlag.data(); d.desc = desc.data(); d.weight = weight.data();
-  const char* e = getenv("B2S_DEVICE");
-  const int rc = b2s_vocabulary_create(&d, e ? atoi(e) : 0, &mpHandle);
+  const int rc = b2s_vocabulary_create(&d, b2s_host::device(), &mpHandle);
   if (rc != B2S_OK) {
-    fprintf(stderr, "ORBVocabulary: libb200slam error %d: %s\n", rc, b2s_last_error());
+    b2s_host::report("ORBVocabulary", rc);
     return false;
   }
   return true;
@@ -70,10 +69,7 @@ void ORBVocabulary::transform(const uint8_t* descriptors, int n, BowVector& v, F
   std::vector<int32_t> word(n), node(n);
   std::vector<double> w(n);
   const int rc = b2s_bow_transform(mpHandle, descriptors, n, levelsup, word.data(), w.data(), node.data());
-  if (rc != B2S_OK) {
-    fprintf(stderr, "ORBVocabulary::transform: libb200slam error %d: %s\n", rc, b2s_last_error());
-    throw std::runtime_error(b2s_last_error());
-  }
+  if (rc != B2S_OK) b2s_host::fail("ORBVocabulary::transform", rc);
   for (int i = 0; i < n; i++) {  // :1145-1160 (TF_IDF): addWeight / addFeature in feature order, stopped words skipped
     if (w[i] > 0) {
       v[(unsigned int)word[i]] += w[i];

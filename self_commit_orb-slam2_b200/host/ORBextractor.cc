@@ -2,19 +2,13 @@
 #include "ORBextractor.h"
 
 #include <cmath>
-#include <cstdio>
-#include <cstdlib>
-#include <stdexcept>
+
+#include "b2s_host.h"
 
 namespace ORB_SLAM2 {
 
 static int g_device = -1;
 void ORBextractor::SetDevice(int device) { g_device = device; }
-static int pick_device() {
-  if (g_device >= 0) return g_device;
-  const char* e = getenv("B2S_DEVICE");
-  return e ? atoi(e) : 0;
-}
 
 ORBextractor::ORBextractor(int _nfeatures, float _scaleFactor, int _nlevels, int _iniThFAST, int _minThFAST)
     : nfeatures(_nfeatures), scaleFactor(_scaleFactor), nlevels(_nlevels), iniThFAST(_iniThFAST), minThFAST(_minThFAST) {
@@ -33,11 +27,11 @@ void ORBextractor::EnsureHandle(int width, int height) {
   mMaxW = std::max(width, mMaxW);
   mMaxH = std::max(height, mMaxH);
   int rc = b2s_extractor_create(nfeatures, (float)scaleFactor, nlevels, iniThFAST, minThFAST, std::max(64, mMaxW),
-                                std::max(64, mMaxH), 1, pick_device(), &mpHandle);
+                                std::max(64, mMaxH), 1, g_device >= 0 ? g_device : b2s_host::device(), &mpHandle);
   if (rc != B2S_OK) {
     // The reference has neither exceptions nor return codes here (SURVEY.md §8b): report on stderr and leave the handle
     // empty; operator() then returns no keypoints, like the reference does for an empty image.  There is no CPU fallback.
-    fprintf(stderr, "ORBextractor: libb200slam error %d: %s\n", rc, b2s_last_error());
+    b2s_host::report("ORBextractor", rc);
     mpHandle = nullptr;
     return;
   }
@@ -86,7 +80,7 @@ void ORBextractor::operator()(b2s_cv::InputArray _image, b2s_cv::InputArray /*_m
   int rc = b2s_extract(mpHandle, image.data, image.cols, image.rows, (int)image.step, mvTmpKeys.data(), desc.data(), cap, &n,
                        mbDownloadPyramid ? pyr.data() : nullptr);
   if (rc != B2S_OK) {
-    fprintf(stderr, "ORBextractor::operator(): libb200slam error %d: %s\n", rc, b2s_last_error());
+    b2s_host::report("ORBextractor::operator()", rc);
     _keypoints.clear();
     _descriptors.release();
     return;

@@ -1,21 +1,13 @@
 #include "ORBmatcher.h"
 
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
-#include <stdexcept>
 #include <vector>
+
+#include "b2s_host.h"
 
 namespace ORB_SLAM2 {
 
-static int dev() {
-  const char* e = getenv("B2S_DEVICE");
-  return e ? atoi(e) : 0;
-}
-static void fail(const char* where, int rc) {
-  fprintf(stderr, "%s: libb200slam error %d: %s\n", where, rc, b2s_last_error());
-  throw std::runtime_error(b2s_last_error());
-}
+using b2s_host::fail;
 
 // ORBmatcher objects are stack temporaries in the reference (one per call site, several per tracked frame); the device
 // handle — a stream and ~30 device buffers — is therefore owned by the calling THREAD, not by the object: created on
@@ -44,7 +36,7 @@ void ORBmatcher::Ensure(int n) {
   if (!t.cur || n > t.cap) {
     const int cap = n < 4096 ? 4096 : n;
     b2s_matcher* h = nullptr;
-    int rc = b2s_matcher_create(cap, 1, dev(), &h);
+    int rc = b2s_matcher_create(cap, 1, b2s_host::device(), &h);
     if (rc != B2S_OK) fail("ORBmatcher", rc);
     t.all.push_back(h);
     t.cur = h;

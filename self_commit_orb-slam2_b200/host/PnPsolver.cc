@@ -1,31 +1,23 @@
 #include "PnPsolver.h"
 
-#include <cstdio>
-#include <cstdlib>
 #include <mutex>
+
+#include "b2s_host.h"
 
 namespace ORB_SLAM2 {
 
 // Tracking's thread: one handle for the process, grown on demand
-static b2s_pnpsolver* g_pnpRansac = nullptr;
-static int g_pnpRansacMatches = 0, g_pnpRansacSets = 0;
-static std::mutex g_pnpRansacMutex;
+static b2s_host::Slot<b2s_pnpsolver, 2, b2s_pnpsolver_destroy> g_pnpRansac;
 
 int PnPRansac::Iterate(const PnPRansacProblem& p, PnPRansacResult& out) {
-  std::lock_guard<std::mutex> lock(g_pnpRansacMutex);
+  std::lock_guard<std::mutex> lock(g_pnpRansac.mutex);
   const int n = (int)(p.P3Dw.size() / 3), k = (int)(p.sets.size() / 4);
-  if (!g_pnpRansac || n > g_pnpRansacMatches || k > g_pnpRansacSets) {
-    b2s_pnpsolver_destroy(g_pnpRansac);
-    g_pnpRansac = nullptr;
-    g_pnpRansacMatches = n > 1024 ? n : 1024;
-    g_pnpRansacSets = k > 300 ? k : 300;
-    const char* e = getenv("B2S_DEVICE");
-    const int rc = b2s_pnpsolver_create(g_pnpRansacMatches, g_pnpRansacSets, 1, e ? atoi(e) : 0, &g_pnpRansac);
-    if (rc != B2S_OK) {
-      fprintf(stderr, "PnPRansac::Iterate: libb200slam error %d: %s\n", rc, b2s_last_error());
-      g_pnpRansac = nullptr;
-      return rc;
-    }
+  int rc = g_pnpRansac.get({n, k}, {1024, 300}, [](const int* c, b2s_pnpsolver** h) {
+    return b2s_pnpsolver_create(c[0], c[1], 1, b2s_host::device(), h);
+  });
+  if (rc != B2S_OK) {
+    b2s_host::report("PnPRansac::Iterate", rc);
+    return rc;
   }
   std::vector<uint8_t> bestIn((size_t)(n > 0 ? n : 1), 0);
   for (int i = 0; i < n && i < (int)p.bestMask.size(); i++) bestIn[(size_t)i] = p.bestMask[(size_t)i];
@@ -53,9 +45,9 @@ int PnPRansac::Iterate(const PnPRansacProblem& p, PnPRansacResult& out) {
   b2s_pnpsolver_result r;
   r.inliers = out.inliers.data();
   r.best_mask = out.bestMask.data();
-  const int rc = b2s_pnpsolver_iterate(g_pnpRansac, 1, &q, &r);
+  rc = b2s_pnpsolver_iterate(g_pnpRansac.h, 1, &q, &r);
   if (rc != B2S_OK) {
-    fprintf(stderr, "PnPRansac::Iterate: libb200slam error %d: %s\n", rc, b2s_last_error());
+    b2s_host::report("PnPRansac::Iterate", rc);
     return rc;
   }
   out.inliers.resize((size_t)n);

@@ -1,31 +1,23 @@
 #include "Sim3Solver.h"
 
-#include <cstdio>
-#include <cstdlib>
 #include <mutex>
+
+#include "b2s_host.h"
 
 namespace ORB_SLAM2 {
 
 // LoopClosing's thread: one handle for the process, grown on demand
-static b2s_sim3solver* g_sim3Ransac = nullptr;
-static int g_sim3RansacMatches = 0, g_sim3RansacSets = 0;
-static std::mutex g_sim3RansacMutex;
+static b2s_host::Slot<b2s_sim3solver, 2, b2s_sim3solver_destroy> g_sim3Ransac;
 
 int Sim3Ransac::Iterate(const Sim3RansacProblem& p, Sim3RansacResult& out) {
-  std::lock_guard<std::mutex> lock(g_sim3RansacMutex);
+  std::lock_guard<std::mutex> lock(g_sim3Ransac.mutex);
   const int n = (int)(p.X1c.size() / 3), k = (int)(p.sets.size() / 3);
-  if (!g_sim3Ransac || n > g_sim3RansacMatches || k > g_sim3RansacSets) {
-    b2s_sim3solver_destroy(g_sim3Ransac);
-    g_sim3Ransac = nullptr;
-    g_sim3RansacMatches = n > 1024 ? n : 1024;
-    g_sim3RansacSets = k > 300 ? k : 300;
-    const char* e = getenv("B2S_DEVICE");
-    const int rc = b2s_sim3solver_create(g_sim3RansacMatches, g_sim3RansacSets, 1, e ? atoi(e) : 0, &g_sim3Ransac);
-    if (rc != B2S_OK) {
-      fprintf(stderr, "Sim3Ransac::Iterate: libb200slam error %d: %s\n", rc, b2s_last_error());
-      g_sim3Ransac = nullptr;
-      return rc;
-    }
+  int rc = g_sim3Ransac.get({n, k}, {1024, 300}, [](const int* c, b2s_sim3solver** h) {
+    return b2s_sim3solver_create(c[0], c[1], 1, b2s_host::device(), h);
+  });
+  if (rc != B2S_OK) {
+    b2s_host::report("Sim3Ransac::Iterate", rc);
+    return rc;
   }
   b2s_sim3solver_problem q;
   q.n = n;
@@ -47,9 +39,9 @@ int Sim3Ransac::Iterate(const Sim3RansacProblem& p, Sim3RansacResult& out) {
   out.inliers.assign((size_t)(n > 0 ? n : 1), 0);
   b2s_sim3solver_result r;
   r.inliers = out.inliers.data();
-  const int rc = b2s_sim3solver_iterate(g_sim3Ransac, 1, &q, &r);
+  rc = b2s_sim3solver_iterate(g_sim3Ransac.h, 1, &q, &r);
   if (rc != B2S_OK) {
-    fprintf(stderr, "Sim3Ransac::Iterate: libb200slam error %d: %s\n", rc, b2s_last_error());
+    b2s_host::report("Sim3Ransac::Iterate", rc);
     return rc;
   }
   out.inliers.resize((size_t)n);

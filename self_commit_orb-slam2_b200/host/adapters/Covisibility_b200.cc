@@ -11,14 +11,13 @@
 #include "adapters/Covisibility_b200.h"
 
 #include <algorithm>
-#include <cstdio>
-#include <cstdlib>
 #include <mutex>
 #include <set>
 #include <unordered_map>
 
 #include "MapPoint.h"
 #include "b200slam.h"
+#include "../b2s_host.h"
 
 namespace ORB_SLAM2 {
 namespace b200 {
@@ -34,29 +33,13 @@ struct Access : KeyFrame {
 };
 
 // One handle for the process (LocalMapping and LoopClosing call it in turn), grown on demand.
-struct CovisSlot {
-  b2s_covis* h = nullptr;
-  int kf = 0, mp = 0, obs = 0, slots = 0, conn = 0, batch = 0;
-  std::mutex m;
-  b2s_covis* get(int nkf, int nmp, int nobs, int nslots, int nconn, int nbatch) {
-    if (h && nkf <= kf && nmp <= mp && nobs <= obs && nslots <= slots && nconn <= conn && nbatch <= batch) return h;
-    b2s_covis_destroy(h);
-    h = nullptr;
-    kf = std::max({nkf, kf, 256});
-    mp = std::max({nmp, mp, 8192});
-    obs = std::max({nobs, obs, 65536});
-    slots = std::max({nslots, slots, 8192});
-    conn = std::max({nconn, conn, 65536});
-    batch = std::max({nbatch, batch, 1});
-    const char* e = getenv("B2S_DEVICE");
-    if (b2s_covis_create(kf, mp, obs, slots, conn, batch, e ? atoi(e) : 0, &h) != B2S_OK) {
-      fprintf(stderr, "UpdateConnections (b200): %s\n", b2s_last_error());
-      h = nullptr;
-      kf = mp = obs = slots = conn = batch = 0;
-    }
-    return h;
-  }
-} g_covis;
+// capacities: keyframes, points, observations, slots, connections, batch
+b2s_host::Slot<b2s_covis, 6, b2s_covis_destroy> g_covis;
+const int kCovisFloor[6] = {256, 8192, 65536, 8192, 65536, 1};
+
+int create_covis(const int* c, b2s_covis** h) {
+  return b2s_covis_create(c[0], c[1], c[2], c[3], c[4], c[5], b2s_host::device(), h);
+}
 
 bool by_id(const KeyFrame* a, const KeyFrame* b) { return a->mnId < b->mnId; }
 
@@ -176,12 +159,11 @@ int UpdateConnections(const std::vector<KeyFrame*>& vpKFs, CovisibilityReads* re
   b2s_covis_result r;
   int rc;
   {
-    std::lock_guard<std::mutex> lock(g_covis.m);
-    b2s_covis* h = g_covis.get(n, nmp, (int)obsKf.size(), (int)slotMp.size(),
-                               (int)std::max(mapKf.size(), listKf.size()), B);
-    if (!h) return B2S_ERR_CUDA;
+    std::lock_guard<std::mutex> lock(g_covis.mutex);
+    rc = g_covis.get({n, nmp, (int)obsKf.size(), (int)slotMp.size(), (int)std::max(mapKf.size(), listKf.size()), B},
+                     kCovisFloor, create_covis);
     size_t cap = 4096;
-    for (;;) {
+    if (rc == B2S_OK) for (;;) {
       rMapKf.resize(cap);
       rMapW.resize(cap);
       rListKf.resize(cap);
@@ -193,22 +175,22 @@ int UpdateConnections(const std::vector<KeyFrame*>& vpKFs, CovisibilityReads* re
                            (int)cap, rListOff.data(), rListKf.data(), rListW.data(), (int)cap, pairs.data(), 0,
                            startOff.data(), startKf.data(), (int)cap, afterOff.data(), afterKf.data(), afterW.data(),
                            (int)cap, 0, 0, 0, 0};
-      rc = b2s_update_connections(h, &p, &r);
+      rc = b2s_update_connections(g_covis.h, &p, &r);
       const int need = std::max({r.map_need, r.list_need, r.start_need, r.after_need});
       if (rc == B2S_ERR_CAPACITY && need > (int)cap) {
         cap = (size_t)need;
         continue;
       }
       if (rc == B2S_ERR_CAPACITY) {  // the handle's output areas: grow them
-        h = g_covis.get(n, nmp, (int)obsKf.size(), (int)slotMp.size(), 2 * std::max(g_covis.conn, 1), B);
-        if (!h) return B2S_ERR_CUDA;
-        continue;
+        rc = g_covis.get({n, nmp, (int)obsKf.size(), (int)slotMp.size(), 2 * std::max(g_covis.cap[4], 1), B},
+                         kCovisFloor, create_covis);
+        if (rc == B2S_OK) continue;
       }
       break;
     }
   }
   if (rc != B2S_OK) {
-    fprintf(stderr, "UpdateConnections (b200): %s\n", b2s_last_error());
+    b2s_host::report("UpdateConnections", rc);
     return rc;
   }
   for (int i = 0; i < n; i++) {

@@ -3,8 +3,6 @@
 // exactly as src/Initializer.cc:82-168 does (so the process consumes the same rand() stream), then makes one
 // b2s_initialize call with batch 1 and writes R21, t21, vP3D and vbTriangulated as the reference does: only on success,
 // except that a failed ReconstructF leaves R21 and t21 empty.  On a library error it prints to stderr and returns false.
-#include <cstdio>
-#include <cstdlib>
 #include <mutex>
 #include <vector>
 
@@ -12,30 +10,13 @@
 #include "Thirdparty/DBoW2/DUtils/Random.h"
 
 #include "b200slam.h"
+#include "../b2s_host.h"
 
 namespace ORB_SLAM2 {
 namespace {
 
 // One handle for the process (Tracking calls Initialize from one thread), grown on demand.
-struct InitSlot {
-  b2s_init_solver* h = nullptr;
-  int keys = 0, iterations = 0;
-  std::mutex m;
-  b2s_init_solver* get(int nKeys, int nIt) {
-    if (h && nKeys <= keys && nIt <= iterations) return h;
-    b2s_init_destroy(h);
-    h = nullptr;
-    keys = nKeys > 4096 ? nKeys : 4096;
-    iterations = nIt > 200 ? nIt : 200;
-    const char* e = getenv("B2S_DEVICE");
-    if (b2s_init_create(keys, iterations, 1, e ? atoi(e) : 0, &h) != B2S_OK) {
-      fprintf(stderr, "Initializer (b200): %s\n", b2s_last_error());
-      h = nullptr;
-      keys = iterations = 0;
-    }
-    return h;
-  }
-} g_init;
+b2s_host::Slot<b2s_init_solver, 2, b2s_init_destroy> g_init;
 
 }  // namespace
 
@@ -114,12 +95,14 @@ bool Initializer::Initialize(const Frame& CurrentFrame, const vector<int>& vMatc
   r.inliers_h = r.inliers_f = nullptr;
   int rc;
   {
-    std::lock_guard<std::mutex> lock(g_init.m);
-    b2s_init_solver* h = g_init.get(n1 > n2 ? n1 : n2, mMaxIterations);
-    rc = h ? b2s_initialize(h, 1, &q, &r) : B2S_ERR_CUDA;
+    std::lock_guard<std::mutex> lock(g_init.mutex);
+    rc = g_init.get({n1 > n2 ? n1 : n2, mMaxIterations}, {4096, 200}, [](const int* c, b2s_init_solver** h) {
+      return b2s_init_create(c[0], c[1], 1, b2s_host::device(), h);
+    });
+    if (rc == B2S_OK) rc = b2s_initialize(g_init.h, 1, &q, &r);
   }
   if (rc != B2S_OK) {
-    fprintf(stderr, "Initializer::Initialize: libb200slam error %d: %s\n", rc, b2s_last_error());
+    b2s_host::report("Initializer::Initialize", rc);
     return false;
   }
   if (r.rt_state == -1) {  // ReconstructF clears its outputs before deciding (:1032-1033)

@@ -14,7 +14,6 @@
 // src/KeyFrameDatabase.cc (libref_kfdb.so) on the same stand-in objects; tests/test_kfdb_gpu.py requires the same
 // vector<KeyFrame*>.
 #include <cstdint>
-#include <cstdlib>
 #include <map>
 #include <mutex>
 #include <stdexcept>
@@ -25,6 +24,7 @@
 #include "KeyFrameDatabase.h"
 
 #include "b200slam.h"
+#include "../b2s_host.h"
 
 using namespace std;
 
@@ -96,9 +96,8 @@ struct Covis {
 
 KeyFrameDatabase::KeyFrameDatabase(const ORBVocabulary& voc) : mpVoc(&voc) {
   // no inverted file on the host: mvInvertedFile stays empty
-  const char* e = getenv("B2S_DEVICE");
   DbState& s = state_of(this);
-  check(b2s_kfdb_create((int)voc.size(), e ? atoi(e) : 0, &s.h), "KeyFrameDatabase");
+  check(b2s_kfdb_create((int)voc.size(), b2s_host::device(), &s.h), "KeyFrameDatabase");
 }
 
 void KeyFrameDatabase::add(KeyFrame* pKF) {

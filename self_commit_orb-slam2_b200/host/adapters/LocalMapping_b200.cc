@@ -22,7 +22,6 @@
 
 #include <algorithm>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <iterator>
 #include <list>
@@ -34,6 +33,7 @@
 
 #include "MapPoint.h"
 #include "b200slam.h"
+#include "../b2s_host.h"
 
 namespace ORB_SLAM2 {
 namespace b200 {
@@ -53,46 +53,13 @@ struct MpAccess : MapPoint {
   static float MapPoint::*maxD() { return &MpAccess::mfMaxDistance; }
 };
 
-// One handle for the process, grown on demand.
-struct CullingSlot {
-  b2s_culling* h = nullptr;
-  int kf = 0, mp = 0, obs = 0, local = 0, slots = 0;
-  std::mutex m;
-  b2s_culling* get(int nkf, int nmp, int nobs, int nlocal, int nslots) {
-    if (h && nkf <= kf && nmp <= mp && nobs <= obs && nlocal <= local && nslots <= slots) return h;
-    b2s_culling_destroy(h);
-    h = nullptr;
-    kf = std::max({nkf, kf, 256});
-    mp = std::max({nmp, mp, 8192});
-    obs = std::max({nobs, obs, 65536});
-    local = std::max({nlocal, local, 256});
-    slots = std::max({nslots, slots, 65536});
-    const char* e = getenv("B2S_DEVICE");
-    if (b2s_culling_create(kf, mp, obs, local, slots, 1, e ? atoi(e) : 0, &h) != B2S_OK) {
-      fprintf(stderr, "KeyFrameCulling (b200): %s\n", b2s_last_error());
-      h = nullptr;
-      kf = mp = obs = local = slots = 0;
-    }
-    return h;
-  }
-} g_culling;
+// One handle for the process, grown on demand; capacities: keyframes, points, observations, local keyframes, slots.
+b2s_host::Slot<b2s_culling, 5, b2s_culling_destroy> g_culling;
 
 bool by_id(const KeyFrame* a, const KeyFrame* b) { return a->mnId < b->mnId; }
 
 // One matcher handle for the process (its buffers grow on demand).
-struct MatcherSlot {
-  b2s_matcher* h = nullptr;
-  std::mutex m;
-  b2s_matcher* get() {
-    if (h) return h;
-    const char* e = getenv("B2S_DEVICE");
-    if (b2s_matcher_create(4096, 1, e ? atoi(e) : 0, &h) != B2S_OK) {
-      fprintf(stderr, "ProcessNewKeyFrame (b200): %s\n", b2s_last_error());
-      h = nullptr;
-    }
-    return h;
-  }
-} g_matcher;
+b2s_host::Slot<b2s_matcher, 1, b2s_matcher_destroy> g_matcher;
 
 }  // namespace
 
@@ -195,13 +162,15 @@ int KeyFrameCulling(KeyFrame* pCurrentKF, bool bMonocular) {
                        0};
   int rc;
   {
-    std::lock_guard<std::mutex> lock(g_culling.m);
-    b2s_culling* h = g_culling.get(n, nmp, (int)obsKf.size(), L, (int)slotMp.size());
-    if (!h) return B2S_ERR_CUDA;
-    rc = b2s_keyframe_culling(h, 1, &p, &r);
+    std::lock_guard<std::mutex> lock(g_culling.mutex);
+    rc = g_culling.get({n, nmp, (int)obsKf.size(), L, (int)slotMp.size()}, {256, 8192, 65536, 256, 65536},
+                       [](const int* c, b2s_culling** h) {
+                         return b2s_culling_create(c[0], c[1], c[2], c[3], c[4], 1, b2s_host::device(), h);
+                       });
+    if (rc == B2S_OK) rc = b2s_keyframe_culling(g_culling.h, 1, &p, &r);
   }
   if (rc != B2S_OK) {
-    fprintf(stderr, "KeyFrameCulling (b200): %s\n", b2s_last_error());
+    b2s_host::report("KeyFrameCulling", rc);
     return rc;
   }
   for (int l = 0; l < L; l++)
@@ -325,13 +294,14 @@ int ProcessNewKeyFrame(KeyFrame* pKF, Map* pMap, std::list<MapPoint*>& lRecent, 
                         rList.data(),  rVerdict.data(), 0,           0};
   int rc;
   {
-    std::lock_guard<std::mutex> lock(g_matcher.m);
-    b2s_matcher* h = g_matcher.get();
-    if (!h) return B2S_ERR_CUDA;
-    rc = b2s_process_new_keyframe(h, 1, &p, &r);
+    std::lock_guard<std::mutex> lock(g_matcher.mutex);
+    rc = g_matcher.get({4096}, {4096}, [](const int* c, b2s_matcher** h) {
+      return b2s_matcher_create(c[0], 1, b2s_host::device(), h);
+    });
+    if (rc == B2S_OK) rc = b2s_process_new_keyframe(g_matcher.h, 1, &p, &r);
   }
   if (rc != B2S_OK) {
-    fprintf(stderr, "ProcessNewKeyFrame (b200): %s\n", b2s_last_error());
+    b2s_host::report("ProcessNewKeyFrame", rc);
     return rc;
   }
 

@@ -23,15 +23,15 @@
 // match arrays and counts for all eleven methods.
 #include <cmath>
 #include <cstdint>
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <set>
+#include <string>
 #include <vector>
 
 #include "ORBmatcher.h"
 
 #include "b200slam.h"
+#include "../b2s_host.h"
 
 using namespace std;
 
@@ -43,37 +43,22 @@ const int ORBmatcher::HISTO_LENGTH = 30;
 
 namespace {
 
-int device_index() {
-  const char* e = getenv("B2S_DEVICE");
-  return e ? atoi(e) : 0;
-}
-
 // ORBmatcher objects are stack temporaries (one per call site); the device handle they use is per THREAD, grown on demand
-// and kept: creating one costs a stream and ~30 cudaMalloc, destroying one synchronises the device.
-struct HandleSlot {
-  b2s_matcher* h = nullptr;
-  int cap = 0;
-  ~HandleSlot() { b2s_matcher_destroy(h); }
-  b2s_matcher* get(int n) {
-    if (h && n <= cap) return h;
-    b2s_matcher_destroy(h);
-    h = nullptr;
-    cap = n < 4096 ? 4096 : n;
-    if (b2s_matcher_create(cap, 1, device_index(), &h) != B2S_OK) {
-      fprintf(stderr, "ORBmatcher (b200): %s\n", b2s_last_error());
-      h = nullptr;
-      cap = 0;
-    }
-    return h;
-  }
+// and destroyed at thread exit: creating one costs a stream and ~30 cudaMalloc, destroying one synchronises the device.
+struct ThreadHandle : b2s_host::Slot<b2s_matcher, 1, b2s_matcher_destroy> {
+  ~ThreadHandle() { b2s_matcher_destroy(h); }
 };
 b2s_matcher* handle_for(int n) {
-  static thread_local HandleSlot slot;
-  return slot.get(n);
+  static thread_local ThreadHandle slot;
+  const int rc = slot.get({n}, {4096}, [](const int* c, b2s_matcher** h) {
+    return b2s_matcher_create(c[0], 1, b2s_host::device(), h);
+  });
+  if (rc != B2S_OK) b2s_host::report("ORBmatcher", rc);
+  return slot.h;
 }
 bool ok(int rc, const char* where) {
   if (rc == B2S_OK) return true;
-  fprintf(stderr, "ORBmatcher::%s (b200): %s\n", where, b2s_last_error());
+  b2s_host::report(("ORBmatcher::" + std::string(where)).c_str(), rc);
   return false;
 }
 

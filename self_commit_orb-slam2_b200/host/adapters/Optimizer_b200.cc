@@ -28,7 +28,6 @@
 #include <algorithm>
 #include <cstdint>
 #include <cstdio>
-#include <cstdlib>
 #include <list>
 #include <map>
 #include <mutex>
@@ -39,101 +38,24 @@
 #include "Optimizer.h"
 
 #include "b200slam.h"
+#include "../b2s_host.h"
 
 namespace ORB_SLAM2 {
 namespace {
 
-int device_index() {
-  const char* e = getenv("B2S_DEVICE");
-  return e ? atoi(e) : 0;
+using b2s_host::report;
+
+int create_ba(const int* cap, b2s_ba_solver** h) {
+  return b2s_ba_create(cap[0], cap[1], cap[2], 1, b2s_host::device(), h);
 }
 
-// One solver handle per calling thread role, grown on demand and kept for the process lifetime (handles own device
-// buffers and a stream; creating one per call would put cudaMalloc / cudaFree on the mapping thread's critical path).
-struct SolverSlot {
-  b2s_ba_solver* h = nullptr;
-  int kf = 0, mp = 0, edges = 0;
-  std::mutex m;
-  b2s_ba_solver* get(int nKF, int nMP, int nE) {
-    if (h && nKF <= kf && nMP <= mp && nE <= edges) return h;
-    b2s_ba_destroy(h);
-    h = nullptr;
-    kf = nKF > 64 ? nKF : 64;
-    mp = nMP > 8192 ? nMP : 8192;
-    edges = nE > 65536 ? nE : 65536;
-    if (b2s_ba_create(kf, mp, edges, 1, device_index(), &h) != B2S_OK) {
-      fprintf(stderr, "Optimizer (b200): %s\n", b2s_last_error());
-      h = nullptr;
-      kf = mp = edges = 0;
-    }
-    return h;
-  }
-};
-SolverSlot g_localBA, g_pose;
-
-// The global bundle adjustment's handle (LoopClosing's GBA thread, or Tracking's monocular initialisation), grown on demand.
-struct GbaSlot {
-  b2s_gba_solver* h = nullptr;
-  int kf = 0, mp = 0, edges = 0;
-  std::mutex m;
-  b2s_gba_solver* get(int nKF, int nMP, int nE) {
-    if (h && nKF <= kf && nMP <= mp && nE <= edges) return h;
-    b2s_gba_destroy(h);
-    h = nullptr;
-    kf = nKF > 256 ? nKF : 256;
-    mp = nMP > 32768 ? nMP : 32768;
-    edges = nE > 262144 ? nE : 262144;
-    if (b2s_gba_create(kf, mp, edges, device_index(), &h) != B2S_OK) {
-      fprintf(stderr, "Optimizer (b200): %s\n", b2s_last_error());
-      h = nullptr;
-      kf = mp = edges = 0;
-    }
-    return h;
-  }
-};
-GbaSlot g_gba;
-
-// The essential graph's handle (LoopClosing::CorrectLoop), grown on demand.
-struct EgSlot {
-  b2s_eg_solver* h = nullptr;
-  int kf = 0, edges = 0, mp = 0;
-  std::mutex m;
-  b2s_eg_solver* get(int nKF, int nE, int nMP) {
-    if (h && nKF <= kf && nE <= edges && nMP <= mp) return h;
-    b2s_eg_destroy(h);
-    h = nullptr;
-    kf = nKF > 1024 ? nKF : 1024;
-    edges = nE > 16384 ? nE : 16384;
-    mp = nMP > 65536 ? nMP : 65536;
-    if (b2s_eg_create(kf, edges, mp, device_index(), &h) != B2S_OK) {
-      fprintf(stderr, "Optimizer (b200): %s\n", b2s_last_error());
-      h = nullptr;
-      kf = edges = mp = 0;
-    }
-    return h;
-  }
-};
-EgSlot g_eg;
-
-// OptimizeSim3's handle (LoopClosing::ComputeSim3), one problem per call, grown on demand.
-struct Sim3Slot {
-  b2s_sim3opt_solver* h = nullptr;
-  int n = 0;
-  std::mutex m;
-  b2s_sim3opt_solver* get(int nMatches) {
-    if (h && nMatches <= n) return h;
-    b2s_sim3opt_destroy(h);
-    h = nullptr;
-    n = nMatches > 4096 ? nMatches : 4096;
-    if (b2s_sim3opt_create(n, 1, device_index(), &h) != B2S_OK) {
-      fprintf(stderr, "Optimizer (b200): %s\n", b2s_last_error());
-      h = nullptr;
-      n = 0;
-    }
-    return h;
-  }
-};
-Sim3Slot g_sim3;
+// One solver handle per calling thread role, grown on demand: LocalBA (LocalMapping), PoseOptimization (Tracking), the
+// global bundle adjustment (LoopClosing's GBA thread, or Tracking's monocular initialisation), the essential graph
+// (LoopClosing::CorrectLoop) and OptimizeSim3 (LoopClosing::ComputeSim3, one problem per call).
+b2s_host::Slot<b2s_ba_solver, 3, b2s_ba_destroy> g_localBA, g_pose;
+b2s_host::Slot<b2s_gba_solver, 3, b2s_gba_destroy> g_gba;
+b2s_host::Slot<b2s_eg_solver, 3, b2s_eg_destroy> g_eg;
+b2s_host::Slot<b2s_sim3opt_solver, 1, b2s_sim3opt_destroy> g_sim3;
 
 b2s_sim3 to_b2s(const g2o::Sim3& S) {
   b2s_sim3 o;
@@ -245,14 +167,14 @@ void Optimizer::LocalBundleAdjustment(KeyFrame* pKF, bool* pbStopFlag, Map* pMap
   res.chi2_final = 0;
   res.n_trials = 0;
   {
-    std::lock_guard<std::mutex> lock(g_localBA.m);
-    b2s_ba_solver* solver = g_localBA.get(nKF, nMP, nE);
-    if (!solver) return;
+    std::lock_guard<std::mutex> lock(g_localBA.mutex);
+    int rc = g_localBA.get({nKF, nMP, nE}, {64, 8192, 65536}, create_ba);
     static_assert(sizeof(bool) == 1, "the stop flag is polled as one byte");
-    const int rc = b2s_local_ba(solver, &prob, reinterpret_cast<const volatile uint8_t*>(pbStopFlag), &res);
+    if (rc == B2S_OK)
+      rc = b2s_local_ba(g_localBA.h, &prob, reinterpret_cast<const volatile uint8_t*>(pbStopFlag), &res);
     if (rc == B2S_ERR_ABORTED) return;
     if (rc != B2S_OK) {
-      fprintf(stderr, "Optimizer::LocalBundleAdjustment (b200): %s\n", b2s_last_error());
+      report("Optimizer::LocalBundleAdjustment", rc);
       return;
     }
   }
@@ -327,11 +249,11 @@ int Optimizer::PoseOptimization(Frame* pFrame) {
   res.n_inliers = 0;
   res.n_trials = 0;
   {
-    std::lock_guard<std::mutex> lock(g_pose.m);
-    b2s_ba_solver* solver = g_pose.get(4, 16, 64);
-    if (!solver) return 0;
-    if (b2s_pose_optimization(solver, &prob, &res) != B2S_OK) {
-      fprintf(stderr, "Optimizer::PoseOptimization (b200): %s\n", b2s_last_error());
+    std::lock_guard<std::mutex> lock(g_pose.mutex);
+    int rc = g_pose.get({0, 0, 0}, {4, 16, 64}, create_ba);
+    if (rc == B2S_OK) rc = b2s_pose_optimization(g_pose.h, &prob, &res);
+    if (rc != B2S_OK) {
+      report("Optimizer::PoseOptimization", rc);
       return 0;
     }
   }
@@ -426,12 +348,14 @@ void Optimizer::BundleAdjustment(const std::vector<KeyFrame*>& vpKFs, const std:
   res.chi2_final = 0;
   res.n_trials = 0;
   {
-    std::lock_guard<std::mutex> lock(g_gba.m);
-    b2s_gba_solver* solver = g_gba.get(nKF, nMP, nE);
-    if (!solver) return;
+    std::lock_guard<std::mutex> lock(g_gba.mutex);
+    int rc = g_gba.get({nKF, nMP, nE}, {256, 32768, 262144}, [](const int* c, b2s_gba_solver** h) {
+      return b2s_gba_create(c[0], c[1], c[2], b2s_host::device(), h);
+    });
     static_assert(sizeof(bool) == 1, "the stop flag is polled as one byte");
-    if (b2s_global_ba(solver, &prob, reinterpret_cast<const volatile uint8_t*>(pbStopFlag), &res) != B2S_OK) {
-      fprintf(stderr, "Optimizer::BundleAdjustment (b200): %s\n", b2s_last_error());
+    if (rc == B2S_OK) rc = b2s_global_ba(g_gba.h, &prob, reinterpret_cast<const volatile uint8_t*>(pbStopFlag), &res);
+    if (rc != B2S_OK) {
+      report("Optimizer::BundleAdjustment", rc);
       return;
     }
   }
@@ -608,11 +532,13 @@ void Optimizer::OptimizeEssentialGraph(Map* pMap, KeyFrame* pLoopKF, KeyFrame* p
   res.chi2_initial = res.chi2_final = 0;
   res.n_trials = 0;
   {
-    std::lock_guard<std::mutex> lock(g_eg.m);
-    b2s_eg_solver* solver = g_eg.get(nKF, nE, nMP);
-    if (!solver) return;
-    if (b2s_optimize_essential_graph(solver, &prob, &res) != B2S_OK) {
-      fprintf(stderr, "Optimizer::OptimizeEssentialGraph (b200): %s\n", b2s_last_error());
+    std::lock_guard<std::mutex> lock(g_eg.mutex);
+    int rc = g_eg.get({nKF, nE, nMP}, {1024, 16384, 65536}, [](const int* c, b2s_eg_solver** h) {
+      return b2s_eg_create(c[0], c[1], c[2], b2s_host::device(), h);
+    });
+    if (rc == B2S_OK) rc = b2s_optimize_essential_graph(g_eg.h, &prob, &res);
+    if (rc != B2S_OK) {
+      report("Optimizer::OptimizeEssentialGraph", rc);
       return;
     }
   }
@@ -696,11 +622,13 @@ int Optimizer::OptimizeSim3(KeyFrame* pKF1, KeyFrame* pKF2, vector<MapPoint*>& v
   res.trace = nullptr;
   res.n_inliers = res.n_trials = 0;
   {
-    std::lock_guard<std::mutex> lock(g_sim3.m);
-    b2s_sim3opt_solver* solver = g_sim3.get(n);
-    if (!solver) return 0;
-    if (b2s_optimize_sim3(solver, 1, &prob, &res) != B2S_OK) {
-      fprintf(stderr, "Optimizer::OptimizeSim3 (b200): %s\n", b2s_last_error());
+    std::lock_guard<std::mutex> lock(g_sim3.mutex);
+    int rc = g_sim3.get({n}, {4096}, [](const int* c, b2s_sim3opt_solver** h) {
+      return b2s_sim3opt_create(c[0], 1, b2s_host::device(), h);
+    });
+    if (rc == B2S_OK) rc = b2s_optimize_sim3(g_sim3.h, 1, &prob, &res);
+    if (rc != B2S_OK) {
+      report("Optimizer::OptimizeSim3", rc);
       return 0;
     }
   }

@@ -12,8 +12,6 @@
 // device the threshold scale the reference folds into mvMaxError.  The EPnP working arrays (pws, us, alphas, pcs) stay
 // unallocated: the device holds them.
 #include <cmath>
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <mutex>
 #include <vector>
@@ -22,30 +20,13 @@
 #include "Thirdparty/DBoW2/DUtils/Random.h"
 
 #include "b200slam.h"
+#include "../b2s_host.h"
 
 namespace ORB_SLAM2 {
 namespace {
 
 // One handle for the process (Tracking runs the solvers from one thread), grown on demand.
-struct PnPsolverSlot {
-  b2s_pnpsolver* h = nullptr;
-  int matches = 0, sets = 0;
-  std::mutex m;
-  b2s_pnpsolver* get(int n, int k) {
-    if (h && n <= matches && k <= sets) return h;
-    b2s_pnpsolver_destroy(h);
-    h = nullptr;
-    matches = n > 1024 ? n : 1024;
-    sets = k > 300 ? k : 300;
-    const char* e = getenv("B2S_DEVICE");
-    if (b2s_pnpsolver_create(matches, sets, 1, e ? atoi(e) : 0, &h) != B2S_OK) {
-      fprintf(stderr, "PnPsolver (b200): %s\n", b2s_last_error());
-      h = nullptr;
-      matches = sets = 0;
-    }
-    return h;
-  }
-} g_pnpsolver;
+b2s_host::Slot<b2s_pnpsolver, 2, b2s_pnpsolver_destroy> g_pnpsolver;
 
 }  // namespace
 
@@ -183,12 +164,14 @@ cv::Mat PnPsolver::iterate(int nIterations, bool& bNoMore, vector<bool>& vbInlie
   r.best_mask = bestOut.data();
   int rc;
   {
-    std::lock_guard<std::mutex> lock(g_pnpsolver.m);
-    b2s_pnpsolver* h = g_pnpsolver.get(N, k);
-    rc = h ? b2s_pnpsolver_iterate(h, 1, &q, &r) : B2S_ERR_CUDA;
+    std::lock_guard<std::mutex> lock(g_pnpsolver.mutex);
+    rc = g_pnpsolver.get({N, k}, {1024, 300}, [](const int* c, b2s_pnpsolver** h) {
+      return b2s_pnpsolver_create(c[0], c[1], 1, b2s_host::device(), h);
+    });
+    if (rc == B2S_OK) rc = b2s_pnpsolver_iterate(g_pnpsolver.h, 1, &q, &r);
   }
   if (rc != B2S_OK) {
-    fprintf(stderr, "PnPsolver::iterate: libb200slam error %d: %s\n", rc, b2s_last_error());
+    b2s_host::report("PnPsolver::iterate", rc);
     return cv::Mat();
   }
   mnIterations = r.iterations_done;

@@ -9,8 +9,6 @@
 //
 // mvSigmaSquare1 / mvSigmaSquare2, which the reference declares and never uses, hold the bit patterns of each
 // correspondence's float sigma2, so that iterate passes the device what the constructor read.
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <mutex>
 #include <vector>
@@ -19,30 +17,13 @@
 #include "Thirdparty/DBoW2/DUtils/Random.h"
 
 #include "b200slam.h"
+#include "../b2s_host.h"
 
 namespace ORB_SLAM2 {
 namespace {
 
 // One handle for the process (LoopClosing runs the solvers from one thread), grown on demand.
-struct Sim3SolverSlot {
-  b2s_sim3solver* h = nullptr;
-  int matches = 0, sets = 0;
-  std::mutex m;
-  b2s_sim3solver* get(int n, int k) {
-    if (h && n <= matches && k <= sets) return h;
-    b2s_sim3solver_destroy(h);
-    h = nullptr;
-    matches = n > 1024 ? n : 1024;
-    sets = k > 300 ? k : 300;
-    const char* e = getenv("B2S_DEVICE");
-    if (b2s_sim3solver_create(matches, sets, 1, e ? atoi(e) : 0, &h) != B2S_OK) {
-      fprintf(stderr, "Sim3Solver (b200): %s\n", b2s_last_error());
-      h = nullptr;
-      matches = sets = 0;
-    }
-    return h;
-  }
-} g_sim3solver;
+b2s_host::Slot<b2s_sim3solver, 2, b2s_sim3solver_destroy> g_sim3solver;
 
 size_t float_bits(float f) {
   uint32_t u;
@@ -185,12 +166,14 @@ cv::Mat Sim3Solver::iterate(int nIterations, bool& bNoMore, std::vector<bool>& v
   r.inliers = inl.data();
   int rc;
   {
-    std::lock_guard<std::mutex> lock(g_sim3solver.m);
-    b2s_sim3solver* h = g_sim3solver.get(N, k);
-    rc = h ? b2s_sim3solver_iterate(h, 1, &q, &r) : B2S_ERR_CUDA;
+    std::lock_guard<std::mutex> lock(g_sim3solver.mutex);
+    rc = g_sim3solver.get({N, k}, {1024, 300}, [](const int* c, b2s_sim3solver** h) {
+      return b2s_sim3solver_create(c[0], c[1], 1, b2s_host::device(), h);
+    });
+    if (rc == B2S_OK) rc = b2s_sim3solver_iterate(g_sim3solver.h, 1, &q, &r);
   }
   if (rc != B2S_OK) {
-    fprintf(stderr, "Sim3Solver::iterate: libb200slam error %d: %s\n", rc, b2s_last_error());
+    b2s_host::report("Sim3Solver::iterate", rc);
     return cv::Mat();
   }
   mnIterations = r.iterations_done;
