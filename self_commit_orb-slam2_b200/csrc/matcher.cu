@@ -415,7 +415,35 @@ __global__ void __launch_bounds__(128) k_bow_resolve(const uint8_t* __restrict__
   }
 }
 
-// rotation-histogram consistency (:356-379) + ComputeThreeMaxima (:1866-1908); one CTA per pair
+// ComputeThreeMaxima (:1866-1908), one thread: the bins of the three largest counts (strict >, so the earlier bin wins
+// a tie); the second and third are dropped (-1) when they hold less than a tenth of the first.
+__device__ __forceinline__ void three_maxima(const int* hist, int (&keep)[3]) {
+  int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
+  for (int i = 0; i < HISTO; i++) {
+    const int s = hist[i];
+    if (s > max1) {
+      max3 = max2; max2 = max1; max1 = s;
+      ind3 = ind2; ind2 = ind1; ind1 = i;
+    } else if (s > max2) {
+      max3 = max2; max2 = s;
+      ind3 = ind2; ind2 = i;
+    } else if (s > max3) {
+      max3 = s;
+      ind3 = i;
+    }
+  }
+  if ((float)max2 < 0.1f * (float)max1) {
+    ind2 = -1;
+    ind3 = -1;
+  } else if ((float)max3 < 0.1f * (float)max1) {
+    ind3 = -1;
+  }
+  keep[0] = ind1;
+  keep[1] = ind2;
+  keep[2] = ind3;
+}
+
+// rotation-histogram consistency (:356-379); one CTA per pair
 __global__ void __launch_bounds__(256) k_rot_cull(const int32_t* __restrict__ nBarr, int capB, int checkOri,
                                                   int32_t* __restrict__ matchB, const int32_t* __restrict__ binB,
                                                   const int32_t* __restrict__ extraCount,
@@ -439,31 +467,7 @@ __global__ void __launch_bounds__(256) k_rot_cull(const int32_t* __restrict__ nB
       if (checkOri) atomicAdd(&hist[bB[j]], 1);
     }
   __syncthreads();
-  if (threadIdx.x == 0) {
-    int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
-    for (int i = 0; i < HISTO; i++) {
-      const int s = hist[i];
-      if (s > max1) {
-        max3 = max2; max2 = max1; max1 = s;
-        ind3 = ind2; ind2 = ind1; ind1 = i;
-      } else if (s > max2) {
-        max3 = max2; max2 = s;
-        ind3 = ind2; ind2 = i;
-      } else if (s > max3) {
-        max3 = s;
-        ind3 = i;
-      }
-    }
-    if ((float)max2 < 0.1f * (float)max1) {
-      ind2 = -1;
-      ind3 = -1;
-    } else if ((float)max3 < 0.1f * (float)max1) {
-      ind3 = -1;
-    }
-    keep[0] = ind1;
-    keep[1] = ind2;
-    keep[2] = ind3;
-  }
+  if (threadIdx.x == 0) three_maxima(hist, keep);
   __syncthreads();
   if (checkOri) {
     for (int j = threadIdx.x; j < nB; j += blockDim.x)
@@ -605,7 +609,7 @@ __device__ __forceinline__ bool win_cells(const Win& w, const ProjGeom& g, int& 
   c1y = min(GRID_ROWS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(w.v, g.minY), w.r), g.invH)));
   return !(c0x >= GRID_COLS || c1x < 0 || c0y >= GRID_ROWS || c1y < 0);
 }
-// one candidate of the window: level gate, |dx|,|dy| < r, occupancy, stereo gate (:1648-1669 / :117-139)
+// one feature of the window's cells: level gate, |dx|,|dy| < r, stereo gate (:1648-1669 / :117-139)
 __device__ __forceinline__ bool win_take(const Win& w, int id, const float* __restrict__ kpx, const float* __restrict__ kpy,
                                          const int32_t* __restrict__ octave, const float* __restrict__ uright) {
   if ((w.minL > 0) || (w.maxL >= 0)) {
@@ -633,6 +637,17 @@ __device__ __forceinline__ bool win_chi2_ok(const Win& w, int id, const float* _
   }
   const float e2 = __fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey));
   return !((double)__fmul_rn(e2, is2) > 5.99);
+}
+// a candidate of the window: win_take, the Fuse gate when it is on, and never a feature occupied on entry (the test of
+// k_proj_topk's loop, which keeps it written out)
+__device__ __forceinline__ bool win_candidate(const Win& w, int id, const float* __restrict__ kpx,
+                                              const float* __restrict__ kpy, const int32_t* __restrict__ octave,
+                                              const float* __restrict__ uright, const uint8_t* __restrict__ occupied,
+                                              const ProjGeom& g) {
+  bool take = win_take(w, id, kpx, kpy, octave, uright);
+  if (take && w.chi2Gate) take = win_chi2_ok(w, id, kpx, kpy, octave, uright, g);
+  if (take && occupied && occupied[id]) take = false;
+  return take;
 }
 
 // stage 1: one warp per query; candidates are enumerated in GetFeaturesInArea order (src/Frame.cc:741-850:
@@ -714,15 +729,16 @@ __global__ void __launch_bounds__(256) k_proj_topk(const QT* __restrict__ q, int
   if (lane == 0) candCnt[i] = ok ? cnt : -1;
 }
 
-// Exact rescan of one query's window in enumeration order against the CURRENT occupancy: the two smallest
-// (distance, order) keys over the warp (key2/id2 = EMPTY/-1 when there is no second candidate).
-template <class QT>
+// Exact rescan of one query's window in enumeration order against the CURRENT state of the greedy loop: the NEED (1 or
+// 2) smallest (distance, order) keys over the warp among the candidates whose distance is below bound(feature)
+// (key2/id2 = EMPTY/-1 when there is no second candidate or NEED == 1).
+template <int NEED, class QT, class Bound>
 __device__ __forceinline__ void win_rescan_top2(const QT& Q, const ProjGeom& g, int lane, const float* __restrict__ kpx,
                                                 const float* __restrict__ kpy, const int32_t* __restrict__ octave,
                                                 const float* __restrict__ uright, const uint8_t* __restrict__ occupied,
-                                                const uint8_t* __restrict__ taken, const uint8_t* __restrict__ desc,
-                                                const int32_t* __restrict__ order, const int32_t* __restrict__ cellStart,
-                                                uint32_t& key1, int& id1, uint32_t& key2, int& id2) {
+                                                const uint8_t* __restrict__ desc, const int32_t* __restrict__ order,
+                                                const int32_t* __restrict__ cellStart, Bound bound, uint32_t& key1,
+                                                int& id1, uint32_t& key2, int& id2) {
   const Win w = make_win(Q, g);
   int c0x, c1x, c0y, c1y;
   win_cells(w, g, c0x, c1x, c0y, c1y);
@@ -734,17 +750,17 @@ __device__ __forceinline__ void win_rescan_top2(const QT& Q, const ProjGeom& g, 
     const int beg = cellStart[ix * GRID_ROWS + c0y], end = cellStart[ix * GRID_ROWS + c1y + 1];
     for (int p = beg + lane; p < end; p += 32) {
       const int fid = order[p];
-      bool take = win_take(w, fid, kpx, kpy, octave, uright);
-      if (take && w.chi2Gate) take = win_chi2_ok(w, fid, kpx, kpy, octave, uright, g);
-      if (take && ((occupied && occupied[fid]) || taken[fid])) take = false;
-      if (take) {
-        const uint32_t key = ((uint32_t)hamming256(dq, ld_desc(desc, fid)) << 20) | (uint32_t)(ord + (p - beg));
-        if (key < k1) {
-          k2 = k1; i2 = i1;
-          k1 = key; i1 = fid;
-        } else if (key < k2) {
-          k2 = key; i2 = fid;
-        }
+      if (!win_candidate(w, fid, kpx, kpy, octave, uright, occupied, g)) continue;
+      const int lim = bound(fid);
+      if (lim <= 0) continue;  // no distance is below it
+      const int d = hamming256(dq, ld_desc(desc, fid));
+      if (d >= lim) continue;
+      const uint32_t key = ((uint32_t)d << 20) | (uint32_t)(ord + (p - beg));
+      if (key < k1) {
+        k2 = k1; i2 = i1;
+        k1 = key; i1 = fid;
+      } else if (key < k2) {
+        k2 = key; i2 = fid;
       }
     }
     ord += end - beg;
@@ -761,6 +777,7 @@ __device__ __forceinline__ void win_rescan_top2(const QT& Q, const ProjGeom& g, 
   const unsigned who = __ballot_sync(0xffffffffu, k1 == m1);
   const int wl = __ffs(who) - 1;
   id1 = __shfl_sync(0xffffffffu, i1, wl);
+  if (NEED == 1) return;  // shuffles are not dead code to the compiler
   // second: the winner lane contributes its own runner-up, every other lane its best
   const uint32_t cand2 = (lane == wl) ? k2 : k1;
   const int cid2 = (lane == wl) ? i2 : i1;
@@ -771,6 +788,40 @@ __device__ __forceinline__ void win_rescan_top2(const QT& Q, const ProjGeom& g, 
     const unsigned who2 = __ballot_sync(0xffffffffu, cand2 == m2);
     key2 = m2;
     id2 = __shfl_sync(0xffffffffu, cid2, __ffs(who2) - 1);
+  }
+}
+
+// The best and (NEED == 2) second-best candidates of query Q that are available NOW — a candidate counts while its
+// distance is below bound(feature) — as keys ascending; key/id = EMPTY/-1 where there is none.  Removing unavailable
+// entries from the query's K-list (topk / topkIdx, sorted by distance, then enumeration order) keeps the reference's
+// first-minimum rule and its runner-up, so the list decides when it holds NEED available entries, or at least one and the
+// window had no more than TOPK candidates (cc; the list is then the whole window).  Otherwise a window with more than TOPK candidates is rescanned exactly; otherwise there is none.
+template <int NEED, class QT, class Bound>
+__device__ __forceinline__ void best_two(const QT& Q, int cc, const uint32_t* __restrict__ topk,
+                                         const int32_t* __restrict__ topkIdx, const ProjGeom& g, int lane,
+                                         const float* __restrict__ kpx, const float* __restrict__ kpy,
+                                         const int32_t* __restrict__ octave, const float* __restrict__ uright,
+                                         const uint8_t* __restrict__ occupied, const uint8_t* __restrict__ desc,
+                                         const int32_t* __restrict__ order, const int32_t* __restrict__ cellStart,
+                                         Bound bound, uint32_t& key1, int& id1, uint32_t& key2, int& id2) {
+  const uint32_t e = (lane < TOPK) ? topk[lane] : EMPTY;
+  const int id = (lane < TOPK) ? topkIdx[lane] : -1;
+  unsigned am = __ballot_sync(0xffffffffu, e != EMPTY && (int)(e >> 20) < bound(id));
+  key1 = EMPTY; id1 = -1;
+  key2 = EMPTY; id2 = -1;
+  if (__popc(am) >= NEED || (am != 0u && cc <= TOPK)) {
+    const int l1 = __ffs(am) - 1;
+    key1 = __shfl_sync(0xffffffffu, e, l1);
+    id1 = __shfl_sync(0xffffffffu, id, l1);
+    am &= am - 1;
+    if (NEED == 2 && am) {
+      const int l2 = __ffs(am) - 1;
+      key2 = __shfl_sync(0xffffffffu, e, l2);
+      id2 = __shfl_sync(0xffffffffu, id, l2);
+    }
+  } else if (cc > TOPK) {
+    win_rescan_top2<NEED>(Q, g, lane, kpx, kpy, octave, uright, occupied, desc, order, cellStart, bound, key1, id1, key2,
+                          id2);
   }
 }
 
@@ -805,86 +856,22 @@ __global__ void __launch_bounds__(32) k_proj_resolve(const ProjQuery* __restrict
   for (int i = 0; i < nq; i++) {
     const int cc = candCnt[i];
     if (cc <= 0) continue;
-    const uint32_t e = (lane < TOPK) ? topk[(size_t)i * TOPK + lane] : EMPTY;
-    const int id = (lane < TOPK) ? topkIdx[(size_t)i * TOPK + lane] : -1;
-    const bool avail = (e != EMPTY) && !taken[id];
-    const unsigned am = __ballot_sync(0xffffffffu, avail);
-    int bestDist = 256, bestIdx = -1;
-    if (am) {
-      const int l1 = __ffs(am) - 1;
-      bestDist = (int)(__shfl_sync(0xffffffffu, e, l1) >> 20);
-      bestIdx = __shfl_sync(0xffffffffu, id, l1);
-    } else if (cc > TOPK) {
-      // exact rescan in enumeration order
-      const ProjQuery& Q = q[i];
-      const float u = Q.u, v = Q.v, invz = Q.invz;
-      const int oct = Q.octave;
-      const float r = __fmul_rn(g.th, g.scale[oct]);
-      int minL, maxL;
-      if (g.mode == 1) { minL = oct; maxL = -1; }
-      else if (g.mode == 2) { minL = 0; maxL = oct; }
-      else { minL = oct - 1; maxL = oct + 1; }
-      const int c0x = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(u, g.minX), r), g.invW)));
-      const int c1x = min(GRID_COLS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(u, g.minX), r), g.invW)));
-      const int c0y = max(0, (int)floorf(__fmul_rn(__fsub_rn(__fsub_rn(v, g.minY), r), g.invH)));
-      const int c1y = min(GRID_ROWS - 1, (int)ceilf(__fmul_rn(__fadd_rn(__fsub_rn(v, g.minY), r), g.invH)));
-      const bool checkLevels = (minL > 0) || (maxL >= 0);
-      const u256 dq = ld_desc_w(Q.desc);
-      const float ur = __fsub_rn(u, __fmul_rn(g.bf, invz));
-      uint32_t bestKey = EMPTY;
-      int bestId = -1;
-      int ord = 0;
-      for (int ix = c0x; ix <= c1x; ix++) {
-        const int beg = cellStart[ix * GRID_ROWS + c0y], end = cellStart[ix * GRID_ROWS + c1y + 1];
-        for (int p = beg + lane; p < end; p += 32) {
-          const int fid = order[p];
-          bool take = true;
-          if (checkLevels) {
-            const int o = octave[fid];
-            if (o < minL) take = false;
-            if (maxL >= 0 && o > maxL) take = false;
-          }
-          if (take) {
-            const float dx = __fsub_rn(kpx[fid], u), dy = __fsub_rn(kpy[fid], v);
-            if (!(fabsf(dx) < r && fabsf(dy) < r)) take = false;
-          }
-          if (take && ((occupied && occupied[fid]) || taken[fid])) take = false;
-          if (take) {
-            const float urr = uright[fid];
-            if (urr > 0 && fabsf(__fsub_rn(ur, urr)) > r) take = false;
-          }
-          if (take) {
-            const uint32_t key = ((uint32_t)hamming256(dq, ld_desc(desc, fid)) << 20) | (uint32_t)(ord + (p - beg));
-            if (key < bestKey) {
-              bestKey = key;
-              bestId = fid;
-            }
-          }
-        }
-        ord += end - beg;
+    uint32_t key1, key2;
+    int id1, id2;
+    best_two<1>(q[i], cc, topk + (size_t)i * TOPK, topkIdx + (size_t)i * TOPK, g, lane, kpx, kpy, octave, uright, occupied,
+                desc, order, cellStart, [=](int f) { return taken[f] ? 0 : 257; }, key1, id1, key2, id2);
+    if (id1 < 0 || (int)(key1 >> 20) > g.thHigh) continue;  // :1683
+    if (lane == 0) {
+      matchCur[id1] = i;
+      taken[id1] = q[i].has_obs ? 1 : 0;
+      if (g.checkOri) {
+        const int bn = rot_bin(q[i].angle, angle[id1]);
+        pushList[nAccepted] = (bn << 20) | id1;  // rotHist[bin].push_back(bestIdx2) (:1700)
+        hist[bn]++;
       }
-      uint32_t m = bestKey;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) m = min(m, __shfl_xor_sync(0xffffffffu, m, o));
-      if (m != EMPTY) {
-        const unsigned who = __ballot_sync(0xffffffffu, bestKey == m);
-        bestDist = (int)(m >> 20);
-        bestIdx = __shfl_sync(0xffffffffu, bestId, __ffs(who) - 1);
-      }
+      nAccepted++;
     }
-    if (bestDist <= g.thHigh) {  // :1683
-      if (lane == 0) {
-        matchCur[bestIdx] = i;
-        taken[bestIdx] = q[i].has_obs ? 1 : 0;
-        if (g.checkOri) {
-          const int bn = rot_bin(q[i].angle, angle[bestIdx]);
-          pushList[nAccepted] = (bn << 20) | bestIdx;  // rotHist[bin].push_back(bestIdx2) (:1700)
-          hist[bn]++;
-        }
-        nAccepted++;
-      }
-      __syncwarp();
-    }
+    __syncwarp();
   }
   __syncwarp();
   if (lane == 0) accepted[0] = nAccepted;
@@ -1067,20 +1054,10 @@ __global__ void __launch_bounds__(32) k_win_resolve(const WinQuery* __restrict__
     const int cc = candCnt[i];
     int outIdx = -1, outDist = 256;
     if (cc > 0) {
-      const uint32_t e = (lane < TOPK) ? topk[(size_t)i * TOPK + lane] : EMPTY;
-      const int id = (lane < TOPK) ? topkIdx[(size_t)i * TOPK + lane] : -1;
-      const bool avail = (e != EMPTY) && !taken[id];
-      const unsigned am = __ballot_sync(0xffffffffu, avail);
-      uint32_t key1 = EMPTY, key2;
-      int id1 = -1, id2;
-      if (am) {
-        const int l1 = __ffs(am) - 1;
-        key1 = __shfl_sync(0xffffffffu, e, l1);
-        id1 = __shfl_sync(0xffffffffu, id, l1);
-      } else if (cc > TOPK) {
-        win_rescan_top2(q[i], g, lane, kpx, kpy, octave, uright, occupied, taken, desc, order, cellStart, key1, id1, key2,
-                        id2);
-      }
+      uint32_t key1, key2;
+      int id1, id2;
+      best_two<1>(q[i], cc, topk + (size_t)i * TOPK, topkIdx + (size_t)i * TOPK, g, lane, kpx, kpy, octave, uright,
+                  occupied, desc, order, cellStart, [=](int f) { return taken[f] ? 0 : 257; }, key1, id1, key2, id2);
       if (id1 >= 0) {
         outDist = (int)(key1 >> 20);
         if (outDist <= thDist) {
@@ -1117,26 +1094,10 @@ __global__ void __launch_bounds__(32) k_map_resolve(const MapQuery* __restrict__
   for (int i = 0; i < nq; i++) {
     const int cc = candCnt[i];
     if (cc <= 0) continue;
-    const uint32_t e = (lane < TOPK) ? topk[(size_t)i * TOPK + lane] : EMPTY;
-    const int id = (lane < TOPK) ? topkIdx[(size_t)i * TOPK + lane] : -1;
-    const bool avail = (e != EMPTY) && !taken[id];
-    unsigned am = __ballot_sync(0xffffffffu, avail);
-    uint32_t key1 = EMPTY, key2 = EMPTY;
-    int id1 = -1, id2 = -1;
-    if (__popc(am) >= 2 || (am != 0u && cc <= TOPK)) {
-      const int l1 = __ffs(am) - 1;
-      key1 = __shfl_sync(0xffffffffu, e, l1);
-      id1 = __shfl_sync(0xffffffffu, id, l1);
-      am &= am - 1;
-      if (am) {
-        const int l2 = __ffs(am) - 1;
-        key2 = __shfl_sync(0xffffffffu, e, l2);
-        id2 = __shfl_sync(0xffffffffu, id, l2);
-      }
-    } else if (cc > TOPK) {
-      win_rescan_top2(q[i], g, lane, kpx, kpy, octave, uright, occupied, taken, desc, order, cellStart, key1, id1, key2,
-                      id2);
-    }
+    uint32_t key1, key2;
+    int id1, id2;
+    best_two<2>(q[i], cc, topk + (size_t)i * TOPK, topkIdx + (size_t)i * TOPK, g, lane, kpx, kpy, octave, uright, occupied,
+                desc, order, cellStart, [=](int f) { return taken[f] ? 0 : 257; }, key1, id1, key2, id2);
     if (id1 < 0) continue;
     const int bestDist = (int)(key1 >> 20);
     if (bestDist > g.thHigh) continue;  // :164
@@ -1167,29 +1128,7 @@ __global__ void __launch_bounds__(256) k_proj_cull(int checkOri, const int32_t* 
   matchCur += (size_t)blockIdx.y * strideF; pushBins += (size_t)blockIdx.y * strideQ;
   if (threadIdx.x == 0) {
     culled = 0;
-    int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
-    for (int i = 0; i < HISTO; i++) {
-      const int s = hist[i];
-      if (s > max1) {
-        max3 = max2; max2 = max1; max1 = s;
-        ind3 = ind2; ind2 = ind1; ind1 = i;
-      } else if (s > max2) {
-        max3 = max2; max2 = s;
-        ind3 = ind2; ind2 = i;
-      } else if (s > max3) {
-        max3 = s;
-        ind3 = i;
-      }
-    }
-    if ((float)max2 < 0.1f * (float)max1) {
-      ind2 = -1;
-      ind3 = -1;
-    } else if ((float)max3 < 0.1f * (float)max1) {
-      ind3 = -1;
-    }
-    keep[0] = ind1;
-    keep[1] = ind2;
-    keep[2] = ind3;
+    three_maxima(hist, keep);
   }
   __syncthreads();
   if (checkOri) {
@@ -1209,53 +1148,6 @@ __global__ void __launch_bounds__(256) k_proj_cull(int checkOri, const int32_t* 
 }
 
 // ---------------------------------------------------------------- SearchForInitialization (src/ORBmatcher.cc:515-643)
-// Exact rescan of one query's window against the CURRENT vMatchedDistance (:563): the two smallest (distance, order)
-// keys among the candidates whose feature is not already matched with a distance <= the candidate's.
-__device__ __forceinline__ void init_rescan_top2(const WinQuery& Q, const ProjGeom& g, int lane, const float* __restrict__ kpx,
-                                                 const float* __restrict__ kpy, const int32_t* __restrict__ octave,
-                                                 const float* __restrict__ uright, const int32_t* __restrict__ matchedDist,
-                                                 const uint8_t* __restrict__ desc, const int32_t* __restrict__ order,
-                                                 const int32_t* __restrict__ cellStart, uint32_t& key1, int& id1,
-                                                 uint32_t& key2) {
-  const Win w = make_win(Q, g);
-  int c0x, c1x, c0y, c1y;
-  win_cells(w, g, c0x, c1x, c0y, c1y);
-  const u256 dq = ld_desc_w(Q.desc);
-  uint32_t k1 = EMPTY, k2 = EMPTY;
-  int i1 = -1;
-  int ord = 0;
-  for (int ix = c0x; ix <= c1x; ix++) {
-    const int beg = cellStart[ix * GRID_ROWS + c0y], end = cellStart[ix * GRID_ROWS + c1y + 1];
-    for (int p = beg + lane; p < end; p += 32) {
-      const int fid = order[p];
-      if (!win_take(w, fid, kpx, kpy, octave, uright)) continue;
-      const int d = hamming256(dq, ld_desc(desc, fid));
-      if (matchedDist[fid] <= d) continue;
-      const uint32_t key = ((uint32_t)d << 20) | (uint32_t)(ord + (p - beg));
-      if (key < k1) {
-        k2 = k1;
-        k1 = key; i1 = fid;
-      } else if (key < k2) {
-        k2 = key;
-      }
-    }
-    ord += end - beg;
-  }
-  uint32_t m1 = k1;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m1 = min(m1, __shfl_xor_sync(0xffffffffu, m1, o));
-  key1 = m1;
-  id1 = -1;
-  key2 = EMPTY;
-  if (m1 == EMPTY) return;
-  const int wl = __ffs(__ballot_sync(0xffffffffu, k1 == m1)) - 1;
-  id1 = __shfl_sync(0xffffffffu, i1, wl);
-  uint32_t m2 = (lane == wl) ? k2 : k1;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m2 = min(m2, __shfl_xor_sync(0xffffffffu, m2, o));
-  key2 = m2;
-}
-
 // The sequential loop of :527-610 — one warp walks F1's keypoints in order over their K-lists (sorted by distance, then
 // enumeration order).  matchedDist / match21 are the reference's vMatchedDistance / vnMatches21; a query whose list cannot
 // prove its best two remaining candidates is rescanned exactly.  Every accepted match is pushed to the rotation histogram
@@ -1279,23 +1171,11 @@ __global__ void __launch_bounds__(32) k_init_resolve(const WinQuery* __restrict_
   for (int i = 0; i < nq; i++) {
     const int cc = candCnt[i];
     if (cc <= 0) continue;
-    const uint32_t e = (lane < TOPK) ? topk[(size_t)i * TOPK + lane] : EMPTY;
-    const int id = (lane < TOPK) ? topkIdx[(size_t)i * TOPK + lane] : -1;
-    const bool avail = (e != EMPTY) && !(matchedDist[id] <= (int)(e >> 20));
-    unsigned am = __ballot_sync(0xffffffffu, avail);
-    uint32_t key1 = EMPTY, key2 = EMPTY;
-    int id1 = -1;
-    if (__popc(am) >= 2 || cc <= TOPK) {  // the list holds the best two remaining candidates (or all candidates)
-      if (am) {
-        const int l1 = __ffs(am) - 1;
-        key1 = __shfl_sync(0xffffffffu, e, l1);
-        id1 = __shfl_sync(0xffffffffu, id, l1);
-        am &= am - 1;
-        if (am) key2 = __shfl_sync(0xffffffffu, e, __ffs(am) - 1);
-      }
-    } else {
-      init_rescan_top2(q[i], g, lane, kpx, kpy, octave, uright, matchedDist, desc, order, cellStart, key1, id1, key2);
-    }
+    uint32_t key1, key2;
+    int id1, id2;
+    // a feature already matched at a distance <= the candidate's is no candidate (:563)
+    best_two<2>(q[i], cc, topk + (size_t)i * TOPK, topkIdx + (size_t)i * TOPK, g, lane, kpx, kpy, octave, uright, nullptr,
+                desc, order, cellStart, [=](int f) { return matchedDist[f]; }, key1, id1, key2, id2);
     if (id1 < 0) continue;
     const int bestDist = (int)(key1 >> 20);
     const int bestDist2 = key2 == EMPTY ? 2147483647 : (int)(key2 >> 20);
@@ -1330,27 +1210,7 @@ __global__ void __launch_bounds__(256) k_init_cull(int checkOri, int n1, const i
   __shared__ int total;
   if (threadIdx.x == 0) {
     total = 0;
-    int max1 = 0, max2 = 0, max3 = 0, ind1 = -1, ind2 = -1, ind3 = -1;
-    for (int i = 0; i < HISTO; i++) {
-      const int s = hist[i];
-      if (s > max1) {
-        max3 = max2; max2 = max1; max1 = s;
-        ind3 = ind2; ind2 = ind1; ind1 = i;
-      } else if (s > max2) {
-        max3 = max2; max2 = s;
-        ind3 = ind2; ind2 = i;
-      } else if (s > max3) {
-        max3 = s;
-        ind3 = i;
-      }
-    }
-    if ((float)max2 < 0.1f * (float)max1) {
-      ind2 = -1;
-      ind3 = -1;
-    } else if ((float)max3 < 0.1f * (float)max1) {
-      ind3 = -1;
-    }
-    keep[0] = ind1; keep[1] = ind2; keep[2] = ind3;
+    three_maxima(hist, keep);
   }
   __syncthreads();
   if (checkOri) {

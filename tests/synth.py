@@ -269,8 +269,14 @@ def synth_local_ba(n_kf=50, n_fixed=10, n_mp=5000, obs_per_mp=6, seed=42, mono_f
                 cy=np.float32(cy), bf=np.float32(bf), Tcw_true=Tcw_true, pts_true=pts_true)
 
 
-def synth_projection(nf=2000, nq=1800, seed=7, w=1241, h=376, cluster=False, th=7.0):
-    """Current-frame features + projected last-frame map points (SURVEY A5 / src/ORBmatcher.cc:1569)."""
+CROWD_F, CROWD_Q = np.arange(100, 112), np.arange(5, 21)
+
+
+def synth_projection(nf=2000, nq=1800, seed=7, w=1241, h=376, cluster=False, th=7.0, crowd=False):
+    """Current-frame features + projected last-frame map points (SURVEY A5 / src/ORBmatcher.cc:1569).
+    crowd: the 12 features CROWD_F share one descriptor inside one window and the 16 queries CROWD_Q (the first valid
+    ones) carry it too, so from the ninth of them on the K-list (8 entries) holds only taken features while the window
+    has more than 8 candidates."""
     rng = np.random.RandomState(seed)
     scale = np.array([np.float32(1.2) ** i for i in range(8)], np.float32)
     if cluster:
@@ -311,15 +317,25 @@ def synth_projection(nf=2000, nq=1800, seed=7, w=1241, h=376, cluster=False, th=
         q["desc"][i] = d
     # a few queries out of bounds
     q["u"][:5] = -3.0
+    if crowd:
+        x0, y0 = np.float32(w / 2), np.float32(h / 2)
+        k = np.arange(len(CROWD_F))
+        kpx[CROWD_F] = x0 + ((k % 4) - np.float32(1.5)) / np.float32(4)
+        kpy[CROWD_F] = y0 + ((k // 4) - np.float32(1)) / np.float32(4)
+        octave[CROWD_F], uright[CROWD_F], occupied[CROWD_F] = 0, -1.0, 0
+        desc[CROWD_F], angle[CROWD_F] = desc[CROWD_F[0]], angle[CROWD_F[0]]
+        q["u"][CROWD_Q], q["v"][CROWD_Q], q["invz"][CROWD_Q] = x0, y0, np.float32(0.1)
+        q["angle"][CROWD_Q], q["octave"][CROWD_Q], q["has_obs"][CROWD_Q] = angle[CROWD_F[0]], 0, 1
+        q["desc"][CROWD_Q] = desc[CROWD_F[0]]
     geom = dict(mnMinX=np.float32(0), mnMinY=np.float32(0), mnMaxX=np.float32(w), mnMaxY=np.float32(h), bf=bf,
                 scale_factors=scale)
     return dict(q=q, kpx=kpx, kpy=kpy, octave=octave, angle=angle, uright=uright, occupied=occupied, desc=desc,
                 geom=geom, th=np.float32(th))
 
 
-def synth_projection_map(nf=2000, nq=2500, seed=9, w=1241, h=376, cluster=False):
+def synth_projection_map(nf=2000, nq=2500, seed=9, w=1241, h=376, cluster=False, crowd=False):
     """Current-frame features + local map points after isInFrustum (SURVEY M4 / src/ORBmatcher.cc:70-175)."""
-    d = synth_projection(nf=nf, nq=nq, seed=seed, w=w, h=h, cluster=cluster)
+    d = synth_projection(nf=nf, nq=nq, seed=seed, w=w, h=h, cluster=cluster, crowd=crowd)
     rng = np.random.RandomState(seed + 77)
     q0 = d["q"]
     qdt = np.dtype([("u", "<f4"), ("v", "<f4"), ("ur", "<f4"), ("view_cos", "<f4"), ("level", "<i4"), ("in_view", "u1"),
@@ -334,14 +350,16 @@ def synth_projection_map(nf=2000, nq=2500, seed=9, w=1241, h=376, cluster=False)
     q["level"] = q0["octave"]
     q["in_view"] = (rng.randint(0, 100, size=nq) < 90).astype(np.uint8)
     q["has_obs"] = (rng.randint(0, 100, size=nq) < 85).astype(np.uint8)
+    if crowd:
+        q["in_view"][CROWD_Q], q["has_obs"][CROWD_Q] = 1, 1
     d = dict(d)
     d["q"] = q
     return d
 
 
-def synth_windows(nf=2000, nq=2500, seed=13, th=3.0, cluster=False):
+def synth_windows(nf=2000, nq=2500, seed=13, th=3.0, cluster=False, crowd=False):
     """Keyframe features + projected map points for the Fuse / SearchByProjection(KeyFrame*, Scw, ...) search core."""
-    d = synth_projection(nf=nf, nq=nq, seed=seed, cluster=cluster)
+    d = synth_projection(nf=nf, nq=nq, seed=seed, cluster=cluster, crowd=crowd)
     rng = np.random.RandomState(seed + 5)
     q0 = d["q"]
     qdt = np.dtype([("u", "<f4"), ("v", "<f4"), ("ur", "<f4"), ("radius", "<f4"), ("min_level", "<i4"), ("max_level", "<i4"),
@@ -357,6 +375,8 @@ def synth_windows(nf=2000, nq=2500, seed=13, th=3.0, cluster=False):
     q["radius"] = (np.float32(th) * d["geom"]["scale_factors"][lvl]).astype(np.float32)
     q["min_level"], q["max_level"] = lvl - 1, lvl
     q["valid"] = (rng.randint(0, 100, size=nq) < 92).astype(np.uint8)
+    if crowd:
+        q["valid"][CROWD_Q] = 1
     d = dict(d)
     d["q"] = q
     d["inv_sigma2"] = (np.float32(1.0) / (d["geom"]["scale_factors"] * d["geom"]["scale_factors"])).astype(np.float32)

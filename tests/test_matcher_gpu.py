@@ -2,7 +2,7 @@
 import numpy as np
 import pytest
 
-from synth import synth_descriptors, synth_projection, synth_projection_map, synth_triangulation, synth_windows
+from synth import CROWD_F, CROWD_Q, synth_descriptors, synth_projection, synth_projection_map, synth_triangulation, synth_windows
 
 pytestmark = pytest.mark.gpu
 
@@ -123,9 +123,10 @@ def test_search_by_bow_ragged(pkg, oracle):
 
 
 @pytest.mark.parametrize("mode", [0, 1, 2])
-@pytest.mark.parametrize("cluster,th", [(False, 7.0), (False, 15.0), (True, 15.0)])
+@pytest.mark.parametrize("cluster,th", [(False, 7.0), (False, 15.0), (True, 15.0), ("crowd", 7.0)])
 def test_search_by_projection(pkg, oracle, mode, cluster, th):
-    d = synth_projection(seed=21 + mode, cluster=cluster, th=th)
+    """cluster = "crowd": the crowded window of synth_projection, whose last queries reach the exact rescan."""
+    d = synth_projection(seed=21 + mode, cluster=cluster is True, th=th, crowd=cluster == "crowd")
     m = pkg.ORBmatcher(0.9, True)
     n, match = m.SearchByProjection(d["q"], d["kpx"], d["kpy"], d["octave"], d["angle"], d["uright"], d["occupied"],
                                     d["desc"], d["geom"], d["th"], mode=mode)
@@ -134,6 +135,17 @@ def test_search_by_projection(pkg, oracle, mode, cluster, th):
     assert n == on
     assert np.array_equal(match, om)
     assert n > 100
+    if cluster == "crowd":
+        assert (match[CROWD_F] >= 0).all()  # features 9..12 of the crowd are only found by the rescan
+        # the batched form (no occupancy on entry) on the same pair
+        kps = np.zeros((1, len(d["kpx"])), pkg.keypoint_dtype)
+        kps["x"][0], kps["y"][0], kps["octave"][0], kps["angle"][0] = d["kpx"], d["kpy"], d["octave"], d["angle"]
+        nb, mb = m.SearchByProjectionBatch(d["q"][None], np.array([len(d["q"])]), kps, d["uright"][None], d["desc"][None],
+                                           np.array([len(d["kpx"])]), d["geom"], d["th"], mode=mode)
+        on, om = oracle.search_by_projection_last(d["q"], d["kpx"], d["kpy"], d["octave"], d["angle"], d["uright"], None,
+                                                  d["desc"], d["geom"], float(d["th"]), mode=mode)
+        assert nb[0] == on and np.array_equal(mb[0], om)
+        assert (mb[0][CROWD_F] >= 0).all()
 
 
 def test_against_committed_golden(pkg):
@@ -154,12 +166,13 @@ def test_against_committed_golden(pkg):
 
 
 @pytest.mark.parametrize("th", [1.0, 3.0])
-@pytest.mark.parametrize("cluster", [False, True])
+@pytest.mark.parametrize("cluster", [False, True, "crowd"])
 @pytest.mark.parametrize("nnratio", [0.8, 0.6])
 def test_search_by_projection_map(pkg, oracle, th, cluster, nnratio):
     """SearchByProjection(Frame&, vector<MapPoint*>&, th) (src/ORBmatcher.cc:70-175): bit-exact match array and count,
-    including the level-gated ratio test, the dynamic occupancy and K-list exhaustion (clustered descriptors)."""
-    d = synth_projection_map(seed=31 + int(th), cluster=cluster)
+    including the level-gated ratio test, the dynamic occupancy and K-list exhaustion (clustered descriptors, and the
+    crowded window of synth_projection, whose queries from the eighth on reach the exact rescan)."""
+    d = synth_projection_map(seed=31 + int(th), cluster=cluster is True, crowd=cluster == "crowd")
     m = pkg.ORBmatcher(nnratio, True)
     n, match = m.SearchByProjectionMap(d["q"], d["kpx"], d["kpy"], d["octave"], d["uright"], d["occupied"], d["desc"],
                                        d["geom"], th=th)
@@ -168,6 +181,8 @@ def test_search_by_projection_map(pkg, oracle, th, cluster, nnratio):
     assert n == on
     assert np.array_equal(match, om)
     assert n > 100
+    if cluster == "crowd":
+        assert (match[CROWD_F] >= 0).all()
 
 
 def test_search_by_projection_map_edge_cases(pkg, oracle):
@@ -189,13 +204,14 @@ def test_search_by_projection_map_edge_cases(pkg, oracle):
     assert n == on and np.array_equal(match, om)
 
 
-@pytest.mark.parametrize("chi2,greedy", [(True, False), (False, False), (False, True)])
-@pytest.mark.parametrize("cluster", [False, True])
+@pytest.mark.parametrize("chi2,greedy", [(True, False), (False, False), (False, True), (True, True)])
+@pytest.mark.parametrize("cluster", [False, True, "crowd"])
 def test_search_windows(pkg, oracle, chi2, greedy, cluster):
     """Search core of Fuse (src/ORBmatcher.cc:1020-1174 with the chi-square gate, :1179-1310 without) and of
     SearchByProjection(KeyFrame*, Scw, vpPoints, vpMatched, th) (:388-512, greedy occupancy): identical best feature per
-    map point, distance and accepted count."""
-    d = synth_windows(seed=13 + int(chi2) + 2 * int(greedy), th=3.0 if not cluster else 6.0, cluster=cluster)
+    map point, distance and accepted count.  cluster = "crowd": the crowded window of synth_projection."""
+    d = synth_windows(seed=13 + int(chi2) + 2 * int(greedy), th=3.0 if not cluster else 6.0, cluster=cluster is True,
+                      crowd=cluster == "crowd")
     occ = d["occupied"] if greedy else None
     m = pkg.ORBmatcher(0.8, True)
     n, best, bd = m.SearchWindows(d["q"], d["kpx"], d["kpy"], d["octave"], d["uright"], d["inv_sigma2"], occ, d["desc"],
@@ -209,6 +225,8 @@ def test_search_windows(pkg, oracle, chi2, greedy, cluster):
     if greedy:  # every feature is given to at most one map point
         used = best[best >= 0]
         assert len(np.unique(used)) == len(used)
+        if cluster == "crowd":  # the greedy search hands the whole crowd out, the last four through the rescan
+            assert set(CROWD_F) <= set(best[CROWD_Q])
 
 
 @pytest.mark.parametrize("only_stereo", [False, True])
@@ -267,3 +285,87 @@ def test_distinctive_descriptors(pkg, oracle):
     obest = oracle.distinctive_descriptors(desc, offsets)
     assert np.array_equal(best, obest)
     assert best[0] == -1 and best[1] == 0
+
+
+def _flip(d, bits):
+    o = d.copy()
+    for b in bits:
+        o[b >> 3] ^= np.uint8(1 << (b & 7))
+    return o
+
+
+_GEOM = dict(mnMinX=np.float32(0), mnMinY=np.float32(0), mnMaxX=np.float32(640), mnMaxY=np.float32(480),
+             bf=np.float32(0), scale_factors=np.array([np.float32(1.2) ** i for i in range(8)], np.float32))
+
+
+@pytest.mark.parametrize("check_ori", [False, True])
+def test_search_for_initialization_crowded(pkg, oracle, check_ori):
+    """SearchForInitialization (src/ORBmatcher.cc:515-643) on one crowded window.  Twelve features, each 20 bits from a
+    base descriptor B on bits of its own, are claimed at distance 0 by the first twelve keypoints.  The later keypoints
+    carry B: their eight nearest features are claimed ones (vMatchedDistance 0 <= 20), and the window holds 15 candidates,
+    so they are decided by the exact rescan, which finds the three unclaimed features at 30, 40 and 45 bits from B."""
+    rng = np.random.RandomState(3)
+    base = rng.randint(0, 256, 32).astype(np.uint8)
+    bits = rng.permutation(256)
+    claimed = [_flip(base, bits[20 * k:20 * k + 20]) for k in range(12)]
+    free = [_flip(base, bits[240:256].tolist() + bits[:n - 16].tolist()) for n in (30, 40, 45)]
+    desc2 = np.array(claimed + free, np.uint8)
+    n2 = len(desc2)
+    kpx2 = (np.float32(320) + (np.arange(n2) % 5 - 2) * np.float32(1.5)).astype(np.float32)
+    kpy2 = (np.float32(240) + (np.arange(n2) // 5 - 1) * np.float32(1.5)).astype(np.float32)
+    desc1 = np.array(claimed + [base] * 5, np.uint8)
+    n1 = len(desc1)
+    prev = np.tile(np.array([[320.0, 240.0]], np.float32), (n1, 1))
+    oct1, oct2 = np.zeros(n1, np.int32), np.zeros(n2, np.int32)
+    ang1 = np.full(n1, 10.0, np.float32)
+    ang2 = np.full(n2, 9.0, np.float32)
+    m = pkg.ORBmatcher(0.9, check_ori)
+    n, m12 = m.SearchForInitialization(prev.copy(), oct1, ang1, desc1, kpx2, kpy2, oct2, ang2, desc2, _GEOM, window=10)
+    on, om = oracle.search_for_initialization(prev.copy(), oct1, ang1, desc1, kpx2, kpy2, oct2, ang2, desc2, _GEOM,
+                                              window=10, nnratio=0.9, check_ori=check_ori)
+    assert n == on and np.array_equal(m12, om)
+    assert np.array_equal(m12[:12], np.arange(12))
+    assert m12[12] >= 12  # only the rescan reaches the unclaimed features
+
+
+# (bin: pairs) of a rotation histogram, and the matches ComputeThreeMaxima (src/ORBmatcher.cc:1866-1908) keeps
+ROT_HISTS = [
+    ({2: 10, 9: 1, 17: 1}, 12),         # second and third at exactly a tenth of the first: kept
+    ({2: 11, 9: 1, 17: 1}, 11),         # just below a tenth: dropped
+    ({4: 5, 11: 5, 20: 5, 25: 5}, 15),  # four equal bins: the earlier three win
+    ({2: 10, 9: 10, 17: 1, 25: 1}, 21),  # a tie for third at a tenth: the earlier bin wins
+]
+
+
+@pytest.mark.parametrize("search", ["bow", "proj", "init"])
+@pytest.mark.parametrize("bins,kept", ROT_HISTS)
+def test_rotation_three_maxima(pkg, oracle, search, bins, kept):
+    """The rotation culls of SearchByBoW, SearchByProjection and SearchForInitialization at ComputeThreeMaxima's edges: one
+    unambiguous match per pair (equal descriptors, one candidate), its rotation put in the bin asked for."""
+    rot = np.concatenate([np.full(c, 12.0 * b + 3.0) for b, c in bins.items()]).astype(np.float32)
+    n = len(rot)
+    rng = np.random.RandomState(n)
+    desc = rng.randint(0, 256, size=(n, 32)).astype(np.uint8)
+    zero = np.zeros(n, np.float32)
+    m = pkg.ORBmatcher(0.9, True)
+    if search == "bow":
+        node, valid = np.arange(n, dtype=np.int32), np.ones(n, np.uint8)
+        got = m.SearchByBoW(desc, node, valid, rot, desc, node, zero)
+        ref = oracle.search_by_bow(desc, node, valid, rot, desc, node, zero, nnratio=0.9, check_ori=True)
+    else:
+        x = (np.float32(40) + np.float32(40) * (np.arange(n) % 14)).astype(np.float32)
+        y = (np.float32(40) + np.float32(40) * (np.arange(n) // 14)).astype(np.float32)
+        octave = np.zeros(n, np.int32)
+        if search == "proj":
+            q = np.zeros(n, pkg.proj_query_dtype)
+            q["u"], q["v"], q["invz"], q["angle"], q["has_obs"], q["desc"] = x, y, np.float32(0.1), rot, 1, desc
+            args = (q, x, y, octave, zero, np.full(n, -1, np.float32), None, desc, _GEOM, np.float32(7))
+            got = m.SearchByProjection(*args)
+            ref = oracle.search_by_projection_last(*args[:-1], 7.0)
+        else:
+            prev = np.stack([x, y], 1)
+            args = (octave, rot, desc, x, y, octave, zero, desc, _GEOM)
+            got = m.SearchForInitialization(prev.copy(), *args, window=10)
+            ref = oracle.search_for_initialization(prev.copy(), *args, window=10, nnratio=0.9, check_ori=True)
+    assert got[0] == ref[0] == kept
+    assert np.array_equal(got[1], ref[1])
