@@ -1,6 +1,8 @@
 // common.cu — error text, device selection, buffers and stage handles, input checks, version for libb200slam.so
 #include <stdarg.h>
 
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace b2s {
@@ -60,6 +62,38 @@ int grow(HostBuf& b, size_t bytes) {
   b.bytes = 0;
   B2S_CUDA(cudaMallocHost(&b.p, bytes));
   b.bytes = bytes;
+  return B2S_OK;
+}
+
+void Packed::reserve(cudaError_t& error, bool pinned) {
+  reserved = true;
+  const size_t bytes = std::max<size_t>(used, 16);
+  if (error == cudaSuccess && (error = cudaMalloc(&d.p, bytes)) == cudaSuccess) d.bytes = bytes;
+  if (pinned && error == cudaSuccess && (error = cudaMallocHost(&h.p, bytes)) == cudaSuccess) h.bytes = bytes;
+}
+
+int Packed::fit(const char* fn) {
+  const size_t cap = std::min(h.bytes, d.bytes);
+  if (cap && used <= cap) return B2S_OK;
+  if (reserved) {
+    set_error("%s: a packed layout of %zu bytes exceeds the %zu bytes reserved at create", fn, used, cap);
+    return B2S_ERR_CAPACITY;
+  }
+  const size_t bytes = std::max(used, 2 * cap);
+  const int rc = grow(d, bytes);
+  return rc == B2S_OK ? grow(h, bytes) : rc;
+}
+
+int Packed::upload(cudaStream_t s) const {
+  B2S_CUDA(cudaMemcpyAsync(d.p, h.p, used, cudaMemcpyHostToDevice, s));
+  return B2S_OK;
+}
+
+int Packed::download(cudaStream_t s, size_t from, size_t to) const {
+  to = std::min(to, used);
+  if (to > from)
+    B2S_CUDA(cudaMemcpyAsync(static_cast<char*>(h.p) + from, static_cast<const char*>(d.p) + from, to - from,
+                             cudaMemcpyDeviceToHost, s));
   return B2S_OK;
 }
 

@@ -27,6 +27,8 @@ void set_error(const char* fmt, ...);
 
 int select_device(int device);  // returns B2S_OK / B2S_ERR_NO_DEVICE
 
+static inline size_t align_up(size_t a, size_t b) { return (a + b - 1) / b * b; }
+
 // Device buffer grown on demand, freed by its destructor.  grow() reallocates when `bytes` exceeds the capacity, without
 // keeping the contents (cudaFree synchronises the device); returns B2S_OK or a B2S_CUDA error.
 struct DevBuf {
@@ -54,6 +56,56 @@ struct HostBuf {
   }
 };
 int grow(HostBuf& b, size_t bytes);
+
+// n values of T at byte offset `off` of a Packed area.
+template <class T>
+struct Seg {
+  size_t off = 0, n = 0;
+  size_t end() const { return off + n * sizeof(T); }
+};
+
+// The arrays of a batched call, packed into one pinned host area and one device area at the same offsets: the host side
+// is filled or read, the device side goes into the kernels' arguments, and each direction is one copy.  Every array
+// starts at a 256-byte boundary, the start alignment of a cudaMalloc of its own.
+//   layout:  clear(), then add<T>(n) for each array in order; `used` is the bytes they span.
+//   sizing:  reserve() once at create, after a layout at the handle's capacities; a later layout that outgrows it is
+//            refused by fit() with B2S_ERR_CAPACITY.  Without reserve(), fit() grows both areas to max(used, 2 x their
+//            size), without keeping their contents: call sizes vary and cudaFree synchronises the device.
+//   moving:  upload() copies [0, used) to the device; download() copies a byte range of it back (by default all of it).
+struct Packed {
+  HostBuf h;
+  DevBuf d;
+  size_t used = 0;
+  bool reserved = false;
+
+  void clear() { used = 0; }
+  template <class T>
+  Seg<T> add(size_t n) {
+    const Seg<T> s{align_up(used, 256), n};
+    used = s.end();
+    return s;
+  }
+  template <class T>
+  T* host(Seg<T> s) const {
+    return reinterpret_cast<T*>(static_cast<char*>(h.p) + s.off);
+  }
+  template <class T>
+  T* dev(Seg<T> s) const {
+    return reinterpret_cast<T*>(static_cast<char*>(d.p) + s.off);
+  }
+  // Copies the segment's n values from src into the host area; returns the segment's device address.
+  template <class T>
+  T* stage(Seg<T> s, const T* src) {
+    if (s.n) memcpy(host(s), src, s.n * sizeof(T));
+    return dev(s);
+  }
+  // Allocates `used` bytes on the device and, when `pinned`, on the host (a device-only area holds scratch no copy
+  // touches).  Like Stage::alloc, it does nothing once `error` is set and records its own failure there.
+  void reserve(cudaError_t& error, bool pinned = true);
+  int fit(const char* fn);  // B2S_OK when both areas hold `used` bytes; `fn` names the entry point in the error
+  int upload(cudaStream_t s) const;
+  int download(cudaStream_t s, size_t from = 0, size_t to = SIZE_MAX) const;
+};
 
 // The host side every device stage's handle shares (the handle struct derives from it): its device, a non-blocking
 // stream, the two events around the timed segment of a call and that segment's device time, and the buffers allocated
@@ -97,7 +149,6 @@ bool entries_ok(const int32_t* off, const int32_t* v, int rows, int lo, int hi, 
 bool sets_ok(const int32_t* sets, int k, int width, int n, int* set, int* entry);
 
 static inline int div_up(int a, int b) { return (a + b - 1) / b; }
-static inline size_t align_up(size_t a, size_t b) { return (a + b - 1) / b * b; }
 
 // ---- device helpers ----
 __device__ __forceinline__ int warp_reduce_sum(int v) {

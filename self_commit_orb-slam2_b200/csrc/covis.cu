@@ -15,7 +15,6 @@
 #include <cub/cub.cuh>
 
 #include <algorithm>
-#include <vector>
 
 #include "common.cuh"
 
@@ -316,14 +315,43 @@ __global__ void __launch_bounds__(kReplayWarps * 32) k_covis_replay(Args a) {
 
 struct b2s_covis : b2s::Stage {
   int maxKf, maxMp, maxObs, maxSlots, maxConn, maxBatch;
-  int* dIn = nullptr;     // the packed problem
-  int* hIn = nullptr;     // its pinned staging copy
-  size_t inCap = 0;
-  int* dScr = nullptr;    // scratch and outputs, one allocation
-  int* hSmall = nullptr;  // pinned copy of the small outputs
-  size_t smallCap = 0;
-  Args a{};
-  std::vector<int> hArea[7];
+  Args a{};      // the scratch pointers; the rest are set per call
+  Packed scr;    // scratch only the device touches
+  Packed in;     // the problem
+  Packed out;    // the small outputs, downloaded first, then the output areas of maxConn entries each
+  Seg<int> mapOff, mapKf, mapW, listOff, listKf, listW, kfFlags, parentIn, mpBad, obsOff, obsKf, member, slotOff, slotMp;
+  Seg<int> flag, outOff, memOff, changed, parent, first, mapN, listN, startN, afterN, pair, area[7];
+  // n keyframes, B calls, M map and L list entries, nmp points with O observers, S slots
+  void lay(size_t n, size_t B, size_t M, size_t L, size_t nmp, size_t O, size_t S) {
+    in.clear();
+    mapOff = in.add<int>(n + 1);
+    mapKf = in.add<int>(M);
+    mapW = in.add<int>(M);
+    listOff = in.add<int>(n + 1);
+    listKf = in.add<int>(L);
+    listW = in.add<int>(L);
+    kfFlags = in.add<int>(n);
+    parentIn = in.add<int>(n);
+    mpBad = in.add<int>(nmp);
+    obsOff = in.add<int>(nmp + 1);
+    obsKf = in.add<int>(O);
+    member = in.add<int>(B);
+    slotOff = in.add<int>(B + 1);
+    slotMp = in.add<int>(S);
+    out.clear();
+    flag = out.add<int>(1);
+    outOff = out.add<int>(n + 1);
+    memOff = out.add<int>(B + 1);
+    changed = out.add<int>(n);
+    parent = out.add<int>(n);
+    first = out.add<int>(n);
+    mapN = out.add<int>(n);
+    listN = out.add<int>(n);
+    startN = out.add<int>(B);
+    afterN = out.add<int>(B);
+    pair = out.add<int>(B);
+    for (Seg<int>& g : area) g = out.add<int>(maxConn);
+  }
 };
 
 extern "C" int b2s_covis_create(int max_kf, int max_mp, int max_obs, int max_slots, int max_conn, int max_batch,
@@ -343,17 +371,18 @@ extern "C" int b2s_covis_create(int max_kf, int max_mp, int max_obs, int max_slo
   h->maxConn = max_conn;
   h->maxBatch = max_batch;
   const size_t K = max_kf, B = max_batch, C = max_conn, KB = K * B;
-  h->inCap = 2 * (K + 1) + 4 * C + 2 * K + 2 * (size_t)max_mp + 1 + max_obs + 2 * B + 1 + max_slots;
-  h->smallCap = 1 + (K + 1) + (B + 1) + 5 * K + 4 * B;
-  // hist, cnt kf/w, str kf/w, ev pos/k: 7 x KB; cntN, strN: 2B; evCnt, evStart, cur, bound: 4(K+1); small; 7 areas of C
-  const size_t scr = 7 * KB + 2 * B + 4 * (K + 1) + h->smallCap + 7 * C;
+  Packed& scr = h->scr;
+  const Seg<int> hist = scr.add<int>(KB), cntKf = scr.add<int>(KB), cntW = scr.add<int>(KB), strKf = scr.add<int>(KB),
+                 strW = scr.add<int>(KB), evPos = scr.add<int>(KB), evK = scr.add<int>(KB), cntN = scr.add<int>(B),
+                 strN = scr.add<int>(B), evCnt = scr.add<int>(K + 1), evStart = scr.add<int>(K + 1),
+                 cur = scr.add<int>(K + 1), bound = scr.add<int>(K + 1);
+  h->lay(K, B, C, C, max_mp, max_obs, max_slots);
   h->open(device);
-  h->alloc(h->dIn, h->inCap * 4);
-  h->alloc_pinned(h->hIn, h->inCap * 4);
-  h->alloc(h->dScr, scr * 4);
-  h->alloc_pinned(h->hSmall, h->smallCap * 4);
+  scr.reserve(h->error, false);
+  h->in.reserve(h->error);
+  h->out.reserve(h->error);
   cudaError_t e = h->error;
-  if (e == cudaSuccess) e = cudaMemset(h->dScr, 0, KB * 4);  // hist
+  if (e == cudaSuccess) e = cudaMemset(scr.dev(hist), 0, KB * 4);
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e != cudaSuccess) {
     set_error("b2s_covis_create: %s", cudaGetErrorString(e));
@@ -361,33 +390,19 @@ extern "C" int b2s_covis_create(int max_kf, int max_mp, int max_obs, int max_slo
     return B2S_ERR_CUDA;
   }
   Args& a = h->a;
-  int* p = h->dScr;
-  auto take = [&p](size_t n) {
-    int* q = p;
-    p += n;
-    return q;
-  };
-  a.hist = take(KB);
-  a.cntKf = take(KB);
-  a.cntW = take(KB);
-  a.strKf = take(KB);
-  a.strW = take(KB);
-  a.evPos = take(KB);
-  a.evK = take(KB);
-  a.cntN = take(B);
-  a.strN = take(B);
-  a.evCnt = take(K + 1);
-  a.evStart = take(K + 1);
-  a.cur = take(K + 1);
-  a.bound = take(K + 1);
-  a.flag = take(h->smallCap);  // the small outputs are laid out per call from here
-  a.oMapKf = take(C);
-  a.oMapW = take(C);
-  a.oListKf = take(C);
-  a.oListW = take(C);
-  a.oStartKf = take(C);
-  a.oAfterKf = take(C);
-  a.oAfterW = take(C);
+  a.hist = scr.dev(hist);
+  a.cntKf = scr.dev(cntKf);
+  a.cntW = scr.dev(cntW);
+  a.strKf = scr.dev(strKf);
+  a.strW = scr.dev(strW);
+  a.evPos = scr.dev(evPos);
+  a.evK = scr.dev(evK);
+  a.cntN = scr.dev(cntN);
+  a.strN = scr.dev(strN);
+  a.evCnt = scr.dev(evCnt);
+  a.evStart = scr.dev(evStart);
+  a.cur = scr.dev(cur);
+  a.bound = scr.dev(bound);
   a.maxConn = max_conn;
   *out = h;
   return B2S_OK;
@@ -448,82 +463,71 @@ extern "C" int b2s_update_connections(b2s_covis* h, const b2s_covis_problem* p, 
   cudaStream_t s = h->stream;
 
   // pack the problem: one upload
+  h->lay(n, B, M, L, nmp, O, S);
+  int rc = h->in.fit("b2s_update_connections");
+  if (rc == B2S_OK) rc = h->out.fit("b2s_update_connections");
+  if (rc != B2S_OK) return rc;
+  Packed &in = h->in, &out = h->out;
   Args a = h->a;
   a.n = n;
   a.B = B;
-  int* q = h->hIn;
-  size_t o = 0;
-  auto put = [&](const int32_t* src, size_t len) {
-    const int* d = h->dIn + o;
-    if (len) memcpy(q + o, src, len * 4);
-    o += len;
-    return d;
-  };
-  a.mapOff = put(p->map_off, n + 1);
-  a.mapKf = put(p->map_kf, M);
-  a.mapW = put(p->map_w, M);
-  a.listOff = put(p->list_off, n + 1);
-  a.listKf = put(p->list_kf, L);
-  a.listW = put(p->list_w, L);
-  a.kfFlags = h->dIn + o;
-  for (int i = 0; i < n; i++) q[o + i] = (p->first_connection[i] ? 1 : 0) | (p->kf_id[i] == 0 ? 2 : 0);
-  o += n;
-  a.parentIn = put(p->parent, n);
-  a.mpBad = h->dIn + o;
-  for (int i = 0; i < nmp; i++) q[o + i] = p->mp_bad[i] ? 1 : 0;
-  o += nmp;
-  a.obsOff = put(p->obs_off, nmp + 1);
-  a.obsKf = put(p->obs_kf, O);
-  a.member = put(p->member, B);
-  a.slotOff = put(p->slot_off, B + 1);
-  a.slotMp = put(p->slot_mp, S);
-  // the small outputs, downloaded in one copy
-  int* sm = a.flag;
-  size_t so = 1;
-  auto small = [&](size_t len) {
-    int* d = sm + so;
-    so += len;
-    return d;
-  };
-  a.outOff = small(n + 1);
-  a.memOff = small(B + 1);
-  a.changed = small(n);
-  a.parent = small(n);
-  a.first = small(n);
-  a.mapN = small(n);
-  a.listN = small(n);
-  a.startN = small(B);
-  a.afterN = small(B);
-  a.pair = small(B);
+  a.mapOff = in.stage(h->mapOff, p->map_off);
+  a.mapKf = in.stage(h->mapKf, p->map_kf);
+  a.mapW = in.stage(h->mapW, p->map_w);
+  a.listOff = in.stage(h->listOff, p->list_off);
+  a.listKf = in.stage(h->listKf, p->list_kf);
+  a.listW = in.stage(h->listW, p->list_w);
+  int* flags = in.host(h->kfFlags);
+  for (int i = 0; i < n; i++) flags[i] = (p->first_connection[i] ? 1 : 0) | (p->kf_id[i] == 0 ? 2 : 0);
+  a.kfFlags = in.dev(h->kfFlags);
+  a.parentIn = in.stage(h->parentIn, p->parent);
+  int* bad = in.host(h->mpBad);
+  for (int i = 0; i < nmp; i++) bad[i] = p->mp_bad[i] ? 1 : 0;
+  a.mpBad = in.dev(h->mpBad);
+  a.obsOff = in.stage(h->obsOff, p->obs_off);
+  a.obsKf = in.stage(h->obsKf, p->obs_kf);
+  a.member = in.stage(h->member, p->member);
+  a.slotOff = in.stage(h->slotOff, p->slot_off);
+  a.slotMp = in.stage(h->slotMp, p->slot_mp);
+  a.flag = out.dev(h->flag);
+  a.outOff = out.dev(h->outOff);
+  a.memOff = out.dev(h->memOff);
+  a.changed = out.dev(h->changed);
+  a.parent = out.dev(h->parent);
+  a.first = out.dev(h->first);
+  a.mapN = out.dev(h->mapN);
+  a.listN = out.dev(h->listN);
+  a.startN = out.dev(h->startN);
+  a.afterN = out.dev(h->afterN);
+  a.pair = out.dev(h->pair);
+  int** areas[7] = {&a.oMapKf, &a.oMapW, &a.oListKf, &a.oListW, &a.oStartKf, &a.oAfterKf, &a.oAfterW};
+  for (int i = 0; i < 7; i++) *areas[i] = out.dev(h->area[i]);
 
-  int rc = h->begin();
-  if (rc != B2S_OK) return rc;
-  B2S_CUDA(cudaMemcpyAsync(h->dIn, h->hIn, o * 4, cudaMemcpyHostToDevice, s));
+  if ((rc = h->begin()) != B2S_OK) return rc;
+  if ((rc = in.upload(s)) != B2S_OK) return rc;
   k_covis_count<<<B, kCountThreads, 0, s>>>(a);
   k_covis_group<<<1, kGroupThreads, 0, s>>>(a);
   k_covis_replay<<<div_up(n, kReplayWarps), kReplayWarps * 32, 0, s>>>(a);
   B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaMemcpyAsync(h->hSmall, sm, so * 4, cudaMemcpyDeviceToHost, s));
+  // the small outputs first: they size the areas
+  if ((rc = out.download(s, 0, h->pair.end())) != B2S_OK) return rc;
   B2S_CUDA(cudaStreamSynchronize(s));
-  const int* hs = h->hSmall;
-  auto at = [&](const int* d) { return hs + (d - sm); };
-  const int *outOff = at(a.outOff), *memOff = at(a.memOff);
-  if (hs[0]) {
+  const int *outOff = out.host(h->outOff), *memOff = out.host(h->memOff);
+  if (*out.host(h->flag)) {
     set_error("b2s_update_connections: the outputs need %d and %d entries, beyond the handle's max_conn %d",
               outOff[n], memOff[B], h->maxConn);
     return B2S_ERR_CAPACITY;
   }
   const int nOut = outOff[n], nMem = memOff[B];
-  int* areas[7] = {a.oMapKf, a.oMapW, a.oListKf, a.oListW, a.oStartKf, a.oAfterKf, a.oAfterW};
   for (int i = 0; i < 7; i++) {
-    const int len = i < 4 ? nOut : nMem;
-    h->hArea[i].resize((size_t)len);
-    if (len) B2S_CUDA(cudaMemcpyAsync(h->hArea[i].data(), areas[i], (size_t)len * 4, cudaMemcpyDeviceToHost, s));
+    const Seg<int>& g = h->area[i];
+    if ((rc = out.download(s, g.off, g.off + (size_t)(i < 4 ? nOut : nMem) * 4)) != B2S_OK) return rc;
   }
   if ((rc = h->finish()) != B2S_OK) return rc;
 
-  const int *changed = at(a.changed), *parent = at(a.parent), *first = at(a.first), *mapN = at(a.mapN),
-            *listN = at(a.listN), *startN = at(a.startN), *afterN = at(a.afterN), *pair = at(a.pair);
+  const int *changed = out.host(h->changed), *parent = out.host(h->parent), *first = out.host(h->first),
+            *mapN = out.host(h->mapN), *listN = out.host(h->listN), *startN = out.host(h->startN),
+            *afterN = out.host(h->afterN), *pair = out.host(h->pair);
   int64_t needMap = 0, needList = 0, needStart = 0, needAfter = 0;
   for (int t = 0; t < n; t++) {
     needMap += mapN[t];
@@ -549,7 +553,8 @@ extern "C" int b2s_update_connections(b2s_covis* h, const b2s_covis_problem* p, 
               (long long)needMap, (long long)needList, (long long)needStart, (long long)needAfter);
     return B2S_ERR_CAPACITY;
   }
-  const std::vector<int>* A = h->hArea;
+  const int* A[7];
+  for (int i = 0; i < 7; i++) A[i] = out.host(h->area[i]);
   int cm = 0, cl = 0;
   r->map_off[0] = r->list_off[0] = 0;
   for (int t = 0; t < n; t++) {
@@ -557,12 +562,12 @@ extern "C" int b2s_update_connections(b2s_covis* h, const b2s_covis_problem* p, 
     r->parent[t] = parent[t];
     r->first_connection[t] = (uint8_t)first[t];
     if (mapN[t]) {
-      memcpy(r->map_kf + cm, A[0].data() + outOff[t], (size_t)mapN[t] * 4);
-      memcpy(r->map_w + cm, A[1].data() + outOff[t], (size_t)mapN[t] * 4);
+      memcpy(r->map_kf + cm, A[0] + outOff[t], (size_t)mapN[t] * 4);
+      memcpy(r->map_w + cm, A[1] + outOff[t], (size_t)mapN[t] * 4);
     }
     if (listN[t]) {
-      memcpy(r->list_kf + cl, A[2].data() + outOff[t], (size_t)listN[t] * 4);
-      memcpy(r->list_w + cl, A[3].data() + outOff[t], (size_t)listN[t] * 4);
+      memcpy(r->list_kf + cl, A[2] + outOff[t], (size_t)listN[t] * 4);
+      memcpy(r->list_w + cl, A[3] + outOff[t], (size_t)listN[t] * 4);
     }
     cm += mapN[t];
     cl += listN[t];
@@ -572,10 +577,10 @@ extern "C" int b2s_update_connections(b2s_covis* h, const b2s_covis_problem* p, 
   int cs = 0, ca = 0, np = 0;
   r->start_off[0] = r->after_off[0] = 0;
   for (int b = 0; b < B; b++) {
-    if (startN[b]) memcpy(r->start_kf + cs, A[4].data() + memOff[b], (size_t)startN[b] * 4);
+    if (startN[b]) memcpy(r->start_kf + cs, A[4] + memOff[b], (size_t)startN[b] * 4);
     if (afterN[b]) {
-      memcpy(r->after_kf + ca, A[5].data() + memOff[b], (size_t)afterN[b] * 4);
-      memcpy(r->after_w + ca, A[6].data() + memOff[b], (size_t)afterN[b] * 4);
+      memcpy(r->after_kf + ca, A[5] + memOff[b], (size_t)afterN[b] * 4);
+      memcpy(r->after_w + ca, A[6] + memOff[b], (size_t)afterN[b] * 4);
     }
     cs += startN[b];
     ca += afterN[b];

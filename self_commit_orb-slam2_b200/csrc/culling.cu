@@ -181,8 +181,7 @@ __global__ void __launch_bounds__(kThreads) k_cull_walk(Args a) {
 
 struct b2s_culling : b2s::Stage {
   int maxKf, maxMp, maxObs, maxLocal, maxSlots, maxBatch;
-  DevBuf dIn, dOut;  // the packed problems; outputs and scratch
-  HostBuf hIn, hOut;
+  Packed in, out;  // the packed problems; outputs, then scratch
 };
 
 extern "C" int b2s_culling_create(int max_kf, int max_mp, int max_obs, int max_local, int max_slots, int max_batch,
@@ -315,98 +314,72 @@ extern "C" int b2s_keyframe_culling(b2s_culling* h, int batch, const b2s_culling
     set_error("b2s_keyframe_culling: the batch is too large for one call");
     return B2S_ERR_CAPACITY;
   }
-  const size_t B = batch, nDesc = B * sizeof(Desc) / 4;
-  const size_t inN = nDesc + L + 2 * K + 2 * M + (M + B) + 4 * O + L + (L + B) + 3 * S;
-  const size_t outN = 3 * L + 2 * M + O + S + B, scrN = 2 * L + K;
-  int rc = grow(h->dIn, inN * 4);
-  if (rc == B2S_OK) rc = grow(h->dOut, (outN + scrN) * 4);
-  if (rc == B2S_OK) rc = grow(h->hIn, inN * 4);
-  if (rc == B2S_OK) rc = grow(h->hOut, outN * 4);
+  Packed &in = h->in, &out = h->out;
+  in.clear();
+  const Seg<Desc> gDesc = in.add<Desc>(batch);
+  const Seg<int> gLocProb = in.add<int>(L), gFlags = in.add<int>(K);
+  const Seg<float> gTh = in.add<float>(K);
+  const Seg<int> gBad = in.add<int>(M), gNobs = in.add<int>(M), gObsOff = in.add<int>(M + batch),
+                 gObsKf = in.add<int>(O), gObsIdx = in.add<int>(O), gObsOct = in.add<int>(O), gObsSt = in.add<int>(O),
+                 gLocal = in.add<int>(L), gSlotOff = in.add<int>(L + batch), gSlotMp = in.add<int>(S),
+                 gSlotOct = in.add<int>(S);
+  const Seg<float> gDepth = in.add<float>(S);
+  out.clear();
+  const Seg<int> gVerdict = out.add<int>(L), gNM = out.add<int>(L), gNR = out.add<int>(L), gBadOut = out.add<int>(M),
+                 gNobsOut = out.add<int>(M), gAlive = out.add<int>(O), gSlot = out.add<int>(S),
+                 gCulled = out.add<int>(batch), gCntM = out.add<int>(L), gCntR = out.add<int>(L),
+                 gLocalPos = out.add<int>(K);
+  int rc = in.fit("b2s_keyframe_culling");
+  if (rc == B2S_OK) rc = out.fit("b2s_keyframe_culling");
   if (rc != B2S_OK) return rc;
 
   // pack: one upload
-  int* q = static_cast<int*>(h->hIn.p);
-  int* dIn = static_cast<int*>(h->dIn.p);
-  size_t o = 0;
-  auto take = [&](size_t n) {
-    const size_t at = o;
-    o += n;
-    return at;
-  };
-  Args a{};
-  memcpy(q, desc.data(), B * sizeof(Desc));
-  a.desc = reinterpret_cast<const Desc*>(dIn + take(nDesc));
-  const size_t oLocProb = take(L), oFlags = take(K), oTh = take(K), oBad = take(M), oNobs = take(M),
-               oObsOff = take(M + B), oObsKf = take(O), oObsIdx = take(O), oObsOct = take(O), oObsSt = take(O),
-               oLocal = take(L), oSlotOff = take(L + B), oSlotMp = take(S), oSlotOct = take(S), oDepth = take(S);
+  memcpy(in.host(gDesc), desc.data(), (size_t)batch * sizeof(Desc));
   for (int b = 0; b < batch; b++) {
     const b2s_culling_problem& pb = p[b];
     const Desc& d = desc[(size_t)b];
     const int nO = pb.obs_off[pb.n_mp], nS = pb.slot_off[pb.n_local];
-    for (int l = 0; l < d.nloc; l++) q[oLocProb + d.loc + l] = b;
-    for (int k = 0; k < d.nkf; k++) q[oFlags + d.kf + k] = (pb.kf_id[k] == 0 ? 1 : 0) | (pb.not_erase[k] ? 2 : 0);
-    if (d.nkf) memcpy(q + oTh + d.kf, pb.th_depth, (size_t)d.nkf * 4);
-    for (int m = 0; m < d.nmp; m++) q[oBad + d.mp + m] = pb.mp_bad[m] ? 1 : 0;
-    if (d.nmp) memcpy(q + oNobs + d.mp, pb.mp_nobs, (size_t)d.nmp * 4);
-    memcpy(q + oObsOff + d.obsOff, pb.obs_off, (size_t)(d.nmp + 1) * 4);
+    for (int l = 0; l < d.nloc; l++) in.host(gLocProb)[d.loc + l] = b;
+    for (int k = 0; k < d.nkf; k++) in.host(gFlags)[d.kf + k] = (pb.kf_id[k] == 0 ? 1 : 0) | (pb.not_erase[k] ? 2 : 0);
+    if (d.nkf) memcpy(in.host(gTh) + d.kf, pb.th_depth, (size_t)d.nkf * 4);
+    for (int m = 0; m < d.nmp; m++) in.host(gBad)[d.mp + m] = pb.mp_bad[m] ? 1 : 0;
+    if (d.nmp) memcpy(in.host(gNobs) + d.mp, pb.mp_nobs, (size_t)d.nmp * 4);
+    memcpy(in.host(gObsOff) + d.obsOff, pb.obs_off, (size_t)(d.nmp + 1) * 4);
     if (nO) {
-      memcpy(q + oObsKf + d.obs, pb.obs_kf, (size_t)nO * 4);
-      memcpy(q + oObsIdx + d.obs, pb.obs_idx, (size_t)nO * 4);
-      memcpy(q + oObsOct + d.obs, pb.obs_octave, (size_t)nO * 4);
-      for (int i = 0; i < nO; i++) q[oObsSt + d.obs + i] = pb.obs_stereo[i] ? 1 : 0;
+      memcpy(in.host(gObsKf) + d.obs, pb.obs_kf, (size_t)nO * 4);
+      memcpy(in.host(gObsIdx) + d.obs, pb.obs_idx, (size_t)nO * 4);
+      memcpy(in.host(gObsOct) + d.obs, pb.obs_octave, (size_t)nO * 4);
+      for (int i = 0; i < nO; i++) in.host(gObsSt)[d.obs + i] = pb.obs_stereo[i] ? 1 : 0;
     }
-    if (d.nloc) memcpy(q + oLocal + d.loc, pb.local_kf, (size_t)d.nloc * 4);
-    memcpy(q + oSlotOff + d.slotOff, pb.slot_off, (size_t)(d.nloc + 1) * 4);
+    if (d.nloc) memcpy(in.host(gLocal) + d.loc, pb.local_kf, (size_t)d.nloc * 4);
+    memcpy(in.host(gSlotOff) + d.slotOff, pb.slot_off, (size_t)(d.nloc + 1) * 4);
     if (nS) {
-      memcpy(q + oSlotMp + d.slot, pb.slot_mp, (size_t)nS * 4);
-      memcpy(q + oSlotOct + d.slot, pb.slot_octave, (size_t)nS * 4);
+      memcpy(in.host(gSlotMp) + d.slot, pb.slot_mp, (size_t)nS * 4);
+      memcpy(in.host(gSlotOct) + d.slot, pb.slot_octave, (size_t)nS * 4);
       if (pb.slot_depth)
-        memcpy(q + oDepth + d.slot, pb.slot_depth, (size_t)nS * 4);
+        memcpy(in.host(gDepth) + d.slot, pb.slot_depth, (size_t)nS * 4);
       else
-        memset(q + oDepth + d.slot, 0, (size_t)nS * 4);
+        memset(in.host(gDepth) + d.slot, 0, (size_t)nS * 4);
     }
   }
-  a.locProb = dIn + oLocProb;
-  a.kfFlags = dIn + oFlags;
-  a.thDepth = reinterpret_cast<const float*>(dIn + oTh);
-  a.mpBad = dIn + oBad;
-  a.mpNobs = dIn + oNobs;
-  a.obsOff = dIn + oObsOff;
-  a.obsKf = dIn + oObsKf;
-  a.obsIdx = dIn + oObsIdx;
-  a.obsOct = dIn + oObsOct;
-  a.obsStereo = dIn + oObsSt;
-  a.localKf = dIn + oLocal;
-  a.slotOff = dIn + oSlotOff;
-  a.slotMp = dIn + oSlotMp;
-  a.slotOct = dIn + oSlotOct;
-  a.slotDepth = reinterpret_cast<const float*>(dIn + oDepth);
-  int* dOut = static_cast<int*>(h->dOut.p);
-  o = 0;
-  a.verdict = dOut + take(L);
-  a.nM = dOut + take(L);
-  a.nR = dOut + take(L);
-  a.bad = dOut + take(M);
-  a.nobs = dOut + take(M);
-  a.alive = dOut + take(O);
-  a.slot = dOut + take(S);
-  a.nCulled = dOut + take(B);
-  a.cntM = dOut + take(L);
-  a.cntR = dOut + take(L);
-  a.localPos = dOut + take(K);
+  const Args a = {in.dev(gDesc),    in.dev(gLocProb),  in.dev(gFlags),   in.dev(gTh),      in.dev(gBad),
+                  in.dev(gNobs),    in.dev(gObsOff),   in.dev(gObsKf),   in.dev(gObsIdx),  in.dev(gObsOct),
+                  in.dev(gObsSt),   in.dev(gLocal),    in.dev(gSlotOff), in.dev(gSlotMp),  in.dev(gSlotOct),
+                  in.dev(gDepth),   out.dev(gCntM),    out.dev(gCntR),   out.dev(gLocalPos), out.dev(gVerdict),
+                  out.dev(gNM),     out.dev(gNR),      out.dev(gBadOut), out.dev(gNobsOut), out.dev(gAlive),
+                  out.dev(gSlot),   out.dev(gCulled)};
 
   if ((rc = h->begin()) != B2S_OK) return rc;
-  B2S_CUDA(cudaMemcpyAsync(dIn, q, inN * 4, cudaMemcpyHostToDevice, s));
+  if ((rc = in.upload(s)) != B2S_OK) return rc;
   if (L) k_cull_count<<<(unsigned)L, kThreads, 0, s>>>(a);
   k_cull_walk<<<batch, kThreads, 0, s>>>(a);
   B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaMemcpyAsync(h->hOut.p, dOut, outN * 4, cudaMemcpyDeviceToHost, s));
+  if ((rc = out.download(s, 0, gCulled.end())) != B2S_OK) return rc;  // not the scratch
   if ((rc = h->finish()) != B2S_OK) return rc;
 
-  const int* ho = static_cast<const int*>(h->hOut.p);
-  auto at = [&](const int* d) { return ho + (d - dOut); };
-  const int *verdict = at(a.verdict), *nM = at(a.nM), *nR = at(a.nR), *bad = at(a.bad), *nobs = at(a.nobs),
-            *alive = at(a.alive), *slot = at(a.slot), *nCulled = at(a.nCulled);
+  const int *verdict = out.host(gVerdict), *nM = out.host(gNM), *nR = out.host(gNR), *bad = out.host(gBadOut),
+            *nobs = out.host(gNobsOut), *alive = out.host(gAlive), *slot = out.host(gSlot),
+            *nCulled = out.host(gCulled);
   for (int b = 0; b < batch; b++) {
     const Desc& d = desc[(size_t)b];
     b2s_culling_result& rb = r[b];

@@ -601,18 +601,31 @@ using namespace b2s::ini;
 // ================================================================================================ host side
 struct b2s_init_solver : b2s::Stage {
   int maxKeys, maxIters, maxBatch;
-  Prob* prob = nullptr;
-  float *kp1 = nullptr, *kp2 = nullptr, *pn1 = nullptr, *pn2 = nullptr, *hyp = nullptr, *score = nullptr;
-  int *m12 = nullptr, *sets = nullptr, *mt = nullptr;
+  float *pn1 = nullptr, *pn2 = nullptr, *hyp = nullptr, *score = nullptr, *p3dh = nullptr;
+  int* mt = nullptr;
   uint32_t* inl = nullptr;
-  St* st = nullptr;
-  float *p3dh = nullptr, *p3d = nullptr;
-  uint8_t *goodh = nullptr, *tri = nullptr, *inlH = nullptr, *inlF = nullptr;
-  std::vector<Prob> hProb;
-  std::vector<float> hKp1, hKp2, hP3d;
-  std::vector<int> hM12, hSets;
-  std::vector<St> hSt;
-  std::vector<uint8_t> hTri, hInlH, hInlF;
+  uint8_t* goodh = nullptr;
+  // a call's inputs and outputs, laid out by lay() for its problems, keypoints of each frame and iterations
+  Packed in, out;
+  Seg<Prob> prob;
+  Seg<float> kp1, kp2, p3d;
+  Seg<int> m12, sets;
+  Seg<St> st;
+  Seg<uint8_t> tri, inlH, inlF;
+  void lay(size_t batch, size_t n1, size_t n2, size_t iters) {
+    in.clear();
+    prob = in.add<Prob>(batch);
+    kp1 = in.add<float>(n1 * 2);
+    kp2 = in.add<float>(n2 * 2);
+    m12 = in.add<int>(n1);
+    sets = in.add<int>(iters * 8);
+    out.clear();
+    st = out.add<St>(batch);
+    p3d = out.add<float>(n1 * 3);
+    tri = out.add<uint8_t>(n1);
+    inlH = out.add<uint8_t>(n1);
+    inlF = out.add<uint8_t>(n1);
+  }
 };
 
 extern "C" int b2s_init_create(int max_keys, int max_iterations, int max_batch, int device, b2s_init_solver** out) {
@@ -630,24 +643,17 @@ extern "C" int b2s_init_create(int max_keys, int max_iterations, int max_batch, 
   const size_t B = max_batch, NK = (size_t)max_keys * B, IT = (size_t)max_iterations * B;
   const size_t W = (size_t)((max_keys + 31) / 32) * 2 * IT;
   h->open(device);
-  h->alloc(h->prob, B * sizeof(Prob));
-  h->alloc(h->kp1, NK * 2 * sizeof(float));
-  h->alloc(h->kp2, NK * 2 * sizeof(float));
+  h->lay(B, NK, NK, IT);
+  h->in.reserve(h->error);
+  h->out.reserve(h->error);
   h->alloc(h->pn1, NK * 2 * sizeof(float));
   h->alloc(h->pn2, NK * 2 * sizeof(float));
-  h->alloc(h->m12, NK * sizeof(int));
   h->alloc(h->mt, NK * 2 * sizeof(int));
-  h->alloc(h->sets, IT * 8 * sizeof(int));
   h->alloc(h->hyp, IT * 2 * 18 * sizeof(float));
   h->alloc(h->score, IT * 2 * sizeof(float));
   h->alloc(h->inl, W * sizeof(uint32_t));
-  h->alloc(h->st, B * sizeof(St));
   h->alloc(h->p3dh, NK * 8 * 3 * sizeof(float));
   h->alloc(h->goodh, NK * 8);
-  h->alloc(h->p3d, NK * 3 * sizeof(float));
-  h->alloc(h->tri, NK);
-  h->alloc(h->inlH, NK);
-  h->alloc(h->inlF, NK);
   cudaError_t e = h->error;
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(k_init_checkrt, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_KEYS * sizeof(float));
@@ -678,6 +684,7 @@ extern "C" int b2s_initialize(b2s_init_solver* h, int batch, const b2s_init_prob
     return B2S_ERR_CAPACITY;
   }
   std::vector<int> nm((size_t)batch);
+  size_t o1 = 0, o2 = 0, oit = 0, oinl = 0;  // keypoints of each frame, iterations and inlier words of the batch
   for (int i = 0; i < batch; i++) {
     const b2s_init_problem& q = p[i];
     if (q.n1 > h->maxKeys || q.n2 > h->maxKeys || q.iterations > h->maxIters) {
@@ -708,16 +715,26 @@ extern "C" int b2s_initialize(b2s_init_solver* h, int batch, const b2s_init_prob
       return B2S_ERR_BAD_ARG;
     }
     nm[(size_t)i] = n;
+    o1 += (size_t)q.n1;
+    o2 += (size_t)q.n2;
+    oit += (size_t)q.iterations;
   }
   B2S_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
 
-  h->hProb.resize((size_t)batch);
-  size_t o1 = 0, o2 = 0, oit = 0, oinl = 0;
+  h->lay((size_t)batch, o1, o2, oit);
+  int rc = h->in.fit("b2s_initialize");
+  if (rc == B2S_OK) rc = h->out.fit("b2s_initialize");
+  if (rc != B2S_OK) return rc;
+  Packed &in = h->in, &out = h->out;
+  Prob* prob = in.host(h->prob);
+  float *kp1 = in.host(h->kp1), *kp2 = in.host(h->kp2);
+  int *m12 = in.host(h->m12), *sets = in.host(h->sets);
+  o1 = o2 = oit = 0;
   int maxIt = 0, maxNm = 0;
   for (int i = 0; i < batch; i++) {
     const b2s_init_problem& q = p[i];
-    Prob& P = h->hProb[(size_t)i];
+    Prob& P = prob[i];
     P.n1 = q.n1;
     P.n2 = q.n2;
     P.off1 = (int)o1;
@@ -728,6 +745,10 @@ extern "C" int b2s_initialize(b2s_init_solver* h, int batch, const b2s_init_prob
     P.offInl = (int)oinl;
     memcpy(P.K, q.K, sizeof(P.K));
     P.sigma = q.sigma;
+    memcpy(kp1 + 2 * o1, q.kp1, 2 * sizeof(float) * q.n1);
+    memcpy(kp2 + 2 * o2, q.kp2, 2 * sizeof(float) * q.n2);
+    memcpy(m12 + o1, q.matches12, sizeof(int) * q.n1);
+    memcpy(sets + 8 * oit, q.sets, 8 * sizeof(int) * q.iterations);
     o1 += (size_t)q.n1;
     o2 += (size_t)q.n2;
     oit += (size_t)q.iterations;
@@ -735,33 +756,12 @@ extern "C" int b2s_initialize(b2s_init_solver* h, int batch, const b2s_init_prob
     maxIt = std::max(maxIt, q.iterations);
     maxNm = std::max(maxNm, nm[(size_t)i]);
   }
-  h->hKp1.resize(o1 * 2);
-  h->hKp2.resize(o2 * 2);
-  h->hM12.resize(o1);
-  h->hSets.resize(oit * 8);
-  for (int i = 0; i < batch; i++) {
-    const b2s_init_problem& q = p[i];
-    const Prob& P = h->hProb[(size_t)i];
-    memcpy(&h->hKp1[2 * (size_t)P.off1], q.kp1, 2 * sizeof(float) * q.n1);
-    memcpy(&h->hKp2[2 * (size_t)P.off2], q.kp2, 2 * sizeof(float) * q.n2);
-    memcpy(&h->hM12[(size_t)P.off1], q.matches12, sizeof(int) * q.n1);
-    memcpy(&h->hSets[8 * (size_t)P.offIt], q.sets, 8 * sizeof(int) * q.iterations);
-  }
-  h->hSt.resize((size_t)batch);
-  h->hP3d.resize(o1 * 3);
-  h->hTri.resize(o1);
-  h->hInlH.resize(o1);
-  h->hInlF.resize(o1);
 
-  int rc = h->begin();
-  if (rc != B2S_OK) return rc;
-  B2S_CUDA(cudaMemcpyAsync(h->prob, h->hProb.data(), (size_t)batch * sizeof(Prob), cudaMemcpyHostToDevice, s));
-  B2S_CUDA(cudaMemcpyAsync(h->kp1, h->hKp1.data(), o1 * 2 * sizeof(float), cudaMemcpyHostToDevice, s));
-  B2S_CUDA(cudaMemcpyAsync(h->kp2, h->hKp2.data(), o2 * 2 * sizeof(float), cudaMemcpyHostToDevice, s));
-  B2S_CUDA(cudaMemcpyAsync(h->m12, h->hM12.data(), o1 * sizeof(int), cudaMemcpyHostToDevice, s));
-  B2S_CUDA(cudaMemcpyAsync(h->sets, h->hSets.data(), oit * 8 * sizeof(int), cudaMemcpyHostToDevice, s));
-  Ptrs a = {h->prob, h->kp1, h->kp2, h->m12, h->sets, h->pn1, h->pn2, h->mt, h->hyp, h->score, h->inl, h->st,
-            h->p3dh, h->goodh, h->p3d, h->tri, h->inlH, h->inlF};
+  if ((rc = h->begin()) != B2S_OK) return rc;
+  if ((rc = in.upload(s)) != B2S_OK) return rc;
+  Ptrs a = {in.dev(h->prob), in.dev(h->kp1),  in.dev(h->kp2),   in.dev(h->m12),   in.dev(h->sets),  h->pn1,
+            h->pn2,          h->mt,           h->hyp,           h->score,         h->inl,           out.dev(h->st),
+            h->p3dh,         h->goodh,        out.dev(h->p3d),  out.dev(h->tri),  out.dev(h->inlH), out.dev(h->inlF)};
   k_init_prepare<<<batch, CT, 0, s>>>(a);
   k_init_hypothesis<<<dim3((2 * maxIt + 63) / 64, batch), 64, 0, s>>>(a);
   k_init_score<<<dim3(2 * maxIt, batch), CT, 0, s>>>(a);
@@ -771,16 +771,15 @@ extern "C" int b2s_initialize(b2s_init_solver* h, int batch, const b2s_init_prob
   k_init_checkrt<<<dim3(8, batch), CT, (size_t)L * sizeof(float), s>>>(a);
   k_init_decide<<<batch, CT, 0, s>>>(a);
   B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaMemcpyAsync(h->hSt.data(), h->st, (size_t)batch * sizeof(St), cudaMemcpyDeviceToHost, s));
-  B2S_CUDA(cudaMemcpyAsync(h->hP3d.data(), h->p3d, o1 * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
-  B2S_CUDA(cudaMemcpyAsync(h->hTri.data(), h->tri, o1, cudaMemcpyDeviceToHost, s));
-  B2S_CUDA(cudaMemcpyAsync(h->hInlH.data(), h->inlH, o1, cudaMemcpyDeviceToHost, s));
-  B2S_CUDA(cudaMemcpyAsync(h->hInlF.data(), h->inlF, o1, cudaMemcpyDeviceToHost, s));
+  if ((rc = out.download(s)) != B2S_OK) return rc;
   if ((rc = h->finish()) != B2S_OK) return rc;
 
+  const St* st = out.host(h->st);
+  const float* p3d = out.host(h->p3d);
+  const uint8_t *tri = out.host(h->tri), *inlH = out.host(h->inlH), *inlF = out.host(h->inlF);
   for (int i = 0; i < batch; i++) {
-    const St& S = h->hSt[(size_t)i];
-    const Prob& P = h->hProb[(size_t)i];
+    const St& S = st[i];
+    const Prob& P = prob[i];
     b2s_init_result& R = r[i];
     R.ret = S.ret;
     R.model = S.model;
@@ -788,11 +787,11 @@ extern "C" int b2s_initialize(b2s_init_solver* h, int batch, const b2s_init_prob
     if (S.ret) {
       memcpy(R.R21, S.R[S.chosen], sizeof(R.R21));
       memcpy(R.t21, S.t[S.chosen], sizeof(R.t21));
-      memcpy(R.p3d, &h->hP3d[3 * (size_t)P.off1], 3 * sizeof(float) * P.n1);
-      memcpy(R.triangulated, &h->hTri[(size_t)P.off1], (size_t)P.n1);
+      memcpy(R.p3d, p3d + 3 * (size_t)P.off1, 3 * sizeof(float) * P.n1);
+      memcpy(R.triangulated, tri + P.off1, (size_t)P.n1);
     }
-    if (R.inliers_h) memcpy(R.inliers_h, &h->hInlH[(size_t)P.off1], (size_t)S.nm);
-    if (R.inliers_f) memcpy(R.inliers_f, &h->hInlF[(size_t)P.off1], (size_t)S.nm);
+    if (R.inliers_h) memcpy(R.inliers_h, inlH + P.off1, (size_t)S.nm);
+    if (R.inliers_f) memcpy(R.inliers_f, inlF + P.off1, (size_t)S.nm);
     R.n_matches = S.nm;
     R.best_h_iter = S.bestH;
     R.best_f_iter = S.bestF;

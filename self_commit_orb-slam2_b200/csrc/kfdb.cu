@@ -319,8 +319,6 @@ __global__ void k_kfdb_move(const uint32_t* __restrict__ ow, const double* __res
   }
 }
 
-size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
-
 }  // namespace
 }  // namespace b2s
 
@@ -343,8 +341,7 @@ struct b2s_kfdb : b2s::Stage {
   DevBuf d_live, d_rec, d_order, d_best, d_acc, d_out;
   HostBuf h_out;
   // one upload per query: query words + values, connected ids, covisibility table
-  HostBuf h_stage;
-  DevBuf d_stage;
+  Packed q;
 };
 
 namespace {
@@ -464,39 +461,32 @@ int query(b2s_kfdb* db, int loop, uint64_t qid, const uint32_t* words, const dou
     db->live_dirty = false;
   }
   const int n_rows = covis ? covis->n_rows : 0;
-  const size_t o_qv = 0, o_qw = align16(o_qv + (size_t)n * 8), o_conn = align16(o_qw + (size_t)n * 4),
-               o_cid = align16(o_conn + (size_t)n_conn * 8), o_cn = align16(o_cid + (size_t)n_rows * 10 * 8),
-               total = align16(o_cn + (size_t)n_rows * 4);
-  if (db->h_stage.bytes < total) rc = grow(db->h_stage, std::max(total, 2 * db->h_stage.bytes));
-  if (rc == B2S_OK && db->d_stage.bytes < total) rc = grow(db->d_stage, std::max(total, 2 * db->d_stage.bytes));
-  if (rc != B2S_OK) return rc;
-  unsigned char* h = (unsigned char*)db->h_stage.p;
-  memcpy(h + o_qv, values, (size_t)n * 8);
-  memcpy(h + o_qw, words, (size_t)n * 4);
-  if (n_conn) {
-    uint64_t* c = reinterpret_cast<uint64_t*>(h + o_conn);
-    memcpy(c, conn, (size_t)n_conn * 8);
-    std::sort(c, c + n_conn);
-  }
-  if (n_rows) {
-    memcpy(h + o_cid, covis->ids, (size_t)n_rows * 10 * 8);
-    memcpy(h + o_cn, covis->n, (size_t)n_rows * 4);
-  }
-  unsigned char* d = (unsigned char*)db->d_stage.p;
-  B2S_CUDA(cudaMemcpyAsync(d, h, total, cudaMemcpyHostToDevice, db->stream));
+  Packed& q = db->q;
+  q.clear();
+  const Seg<double> qv = q.add<double>(n);
+  const Seg<uint32_t> qw = q.add<uint32_t>(n);
+  const Seg<uint64_t> qc = q.add<uint64_t>(n_conn), cid = q.add<uint64_t>((size_t)n_rows * 10);
+  const Seg<int32_t> cn = q.add<int32_t>(n_rows);
+  if ((rc = q.fit(fn)) != B2S_OK) return rc;
+  q.stage(qv, values);
+  q.stage(qw, words);
+  q.stage(qc, conn);
+  std::sort(q.host(qc), q.host(qc) + n_conn);
+  q.stage(cid, n_rows ? covis->ids : nullptr);
+  q.stage(cn, n_rows ? covis->n : nullptr);
+  if ((rc = q.upload(db->stream)) != B2S_OK) return rc;
   const LiveRec* live = (const LiveRec*)db->d_live.p;
   SlotRec* rec = (SlotRec*)db->d_rec.p;
   b2s_kfdb_state* state = (b2s_kfdb_state*)db->d_state.p;
   if ((rc = db->begin()) != B2S_OK) return rc;
   k_kfdb_match<<<div_up(n_live, kMatchWarps), kMatchWarps * 32, (size_t)n * 12, db->stream>>>(
-      (const uint32_t*)db->d_pw.p, (const double*)db->d_pv.p, live, n_live, reinterpret_cast<const uint32_t*>(d + o_qw),
-      reinterpret_cast<const double*>(d + o_qv), n, reinterpret_cast<const uint64_t*>(d + o_conn), n_conn, loop,
-      (unsigned long long)qid, state, rec);
+      (const uint32_t*)db->d_pw.p, (const double*)db->d_pv.p, live, n_live, q.dev(qw), q.dev(qv), n, q.dev(qc), n_conn,
+      loop, (unsigned long long)qid, state, rec);
   B2S_CUDA(cudaGetLastError());
-  k_kfdb_finish<<<1, kFinThreads, 0, db->stream>>>(
-      live, n_live, rec, n, loop, (unsigned long long)qid, min_score, reinterpret_cast<const uint64_t*>(d + o_cid),
-      reinterpret_cast<const int32_t*>(d + o_cn), n_rows, state, db->state_cap, (int32_t*)db->d_order.p,
-      (float*)db->d_acc.p, (int32_t*)db->d_best.p, (int32_t*)db->d_first_pos.p, (int32_t*)db->d_out.p);
+  k_kfdb_finish<<<1, kFinThreads, 0, db->stream>>>(live, n_live, rec, n, loop, (unsigned long long)qid, min_score,
+                                                   q.dev(cid), q.dev(cn), n_rows, state, db->state_cap,
+                                                   (int32_t*)db->d_order.p, (float*)db->d_acc.p, (int32_t*)db->d_best.p,
+                                                   (int32_t*)db->d_first_pos.p, (int32_t*)db->d_out.p);
   B2S_CUDA(cudaGetLastError());
   B2S_CUDA(cudaEventRecord(db->ev[1], db->stream));  // the kernels only: the download is not timed
   const int n_dl = 1 + std::min(cap, n_live);

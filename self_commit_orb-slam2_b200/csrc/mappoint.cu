@@ -354,7 +354,7 @@ int check_kfinsert(int b, const b2s_kfinsert_problem& p, const b2s_kfinsert_resu
   return B2S_OK;
 }
 
-// Sizes of one packing: ints (and floats) of the input area, of the output area, of the scratch
+// Extents of a batch: keyframes, points, observations, slots, recent entries, scale levels, problems
 struct Sizes {
   size_t K = 0, M = 0, O = 0, S = 0, R = 0, F = 0, B = 0;
 };
@@ -390,72 +390,58 @@ extern "C" int b2s_update_normal_and_depth(b2s_matcher* h, const b2s_normal_dept
   B2S_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = h->stream;
 
-  const size_t nDesc = (sizeof(Desc) + 3) / 4;
-  const size_t inN = nDesc + 3 * (size_t)nK + 3 * (size_t)nM + 2 * (size_t)nM + (nM + 1) + 2 * (size_t)O + p->n_levels;
-  const size_t outN = (size_t)nM * 6;
-  int rc = grow(h->dMpIn, inN * 4);
-  if (rc == B2S_OK) rc = grow(h->dMpOut, outN * 4);
-  if (rc == B2S_OK) rc = grow(h->hMpIn, inN * 4);
-  if (rc == B2S_OK) rc = grow(h->hMpOut, outN * 4);
+  Packed &in = h->mpIn, &out = h->mpOut;
+  in.clear();
+  const Seg<Desc> gDesc = in.add<Desc>(1);
+  const Seg<float> gC = in.add<float>(3 * (size_t)nK), gP = in.add<float>(3 * (size_t)nM);
+  const Seg<int> gBad = in.add<int>(nM), gRef = in.add<int>(nM), gOff = in.add<int>(nM + 1), gKf = in.add<int>(O),
+                 gOct = in.add<int>(O);
+  const Seg<float> gSf = in.add<float>(p->n_levels);
+  out.clear();
+  const Seg<float> gNormal = out.add<float>(3 * (size_t)nM), gMinD = out.add<float>(nM), gMaxD = out.add<float>(nM);
+  const Seg<int> gUpdated = out.add<int>(nM);
+  int rc = in.fit(fn);
+  if (rc == B2S_OK) rc = out.fit(fn);
   if (rc != B2S_OK) return rc;
-  int* q = static_cast<int*>(h->hMpIn.p);
-  int* dIn = static_cast<int*>(h->dMpIn.p);
-  size_t o = 0;
-  auto take = [&](size_t n) {
-    const size_t at = o;
-    o += n;
-    return at;
-  };
-  Desc d{};
-  d.nkf = nK;
-  d.nmp = nM;
-  d.nlev = p->n_levels;
-  d.cur = -1;
-  memcpy(q, &d, sizeof(Desc));
+  Desc* d = in.host(gDesc);
+  *d = Desc{};
+  d->nkf = nK;
+  d->nmp = nM;
+  d->nlev = p->n_levels;
+  d->cur = -1;
   Args a{};
-  a.desc = reinterpret_cast<const Desc*>(dIn + take(nDesc));
-  const size_t oC = take(3 * (size_t)nK), oP = take(3 * (size_t)nM), oBad = take(nM), oRef = take(nM),
-               oOff = take(nM + 1), oKf = take(O), oOct = take(O), oSf = take(p->n_levels);
-  if (nK) memcpy(q + oC, p->kf_center, 12 * (size_t)nK);
-  memcpy(q + oP, p->mp_pos, 12 * (size_t)nM);
-  for (int m = 0; m < nM; m++) q[oBad + m] = p->mp_bad[m] ? 1 : 0;
-  memcpy(q + oRef, p->mp_ref, 4 * (size_t)nM);
-  memcpy(q + oOff, p->obs_off, 4 * (size_t)(nM + 1));
-  if (O) {
-    memcpy(q + oKf, p->obs_kf, 4 * (size_t)O);
-    memcpy(q + oOct, p->obs_octave, 4 * (size_t)O);
-  }
-  memcpy(q + oSf, p->scale_factors, 4 * (size_t)p->n_levels);
-  a.kfC = reinterpret_cast<const float*>(dIn + oC);
-  a.mpPos = reinterpret_cast<const float*>(dIn + oP);
-  a.mpBad = dIn + oBad;
-  a.mpRef = dIn + oRef;
-  a.obsOff = dIn + oOff;
-  a.obsKf = dIn + oKf;
-  a.obsOct = dIn + oOct;
-  a.sf = reinterpret_cast<const float*>(dIn + oSf);
-  int* dOut = static_cast<int*>(h->dMpOut.p);
-  a.normal = reinterpret_cast<float*>(dOut);
-  a.minD = reinterpret_cast<float*>(dOut + 3 * (size_t)nM);
-  a.maxD = reinterpret_cast<float*>(dOut + 4 * (size_t)nM);
-  a.updated = dOut + 5 * (size_t)nM;
+  a.desc = in.dev(gDesc);
+  a.kfC = in.stage(gC, p->kf_center);
+  a.mpPos = in.stage(gP, p->mp_pos);
+  int* bad = in.host(gBad);
+  for (int m = 0; m < nM; m++) bad[m] = p->mp_bad[m] ? 1 : 0;
+  a.mpBad = in.dev(gBad);
+  a.mpRef = in.stage(gRef, p->mp_ref);
+  a.obsOff = in.stage(gOff, p->obs_off);
+  a.obsKf = in.stage(gKf, p->obs_kf);
+  a.obsOct = in.stage(gOct, p->obs_octave);
+  a.sf = in.stage(gSf, p->scale_factors);
+  a.normal = out.dev(gNormal);
+  a.minD = out.dev(gMinD);
+  a.maxD = out.dev(gMaxD);
+  a.updated = out.dev(gUpdated);
 
   if ((rc = h->begin()) != B2S_OK) return rc;
-  B2S_CUDA(cudaMemcpyAsync(dIn, q, inN * 4, cudaMemcpyHostToDevice, st));
+  if ((rc = in.upload(st)) != B2S_OK) return rc;
   k_mp_point<false><<<div_up(nM, kWarps), kThreads, 0, st>>>(a, nM);
   h->launches++;
   B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaMemcpyAsync(h->hMpOut.p, dOut, outN * 4, cudaMemcpyDeviceToHost, st));
+  if ((rc = out.download(st)) != B2S_OK) return rc;
   if ((rc = h->finish()) != B2S_OK) return rc;
 
-  const int* ho = static_cast<const int*>(h->hMpOut.p);
-  const float* hf = reinterpret_cast<const float*>(ho);
+  const float *normal = out.host(gNormal), *minD = out.host(gMinD), *maxD = out.host(gMaxD);
+  const int* updated = out.host(gUpdated);
   for (int m = 0; m < nM; m++) {
-    r->updated[m] = (uint8_t)ho[5 * (size_t)nM + m];
+    r->updated[m] = (uint8_t)updated[m];
     if (!r->updated[m]) continue;
-    memcpy(r->normal + 3 * (size_t)m, hf + 3 * (size_t)m, 12);
-    r->min_dist[m] = hf[3 * (size_t)nM + m];
-    r->max_dist[m] = hf[4 * (size_t)nM + m];
+    memcpy(r->normal + 3 * (size_t)m, normal + 3 * (size_t)m, 12);
+    r->min_dist[m] = minD[m];
+    r->max_dist[m] = maxD[m];
   }
   return B2S_OK;
 }
@@ -507,110 +493,77 @@ extern "C" int b2s_process_new_keyframe(b2s_matcher* h, int batch, const b2s_kfi
   B2S_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = h->stream;
   const size_t B = z.B, K = z.K, M = z.M, O = z.O, S = z.S, R = z.R, L = R + S;
-  const size_t nDesc = (B * sizeof(Desc) + 3) / 4;
-  const size_t inN = nDesc + M + 3 * K + K + 2 * S + 3 * M + 6 * M + (M + B) + 3 * O + R + z.F;
-  const size_t outN = 5 * M + O + 3 * M + 2 * M + S + 2 * L + 2 * B, scrN = 2 * M + 2 * (O + M);
-  int rc = grow(h->dMpIn, inN * 4);
-  if (rc == B2S_OK) rc = grow(h->dMpDesc, (O + S) * 32 + 32);
-  if (rc == B2S_OK) rc = grow(h->dMpOut, (outN + scrN) * 4);
-  if (rc == B2S_OK) rc = grow(h->hMpIn, inN * 4 + (O + S) * 32 + 32);
-  if (rc == B2S_OK) rc = grow(h->hMpOut, outN * 4);
+  Packed &in = h->mpIn, &out = h->mpOut;
+  in.clear();
+  const Seg<Desc> gDesc = in.add<Desc>(B);
+  const Seg<int> gProb = in.add<int>(M);
+  const Seg<float> gC = in.add<float>(3 * K);
+  const Seg<int> gKb = in.add<int>(K), gSm = in.add<int>(S), gSs = in.add<int>(S);
+  const Seg<float> gP = in.add<float>(3 * M);
+  const Seg<int> gBad = in.add<int>(M), gRef = in.add<int>(M), gNobs = in.add<int>(M), gFound = in.add<int>(M),
+                 gVis = in.add<int>(M), gFirst = in.add<int>(M), gOff = in.add<int>(M + B), gKf = in.add<int>(O),
+                 gIdx = in.add<int>(O), gOct = in.add<int>(O), gRec = in.add<int>(R);
+  const Seg<float> gSf = in.add<float>(z.F);
+  const Seg<uint8_t> gObsDesc = in.add<uint8_t>(32 * O), gSlotDesc = in.add<uint8_t>(32 * S);
+  out.clear();
+  const Seg<int> gNobsOut = out.add<int>(M), gBadOut = out.add<int>(M), gAdded = out.add<int>(M),
+                 gUpdated = out.add<int>(M), gDescPos = out.add<int>(M), gAlive = out.add<int>(O);
+  const Seg<float> gNormal = out.add<float>(3 * M), gMinD = out.add<float>(M), gMaxD = out.add<float>(M);
+  const Seg<int> gSlot = out.add<int>(S), gList = out.add<int>(L), gVerdict = out.add<int>(L), gNList = out.add<int>(B),
+                 gCulled = out.add<int>(B), gFirstSlot = out.add<int>(M), gFirstEntry = out.add<int>(M),
+                 gGather = out.add<int>(O + M), gGatherPos = out.add<int>(O + M);
+  int rc = in.fit(fn);
+  if (rc == B2S_OK) rc = out.fit(fn);
   if (rc != B2S_OK) return rc;
 
-  // pack: one upload of the ints and floats, one of the descriptors
-  int* q = static_cast<int*>(h->hMpIn.p);
-  uint8_t* qd = reinterpret_cast<uint8_t*>(q + inN);
-  int* dIn = static_cast<int*>(h->dMpIn.p);
-  uint8_t* dDesc = static_cast<uint8_t*>(h->dMpDesc.p);
-  size_t o = 0;
-  auto take = [&](size_t n) {
-    const size_t at = o;
-    o += n;
-    return at;
-  };
-  Args a{};
-  memcpy(q, desc.data(), B * sizeof(Desc));
-  a.desc = reinterpret_cast<const Desc*>(dIn + take(nDesc));
-  const size_t oProb = take(M), oC = take(3 * K), oKb = take(K), oSm = take(S), oSs = take(S), oP = take(3 * M),
-               oBad = take(M), oRef = take(M), oNobs = take(M), oFound = take(M), oVis = take(M), oFirst = take(M),
-               oOff = take(M + B), oKf = take(O), oIdx = take(O), oOct = take(O), oRec = take(R), oSf = take(z.F);
+  // pack: one upload
+  memcpy(in.host(gDesc), desc.data(), B * sizeof(Desc));
   for (int b = 0; b < batch; b++) {
     const b2s_kfinsert_problem& pb = p[b];
     const Desc& d = desc[(size_t)b];
     const int nO = pb.obs_off[pb.n_mp];
     for (int m = 0; m < d.nmp; m++) {
-      q[oProb + d.mp + m] = b;
-      q[oBad + d.mp + m] = pb.mp_bad[m] ? 1 : 0;
-      q[oFirst + d.mp + m] = (int)(uint32_t)(uint64_t)pb.mp_first_kf[m];  // (int)mnFirstKFid
+      in.host(gProb)[d.mp + m] = b;
+      in.host(gBad)[d.mp + m] = pb.mp_bad[m] ? 1 : 0;
+      in.host(gFirst)[d.mp + m] = (int)(uint32_t)(uint64_t)pb.mp_first_kf[m];  // (int)mnFirstKFid
     }
-    memcpy(q + oC + 3 * (size_t)d.kf, pb.kf_center, 12 * (size_t)d.nkf);
-    for (int k = 0; k < d.nkf; k++) q[oKb + d.kf + k] = pb.kf_bad[k] ? 1 : 0;
+    memcpy(in.host(gC) + 3 * (size_t)d.kf, pb.kf_center, 12 * (size_t)d.nkf);
+    for (int k = 0; k < d.nkf; k++) in.host(gKb)[d.kf + k] = pb.kf_bad[k] ? 1 : 0;
     if (d.nslot) {
-      memcpy(q + oSm + d.slot, pb.slot_mp, 4 * (size_t)d.nslot);
-      for (int s = 0; s < d.nslot; s++) q[oSs + d.slot + s] = pb.slot_stereo[s] ? 1 : 0;
-      memcpy(qd + 32 * (O + (size_t)d.slot), pb.slot_desc, 32 * (size_t)d.nslot);
+      memcpy(in.host(gSm) + d.slot, pb.slot_mp, 4 * (size_t)d.nslot);
+      for (int s = 0; s < d.nslot; s++) in.host(gSs)[d.slot + s] = pb.slot_stereo[s] ? 1 : 0;
+      memcpy(in.host(gSlotDesc) + 32 * (size_t)d.slot, pb.slot_desc, 32 * (size_t)d.nslot);
     }
     if (d.nmp) {
-      memcpy(q + oP + 3 * (size_t)d.mp, pb.mp_pos, 12 * (size_t)d.nmp);
-      memcpy(q + oRef + d.mp, pb.mp_ref, 4 * (size_t)d.nmp);
-      memcpy(q + oNobs + d.mp, pb.mp_nobs, 4 * (size_t)d.nmp);
-      memcpy(q + oFound + d.mp, pb.mp_found, 4 * (size_t)d.nmp);
-      memcpy(q + oVis + d.mp, pb.mp_visible, 4 * (size_t)d.nmp);
+      memcpy(in.host(gP) + 3 * (size_t)d.mp, pb.mp_pos, 12 * (size_t)d.nmp);
+      memcpy(in.host(gRef) + d.mp, pb.mp_ref, 4 * (size_t)d.nmp);
+      memcpy(in.host(gNobs) + d.mp, pb.mp_nobs, 4 * (size_t)d.nmp);
+      memcpy(in.host(gFound) + d.mp, pb.mp_found, 4 * (size_t)d.nmp);
+      memcpy(in.host(gVis) + d.mp, pb.mp_visible, 4 * (size_t)d.nmp);
     }
-    memcpy(q + oOff + d.obsOff, pb.obs_off, 4 * (size_t)(d.nmp + 1));
+    memcpy(in.host(gOff) + d.obsOff, pb.obs_off, 4 * (size_t)(d.nmp + 1));
     if (nO) {
-      memcpy(q + oKf + d.obs, pb.obs_kf, 4 * (size_t)nO);
-      memcpy(q + oIdx + d.obs, pb.obs_idx, 4 * (size_t)nO);
-      memcpy(q + oOct + d.obs, pb.obs_octave, 4 * (size_t)nO);
-      memcpy(qd + 32 * (size_t)d.obs, pb.obs_desc, 32 * (size_t)nO);
+      memcpy(in.host(gKf) + d.obs, pb.obs_kf, 4 * (size_t)nO);
+      memcpy(in.host(gIdx) + d.obs, pb.obs_idx, 4 * (size_t)nO);
+      memcpy(in.host(gOct) + d.obs, pb.obs_octave, 4 * (size_t)nO);
+      memcpy(in.host(gObsDesc) + 32 * (size_t)d.obs, pb.obs_desc, 32 * (size_t)nO);
     }
-    if (d.nrec) memcpy(q + oRec + d.rec, pb.recent, 4 * (size_t)d.nrec);
-    memcpy(q + oSf + d.sf, pb.scale_factors, 4 * (size_t)d.nlev);
+    if (d.nrec) memcpy(in.host(gRec) + d.rec, pb.recent, 4 * (size_t)d.nrec);
+    memcpy(in.host(gSf) + d.sf, pb.scale_factors, 4 * (size_t)d.nlev);
   }
-  a.mpProb = dIn + oProb;
-  a.kfC = reinterpret_cast<const float*>(dIn + oC);
-  a.kfBad = dIn + oKb;
-  a.slotMp = dIn + oSm;
-  a.slotSt = dIn + oSs;
-  a.mpPos = reinterpret_cast<const float*>(dIn + oP);
-  a.mpBad = dIn + oBad;
-  a.mpRef = dIn + oRef;
-  a.mpNobs = dIn + oNobs;
-  a.mpFound = dIn + oFound;
-  a.mpVis = dIn + oVis;
-  a.mpFirst = dIn + oFirst;
-  a.obsOff = dIn + oOff;
-  a.obsKf = dIn + oKf;
-  a.obsIdx = dIn + oIdx;
-  a.obsOct = dIn + oOct;
-  a.recent = dIn + oRec;
-  a.sf = reinterpret_cast<const float*>(dIn + oSf);
-  a.obsDesc = dDesc;
-  a.slotDesc = dDesc + 32 * O;
-  int* dOut = static_cast<int*>(h->dMpOut.p);
-  o = 0;
-  a.nobs = dOut + take(M);
-  a.bad = dOut + take(M);
-  a.added = dOut + take(M);
-  a.updated = dOut + take(M);
-  a.descPos = dOut + take(M);
-  a.alive = dOut + take(O);
-  a.normal = reinterpret_cast<float*>(dOut + take(3 * M));
-  a.minD = reinterpret_cast<float*>(dOut + take(M));
-  a.maxD = reinterpret_cast<float*>(dOut + take(M));
-  a.slot = dOut + take(S);
-  a.list = dOut + take(L);
-  a.verdict = dOut + take(L);
-  a.nList = dOut + take(B);
-  a.nCulled = dOut + take(B);
-  a.firstSlot = dOut + take(M);
-  a.firstEntry = dOut + take(M);
-  a.gather = dOut + take(O + M);
-  a.gatherPos = dOut + take(O + M);
+  const Args a = {in.dev(gDesc),       in.dev(gProb),        in.dev(gC),           in.dev(gP),
+                  in.dev(gSf),         in.dev(gKb),          in.dev(gSm),          in.dev(gSs),
+                  in.dev(gBad),        in.dev(gRef),         in.dev(gNobs),        in.dev(gFound),
+                  in.dev(gVis),        in.dev(gFirst),       in.dev(gOff),         in.dev(gKf),
+                  in.dev(gIdx),        in.dev(gOct),         in.dev(gRec),         in.dev(gObsDesc),
+                  in.dev(gSlotDesc),   out.dev(gNobsOut),    out.dev(gBadOut),     out.dev(gAdded),
+                  out.dev(gAlive),     out.dev(gUpdated),    out.dev(gDescPos),    out.dev(gSlot),
+                  out.dev(gList),      out.dev(gVerdict),    out.dev(gNList),      out.dev(gCulled),
+                  out.dev(gNormal),    out.dev(gMinD),       out.dev(gMaxD),       out.dev(gFirstSlot),
+                  out.dev(gFirstEntry), out.dev(gGather),    out.dev(gGatherPos)};
 
   if ((rc = h->begin()) != B2S_OK) return rc;
-  B2S_CUDA(cudaMemcpyAsync(dIn, q, inN * 4, cudaMemcpyHostToDevice, st));
-  if (O + S) B2S_CUDA(cudaMemcpyAsync(dDesc, qd, (O + S) * 32, cudaMemcpyHostToDevice, st));
+  if ((rc = in.upload(st)) != B2S_OK) return rc;
   k_kfi_list<<<batch, kThreads, 0, st>>>(a);
   h->launches++;
   if (M) {
@@ -618,16 +571,14 @@ extern "C" int b2s_process_new_keyframe(b2s_matcher* h, int batch, const b2s_kfi
     h->launches++;
   }
   B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaMemcpyAsync(h->hMpOut.p, dOut, outN * 4, cudaMemcpyDeviceToHost, st));
+  if ((rc = out.download(st, 0, gCulled.end())) != B2S_OK) return rc;  // not the scratch
   if ((rc = h->finish()) != B2S_OK) return rc;
 
-  const int* ho = static_cast<const int*>(h->hMpOut.p);
-  auto at = [&](const void* d) { return ho + (static_cast<const int*>(d) - dOut); };
-  const int *nobs = at(a.nobs), *bad = at(a.bad), *added = at(a.added), *updated = at(a.updated),
-            *descPos = at(a.descPos), *alive = at(a.alive), *slot = at(a.slot), *list = at(a.list),
-            *verdict = at(a.verdict), *nList = at(a.nList), *nCulled = at(a.nCulled);
-  const float *normal = reinterpret_cast<const float*>(at(a.normal)), *minD = reinterpret_cast<const float*>(at(a.minD)),
-              *maxD = reinterpret_cast<const float*>(at(a.maxD));
+  const int *nobs = out.host(gNobsOut), *bad = out.host(gBadOut), *added = out.host(gAdded),
+            *updated = out.host(gUpdated), *descPos = out.host(gDescPos), *alive = out.host(gAlive),
+            *slot = out.host(gSlot), *list = out.host(gList), *verdict = out.host(gVerdict), *nList = out.host(gNList),
+            *nCulled = out.host(gCulled);
+  const float *normal = out.host(gNormal), *minD = out.host(gMinD), *maxD = out.host(gMaxD);
   for (int b = 0; b < batch; b++) {
     const Desc& d = desc[(size_t)b];
     b2s_kfinsert_result& rb = r[b];

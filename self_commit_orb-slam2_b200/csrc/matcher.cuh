@@ -23,7 +23,6 @@ struct b2s_matcher : b2s::Stage {
   b2s::DevBuf dSeqDesc, dSeqDepth, dSeqT, dSeqN;
   // b2s_distinctive_descriptors: descriptors, point offsets and results
   b2s::DevBuf dDistDesc, dDistOff, dDistBest;
-  // b2s_update_normal_and_depth and b2s_process_new_keyframe: packed inputs, descriptors, outputs and scratch
-  b2s::DevBuf dMpIn, dMpDesc, dMpOut;
-  b2s::HostBuf hMpIn, hMpOut;
+  // b2s_update_normal_and_depth and b2s_process_new_keyframe: packed inputs (descriptors included); outputs, then scratch
+  b2s::Packed mpIn, mpOut;
 };

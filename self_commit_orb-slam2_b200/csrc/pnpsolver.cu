@@ -27,7 +27,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <vector>
 
 #include "common.cuh"
 #include "jacobi.cuh"
@@ -695,18 +694,30 @@ using namespace b2s::pnp;
 // ================================================================================================ host side
 struct b2s_pnpsolver : b2s::Stage {
   int maxMatches, maxSets, maxBatch;
-  Prob* prob = nullptr;
-  float *P3Dw = nullptr, *P2D = nullptr, *sig = nullptr, *bestTcw = nullptr;
-  int *sets = nullptr, *cnt = nullptr, *idx = nullptr;
-  uint8_t *bestIn = nullptr, *inl = nullptr, *bestOut = nullptr;
+  int *cnt = nullptr, *idx = nullptr;
   double *hyp = nullptr, *scratch = nullptr;
   uint32_t *mask = nullptr, *carried = nullptr, *refined = nullptr;
-  St* st = nullptr;
-  std::vector<Prob> hProb;
-  std::vector<float> hP3Dw, hP2D, hSig, hBestTcw;
-  std::vector<int> hSets;
-  std::vector<uint8_t> hBestIn, hInl, hBestOut;
-  std::vector<St> hSt;
+  // a call's inputs and outputs, laid out by lay() for its problems, correspondences and sets
+  Packed in, out;
+  Seg<Prob> prob;
+  Seg<float> P3Dw, P2D, sig, bestTcw;
+  Seg<uint8_t> bestIn, inl, bestOut;
+  Seg<int> sets;
+  Seg<St> st;
+  void lay(size_t batch, size_t nm, size_t ns) {
+    in.clear();
+    prob = in.add<Prob>(batch);
+    P3Dw = in.add<float>(nm * 3);
+    P2D = in.add<float>(nm * 2);
+    sig = in.add<float>(nm);
+    bestTcw = in.add<float>(batch * 16);
+    bestIn = in.add<uint8_t>(nm);
+    sets = in.add<int>(ns * 4);
+    out.clear();
+    st = out.add<St>(batch);
+    inl = out.add<uint8_t>(nm);
+    bestOut = out.add<uint8_t>(nm);
+  }
 };
 
 extern "C" int b2s_pnpsolver_create(int max_matches, int max_sets, int max_batch, int device, b2s_pnpsolver** out) {
@@ -726,13 +737,9 @@ extern "C" int b2s_pnpsolver_create(int max_matches, int max_sets, int max_batch
   const size_t B = max_batch, NM = (size_t)max_matches * B, NS = (size_t)max_sets * B;
   const size_t WPB = (size_t)((max_matches + 31) / 32) * B, W = (size_t)((max_matches + 31) / 32) * NS;
   h->open(device);
-  h->alloc(h->prob, B * sizeof(Prob));
-  h->alloc(h->P3Dw, NM * 3 * sizeof(float));
-  h->alloc(h->P2D, NM * 2 * sizeof(float));
-  h->alloc(h->sig, NM * sizeof(float));
-  h->alloc(h->bestTcw, B * 16 * sizeof(float));
-  h->alloc(h->bestIn, NM);
-  h->alloc(h->sets, NS * 4 * sizeof(int));
+  h->lay(B, NM, NS);
+  h->in.reserve(h->error);
+  h->out.reserve(h->error);
   h->alloc(h->hyp, NS * HYP * sizeof(double));
   h->alloc(h->cnt, NS * sizeof(int));
   h->alloc(h->mask, W * sizeof(uint32_t));
@@ -740,9 +747,6 @@ extern "C" int b2s_pnpsolver_create(int max_matches, int max_sets, int max_batch
   h->alloc(h->refined, WPB * sizeof(uint32_t));
   h->alloc(h->scratch, NM * SCR * sizeof(double));
   h->alloc(h->idx, NM * sizeof(int));
-  h->alloc(h->st, B * sizeof(St));
-  h->alloc(h->inl, NM);
-  h->alloc(h->bestOut, NM);
   if (h->error != cudaSuccess) {
     set_error("b2s_pnpsolver_create: %s", cudaGetErrorString(h->error));
     b2s_pnpsolver_destroy(h);
@@ -775,6 +779,7 @@ extern "C" int b2s_pnpsolver_iterate(b2s_pnpsolver* h, int batch, const b2s_pnps
     set_error("b2s_pnpsolver_iterate: batch %d exceeds the handle's capacity %d", batch, h->maxBatch);
     return B2S_ERR_CAPACITY;
   }
+  size_t on = 0, os = 0, om = 0, ow = 0;  // correspondences, sets, mask words and words per problem of the batch
   for (int i = 0; i < batch; i++) {
     const b2s_pnpsolver_problem& q = p[i];
     if (q.n > h->maxMatches || q.k > h->maxSets) {
@@ -801,16 +806,26 @@ extern "C" int b2s_pnpsolver_iterate(b2s_pnpsolver* h, int batch, const b2s_pnps
       set_error("b2s_pnpsolver_iterate: problem %d: set %d entry %d = %d (n = %d)", i, j, l, q.sets[4 * j + l], q.n);
       return B2S_ERR_BAD_ARG;
     }
+    on += (size_t)q.n;
+    os += (size_t)(run ? q.k : 0);
   }
   B2S_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
 
-  h->hProb.resize((size_t)batch);
-  size_t on = 0, os = 0, om = 0, ow = 0;
+  h->lay((size_t)batch, on, os);
+  int rc = h->in.fit("b2s_pnpsolver_iterate");
+  if (rc == B2S_OK) rc = h->out.fit("b2s_pnpsolver_iterate");
+  if (rc != B2S_OK) return rc;
+  Packed &in = h->in, &out = h->out;
+  Prob* prob = in.host(h->prob);
+  float *P3Dw = in.host(h->P3Dw), *P2D = in.host(h->P2D), *sig = in.host(h->sig), *bestTcw = in.host(h->bestTcw);
+  uint8_t* bestIn = in.host(h->bestIn);
+  int* sets = in.host(h->sets);
+  on = os = 0;
   int maxK = 0;
   for (int i = 0; i < batch; i++) {
     const b2s_pnpsolver_problem& q = p[i];
-    Prob& P = h->hProb[(size_t)i];
+    Prob& P = prob[i];
     P.n = q.n;
     P.off = (int)on;
     P.k = q.n >= q.min_inliers ? q.k : 0;
@@ -827,70 +842,46 @@ extern "C" int b2s_pnpsolver_iterate(b2s_pnpsolver* h, int batch, const b2s_pnps
     P.uc = q.uc;
     P.vc = q.vc;
     P.th2 = q.th2;
+    if (q.n > 0) {
+      memcpy(P3Dw + 3 * on, q.P3Dw, 3 * sizeof(float) * q.n);
+      memcpy(P2D + 2 * on, q.P2D, 2 * sizeof(float) * q.n);
+      memcpy(sig + on, q.sigma2, sizeof(float) * q.n);
+      memcpy(bestIn + on, q.best_mask, (size_t)q.n);
+    }
+    memcpy(bestTcw + 16 * (size_t)i, q.best_Tcw, 16 * sizeof(float));
+    if (P.k > 0) memcpy(sets + 4 * os, q.sets, 4 * sizeof(int) * P.k);
     on += (size_t)q.n;
     os += (size_t)P.k;
     om += (size_t)P.k * P.words;
     ow += (size_t)P.words;
     maxK = std::max(maxK, P.k);
   }
-  h->hP3Dw.resize(on * 3);
-  h->hP2D.resize(on * 2);
-  h->hSig.resize(on);
-  h->hBestIn.resize(on);
-  h->hBestTcw.resize((size_t)batch * 16);
-  h->hSets.resize(os * 4);
-  for (int i = 0; i < batch; i++) {
-    const b2s_pnpsolver_problem& q = p[i];
-    const Prob& P = h->hProb[(size_t)i];
-    if (q.n > 0) {
-      memcpy(&h->hP3Dw[3 * (size_t)P.off], q.P3Dw, 3 * sizeof(float) * q.n);
-      memcpy(&h->hP2D[2 * (size_t)P.off], q.P2D, 2 * sizeof(float) * q.n);
-      memcpy(&h->hSig[(size_t)P.off], q.sigma2, sizeof(float) * q.n);
-      memcpy(&h->hBestIn[(size_t)P.off], q.best_mask, (size_t)q.n);
-    }
-    memcpy(&h->hBestTcw[16 * (size_t)i], q.best_Tcw, 16 * sizeof(float));
-    if (P.k > 0) memcpy(&h->hSets[4 * (size_t)P.offSet], q.sets, 4 * sizeof(int) * P.k);
-  }
-  h->hSt.resize((size_t)batch);
-  h->hInl.resize(on);
-  h->hBestOut.resize(on);
 
-  int rc = h->begin();
-  if (rc != B2S_OK) return rc;
-  B2S_CUDA(cudaMemcpyAsync(h->prob, h->hProb.data(), (size_t)batch * sizeof(Prob), cudaMemcpyHostToDevice, s));
-  B2S_CUDA(cudaMemcpyAsync(h->bestTcw, h->hBestTcw.data(), (size_t)batch * 16 * sizeof(float), cudaMemcpyHostToDevice,
-                           s));
-  if (on) {
-    B2S_CUDA(cudaMemcpyAsync(h->P3Dw, h->hP3Dw.data(), on * 3 * sizeof(float), cudaMemcpyHostToDevice, s));
-    B2S_CUDA(cudaMemcpyAsync(h->P2D, h->hP2D.data(), on * 2 * sizeof(float), cudaMemcpyHostToDevice, s));
-    B2S_CUDA(cudaMemcpyAsync(h->sig, h->hSig.data(), on * sizeof(float), cudaMemcpyHostToDevice, s));
-    B2S_CUDA(cudaMemcpyAsync(h->bestIn, h->hBestIn.data(), on, cudaMemcpyHostToDevice, s));
-  }
-  if (os) B2S_CUDA(cudaMemcpyAsync(h->sets, h->hSets.data(), os * 4 * sizeof(int), cudaMemcpyHostToDevice, s));
-  Ptrs a = {h->prob, h->P3Dw,    h->P2D,     h->sig,     h->bestTcw, h->sets, h->bestIn, h->hyp, h->cnt,
-            h->mask, h->carried, h->refined, h->scratch, h->idx,     h->st,   h->inl,    h->bestOut};
+  if ((rc = h->begin()) != B2S_OK) return rc;
+  if ((rc = in.upload(s)) != B2S_OK) return rc;
+  Ptrs a = {in.dev(h->prob), in.dev(h->P3Dw), in.dev(h->P2D), in.dev(h->sig),     in.dev(h->bestTcw), in.dev(h->sets),
+            in.dev(h->bestIn), h->hyp,        h->cnt,         h->mask,            h->carried,         h->refined,
+            h->scratch,        h->idx,        out.dev(h->st), out.dev(h->inl),    out.dev(h->bestOut)};
   if (maxK > 0) {
     k_pnp_hypothesis<<<dim3(maxK, batch), HT, 0, s>>>(a);
     k_pnp_inliers<<<dim3(maxK, batch), CT, 0, s>>>(a);
   }
   k_pnp_scan<<<batch, CT, 0, s>>>(a);
   B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaMemcpyAsync(h->hSt.data(), h->st, (size_t)batch * sizeof(St), cudaMemcpyDeviceToHost, s));
-  if (on) {
-    B2S_CUDA(cudaMemcpyAsync(h->hInl.data(), h->inl, on, cudaMemcpyDeviceToHost, s));
-    B2S_CUDA(cudaMemcpyAsync(h->hBestOut.data(), h->bestOut, on, cudaMemcpyDeviceToHost, s));
-  }
+  if ((rc = out.download(s)) != B2S_OK) return rc;
   if ((rc = h->finish()) != B2S_OK) return rc;
 
+  const St* st = out.host(h->st);
+  const uint8_t *inl = out.host(h->inl), *bestOut = out.host(h->bestOut);
   for (int i = 0; i < batch; i++) {
-    const St& S = h->hSt[(size_t)i];
-    const Prob& P = h->hProb[(size_t)i];
+    const St& S = st[i];
+    const Prob& P = prob[i];
     b2s_pnpsolver_result& R = r[i];
     R.returned = S.returned;
     if (S.returned) memcpy(R.Tcw, S.Tcw, sizeof(R.Tcw));
     if (P.n > 0) {
-      memcpy(R.inliers, &h->hInl[(size_t)P.off], (size_t)P.n);
-      memcpy(R.best_mask, &h->hBestOut[(size_t)P.off], (size_t)P.n);
+      memcpy(R.inliers, inl + P.off, (size_t)P.n);
+      memcpy(R.best_mask, bestOut + P.off, (size_t)P.n);
     }
     R.n_inliers = S.nInl;
     R.no_more = S.noMore;

@@ -24,7 +24,6 @@
 #include <stddef.h>
 
 #include <algorithm>
-#include <vector>
 
 #include "ba_math.cuh"
 #include "common.cuh"
@@ -339,16 +338,23 @@ using namespace b2s::s3o;
 struct b2s_sim3opt_solver : b2s::Stage {
   int maxN, maxBatch;
   long long lastTrials = 0;
-  Prob* prob = nullptr;
-  float* in = nullptr;
-  double *scr = nullptr, *Sout = nullptr;
-  uint8_t* keep = nullptr;
-  int* outI = nullptr;
-  std::vector<Prob> hProb;
-  std::vector<float> hIn;
-  std::vector<double> hSout;
-  std::vector<int> hOutI;
-  std::vector<uint8_t> hKeep;
+  double* scr = nullptr;
+  // a call's inputs and outputs, laid out by lay() for its problems and correspondences
+  Packed in, out;
+  Seg<Prob> prob;
+  Seg<float> corr;
+  Seg<double> Sout;
+  Seg<int> outI;
+  Seg<uint8_t> keep;
+  void lay(size_t batch, size_t n) {
+    in.clear();
+    prob = in.add<Prob>(batch);
+    corr = in.add<float>(n * IN);
+    out.clear();
+    Sout = out.add<double>(batch * 8);
+    outI = out.add<int>(batch * OUT_I);
+    keep = out.add<uint8_t>(n);
+  }
 };
 
 extern "C" int b2s_sim3opt_create(int max_matches, int max_batch, int device, b2s_sim3opt_solver** out) {
@@ -364,12 +370,10 @@ extern "C" int b2s_sim3opt_create(int max_matches, int max_batch, int device, b2
   h->maxBatch = max_batch;
   const size_t M = (size_t)max_matches * max_batch, B = max_batch;
   h->open(device);
-  h->alloc(h->prob, B * sizeof(Prob));
-  h->alloc(h->in, M * IN * sizeof(float));
+  h->lay(B, M);
+  h->in.reserve(h->error);
+  h->out.reserve(h->error);
   h->alloc(h->scr, M * 2 * ES * sizeof(double));
-  h->alloc(h->keep, M);
-  h->alloc(h->Sout, B * 8 * sizeof(double));
-  h->alloc(h->outI, B * OUT_I * sizeof(int));
   cudaError_t e = h->error;
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(k_optimize_sim3, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_N);
@@ -421,13 +425,18 @@ extern "C" int b2s_optimize_sim3(b2s_sim3opt_solver* h, int batch, const b2s_sim
   cudaStream_t s = h->stream;
 
   // ---- pack: one Prob per problem, IN floats per correspondence, problems back to back
-  h->hProb.resize((size_t)batch);
-  h->hIn.resize(std::max<size_t>(total, 1) * IN);
+  h->lay((size_t)batch, total);
+  int rc = h->in.fit("b2s_optimize_sim3");
+  if (rc == B2S_OK) rc = h->out.fit("b2s_optimize_sim3");
+  if (rc != B2S_OK) return rc;
+  Packed &in = h->in, &out = h->out;
+  Prob* prob = in.host(h->prob);
+  float* corr = in.host(h->corr);
   int maxN = 0;
   size_t off = 0;
   for (int i = 0; i < batch; i++) {
     const b2s_sim3_problem& q = p[i];
-    Prob& P = h->hProb[(size_t)i];
+    Prob& P = prob[i];
     P.n = q.n;
     P.off = (int)off;
     P.fixScale = q.fix_scale != 0;
@@ -439,7 +448,7 @@ extern "C" int b2s_optimize_sim3(b2s_sim3opt_solver* h, int batch, const b2s_sim
     for (int k = 0; k < 8; k++) P.K[k] = (double)K[k];
     memcpy(P.S, &q.S12, sizeof(P.S));
     for (int m = 0; m < q.n; m++) {
-      float* c = &h->hIn[(off + (size_t)m) * IN];
+      float* c = corr + (off + (size_t)m) * IN;
       for (int k = 0; k < 3; k++) {
         c[k] = q.X1c[3 * m + k];
         c[3 + k] = q.X2c[3 * m + k];
@@ -454,29 +463,25 @@ extern "C" int b2s_optimize_sim3(b2s_sim3opt_solver* h, int batch, const b2s_sim
     off += (size_t)q.n;
     maxN = std::max(maxN, q.n);
   }
-  h->hSout.resize((size_t)batch * 8);
-  h->hOutI.resize((size_t)batch * OUT_I);
-  h->hKeep.resize(std::max<size_t>(total, 1));
 
-  int rc = h->begin();
-  if (rc != B2S_OK) return rc;
-  B2S_CUDA(cudaMemcpyAsync(h->prob, h->hProb.data(), (size_t)batch * sizeof(Prob), cudaMemcpyHostToDevice, s));
-  if (total) B2S_CUDA(cudaMemcpyAsync(h->in, h->hIn.data(), total * IN * sizeof(float), cudaMemcpyHostToDevice, s));
-  Ptrs a = {h->prob, h->in, h->scr, h->keep, h->Sout, h->outI};
+  if ((rc = h->begin()) != B2S_OK) return rc;
+  if ((rc = in.upload(s)) != B2S_OK) return rc;
+  Ptrs a = {in.dev(h->prob), in.dev(h->corr), h->scr, out.dev(h->keep), out.dev(h->Sout), out.dev(h->outI)};
   const size_t smem = (size_t)((maxN + 15) / 16 * 16);
   k_optimize_sim3<<<batch, T, smem, s>>>(a);
   B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaMemcpyAsync(h->hSout.data(), h->Sout, (size_t)batch * 8 * sizeof(double), cudaMemcpyDeviceToHost, s));
-  B2S_CUDA(cudaMemcpyAsync(h->hOutI.data(), h->outI, (size_t)batch * OUT_I * sizeof(int), cudaMemcpyDeviceToHost, s));
-  if (total) B2S_CUDA(cudaMemcpyAsync(h->hKeep.data(), h->keep, total, cudaMemcpyDeviceToHost, s));
+  if ((rc = out.download(s)) != B2S_OK) return rc;
   if ((rc = h->finish()) != B2S_OK) return rc;
 
+  const double* Sout = out.host(h->Sout);
+  const int* outI = out.host(h->outI);
+  const uint8_t* keep = out.host(h->keep);
   long long trials = 0;
   for (int i = 0; i < batch; i++) {
     b2s_sim3_result& R = r[i];
-    const int* o = &h->hOutI[(size_t)i * OUT_I];
-    memcpy(&R.S12_out, &h->hSout[(size_t)i * 8], 8 * sizeof(double));
-    if (p[i].n) memcpy(R.keep, &h->hKeep[(size_t)h->hProb[(size_t)i].off], (size_t)p[i].n);
+    const int* o = outI + (size_t)i * OUT_I;
+    memcpy(&R.S12_out, Sout + (size_t)i * 8, 8 * sizeof(double));
+    if (p[i].n) memcpy(R.keep, keep + prob[i].off, (size_t)p[i].n);
     R.n_inliers = o[0];
     R.n_trials = o[1];
     if (R.trace) {

@@ -19,7 +19,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <vector>
 
 #include "common.cuh"
 
@@ -389,17 +388,28 @@ using namespace b2s::s3s;
 // ================================================================================================ host side
 struct b2s_sim3solver : b2s::Stage {
   int maxMatches, maxSets, maxBatch;
-  Prob* prob = nullptr;
-  float *X1 = nullptr, *X2 = nullptr, *sig1 = nullptr, *sig2 = nullptr, *hyp = nullptr;
-  int *sets = nullptr, *cnt = nullptr;
+  float* hyp = nullptr;
+  int* cnt = nullptr;
   uint32_t* mask = nullptr;
-  St* st = nullptr;
-  uint8_t* inl = nullptr;
-  std::vector<Prob> hProb;
-  std::vector<float> hX1, hX2, hSig1, hSig2;
-  std::vector<int> hSets;
-  std::vector<St> hSt;
-  std::vector<uint8_t> hInl;
+  // a call's inputs and outputs, laid out by lay() for its problems, correspondences and sets
+  Packed in, out;
+  Seg<Prob> prob;
+  Seg<float> X1, X2, sig1, sig2;
+  Seg<int> sets;
+  Seg<St> st;
+  Seg<uint8_t> inl;
+  void lay(size_t batch, size_t nm, size_t ns) {
+    in.clear();
+    prob = in.add<Prob>(batch);
+    X1 = in.add<float>(nm * 3);
+    X2 = in.add<float>(nm * 3);
+    sig1 = in.add<float>(nm);
+    sig2 = in.add<float>(nm);
+    sets = in.add<int>(ns * 3);
+    out.clear();
+    st = out.add<St>(batch);
+    inl = out.add<uint8_t>(nm);
+  }
 };
 
 extern "C" int b2s_sim3solver_create(int max_matches, int max_sets, int max_batch, int device, b2s_sim3solver** out) {
@@ -418,17 +428,12 @@ extern "C" int b2s_sim3solver_create(int max_matches, int max_sets, int max_batc
   const size_t B = max_batch, NM = (size_t)max_matches * B, NS = (size_t)max_sets * B;
   const size_t W = (size_t)((max_matches + 31) / 32) * NS;
   h->open(device);
-  h->alloc(h->prob, B * sizeof(Prob));
-  h->alloc(h->X1, NM * 3 * sizeof(float));
-  h->alloc(h->X2, NM * 3 * sizeof(float));
-  h->alloc(h->sig1, NM * sizeof(float));
-  h->alloc(h->sig2, NM * sizeof(float));
-  h->alloc(h->sets, NS * 3 * sizeof(int));
+  h->lay(B, NM, NS);
+  h->in.reserve(h->error);
+  h->out.reserve(h->error);
   h->alloc(h->hyp, NS * HYP * sizeof(float));
   h->alloc(h->cnt, NS * sizeof(int));
   h->alloc(h->mask, W * sizeof(uint32_t));
-  h->alloc(h->st, B * sizeof(St));
-  h->alloc(h->inl, NM);
   if (h->error != cudaSuccess) {
     set_error("b2s_sim3solver_create: %s", cudaGetErrorString(h->error));
     b2s_sim3solver_destroy(h);
@@ -456,6 +461,7 @@ extern "C" int b2s_sim3solver_iterate(b2s_sim3solver* h, int batch, const b2s_si
     set_error("b2s_sim3solver_iterate: batch %d exceeds the handle's capacity %d", batch, h->maxBatch);
     return B2S_ERR_CAPACITY;
   }
+  size_t on = 0, os = 0, om = 0;  // correspondences, sets and mask words of the batch
   for (int i = 0; i < batch; i++) {
     const b2s_sim3solver_problem& q = p[i];
     if (q.n > h->maxMatches || q.k > h->maxSets) {
@@ -480,16 +486,24 @@ extern "C" int b2s_sim3solver_iterate(b2s_sim3solver* h, int batch, const b2s_si
       set_error("b2s_sim3solver_iterate: problem %d: set %d entry %d = %d (n = %d)", i, j, l, q.sets[3 * j + l], q.n);
       return B2S_ERR_BAD_ARG;
     }
+    on += (size_t)q.n;
+    os += (size_t)(run ? q.k : 0);
   }
   B2S_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
 
-  h->hProb.resize((size_t)batch);
-  size_t on = 0, os = 0, om = 0;
+  h->lay((size_t)batch, on, os);
+  int rc = h->in.fit("b2s_sim3solver_iterate");
+  if (rc == B2S_OK) rc = h->out.fit("b2s_sim3solver_iterate");
+  if (rc != B2S_OK) return rc;
+  Prob* prob = h->in.host(h->prob);
+  float *X1 = h->in.host(h->X1), *X2 = h->in.host(h->X2), *sig1 = h->in.host(h->sig1), *sig2 = h->in.host(h->sig2);
+  int* sets = h->in.host(h->sets);
+  on = os = 0;
   int maxK = 0;
   for (int i = 0; i < batch; i++) {
     const b2s_sim3solver_problem& q = p[i];
-    Prob& P = h->hProb[(size_t)i];
+    Prob& P = prob[i];
     P.n = q.n;
     P.off = (int)on;
     P.k = q.n >= q.min_inliers ? q.k : 0;
@@ -503,54 +517,38 @@ extern "C" int b2s_sim3solver_iterate(b2s_sim3solver* h, int batch, const b2s_si
     P.best = q.best_inliers;
     memcpy(P.K1, q.K1, sizeof(P.K1));
     memcpy(P.K2, q.K2, sizeof(P.K2));
+    if (q.n > 0) {
+      memcpy(X1 + 3 * on, q.X1c, 3 * sizeof(float) * q.n);
+      memcpy(X2 + 3 * on, q.X2c, 3 * sizeof(float) * q.n);
+      memcpy(sig1 + on, q.sigma2_1, sizeof(float) * q.n);
+      memcpy(sig2 + on, q.sigma2_2, sizeof(float) * q.n);
+    }
+    if (P.k > 0) memcpy(sets + 3 * os, q.sets, 3 * sizeof(int) * P.k);
     on += (size_t)q.n;
     os += (size_t)P.k;
     om += (size_t)P.k * P.words;
     maxK = std::max(maxK, P.k);
   }
-  h->hX1.resize(on * 3);
-  h->hX2.resize(on * 3);
-  h->hSig1.resize(on);
-  h->hSig2.resize(on);
-  h->hSets.resize(os * 3);
-  for (int i = 0; i < batch; i++) {
-    const b2s_sim3solver_problem& q = p[i];
-    const Prob& P = h->hProb[(size_t)i];
-    if (q.n > 0) {
-      memcpy(&h->hX1[3 * (size_t)P.off], q.X1c, 3 * sizeof(float) * q.n);
-      memcpy(&h->hX2[3 * (size_t)P.off], q.X2c, 3 * sizeof(float) * q.n);
-      memcpy(&h->hSig1[(size_t)P.off], q.sigma2_1, sizeof(float) * q.n);
-      memcpy(&h->hSig2[(size_t)P.off], q.sigma2_2, sizeof(float) * q.n);
-    }
-    if (P.k > 0) memcpy(&h->hSets[3 * (size_t)P.offSet], q.sets, 3 * sizeof(int) * P.k);
-  }
-  h->hSt.resize((size_t)batch);
-  h->hInl.resize(on);
 
-  int rc = h->begin();
-  if (rc != B2S_OK) return rc;
-  B2S_CUDA(cudaMemcpyAsync(h->prob, h->hProb.data(), (size_t)batch * sizeof(Prob), cudaMemcpyHostToDevice, s));
-  if (on) {
-    B2S_CUDA(cudaMemcpyAsync(h->X1, h->hX1.data(), on * 3 * sizeof(float), cudaMemcpyHostToDevice, s));
-    B2S_CUDA(cudaMemcpyAsync(h->X2, h->hX2.data(), on * 3 * sizeof(float), cudaMemcpyHostToDevice, s));
-    B2S_CUDA(cudaMemcpyAsync(h->sig1, h->hSig1.data(), on * sizeof(float), cudaMemcpyHostToDevice, s));
-    B2S_CUDA(cudaMemcpyAsync(h->sig2, h->hSig2.data(), on * sizeof(float), cudaMemcpyHostToDevice, s));
-  }
-  if (os) B2S_CUDA(cudaMemcpyAsync(h->sets, h->hSets.data(), os * 3 * sizeof(int), cudaMemcpyHostToDevice, s));
-  Ptrs a = {h->prob, h->X1, h->X2, h->sig1, h->sig2, h->sets, h->hyp, h->cnt, h->mask, h->st, h->inl};
+  if ((rc = h->begin()) != B2S_OK) return rc;
+  if ((rc = h->in.upload(s)) != B2S_OK) return rc;
+  const Packed &in = h->in, &out = h->out;
+  Ptrs a = {in.dev(h->prob), in.dev(h->X1), in.dev(h->X2), in.dev(h->sig1), in.dev(h->sig2), in.dev(h->sets),
+            h->hyp,          h->cnt,        h->mask,       out.dev(h->st),  out.dev(h->inl)};
   if (maxK > 0) {
     k_s3s_hypothesis<<<dim3((maxK + 63) / 64, batch), 64, 0, s>>>(a);
     k_s3s_inliers<<<dim3(maxK, batch), CT, 0, s>>>(a);
   }
   k_s3s_scan<<<batch, CT, 0, s>>>(a);
   B2S_CUDA(cudaGetLastError());
-  B2S_CUDA(cudaMemcpyAsync(h->hSt.data(), h->st, (size_t)batch * sizeof(St), cudaMemcpyDeviceToHost, s));
-  if (on) B2S_CUDA(cudaMemcpyAsync(h->hInl.data(), h->inl, on, cudaMemcpyDeviceToHost, s));
+  if ((rc = out.download(s)) != B2S_OK) return rc;
   if ((rc = h->finish()) != B2S_OK) return rc;
 
+  const St* st = out.host(h->st);
+  const uint8_t* inl = out.host(h->inl);
   for (int i = 0; i < batch; i++) {
-    const St& S = h->hSt[(size_t)i];
-    const Prob& P = h->hProb[(size_t)i];
+    const St& S = st[i];
+    const Prob& P = prob[i];
     b2s_sim3solver_result& R = r[i];
     R.returned = S.returned;
     R.best_changed = S.changedIdx >= 0;
@@ -561,7 +559,7 @@ extern "C" int b2s_sim3solver_iterate(b2s_sim3solver* h, int batch, const b2s_si
       R.s = hy[12];
       if (S.returned) memcpy(R.T12, hy + 13, sizeof(R.T12));
     }
-    if (P.n > 0) memcpy(R.inliers, &h->hInl[(size_t)P.off], (size_t)P.n);
+    if (P.n > 0) memcpy(R.inliers, inl + P.off, (size_t)P.n);
     R.n_inliers = S.nInl;
     R.no_more = S.noMore;
     R.iterations_used = S.used;
