@@ -143,6 +143,8 @@ def build_oracle_ref():
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "culling.mk", "culling-ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "kfinsert.mk", "kfinsert-ref", "REF=" + ref])
     subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "undistort.mk", "undistort-ref", "REF=" + ref])
+    # the reference's Frame.cc and the drop-in Frame_b200.cc behind one glue (oracle/frame.mk)
+    subprocess.check_call(["make", "-s", "-j8", "-C", ORACLE_DIR, "-f", "frame.mk", "frame-ref", "REF=" + ref])
     return os.path.join(ORACLE_DIR, "_ref")
 
 

@@ -1,5 +1,7 @@
 // cv_compat.h — the few OpenCV types the hot-path signatures mention.
-// With -DB2S_HAVE_OPENCV the real OpenCV headers are used (drop-in build inside ORB-SLAM2); otherwise
+// With -DB2S_HAVE_OPENCV the real OpenCV headers are used (drop-in build inside ORB-SLAM2), or whichever
+// <opencv2/core/core.hpp> the include path finds first: the parity builds of oracle/frame.mk put oracle/refshim's cv
+// stand-in there, so the drop-in ORBextractor and Frame compile behind the reference's glue without OpenCV; otherwise
 // layout-compatible stand-ins are declared so the shim and its tests build where OpenCV C++ is absent.
 #pragma once
 #ifdef B2S_HAVE_OPENCV
