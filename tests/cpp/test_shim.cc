@@ -1,11 +1,10 @@
-// C++ test of the reference-signature shim classes (ORB_SLAM2::ORBextractor / ORBmatcher / Optimizer).
+// C++ test of the reference-signature drop-in ORB_SLAM2::ORBextractor.
 // Reads a raw 8-bit image, runs operator(), writes keypoints+descriptors for the Python side to compare with the oracle.
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
 
 #include "../../self_commit_orb-slam2_b200/host/ORBextractor.h"
-#include "../../self_commit_orb-slam2_b200/host/ORBmatcher.h"
 
 int main(int argc, char** argv) {
   if (argc < 5) return 2;
@@ -33,7 +32,6 @@ int main(int argc, char** argv) {
   std::vector<b2s_cv::KeyPoint> k2(3);
   ex(empty, mask, k2, desc);
   if (k2.size() != 3) return 7;
-  if (ORB_SLAM2::ORBmatcher::DescriptorDistance(desc.ptr(0), desc.ptr(0)) != 0) return 8;
   printf("shim ok %d keypoints\n", n);
   return 0;
 }

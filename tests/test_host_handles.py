@@ -1,7 +1,7 @@
-"""The host layer's handle policy (self_commit_orb-slam2_b200/host/b2s_host.h), which the flattened entries (host/*.cc)
-and the drop-in adapters (host/adapters/*.cc) share: the grow-on-demand slot against a fake handle, the device choice,
-the error line, that every flattened entry compiles, and that no stage's result depends on the capacity of the handle
-it runs on (a slot only grows, so a call may run on a handle larger than the one it needed)."""
+"""The host layer's handle policy (self_commit_orb-slam2_b200/host/b2s_host.h), which the drop-ins (host/*.cc and
+host/adapters/*.cc) share: the grow-on-demand slot against a fake handle, the device choice, the error line, that every
+host/*.cc compiles on its own, and that no stage's result depends on the capacity of the handle it runs on (a slot only
+grows, so a call may run on a handle larger than the one it needed)."""
 import glob
 import os
 import shutil
@@ -59,7 +59,9 @@ def test_report_and_fail(harness):
 
 
 @pytest.mark.parametrize("source", sorted(os.path.basename(p) for p in glob.glob(os.path.join(HOST, "*.cc"))))
-def test_flattened_entry_compiles(source):
+def test_host_source_compiles(source):
+    """Each drop-in under host/ (ORBextractor.cc, ORBVocabulary.cc) compiles warning-free against the C ABI header,
+    without OpenCV or the reference's headers."""
     out = subprocess.run([_gxx(), "-std=c++14", "-fsyntax-only", "-Wall", "-Wextra", "-Werror",
                           "-I", os.path.join(ROOT, "include"), os.path.join(HOST, source)],
                          stdout=subprocess.PIPE, stderr=subprocess.STDOUT)

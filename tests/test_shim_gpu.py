@@ -15,7 +15,7 @@ def test_cpp_extractor_shim(pkg, oracle, tmp_path):
     host = os.path.join(ROOT, "self_commit_orb-slam2_b200", "host")
     exe = str(tmp_path / "test_shim")
     subprocess.check_call(["g++", "-O2", "-std=c++17", "-o", exe, os.path.join(ROOT, "tests", "cpp", "test_shim.cc"),
-                           os.path.join(host, "ORBextractor.cc"), os.path.join(host, "ORBmatcher.cc"), pkg.LIB_PATH,
+                           os.path.join(host, "ORBextractor.cc"), pkg.LIB_PATH,
                            "-Wl,-rpath," + os.path.dirname(pkg.LIB_PATH)])
     img = synth_image(640, 480, 6)
     raw = str(tmp_path / "img.raw")
